@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py - augmented images/sec of the Fast AutoAugment hot path on B200.
+"""bench.py - augmented images/sec of the Fast AutoAugment hot path on H100.
 
     python bench.py --gpus N --steps K --warmup W            (ours; N>1 via torchrun)
     python bench.py --impl reference --gpus N --steps K --warmup W   (CPU PIL path, rank 0 only)
+    python bench.py ... --dump-outputs DIR     (also write the last timed step's output, rank 0, as DIR/*.npy)
 
 A "step" is one pass of the hot path over one batch of synthetic uint8 HWC images:
 policy ops -> HFlip -> ToTensor -> Normalize -> NCHW fp16, with the per-sample decisions
@@ -12,8 +13,8 @@ every rank processes its own 512-image shard, no data-path collective (images ar
 independent; SURVEY.md 8e).
 
 The JSON line carries the device-timed `value`, the host-buffer `e2e`, the HBM `roofline`
-of the fused kernel (algorithmic bytes 9*H*W per image / measured launch time / measured
-copy peak) and the CPU `cpu_baseline` (the reference's PIL/torchvision call sequence as
+of the fused kernel (algorithmic bytes 9*H*W per image / measured launch time / the measured copy
+peak of MEASURED_PEAKS.json, or the H100 SXM data-sheet HBM3 bandwidth without it) and the CPU `cpu_baseline` (the reference's PIL/torchvision call sequence as
 restated in oracle/pil_path.py, run through a torch DataLoader like reference data.py:214).
 """
 from __future__ import annotations
@@ -92,8 +93,12 @@ def _cpu_chain(workload):
     try:
         from oracle import build_ref
         mods = build_ref.import_ref()
-    except Exception:
+    except Exception as e:          # noqa: BLE001 - reported below, the port is timed instead
         mods = None
+        sys.stderr.write("[bench] oracle/_ref could not be imported (%s: %s)\n" % (type(e).__name__, e))
+    if mods is None:
+        sys.stderr.write("[bench] cpu_baseline times the oracle's restatement of the reference (kind \"port\"), "
+                         "not the reference's own classes: oracle/_ref is not available\n")
     if mods is not None:
         from torchvision import transforms
         _, ref_archive, _, ref_data = mods
@@ -147,6 +152,16 @@ def cpu_throughput(workload, n_batches, warm_batches, workers):
     dt = time.perf_counter() - t0
     del it
     return n / dt, dt, kind
+
+
+def gpu_power_limit(gpu_index):
+    """the card's power limit in W (part of every number measured on it), None when nvidia-smi is unavailable"""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(gpu_index), "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=30).stdout
+        return float(out.strip().splitlines()[0])
+    except Exception:
+        return None
 
 
 def host_cores():
@@ -212,22 +227,28 @@ class ClockSampler:
                 "samples": len(sm)}
 
 
-def measured_peak():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
+def hbm_peak():
+    """(GB/s, source): a measured copy peak when the machine provides MEASURED_PEAKS.json, else the data sheet"""
     try:
-        with open(p) as f:
+        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, STREAM-style copy)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback: H100 SXM data sheet (3.35 TB/s HBM3, 700 W card); not a measured copy rate"
 
 
-def ncu_traffic(workload):
-    """per-launch DRAM bytes of the fused kernel from the committed ncu capture, if any"""
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            return json.load(f).get(workload)
-    except Exception:
-        return None
+DUMP_BYTES = 64_000_000          # --dump-outputs: at most this many bytes of .npy data
+
+
+def dump_outputs(out_dir, out):
+    """The output tensor of the last timed step as float32 DIR/augmented.npy: every image when they fit DUMP_BYTES,
+    else a fixed sample of images (numpy default_rng(0), sorted indices) - the same images in every run."""
+    import numpy as np
+    import torch
+    n = out.shape[0]
+    k = min(n, (DUMP_BYTES - 4096) // (out[0].numel() * 4))
+    idx = np.arange(n) if k == n else np.sort(np.random.default_rng(0).choice(n, k, replace=False))
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "augmented.npy"), out[torch.from_numpy(idx).to(out.device)].float().cpu().numpy())
 
 
 # --------------------------------------------------------------------------------------
@@ -242,7 +263,7 @@ def workload_string(name):
 
 class _Workload:
     """Device-resident buffers + the pre-bound launch of one workload on this rank."""
-    NSETS = 4      # input/output sets rotate so that no step finds its data in the 126 MB L2
+    NSETS = 4      # input/output sets rotate so that no step finds its data in L2 (50 MB on H100)
 
     def __init__(self, name, seed, rank, world):
         import torch
@@ -286,11 +307,11 @@ class _Workload:
         return ev0.elapsed_time(ev1), t0, time.perf_counter()
 
     def roofline(self, ms_per_step):
-        peak, peak_src = measured_peak()
+        peak, peak_src = hbm_peak()
         alg = self.in_bytes + self.out_bytes          # 3HW read + 6 out_h out_w written (= 9HW when no crop)
         ach = alg / (ms_per_step / 1e3) / 1e9
         return {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                "traffic": ncu_traffic(self.name), "peak_source": peak_src, "algorithmic_bytes_per_launch": alg,
+                "peak_source": peak_src, "algorithmic_bytes_per_launch": alg,
                 "kernel": "faa_augment_mid_kernel + faa_augment_light_kernel (+ faa_augment_kernel for crops / odd widths); one step = one pass over the batch"}
 
 
@@ -310,7 +331,7 @@ def measure_mixup(args, rank, world, barrier, max_over_ranks):
     tail = TailSpec.imagenet(0, torch.float16)
     xs = [torch.from_numpy(synth_batch(b, H, W, 4321 + rank + 17 * i)).cuda() for i in range(2)]
     y = torch.arange(rank * b, (rank + 1) * b, device="cuda")
-    steps = max(10, min(args.steps, 50))
+    steps = args.steps
     tim = {}
     # world > 1: the exchange is fused into the mix kernel (partners read over NVLink peer memory); FAA_MIXUP_A2A=1 or a
     # failing peer mapping selects the NCCL all-to-all route
@@ -353,7 +374,7 @@ def measure_mixup(args, rank, world, barrier, max_over_ranks):
     mix_ms = sum(t["m0"].elapsed_time(t["m1"]) for t in pairs) / steps
     ms, ex_ms, aug_ms, mix_ms = max_over_ranks([ms, ex_ms, aug_ms, mix_ms])
     alg = G * 9 * H * W
-    peak, _ = measured_peak()
+    peak, _ = hbm_peak()
     return {"workload": "imagenet224_b2048_mixup: synthetic uint8 HWC 224x224, GLOBAL batch 2048 (%d per GPU), fa_resnet50_rimagenet policy, "
                         "HFlip+ToTensor+Normalize(ImageNet), Mixup alpha 0.2 with global pairing -> NCHW fp16" % b,
             "value": G * steps / (ms / 1e3), "unit": "images/s", "steps": steps, "ms_per_step": ms / steps, "scaling": "strong",
@@ -501,6 +522,8 @@ def run_ours(args):
     launches0 = _lib.lib.faa_launch_count()
     ms_local, t0, t1 = wl.timed(args.steps, args.warmup, barrier)
     launches = int(_lib.lib.faa_launch_count() - launches0)
+    if args.dump_outputs and rank == 0:        # before any later step rewrites the rotating output buffers
+        dump_outputs(args.dump_outputs, wl.outs[(args.warmup + args.steps - 1) % wl.NSETS])
     # keep the GPU busy a little longer if the region was too short for a clock sample
     if t1 - t0 < 0.4:
         tb = time.perf_counter()
@@ -542,7 +565,7 @@ def run_ours(args):
     also = {}
     for name in ([] if args.no_also else [n for n in ("cifar32_b512", "effnetb4_380_b256") if n != args.workload]):
         w2 = _Workload(name, args.seed, rank, world)
-        k2 = max(args.steps, 300)
+        k2 = args.steps
         ms2, _, _ = w2.timed(k2, max(args.warmup, 5), barrier)
         ms2 = max_over_ranks([ms2])[0]
         also[name] = {"value": world * w2.B * k2 / (ms2 / 1e3), "unit": "images/s", "steps": k2, "ms_per_step": ms2 / k2,
@@ -572,8 +595,10 @@ def run_ours(args):
             "scaling": "weak", "vs_baseline": None, "dtype": "u8", "data": "synthetic",
             "config": {"workload": workload_string(args.workload), "out_dtype": "fp16", "sampler": "fused Philox4x32-10 (device)",
                        "global_batch": world * B, "parallelism": "dp%d (independent shards, no collective)" % world,
-                       "l2": "inputs/outputs rotate over %d buffer sets (%.0f MB) > 126 MB L2" % (
-                           wl.NSETS, wl.NSETS * (wl.in_bytes + wl.out_bytes) / 1e6)},
+                       "l2": "inputs/outputs rotate over %d buffer sets (%.0f MB) > %.0f MB L2" % (
+                           wl.NSETS, wl.NSETS * (wl.in_bytes + wl.out_bytes) / 1e6,
+                           torch.cuda.get_device_properties(local).L2_cache_size / 1e6)},
+            "gpu": {"name": torch.cuda.get_device_name(local), "power_limit_w": gpu_power_limit(local)},
             "clocks": clk,
             "e2e": {"value": total / (ms_rt / 1e3), "unit": "images/s", "h2d_bytes_per_step": wl.in_bytes,
                     "d2h_bytes_per_step": wl.out_bytes,
@@ -601,8 +626,8 @@ def run_ours(args):
                                     "sample": "%d batches of %d through the reference's Augmentation + torchvision chain in a torch "
                                               "DataLoader with %d workers (reference data.py:215), first batches excluded; %.1f s; "
                                               "one_core = the same chain in the main process (num_workers=0)" % (nb, B, workers, dt),
-                                    "note": "the reference's DataLoader architecture is main-process-bound beyond ~8 workers "
-                                            "(per-worker rate drops from ~700 to ~60 img/s at 128 workers): see --impl reference"}
+                                    "note": "the reference's DataLoader architecture is main-process-bound with many workers: "
+                                            "see --impl reference"}
         print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()
@@ -647,6 +672,8 @@ def main():
     ap.add_argument("--seed", type=int, default=2024)
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-also", action="store_true", help="skip the extra single-GPU configurations (CIFAR b512, 380x380 b256)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's output (rank 0) as DIR/augmented.npy, "
+                                                          "float32, at most 64 MB (a fixed sample of images beyond that)")
     args = ap.parse_args()
     args.warmup = max(3, args.warmup) if args.impl == "ours" else args.warmup
     if args.impl == "reference":

@@ -1,4 +1,4 @@
-"""fast_autoaugment_b200 - B200-native (sm_100a CUDA) implementation of Fast AutoAugment's
+"""fast_autoaugment_b200 - H100-native (sm_90a CUDA) implementation of Fast AutoAugment's
 per-batch augmentation hot path, behind the reference's own Python surface.
 
 Reference (kakaobrain/fast-autoaugment) module  ->  this package

@@ -1,6 +1,6 @@
 """ctypes binding of ``libfaa_b200.so`` (the C ABI of ``include/faa_b200.h``).
 
-The shared library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_100a).
+The shared library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_90a).
 There is no Python / CPU implementation of the pixel path behind this module: if the
 library is missing, importing the package fails loudly.
 """
@@ -42,7 +42,7 @@ class Rng(C.Structure):           # faa_rng_t
 def _load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
-            "fast_autoaugment_b200: %s is missing. The augmentation path is CUDA-only (sm_100a) "
+            "fast_autoaugment_b200: %s is missing. The augmentation path is CUDA-only (sm_90a) "
             "and has no CPU fallback - build it with `python -c 'import __graft_entry__ as g; "
             "g.build()'` (needs nvcc)." % LIB_PATH)
     lib = C.CDLL(LIB_PATH)

@@ -707,7 +707,7 @@ static int augment_common(faa_policy_t* p, const uint8_t* d_in_all, int n_all, i
     // overlap (the next step's CTAs fill the slots the previous step's tail frees); the only true dependency -
     // programs written by the resolve kernel - is a ticket word the pixel kernels poll.  FAA_CHAIN=0: the
     // two-stream schedule with events (light kernel on the caller's stream, cluster kernel on a priority stream).
-    int chain_mode = 1;                                   // measured (profiles/r02_schedules.txt): 62.4 us chained vs 65.6 us with events
+    int chain_mode = 1;
     if (const char* e = getenv("FAA_CHAIN")) chain_mode = atoi(e);
     // (launches too small to split are chained as well: resolve(N+1), cluster(N) - their step is bound by kernel latencies,
     //  which only overlap across steps on one stream; uint8 output stays on the event schedule)
@@ -804,7 +804,7 @@ static int augment_common(faa_policy_t* p, const uint8_t* d_in_all, int n_all, i
         // its program; a step that touches the previous step's buffers is launched as a plain stream-ordered kernel instead
         Ps.chain = overlap_ok ? 1 : 0; Ps.pdl = 0;
         // Only for tiny images (CIFAR): there the one-block resolve kernel is as long as the pixel kernel; for larger images
-        // every band CTA would repeat ~10 us of serial work (measured: 224x224 b2048 uint8 launches 0.90 -> 0.97 ms).
+        // every band CTA would repeat the whole serial resolve work.
         // Sharpness -> gather programs are evaluated lazily instead of through the scratch image - the last thing consecutive
         // steps shared - and every CTA releases the next step at once (chain = 3).
         Ps.sr_allow &= ~2; Ps.scratch = nullptr;
@@ -906,8 +906,7 @@ static int augment_common(faa_policy_t* p, const uint8_t* d_in_all, int n_all, i
             static const int rows_m = [] { const char* e = getenv("FAA_ROWS_MID"); return e ? atoi(e) : 0; }();
             const int lb = P.geo[1].bands > 0 ? P.geo[1].bands : 1;
             Pc.grid_y = rows_l > 0 ? rows_l : (p->sm_count * resident_ctas_per_sm(1)) / lb;
-            // (mid rows: ONE CTA per SM measured best - 58.1 us vs 58.9 us with both slots - the light CTAs that follow
-            //  share the SM with it from the start; profiles/r02_schedules.txt)
+            // (mid rows: ONE CTA per SM, so that the light CTAs that follow share the SM with it from the start)
             Pm.grid_y = rows_m > 0 ? rows_m : p->sm_count / (Pm.bands > 0 ? Pm.bands : 1);
             if (Pc.grid_y < 1) Pc.grid_y = 1;
             if (Pm.grid_y < 1) Pm.grid_y = 1;
@@ -1004,7 +1003,7 @@ static int augment_common(faa_policy_t* p, const uint8_t* d_in_all, int n_all, i
             if (use_mid && !mid_same) CK(cudaStreamWaitEvent(p->mid_stream, p->ev_res, 0));
             // the streaming kernel goes FIRST: it fills the machine at once; the priority streams' clusters then take
             // the slots its CTAs free (launched first, the thousands of exiting CTAs of the cluster kernels would hold
-            // up the work distributor: measured +10 us per step)
+            // up the work distributor)
             if (order_knob == 0) CK(launch_augment(P, tail->out_dtype, use_tab, 1, stream));
             if (!no_heavy) CK(launch_augment(Ph, tail->out_dtype, use_tab, 0, p->light_stream)); else g_launches--;
             if (order_knob == 1) CK(launch_augment(P, tail->out_dtype, use_tab, 1, stream));

@@ -1,5 +1,5 @@
 // faa_core.cuh - per-pixel arithmetic of the augmentation hot path, shared by the
-// sm_100a kernels (faa_kernels.cu) and by the host-side emulation used in the CPU
+// sm_90a kernels (faa_kernels.cu) and by the host-side emulation used in the CPU
 // tests (tests/emu).  Every function states the reference call it reproduces
 // (file:line relative to kakaobrain/fast-autoaugment @ 2424224) and the Pillow /
 // torchvision arithmetic behind that call (SURVEY.md 8a).

@@ -11,7 +11,7 @@
 //                       global memory (L1), no staged-copy test, no branches between the loads
 //   Color               ImageEnhance.Color (augmentations.py:102-104) with the fp32 blend kept on the FMA
 //                       pipe: byte -> float through the 1.5*2^23 bias trick, truncation through a
-//                       round-toward-zero add, no I2F / F2I (the conversion unit is 1/8 rate on sm_100)
+//                       round-toward-zero add, no I2F / F2I (the conversion unit runs at a fraction of the FMA rate)
 //   Cutout              the streaming loop plus a box test per octet (augmentations.py:126-144)
 // A per-channel LUT in the program's other slot rides for free: the float table already composes
 // LUT o ToTensor o Normalize; only the fill colour depends on the order of the two ops.
@@ -295,10 +295,8 @@ __device__ __forceinline__ void final_rows_gather_t(const AugParams& P, const fl
 #pragma unroll
                     for (int k = 0; k < 4; ++k) v[k] = tab[ch * 256 + ((px[k] >> (8 * ch)) & 255u)];
                 } else {
-                    const float2 sc = make_float2(P.scale[ch], P.scale[ch]), bi = make_float2(P.bias[ch], P.bias[ch]);
-                    const float2 r0 = __ffma2_rn(make_float2((float)((px[0] >> (8 * ch)) & 255u), (float)((px[1] >> (8 * ch)) & 255u)), sc, bi);
-                    const float2 r1 = __ffma2_rn(make_float2((float)((px[2] >> (8 * ch)) & 255u), (float)((px[3] >> (8 * ch)) & 255u)), sc, bi);
-                    v[0] = r0.x; v[1] = r0.y; v[2] = r1.x; v[3] = r1.y;
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) v[k] = __fmaf_rn((float)((px[k] >> (8 * ch)) & 255u), P.scale[ch], P.bias[ch]);
                 }
                 if (patch) {
 #pragma unroll
@@ -426,12 +424,8 @@ __device__ __forceinline__ void final_rows_color(const AugParams& P, const float
 #pragma unroll
                 for (int k = 0; k < 8; ++k) nv[k] = s_norm[ch * 256 + (int)v[ch][k]];
             } else {
-                const float2 sc = make_float2(P.scale[ch], P.scale[ch]), bi = make_float2(P.bias[ch], P.bias[ch]);
 #pragma unroll
-                for (int k = 0; k < 8; k += 2) {
-                    const float2 rr = __ffma2_rn(make_float2(v[ch][k], v[ch][k + 1]), sc, bi);
-                    nv[k] = rr.x; nv[k + 1] = rr.y;
-                }
+                for (int k = 0; k < 8; ++k) nv[k] = __fmaf_rn(v[ch][k], P.scale[ch], P.bias[ch]);
             }
             store_plane8<OUT>(o + ch * plane, nv);
         }
@@ -530,12 +524,9 @@ __device__ __forceinline__ void sharp_emit(const AugParams& P, const float* tab,
 #pragma unroll
             for (int k = 0; k < 4; ++k) v[k] = tab[ch * 256 + (__float_as_uint(zb[3 * (FLIP ? 3 - k : k) + ch]) & 255u)];
         } else {
-            const float2 nk = make_float2(-kBias15, -kBias15);
-            const float2 sc = make_float2(P.scale[ch], P.scale[ch]), bi = make_float2(P.bias[ch], P.bias[ch]);
-            const float2 a = __fadd2_rn(make_float2(zb[3 * (FLIP ? 3 : 0) + ch], zb[3 * (FLIP ? 2 : 1) + ch]), nk);
-            const float2 b = __fadd2_rn(make_float2(zb[3 * (FLIP ? 1 : 2) + ch], zb[3 * (FLIP ? 0 : 3) + ch]), nk);
-            const float2 r0 = __ffma2_rn(a, sc, bi), r1 = __ffma2_rn(b, sc, bi);
-            v[0] = r0.x; v[1] = r0.y; v[2] = r1.x; v[3] = r1.y;
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+                v[k] = __fmaf_rn(__fadd_rn(zb[3 * (FLIP ? 3 - k : k) + ch], -kBias15), P.scale[ch], P.bias[ch]);
         }
         store_plane4<OUT>(o + ch * plane, v, true, 4);
     }
@@ -591,24 +582,18 @@ __device__ __forceinline__ void final_rows_sharp4(const AugParams& P, const floa
             for (int m = 2; m < 8; ++m) {                                 // output bytes 2m-4, 2m-3
                 const uint32_t t = sh[m - 2] + colp[m] + sh[m + 1];      // col[k-3] + col[k] + col[k+3]
                 const uint32_t x2 = 2u * t + 8u * ctr[m] + 0x000D000Du;  // 2 S + 13 per lane (< 6644)
-                // the two bytes of the pair as packed fp32x2 (sm_100 FADD2 / FMUL2 / FFMA2: half the issue slots)
-                const int k0 = 2 * m, k1 = 2 * m + 1;                    // byte indices from byte -4
-                const float2 kk = make_float2(kBias15, kBias15), nk = make_float2(-kBias15, -kBias15);
-                const float2 fx = make_float2(__uint_as_float(__byte_perm(x2, kBias15Bits, 0x7610)),
-                                              __uint_as_float(__byte_perm(x2, kBias15Bits, 0x7632)));    // kBias15 + (2S+13)
-                const float2 u = __ffma2_rn(__fadd2_rn(fx, nk), make_float2(k26, k26), make_float2(h26, h26));   // (2S+13+.5)/26
-                const float2 fdeg = __fadd2_rz(u, kk);                                                  // kBias15 + floor(u)
-                const float2 fctr = make_float2(biased_byte(wb[k0 >> 2], k0 & 3), biased_byte(wb[k1 >> 2], k1 & 3));
-                const float2 d = __ffma2_rn(fdeg, make_float2(-1.0f, -1.0f), fctr);                    // (float)(px - deg), exact
-                // Blend.c: product and sum are rounded SEPARATELY.  The product stays scalar: __fmul_rn is never contracted,
-                // whereas ptxas fuses a packed mul.f32x2 + add.f32x2 pair into one FFMA2 (seen with alpha = 1.72: wrong bytes)
-                const float2 tt = __fadd2_rn(__fadd2_rn(fdeg, nk), make_float2(__fmul_rn(alpha, d.x), __fmul_rn(alpha, d.y)));
-                float2 z = __fadd2_rz(tt, kk);
-                if (CLIP) {
-                    z.x = fminf(fmaxf(z.x, kBias15), kBias15 + 255.0f);
-                    z.y = fminf(fmaxf(z.y, kBias15), kBias15 + 255.0f);
+#pragma unroll
+                for (int l = 0; l < 2; ++l) {                            // the two bytes of the pair
+                    const int k = 2 * m + l;                             // byte index from byte -4
+                    const float fx = __uint_as_float(__byte_perm(x2, kBias15Bits, l ? 0x7632 : 0x7610));   // kBias15 + (2S+13)
+                    const float u = __fmaf_rn(__fadd_rn(fx, -kBias15), k26, h26);                         // (2S+13+.5)/26
+                    const float fdeg = __fadd_rz(u, kBias15);                                              // kBias15 + floor(u)
+                    const float d = __fmaf_rn(fdeg, -1.0f, biased_byte(wb[k >> 2], k & 3));               // (float)(px - deg), exact
+                    // Blend.c: product and sum are rounded SEPARATELY (__fmul_rn / __fadd_rn are never contracted into an fma)
+                    float z = __fadd_rz(__fadd_rn(__fadd_rn(fdeg, -kBias15), __fmul_rn(alpha, d)), kBias15);
+                    if (CLIP) z = fminf(fmaxf(z, kBias15), kBias15 + 255.0f);
+                    zb[k - 4] = z;
                 }
-                zb[k0 - 4] = z.x; zb[k1 - 4] = z.y;
             }
             // first / last pixel of the row are image border: copied
             if (!has_l) {

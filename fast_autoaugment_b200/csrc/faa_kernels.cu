@@ -1,4 +1,4 @@
-// faa_kernels.cu - sm_100a kernels of the augmentation hot path.
+// faa_kernels.cu - sm_90a kernels of the augmentation hot path.
 //
 // Two launches per batch:
 //   faa_resolve_kernel   ONE block: per-sample decisions (given records, or drawn with
@@ -56,8 +56,12 @@ namespace faa {
 
 constexpr int kThreads = 256;
 constexpr int kMaxDevices = 64;
+// Resident CTAs per SM of the single-source cluster kernel and of the light kernel (launch bounds; the persistent light
+// grid is sized from it).  3 (an 80-register budget) rather than 4 (64 registers): on sm_90a the 64-register build
+// spills (light kernel 232 B stores / 808 B loads, cluster kernel 628 / 720 B), and 3 was faster on every bench.py
+// workload on an H100 SXM (DESIGN.md 4.3).
 #ifndef FAA_MIN_CTAS
-#define FAA_MIN_CTAS 4
+#define FAA_MIN_CTAS 3
 #endif
 constexpr int kCostBuckets = 8;       // per weight class; heavy programs sort before light ones
 
@@ -872,7 +876,7 @@ __device__ __forceinline__ void final_rows_stream(const AugParams& P, const floa
 
 // ---- octet (8-pixel) streaming: W % 8 == 0, output size == image size, no crop --------------------
 // Eight consecutive pixels of one row are 24 contiguous, 8-byte aligned bytes; each plane gets ONE 16-byte
-// store (fp16 / bf16) and the normalisation runs as packed fp32x2 fused multiply-adds (sm_100 FFMA2).
+// store (fp16 / bf16) and the normalisation is one fused multiply-add per value.
 template <int OUT>
 __device__ __forceinline__ void store_plane8(typename OutElem<OUT>::T* o, const float v[8]) {
     if constexpr (OUT == OUT_U8_HWC) {
@@ -895,19 +899,16 @@ __device__ __forceinline__ void store_plane8(typename OutElem<OUT>::T* o, const 
     }
 }
 
-// normalised values of one plane from eight byte values: table lookups, or packed fma
+// normalised values of one plane from eight byte values: table lookups, or fma
 template <bool USE_TAB>
 __device__ __forceinline__ void norm8(const AugParams& P, const float* tab, int ch, const uint32_t u[8], float v[8]) {
     if (USE_TAB) {
 #pragma unroll
         for (int k = 0; k < 8; ++k) v[k] = tab[ch * 256 + u[k]];
     } else {
-        const float2 sc = make_float2(P.scale[ch], P.scale[ch]), bi = make_float2(P.bias[ch], P.bias[ch]);
+        const float sc = P.scale[ch], bi = P.bias[ch];
 #pragma unroll
-        for (int k = 0; k < 8; k += 2) {
-            const float2 r = __ffma2_rn(make_float2((float)u[k], (float)u[k + 1]), sc, bi);
-            v[k] = r.x; v[k + 1] = r.y;
-        }
+        for (int k = 0; k < 8; ++k) v[k] = __fmaf_rn((float)u[k], sc, bi);
     }
 }
 
@@ -1716,7 +1717,7 @@ __global__ void __launch_bounds__(kMidThreadsMax, 2) faa_augment_mid_kernel(cons
 // PLAIN / LUT / POINT / GEOM classes only - no cluster, 3 KB of static shared memory, a fraction of
 // the cluster kernel's registers and code.  It owns schedule entries [n_heavy, B).
 #ifndef FAA_LIGHT_CTAS
-#define FAA_LIGHT_CTAS 4
+#define FAA_LIGHT_CTAS 3                  // (see FAA_MIN_CTAS)
 #endif
 template <int OUT, bool TAB>
 __global__ void __launch_bounds__(kThreads, FAA_LIGHT_CTAS) faa_augment_light_kernel(const __grid_constant__ AugParams P) {

@@ -1,5 +1,5 @@
 /*
- * faa_b200.h - C ABI of the B200-native Fast AutoAugment augmentation hot path.
+ * faa_b200.h - C ABI of the H100-native Fast AutoAugment augmentation hot path.
  *
  * Plain C: opaque handle, plain pointers and sizes, int status returns, no C++
  * or torch types, no exceptions across the boundary.  Every device entry point

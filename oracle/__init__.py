@@ -7,7 +7,7 @@ checker (or as the timed CPU baseline), never as the thing that is measured as
 "ours" or shipped.  The product path (``fast_autoaugment_b200``) never imports
 this package and fails loudly when its CUDA library is missing.
 
-Two layers, both restating ``/root/reference`` (kakaobrain/fast-autoaugment @
+Two layers, both restating the reference (kakaobrain/fast-autoaugment @
 2424224) for the path named by BASELINE.json:
 
 * ``oracle.pil_path``  - the reference's own call sequence into Pillow /
@@ -23,9 +23,8 @@ Two layers, both restating ``/root/reference`` (kakaobrain/fast-autoaugment @
 Pinning: the reference has no tests and no golden vectors of its own
 (SURVEY.md section 4), and its arithmetic lives in an un-vendored, un-pinned
 Pillow.  The oracle is therefore pinned against *outputs of the reference
-itself run in the build container* (Pillow 12.2.0, torchvision 0.26.0, numpy
-2.3.5, CPython 3.12): ``tests/golden/make_golden.py`` imports
-``/root/reference`` and writes the fixtures under ``tests/golden/``; the
-``-m "not gpu"`` tests check both oracle layers against those fixtures, and,
-whenever ``/root/reference`` is present, against the live reference.
+itself* (Pillow 12.2.0, torchvision 0.26.0, numpy 2.3.5, CPython 3.12):
+``tests/golden/make_golden.py <checkout>`` imports the reference and writes the
+fixtures under ``tests/golden/``; the ``-m "not gpu"`` tests check both oracle
+layers against those fixtures.
 """

@@ -5,7 +5,7 @@ TEST INFRASTRUCTURE ONLY (see ``oracle/__init__.py``).
 
 Third-party algorithm notice.  The per-pixel arithmetic of the reference lives
 in **Pillow** (C ``libImaging``), which is neither vendored under
-``/root/reference`` nor pinned by its ``requirements.txt``; the build image has
+the reference nor pinned by its ``requirements.txt``; the build image has
 Pillow 12.2.0 (binary wheel, C sources absent).  The functions below restate
 Pillow's published algorithms (``Geometry.c`` affine_fixed / ImagingScaleAffine,
 ``Blend.c``, ``Convert.c`` rgb2l, ``Filter.c`` 3x3, ``Point.c``, ``Histo.c``,

@@ -2,7 +2,7 @@
 
 TEST INFRASTRUCTURE ONLY (see ``oracle/__init__.py``).
 
-Every function restates one piece of ``/root/reference`` and cites it.  The
+Every function restates one piece of the reference and cites it.  The
 per-pixel arithmetic is *not* here - it is inside Pillow's C library, exactly as
 for the reference - so this layer has the reference's CPU cost profile and is
 what ``bench.py`` times as ``cpu_baseline`` (kind "port").  The RNG streams that

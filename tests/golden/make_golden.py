@@ -1,16 +1,19 @@
 #!/usr/bin/env python
 """Generate the golden fixtures from the LIVE reference.
 
-Run in the build container only (needs ``/root/reference``; it does not exist on
-the GPU box).  Imports the reference in place, read-only, with two import shims
+    python tests/golden/make_golden.py <checkout of kakaobrain/fast-autoaugment>
+
+Imports the reference in place, read-only, with two import shims
 (``theconf`` is not installed; ``torch._six`` no longer exists - SURVEY.md 8c),
 runs the reference's own ``apply_augment`` / ``Augmentation`` / ``CutoutDefault``
 / ``mixup`` and the exact ``transform_train`` of ``data.py:39-44,92,112`` on
 seeded synthetic inputs, and writes
 
     tests/golden/golden_ops.npz      per-op outputs (19 ops x levels x 3 input kinds, 32x32 + 24x40)
-    tests/golden/golden_chain.npz    policy outputs + full CIFAR chain fp32 + mixup
-    tests/golden/golden_hashes.json  sha256 digests (incl. the SURVEY.md 8c table at 32 and 224)
+    tests/golden/golden_chain.npz    policy outputs + full CIFAR chain fp32 + mixup (the first images of
+                                     each seeded batch: every file stays under 1 MB)
+    tests/golden/golden_hashes.json  sha256 digests (incl. the SURVEY.md 8c table at 32 and 224, and one
+                                     digest per image of the reference's sub-policy draw on fresh inputs)
 
 Environment that produced the committed files: Pillow 12.2.0, numpy 2.3.5,
 torch 2.11.0, torchvision 0.26.0, CPython 3.12.3.
@@ -29,10 +32,14 @@ import PIL.Image
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = "/root/reference"
+# policy batches are drawn in full (the RNG streams stay those of the original fixtures) and stored up to KEEP images
+KEEP = {"fa_reduced_cifar10": 32, "autoaug_policy": 32, "fa_reduced_svhn": 16, "arsaug_policy": 16,
+        "fa_resnet50_rimagenet": 16, "cifar_chain": 32}
+# (policy, size, images): fresh inputs through the reference's own sub-policy draw (tests/test_oracle_golden.py)
+LIVE_CASES = (("fa_reduced_cifar10", 32, 400), ("autoaug_policy", 32, 400), ("fa_resnet50_rimagenet", 64, 100))
 
 
-def import_reference():
+def import_reference(ref):
     # shim 1: theconf (data.py:16)
     tc = types.ModuleType("theconf")
 
@@ -49,7 +56,7 @@ def import_reference():
     six = types.ModuleType("torch._six")
     six.container_abcs = collections.abc
     sys.modules["torch._six"] = six
-    sys.path.insert(0, REF)
+    sys.path.insert(0, ref)
     from FastAutoAugment import augmentations, archive, aug_mixup, data
     return augmentations, archive, aug_mixup, data
 
@@ -77,8 +84,19 @@ ALL_OPS = ["ShearX", "ShearY", "TranslateX", "TranslateY", "Rotate", "AutoContra
 LEVELS = [0.0, 0.13, 0.5, 0.7, 1.0]
 
 
-def main():
-    aug, archive, aug_mixup, data = import_reference()
+def live_input(rng, i, s):
+    """input i of a LIVE_CASES run: noise (odd i) or a low-contrast ramp + noise (even i)"""
+    if i % 2:
+        return rng.integers(0, 256, (s, s, 3), dtype=np.uint8)
+    return np.clip(np.linspace(60, 180, s)[None, :, None] + rng.normal(0, 6, (s, s, 3)), 0, 255).astype(np.uint8)
+
+
+def policy_sha(policies) -> str:
+    return hashlib.sha256(json.dumps([[list(o) for o in sub] for sub in policies]).encode()).hexdigest()
+
+
+def main(ref):
+    aug, archive, aug_mixup, data = import_reference(ref)
     hashes = {"env": {"pillow": PIL.__version__, "numpy": np.__version__, "torch": torch.__version__}}
 
     # ---- (1) SURVEY 8c table: rng(1234) noise, seed 0, level 0.7 (Posterize 0.3)
@@ -144,8 +162,8 @@ def main():
         np.random.seed(5)
         torch.manual_seed(5)
         out = np.stack([np.asarray(A(PIL.Image.fromarray(a))) for a in batch])
-        chain["policy_%s_in" % pol] = batch
-        chain["policy_%s_out" % pol] = out
+        chain["policy_%s_in" % pol] = batch[:KEEP[pol]]
+        chain["policy_%s_out" % pol] = out[:KEEP[pol]]
 
     # ---- (5) the exact CIFAR transform_train (data.py:39-44 + :92 + :112), fp32
     from torchvision.transforms import transforms as T
@@ -160,8 +178,8 @@ def main():
     np.random.seed(11)
     torch.manual_seed(11)
     out = torch.stack([tt(PIL.Image.fromarray(a)) for a in batch]).numpy()
-    chain["cifar_chain_in"] = batch
-    chain["cifar_chain_out_f32"] = out
+    chain["cifar_chain_in"] = batch[:KEEP["cifar_chain"]]
+    chain["cifar_chain_out_f32"] = out[:KEEP["cifar_chain"]]
     hashes["cifar_chain_sha"] = sha(out)
 
     # ---- (6) mixup (aug_mixup.py:13-23)
@@ -175,6 +193,26 @@ def main():
     chain["mixup_t2"] = t2.numpy()
     chain["mixup_lam"] = np.array([lam], dtype=np.float64)
 
+    # ---- (7) fresh inputs, the reference's sub-policy draw (data.py:257-264) on its own apply_augment: one digest per image
+    live = []                                   # in LIVE_CASES order: the cases share one input generator
+    rng = np.random.default_rng(5)
+    for pol, s, n in LIVE_CASES:
+        policies = archive.__dict__[pol]()
+        digests = []
+        for i in range(n):
+            img = live_input(rng, i, s)
+            random.seed(i)
+            np.random.seed(i)
+            policy = random.choice(policies)
+            out = PIL.Image.fromarray(img)
+            for name, pr, level in policy:
+                if random.random() > pr:
+                    continue
+                out = aug.apply_augment(out, name, level)
+            digests.append(sha(np.asarray(out))[:16])          # 64 bits per image
+        live.append({"policy": pol, "size": s, "policy_sha": policy_sha(policies), "digests": digests})
+    hashes["live_reference"] = live
+
     np.savez_compressed(os.path.join(HERE, "golden_chain.npz"), **chain)
     with open(os.path.join(HERE, "golden_hashes.json"), "w") as f:
         json.dump(hashes, f, indent=1, sort_keys=True)
@@ -183,4 +221,6 @@ def main():
 
 
 if __name__ == "__main__":
-    main()
+    if len(sys.argv) != 2:
+        sys.exit(__doc__)
+    main(sys.argv[1])

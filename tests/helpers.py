@@ -33,6 +33,20 @@ def synth_batch(n, shape, seed):
     return np.stack([synth(shape, i % 3, rng) for i in range(n)])
 
 
+def live_input(rng, i, s):
+    """input i of a make_golden.py LIVE_CASES run (same generator): noise (odd i) or a low-contrast ramp + noise"""
+    if i % 2:
+        return rng.integers(0, 256, (s, s, 3), dtype=np.uint8)
+    return np.clip(np.linspace(60, 180, s)[None, :, None] + rng.normal(0, 6, (s, s, 3)), 0, 255).astype(np.uint8)
+
+
+def policy_sha(policies) -> str:
+    """digest of a policy table, as make_golden.py stores it for the reference's archive"""
+    import hashlib
+    import json
+    return hashlib.sha256(json.dumps([[list(o) for o in sub] for sub in policies]).encode()).hexdigest()
+
+
 def exact_norm_table(mean, std):
     """fp32 ToTensor+Normalize value of every byte, computed with torch itself."""
     import torch

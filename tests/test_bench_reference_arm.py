@@ -16,7 +16,9 @@ def test_reference_arm_json_line():
               "scaling", "vs_baseline", "dtype", "data", "config", "cpu_baseline", "e2e"):
         assert k in line, k
     assert line["impl"] == "reference" and line["value"] > 0 and line["unit"] == "images/s"
-    ref_there = os.path.isdir(os.path.join(ROOT, "oracle", "_ref", "FastAutoAugment")) or os.path.isdir("/root/reference")
+    from oracle import build_ref
+    ref_there = os.path.isdir(os.path.join(build_ref.DST, "FastAutoAugment")) or \
+        bool(build_ref.REF_ROOT and os.path.isdir(os.path.join(build_ref.REF_ROOT, "FastAutoAugment")))
     assert line["cpu_baseline"]["kind"] == ("reference" if ref_there else "port") and line["cpu_baseline"]["cores"] >= 1
     assert line["e2e"]["h2d_bytes_per_step"] == 0 and line["e2e"]["d2h_bytes_per_step"] == 0
     # other ranks of a torchrun launch stay silent
@@ -38,6 +40,22 @@ def test_reference_arm_never_loads_the_cuda_library():
     out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300, cwd=ROOT)
     assert out.returncode == 0, out.stderr[-2000:]
     assert out.stdout.strip().splitlines()[-1] in ("reference", "port")
+
+
+def test_reference_imports_without_scikit_learn():
+    """reference data.py:15 imports sklearn.model_selection at module level; the oracle/_ref loader shims it when
+    scikit-learn is absent, so the reference arm times the reference's own classes either way"""
+    code = ("import sys\n"
+            "sys.modules['sklearn'] = sys.modules['sklearn.model_selection'] = None   # as if not installed\n"
+            "from oracle import build_ref\n"
+            "build_ref.install_sklearn_shim()\n"
+            "from sklearn.model_selection import StratifiedShuffleSplit\n"
+            "import os\n"
+            "if os.path.isdir(os.path.join(build_ref.DST, 'FastAutoAugment')):\n"
+            "    assert build_ref.import_ref() is not None\n"
+            "print('ok')\n")
+    out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300, cwd=ROOT)
+    assert out.returncode == 0 and out.stdout.strip().endswith("ok"), out.stderr[-2000:]
 
 
 def test_workload_string_is_shared_by_both_arms():

@@ -1,6 +1,6 @@
 """Kernel arithmetic (faa_core.cuh, compiled for the host by tests/emu) vs the oracle.
 
-These tests execute, on the CPU, the same per-pixel source the sm_100a kernels execute -
+These tests execute, on the CPU, the same per-pixel source the sm_90a kernels execute -
 policy compilation comes from the real C-ABI library (host functions, no GPU needed), the
 pixel evaluation from tests/emu - and demand bit-exact agreement with the oracle
 (oracle.pil_path = the reference's calls into Pillow) on every op, policy and chain.

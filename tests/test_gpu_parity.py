@@ -1,4 +1,4 @@
-"""GPU parity tests: the sm_100a kernels, called through the C ABI, against the oracle.
+"""GPU parity tests: the sm_90a kernels, called through the C ABI, against the oracle.
 
 Bit-exact for every uint8 result and for the fp32 chain; fp16/bf16 outputs must equal the
 fp32 oracle rounded to that dtype.  Full-size cases (BASELINE.json configs) are checked

@@ -1,5 +1,6 @@
 import os, sys
-sys.path.insert(0, "/root/repo"); sys.path.insert(0, "/root/repo/tests")
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 os.environ["FAA_SPLIT_MIN"] = "0"
 import numpy as np, PIL.Image, torch
 from helpers import exact_norm_table, seed_all, synth_batch

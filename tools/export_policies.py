@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Export the reference's policy archive into compact data files.
 
-Run in the build container (needs ``/root/reference``); the outputs
+``python tools/export_policies.py <checkout of kakaobrain/fast-autoaugment>``; the outputs
 ``fast_autoaugment_b200/policies/<name>.json`` are committed so the package has
 the searched policies (the *data* the reference publishes - its README result
 tables are produced with them) without importing the reference.
@@ -14,9 +14,6 @@ S*K rows).  ``level`` is what ``Augmentation`` receives, i.e. AFTER the
 import json
 import os
 import sys
-
-sys.path.insert(0, "/root/reference")
-from FastAutoAugment import archive  # noqa: E402
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 OUT = os.path.join(HERE, "..", "fast_autoaugment_b200", "policies")
@@ -31,7 +28,9 @@ SETS = {
 }
 
 
-def main():
+def main(ref):
+    sys.path.insert(0, ref)
+    from FastAutoAugment import archive
     os.makedirs(OUT, exist_ok=True)
     for name, src in SETS.items():
         subs = getattr(archive, name)()
@@ -46,4 +45,6 @@ def main():
 
 
 if __name__ == "__main__":
-    main()
+    if len(sys.argv) != 2:
+        sys.exit(__doc__)
+    main(sys.argv[1])

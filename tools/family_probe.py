@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Device time of single-op policies per input family (noise / ramp / constant): shows how much of a
-statistics op's cost is histogram contention.  Usage (GPU box): python tools/family_probe.py"""
+statistics op's cost is histogram contention.  Usage (on an H100): python tools/family_probe.py"""
 import os
 import sys
 

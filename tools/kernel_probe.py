@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Device-time decomposition of the fused kernel: which program classes cost what.
-Usage (GPU box): python tools/kernel_probe.py [H W B]"""
+Usage (on an H100): python tools/kernel_probe.py [H W B]"""
 import os
 import sys
 import time
@@ -15,6 +15,7 @@ from fast_autoaugment_b200 import archive
 from fast_autoaugment_b200.engine import CompiledPolicy, FusedAugmenter, TailSpec
 
 H, W, B = (int(a) for a in sys.argv[1:4]) if len(sys.argv) >= 4 else (224, 224, 512)
+PEAK = bench.hbm_peak()[0]
 x = [torch.from_numpy(bench.synth_batch(B, H, W, 1 + i)).cuda() for i in range(4)]
 
 
@@ -34,7 +35,7 @@ def timeit(name, policies, tail, n=int(os.environ.get("PROBE_N", "200"))):
     us = e0.elapsed_time(e1) * 1e3 / n
     out_b = outs[0].numel() * outs[0].element_size()
     gbs = (B * H * W * 3 + out_b) / us / 1e3
-    print("%-34s %8.1f us  %7.0f GB/s  %5.1f%% of 6575" % (name, us, gbs, gbs / 65.75), flush=True)
+    print("%-34s %8.1f us  %7.0f GB/s  %5.1f%% of %.0f" % (name, us, gbs, 100 * gbs / PEAK, PEAK), flush=True)
 
 
 t16 = TailSpec.imagenet(0, torch.float16) if H != 32 else TailSpec.cifar(16, torch.float16)

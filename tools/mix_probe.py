@@ -21,4 +21,5 @@ e0.record()
 for i in range(n): f(x[i % 4], outs[i % 4], i * B)
 e1.record(); torch.cuda.synchronize()
 us = e0.elapsed_time(e1) * 1e3 / n
-print("%-40s %7.1f us  %5.1f%% of 6575 GB/s" % (" ".join("%s=%s" % (k, v) for k, v in os.environ.items() if k.startswith("FAA_")) or "default", us, B * H * W * 9 / us / 1e3 / 65.75), flush=True)
+peak = bench.hbm_peak()[0]
+print("%-40s %7.1f us  %5.1f%% of %.0f GB/s" % (" ".join("%s=%s" % (k, v) for k, v in os.environ.items() if k.startswith("FAA_")) or "default", us, 100 * B * H * W * 9 / us / 1e3 / peak, peak), flush=True)

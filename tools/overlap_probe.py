@@ -2,7 +2,7 @@
 """How much of a step is the per-step barrier (both pixel kernels drain before the next step starts)?
 Runs the bench workload (a) as bench.py does - one policy handle, one stream - and (b) alternating between
 two handles on two streams, so that consecutive steps have no stream-order dependency and may overlap.
-Usage (GPU box): python tools/overlap_probe.py"""
+Usage (on an H100): python tools/overlap_probe.py"""
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)

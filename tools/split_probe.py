@@ -1,5 +1,5 @@
 import os, sys
-sys.path.insert(0, '/root/repo')
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch, bench
 from fast_autoaugment_b200.engine import CompiledPolicy, FusedAugmenter, TailSpec
 H=W=224; B=512
