@@ -209,7 +209,7 @@ struct faa_policy {
     // pixels are computed; a call whose (rng, shapes, ...) key matches the speculation skips its resolve launch
     struct AheadKey { uint64_t seed, first_index; int32_t v[16]; };
     AheadKey ahead_key{}; bool ahead_valid = false; int ahead_slot = 0, cur_slot = 0;
-    uint64_t last_first_index = 0; bool have_last = false; AheadKey last_key{};
+    bool have_last = false; AheadKey last_key{};
     cudaStream_t ahead_stream = nullptr; cudaEvent_t ev_ahead = nullptr;
     void* d_scratch = nullptr; size_t d_scratch_bytes = 0;   // Sharpness->gather scratch images
     bool overlap_calls = false;          // faa_policy_set_overlap: consecutive calls on one stream may overlap (see augment_common)
@@ -586,6 +586,257 @@ int faa_sample_philox(faa_policy_t* p, int batch, int h, int w, const faa_tail_t
     return FAA_OK;
 }
 
+// What augment_common decided for one call: which kernels run, on which schedule, and how their buffers are bound.
+struct Schedule {
+    bool use_order;             // the resolve kernel writes a cost-sorted schedule (order / n_heavy)
+    bool use_split;             // the light streaming kernel (and the mid kernel) take the programs they cover
+    bool use_mid;               // three-way split: statistics-LUT and Sharpness programs run in the mid kernel
+    bool use_chain;             // chained schedule (else the event schedule)
+    bool no_heavy;              // every program is light or mid: the cluster kernel is not launched
+    bool use_tab;               // exact normalisation table instead of one fma
+    bool speculate;             // resolve the next call's batch ahead (resolve-ahead)
+    bool hit;                   // ... and the previous call already resolved exactly this one
+    size_t scratch_slot_bytes;  // scratch images per program slot
+};
+
+// Program / schedule buffers come in two slots; a slot = progs[cap] + order[cap] + counters[2 cap] + ready[cap] + done word.
+// The segment counters of a split launch live behind the order array, indexed by `first` so that concurrent chunk launches
+// do not share them (same for the ready word).  Chained steps also own a completion counter and a scratch image per slot.
+static void bind_slot(const faa_policy* p, const Schedule& s, int first, int slot, ResolveParams& r, AugParams* a) {
+    const size_t cap_imgs = p->d_progs_bytes / sizeof(Prog);
+    Prog* progs = reinterpret_cast<Prog*>((uint8_t*)p->d_progs + (size_t)slot * p->d_progs_bytes);
+    int32_t* order = reinterpret_cast<int32_t*>(p->d_order) + (size_t)slot * (4 * cap_imgs + 8);
+    int32_t* counter = order + cap_imgs + 2 * (size_t)first;
+    int32_t* ready = order + 3 * cap_imgs + first;
+    uint32_t* done = reinterpret_cast<uint32_t*>(order + 4 * cap_imgs);     // the slot's completion counter
+    r.progs = progs; r.order = s.use_order ? order : nullptr; r.n_heavy = s.use_split ? counter : nullptr;
+    r.ready = s.use_chain ? ready : nullptr;
+    // (the pixel kernels that last read the slot release their dependents before they finish: the resolve kernel that
+    //  rewrites it first waits until all of them have counted themselves)
+    if (s.use_chain) { r.wait_done = done; r.wait_target = p->done_target[slot]; }
+    if (a) {
+        a->progs = progs; a->order = r.order; a->n_heavy = r.n_heavy; a->ready = r.ready;
+        if (s.use_chain) {
+            a->done = done;
+            if (a->scratch) a->scratch = (uint8_t*)p->d_scratch + (size_t)slot * s.scratch_slot_bytes;
+        }
+    }
+}
+
+// the mid kernel's launch: its own (taller) bands in bands / geo[0] - the band count is halved while a band (+ halo)
+// stays <= 80 KB (2 CTAs / SM)
+static AugParams mid_params(AugParams a) {
+    int mb = a.bands;
+    while (mb > 1 && band_capacity(mb / 2, a.H, a.W, a.out_h, 0) <= 80 * 1024) mb /= 2;
+    a.bands = mb;
+    fill_geom(a.geo[0], mb, a.H, a.W, a.out_h, 0, true);
+    a.band_cap = a.geo[0].band_cap; a.mat_cap = 0;
+    return a;
+}
+
+// the byte ranges the step P describes reads and writes
+static void step_ranges(const AugParams& P, int out_dtype, uintptr_t in[2], uintptr_t out[2]) {
+    const size_t img_bytes = (size_t)P.H * P.W * 3;
+    in[0] = (uintptr_t)P.in + (P.in_mod ? 0 : (size_t)P.first * img_bytes);
+    in[1] = in[0] + (size_t)(P.in_mod ? P.in_mod : P.B) * img_bytes;
+    out[0] = (uintptr_t)P.out;
+    out[1] = out[0] + (size_t)P.B * P.out_h * P.out_w * 3 * out_elem_size(out_dtype);
+}
+
+// A step may only overlap the previous one if it follows it on the same stream and neither reads what that step wrote
+// nor writes what it read or wrote; otherwise its first kernel is a plain dependent launch.  And only if the caller has
+// promised that this call's inputs were complete before the previous call was issued (faa_policy_set_overlap /
+// faa_augment_many): a kernel launched with programmatic serialization that does not execute griddepcontrol.wait has no
+// visibility guarantee for what the kernel right in front of it wrote, and that kernel may be the producer of this batch
+// (a gather, a copy).  Within a call every kernel only consumes what its own call's first - stream-ordered - kernel
+// already waited for.
+static bool may_overlap_previous(const faa_policy* p, const AugParams& P, int out_dtype, cudaStream_t stream) {
+    uintptr_t in[2], out[2];
+    step_ranges(P, out_dtype, in, out);
+    auto overlap = [](const uintptr_t a[2], const uintptr_t b[2]) { return a[0] < b[1] && b[0] < a[1]; };
+    return p->overlap_calls && p->chain_live && p->chain_stream == stream && !overlap(in, p->prev_out) &&
+           !overlap(out, p->prev_out) && !overlap(out, p->prev_in);
+}
+
+// this step is the one the next call on `stream` may overlap
+static void record_step(faa_policy* p, const AugParams& P, int out_dtype, cudaStream_t stream) {
+    step_ranges(P, out_dtype, p->prev_in, p->prev_out);
+    p->chain_live = true; p->chain_stream = stream;
+}
+
+// Resolve-ahead: speculate that the next call is this one (`key`) with first_index advanced by the stride seen so far.
+// Returns the resolve parameters of that call; the caller binds them to the other slot, launches them and then sets
+// ahead_valid.
+static ResolveParams speculate_next(faa_policy* p, const faa_policy::AheadKey& key, const ResolveParams& R, int batch) {
+    uint64_t stride = (uint64_t)batch;
+    faa_policy::AheadKey base = key; base.first_index = 0;
+    faa_policy::AheadKey lastb = p->last_key; lastb.first_index = 0;
+    if (p->have_last && memcmp(&base, &lastb, sizeof base) == 0 && key.first_index > p->last_key.first_index)
+        stride = key.first_index - p->last_key.first_index;
+    p->last_key = key; p->have_last = true;
+    ResolveParams R2 = R;
+    R2.rng.first_index = key.first_index + stride;
+    p->ahead_key = key; p->ahead_key.first_index = R2.rng.first_index;
+    p->ahead_slot = p->cur_slot ^ 1;
+    return R2;
+}
+
+// Self-resolving launch: a launch of tiny images is bound by kernel latencies and by the host's launch rate, not by
+// bytes.  Thread 0 of every CTA draws its image's decisions and builds the program itself (same Philox counters, same
+// build_prog): ONE kernel per step, no program array, no ticket - consecutive steps have no dependency left and overlap
+// through programmatic dependent launch.
+static int launch_self_resolving(faa_policy* p, const AugParams& P, const ResolveParams& R, bool use_tab, int out_dtype,
+                                 cudaStream_t stream) {
+    const bool overlap_ok = may_overlap_previous(p, P, out_dtype, stream) && !P.norm_stride;
+    AugParams Ps = P;
+    Ps.progs = nullptr; Ps.order = nullptr; Ps.n_heavy = nullptr; Ps.ready = nullptr; Ps.done = nullptr; Ps.grid_y = 0;
+    Ps.self_resolve = 1;
+    Ps.sr_ops = R.ops; Ps.sr_probs = R.probs; Ps.sr_rng = R.rng;
+    Ps.sr_n_sub = R.n_sub; Ps.sr_n_op = R.n_op; Ps.sr_op_base = R.op_base; Ps.sr_apply_tail = R.apply_tail;
+    // Sharpness -> gather programs are evaluated lazily instead of through the scratch image - the last thing consecutive
+    // steps shared - so every CTA may release the next step at once; a step that touches the previous step's buffers is
+    // launched as a plain stream-ordered kernel instead
+    Ps.sr_allow = R.allow & ~2; Ps.scratch = nullptr;
+    Ps.chain = overlap_ok ? CHAIN_SELF_RESOLVING : CHAIN_STREAM_ORDERED; Ps.pdl = 0;
+    CK(launch_augment(Ps, out_dtype, use_tab, 0, stream));
+    g_launches++;
+    p->ahead_valid = false;
+    record_step(p, P, out_dtype, stream);
+    return FAA_OK;
+}
+
+// Chained schedule: resolve(N+1), [cluster(N),] mid(N), light(N) all on the caller's stream with programmatic dependent
+// launches, no events and no side streams.  Consecutive steps overlap (the next step's CTAs fill the slots the previous
+// step's tail frees); the only true dependency - programs written by the resolve kernel - is a ticket word the pixel
+// kernels poll.  The mid and light kernels are persistent: one resident wave each, whose rows loop over their entries,
+// so a kernel releases its dependents immediately and consecutive kernels - and steps - overlap for their whole length.
+// What the early release no longer orders is ordered explicitly: program slots by completion counters the next resolve
+// kernel of the slot waits for, scratch images by a copy per slot.
+static int launch_chained(faa_policy* p, const AugParams& P, ResolveParams& R, const Schedule& s,
+                          const faa_policy::AheadKey& key, int out_dtype, cudaStream_t stream) {
+    bool overlap_ok = may_overlap_previous(p, P, out_dtype, stream);
+    AugParams Pc = P;
+    Pc.chain = CHAIN_STEP; Pc.pdl = 0;
+    int slot = p->cur_slot;
+    if (s.hit) {
+        slot = p->ahead_slot;
+        Pc.ticket = p->ahead_ticket;
+        bind_slot(p, s, P.first, slot, R, &Pc);
+    } else {
+        bind_slot(p, s, P.first, slot, R, &Pc);
+        R.ticket = ++p->ticket; R.pdl = overlap_ok ? 1 : 0;
+        Pc.ticket = R.ticket;
+        CK(launch_resolve(R, stream));
+        g_launches++;
+        overlap_ok = true;                              // the kernels behind it may overlap IT
+    }
+    p->cur_slot = slot;
+    p->ahead_valid = false;
+    ResolveParams R2 = speculate_next(p, key, R, P.B);
+    bind_slot(p, s, P.first, slot ^ 1, R2, nullptr);
+    R2.ticket = ++p->ticket; R2.pdl = overlap_ok ? 1 : 0;
+    CK(launch_resolve(R2, stream));
+    g_launches++;
+    p->ahead_valid = true; p->ahead_ticket = R2.ticket;
+
+    if (!p->sm_count) CK(cudaDeviceGetAttribute(&p->sm_count, cudaDevAttrMultiProcessorCount, p->device));
+    AugParams Pm = s.use_mid ? mid_params(Pc) : Pc;
+    // one resident wave each (launch bounds: light CTAs / SM; mid rows: ONE CTA per SM, so that the light CTAs that
+    // follow share the SM with it from the start)
+    const int lb = P.geo[1].bands > 0 ? P.geo[1].bands : 1;
+    Pc.grid_y = (p->sm_count * resident_ctas_per_sm(1)) / lb;
+    Pm.grid_y = p->sm_count / (Pm.bands > 0 ? Pm.bands : 1);
+    if (Pc.grid_y < 1) Pc.grid_y = 1;
+    if (Pm.grid_y < 1) Pm.grid_y = 1;
+    auto launch = [&](const AugParams& a, int which) -> int {
+        CK(launch_augment(a, out_dtype, s.use_tab, which, stream));
+        g_launches++;
+        p->done_target[slot] += augment_cta_count(a, which);
+        return FAA_OK;
+    };
+    if (!s.no_heavy) {                                  // the cluster kernel keeps one cluster per entry
+        AugParams Pk = Pc; Pk.grid_y = 0;
+        if (int e = launch(Pk, 0)) return e;
+    }
+    if (s.use_split) {
+        if (s.use_mid) { if (int e = launch(Pm, 2)) return e; }
+        if (int e = launch(Pc, 1)) return e;
+    }
+    record_step(p, P, out_dtype, stream);
+    return FAA_OK;
+}
+
+// Event schedule, for what cannot be chained (resolved samples, fused Mixup, the host-buffer entry, the windows of
+// policies of more than two ops, uint8 output of one pixel kernel): the resolve kernel and the light streaming kernel on
+// the caller's stream, the cluster and mid kernels on high-priority side streams, joined by events.
+static int launch_event(faa_policy* p, AugParams& P, ResolveParams& R, const Schedule& s, const faa_policy::AheadKey& key,
+                        int out_dtype, cudaStream_t stream) {
+    p->chain_live = false;
+    int slot = p->cur_slot;
+    if (s.hit) {
+        slot = p->ahead_slot;
+        CK(cudaStreamWaitEvent(stream, p->ev_ahead, 0));
+        P.pdl = 0;                                          // no resolve kernel right in front of the pixel kernel
+        bind_slot(p, s, P.first, slot, R, &P);
+    } else {
+        bind_slot(p, s, P.first, slot, R, &P);
+        CK(launch_resolve(R, stream));
+        g_launches++;
+    }
+    p->cur_slot = slot;
+    p->ahead_valid = false;
+    if (P.n_heavy || s.speculate) {
+        if (!p->light_stream) {
+            int lo = 0, hi = 0;
+            CK(cudaDeviceGetStreamPriorityRange(&lo, &hi));       // hi = numerically lowest = greatest priority
+            CK(cudaStreamCreateWithPriority(&p->light_stream, cudaStreamNonBlocking, hi));
+            CK(cudaStreamCreateWithPriority(&p->ahead_stream, cudaStreamNonBlocking, hi));   // one block: get a slot promptly
+            CK(cudaStreamCreateWithPriority(&p->mid_stream, cudaStreamNonBlocking, hi));
+            CK(cudaEventCreateWithFlags(&p->ev_mid, cudaEventDisableTiming));
+            CK(cudaEventCreateWithFlags(&p->ev_res, cudaEventDisableTiming));
+            CK(cudaEventCreateWithFlags(&p->ev_light, cudaEventDisableTiming));
+            CK(cudaEventCreateWithFlags(&p->ev_ahead, cudaEventDisableTiming));
+        }
+        CK(cudaEventRecord(p->ev_res, stream));               // this batch's programs are ready
+    }
+    if (s.speculate) {
+        ResolveParams R2 = speculate_next(p, key, R, P.B);
+        bind_slot(p, s, P.first, slot ^ 1, R2, nullptr);
+        CK(cudaStreamWaitEvent(p->ahead_stream, p->ev_res, 0));      // the other slot's last readers are done
+        CK(launch_resolve(R2, p->ahead_stream));
+        CK(cudaEventRecord(p->ev_ahead, p->ahead_stream));
+        g_launches++;
+        p->ahead_valid = true;
+    }
+    if (!P.n_heavy) {                                       // one pixel kernel
+        CK(launch_augment(P, out_dtype, s.use_tab, 0, stream));
+        g_launches++;
+        return FAA_OK;
+    }
+    // Split pixel kernels, concurrently: the streaming kernel goes FIRST on the caller's stream and fills the machine at
+    // once; the clusters of the cluster and mid kernels on the high-priority side streams then take the CTA slots its CTAs
+    // free (heavy images finish early, light work fills the gaps; launched first, the thousands of exiting CTAs of the
+    // cluster kernels would hold up the work distributor).
+    AugParams Ph = P; Ph.pdl = 0;                           // not behind the resolve kernel in its stream
+    CK(cudaStreamWaitEvent(p->light_stream, p->ev_res, 0));
+    if (s.use_mid) CK(cudaStreamWaitEvent(p->mid_stream, p->ev_res, 0));
+    CK(launch_augment(P, out_dtype, s.use_tab, 1, stream));
+    g_launches++;
+    if (!s.no_heavy) {
+        CK(launch_augment(Ph, out_dtype, s.use_tab, 0, p->light_stream));
+        g_launches++;
+    }
+    if (s.use_mid) {
+        CK(launch_augment(mid_params(Ph), out_dtype, s.use_tab, 2, p->mid_stream));
+        g_launches++;
+        CK(cudaEventRecord(p->ev_mid, p->mid_stream));
+    }
+    CK(cudaEventRecord(p->ev_light, p->light_stream));
+    if (s.use_mid) CK(cudaStreamWaitEvent(stream, p->ev_mid, 0));
+    CK(cudaStreamWaitEvent(stream, p->ev_light, 0));
+    return FAA_OK;
+}
+
 static int augment_common(faa_policy_t* p, const uint8_t* d_in_all, int n_all, int first, void* d_out, int batch,
                           int h, int w, const faa_tail_t* tail, const faa_sample_t* d_samples,
                           const faa_box_t* d_boxes, const faa_rng_t* rng, int op_base, const int32_t* d_partner,
@@ -633,7 +884,6 @@ static int augment_common(faa_policy_t* p, const uint8_t* d_in_all, int n_all, i
     P.use_zero_box = (tail->use_zero_box && apply_tail) ? 1 : 0;
     P.lam = lam; P.one_minus_lam = oml;
     P.bands = pick_bands(h, w, tail->out_h, tail->out_w);
-    static const bool lpt_off = [] { const char* e = getenv("FAA_LPT"); return e && e[0] == '0'; }();
     // TMA band staging needs 16-byte aligned image bases and a band that fits shared memory
     // (crop_pad only sizes the staged band; rows outside it are read from global memory)
     P.crop_pad = tail->crop_pad > 0 ? tail->crop_pad : 0;
@@ -642,11 +892,7 @@ static int augment_common(faa_policy_t* p, const uint8_t* d_in_all, int n_all, i
     P.band_cap = (int32_t)band_capacity(P.bands, h, w, tail->out_h, P.crop_pad);
     const size_t img_bytes = (size_t)h * w * 3;
     const int nsrc = d_partner ? 2 : 1;
-    static const bool stage_off = [] { const char* e = getenv("FAA_STAGE"); return e && e[0] == '0'; }();
-    static const bool mat_off = [] { const char* e = getenv("FAA_MAT"); return e && e[0] == '0'; }();
-    static const bool pdl_off = [] { const char* e = getenv("FAA_PDL"); return e && e[0] == '0'; }();
-    P.stage = (!stage_off && img_bytes % 16 == 0 && ((uintptr_t)d_in_all % 16) == 0 &&
-               (size_t)P.band_cap * nsrc <= 150 * 1024) ? 1 : 0;
+    P.stage = (img_bytes % 16 == 0 && ((uintptr_t)d_in_all % 16) == 0 && (size_t)P.band_cap * nsrc <= 150 * 1024) ? 1 : 0;
     if (!P.stage) P.band_cap = 0;
     {   // per-kernel band geometry and fastdiv reciprocals (host side: no divisions in the kernels)
         fill_geom(P.geo[0], P.bands, h, w, tail->out_h, P.crop_pad, P.stage != 0);
@@ -663,14 +909,11 @@ static int augment_common(faa_policy_t* p, const uint8_t* d_in_all, int n_all, i
                 if (eff > best + 0.02) { best = eff; lb = b; }
             }
         }
-        static const int light_bands = [] { const char* e = getenv("FAA_LIGHT_BANDS"); return e ? atoi(e) : 0; }();
-        if (light_bands >= 1 && light_bands <= 8 && light_bands <= h && light_bands <= tail->out_h) lb = light_bands;
         fill_geom(P.geo[1], lb, h, w, tail->out_h, P.crop_pad, P.stage != 0 && (size_t)band_capacity(lb, h, w, tail->out_h, P.crop_pad) <= 100 * 1024);
         auto rcp = [](uint32_t d) { return d <= 1 ? 0u : (uint32_t)((0x100000000ull + d - 1) / d); };
         P.rcp_out_qpr = rcp((uint32_t)(tail->out_w + 3) / 4); P.rcp_w = rcp((uint32_t)w); P.rcp_wq = rcp((uint32_t)w / 4);
         P.rcp_opr = (w & 7) ? 0u : rcp((uint32_t)w / 8);
-        static const bool oct_off = [] { const char* e = getenv("FAA_OCTETS"); return e && e[0] == '0'; }();
-        P.octets = (!oct_off && (w & 7) == 0 && tail->out_w == w && tail->out_h == h &&
+        P.octets = ((w & 7) == 0 && tail->out_w == w && tail->out_h == h &&
                     ((uintptr_t)d_out % 16) == 0 && P.stage) ? 1 : 0;          // (uint8 HWC included: 24-byte octets, 8-byte aligned)
     }
     // materialisation chunk: as many rows as fit ~16 KB, at least 3 (single-source launches only)
@@ -680,9 +923,9 @@ static int augment_common(faa_policy_t* p, const uint8_t* d_in_all, int n_all, i
         const int band_rows = (h + P.bands - 1) / P.bands + 2 + 2 * P.crop_pad;
         int rows = (band_rows * pitch <= 24576) ? band_rows : 16384 / pitch;
         if (rows > h + 2) rows = h + 2;
-        P.mat_cap = (!mat_off && !d_partner && rows >= 3) ? ((rows * pitch + 32 + 15) & ~15) : 0;   // + 2 guard bands
+        P.mat_cap = (!d_partner && rows >= 3) ? ((rows * pitch + 32 + 15) & ~15) : 0;   // + 2 guard bands
     }
-    P.pdl = pdl_off ? 0 : 1;
+    P.pdl = 1;
     // launch 1: decisions -> programs (the whole pool when partners may be anywhere in it)
     ResolveParams R; memset(&R, 0, sizeof R);
     R.ops = d_ops; R.probs = p->d_probs;
@@ -692,63 +935,30 @@ static int augment_common(faa_policy_t* p, const uint8_t* d_in_all, int n_all, i
     R.H = h; R.W = w; R.out_h = tail->out_h; R.out_w = tail->out_w;
     R.n_sub = p->n_sub; R.n_op = p->n_op; R.op_base = op_base; R.apply_tail = apply_tail;
     R.allow = P.mat_cap > 0 ? 1 : 0;
-    static const bool split_off = [] { const char* e = getenv("FAA_SPLIT"); return e && e[0] == '0'; }();
-    static const bool ahead_off = [] { const char* e = getenv("FAA_AHEAD"); return e && e[0] == '0'; }();
-    const bool use_order = !(d_partner || lpt_off);
+    Schedule s{};
+    s.use_order = !d_partner;
     // (small launches are launch-latency bound: one pixel kernel is faster there)
     size_t split_min = (size_t)4 << 20;                   // pixels per launch from which two pixel kernels pay off
     if (const char* e = getenv("FAA_SPLIT_MIN")) split_min = (size_t)strtoull(e, nullptr, 10);   // tests: force either path
     // (uint8 HWC output - the Mixup exchange format - splits when the lean octet paths can write it)
-    const bool use_split = use_order && !split_off && (tail->out_dtype != FAA_U8_HWC || (P.octets && P.crop_pad == 0 && apply_tail)) &&
-                           (size_t)batch * h * w >= split_min;
-    R.split = use_split ? 1 : 0;
-    // Chained steps (default; FAA_CHAIN=0 selects the event schedule): resolve(N+1), [cluster(N),] mid(N), light(N) all on the
-    // caller's stream with programmatic dependent launches, no events and no side streams.  Consecutive steps
-    // overlap (the next step's CTAs fill the slots the previous step's tail frees); the only true dependency -
-    // programs written by the resolve kernel - is a ticket word the pixel kernels poll.  FAA_CHAIN=0: the
-    // two-stream schedule with events (light kernel on the caller's stream, cluster kernel on a priority stream).
-    int chain_mode = 1;
-    if (const char* e = getenv("FAA_CHAIN")) chain_mode = atoi(e);
-    // (launches too small to split are chained as well: resolve(N+1), cluster(N) - their step is bound by kernel latencies,
-    //  which only overlap across steps on one stream; uint8 output stays on the event schedule)
-    static const bool chain_small_off = [] { const char* e = getenv("FAA_CHAIN_SMALL"); return e && e[0] == '0'; }();
-    const bool chain_small = !use_split && !chain_small_off && use_order && tail->out_dtype != FAA_U8_HWC;
-    const bool use_chain = chain_mode != 0 && (use_split || chain_small) && allow_ahead && rng && !d_samples && !d_partner &&
-                           !(getenv("FAA_AHEAD") && getenv("FAA_AHEAD")[0] == '0');
+    s.use_split = s.use_order && (tail->out_dtype != FAA_U8_HWC || (P.octets && P.crop_pad == 0 && apply_tail)) &&
+                  (size_t)batch * h * w >= split_min;
+    R.split = s.use_split ? 1 : 0;
+    // Chained steps need the Philox sampler on the device and a caller that allows the next batch to be resolved ahead.
+    // Launches too small to split are chained as well (resolve(N+1), cluster(N)): their step is bound by kernel latencies,
+    // which only overlap across steps on one stream; uint8 output of one pixel kernel stays on the event schedule.
+    s.use_chain = (s.use_split || tail->out_dtype != FAA_U8_HWC) && allow_ahead && rng && !d_samples && !d_partner;
     // Three-way split: statistics-LUT and Sharpness programs run in the lean mid kernel.
     // Needs the geometry its paths assume: float planes of the image's own size, no crop, W % 4 == 0, staged bands.
-    static const bool mid_off = [] { const char* e = getenv("FAA_MID"); return e && e[0] == '0'; }();
-    const bool use_mid = use_split && !mid_off && P.stage && (w & 3) == 0 && tail->out_w == w && tail->out_h == h &&
-                         P.crop_pad == 0 && ((uintptr_t)d_out % 16) == 0;
-    if (use_mid) R.split = 2;
-    if (use_split && P.octets && P.crop_pad == 0) R.allow |= 4;     // the lean gather paths exist in this launch
-    // program / schedule buffers come in two slots; a slot = progs[cap] + order[cap] + counters[2 cap] + ready[cap]
-    const size_t cap_imgs = p->d_progs_bytes / sizeof(Prog);
-    auto bind_slot = [&](int slot, ResolveParams& r, AugParams* a) {
-        Prog* progs = reinterpret_cast<Prog*>((uint8_t*)p->d_progs + (size_t)slot * p->d_progs_bytes);
-        int32_t* order = reinterpret_cast<int32_t*>(p->d_order) + (size_t)slot * (4 * cap_imgs + 8);
-        // the segment counters of a split launch live behind the order array, indexed by `first` so that
-        // concurrent chunk launches do not share them (same for the ready word)
-        int32_t* counter = order + cap_imgs + 2 * (size_t)first;
-        int32_t* ready = order + 3 * cap_imgs + first;
-        r.progs = progs; r.order = use_order ? order : nullptr; r.n_heavy = use_split ? counter : nullptr;
-        r.ready = use_chain ? ready : nullptr;
-        if (a) {
-            a->progs = progs; a->order = use_order ? order : nullptr; a->n_heavy = use_split ? counter : nullptr;
-            a->ready = use_chain ? ready : nullptr;
-        }
-    };
-    // scratch images: Sharpness -> gather programs of the cluster kernel, every Sharpness-first two-op program of the mid kernel
-    // Persistent mid / light kernels (chained schedule only; FAA_PERSIST=0 keeps one CTA row per image): rows loop over
-    // their entries, all CTAs of a kernel are resident at once, so it releases its dependents immediately and consecutive
-    // kernels - and steps - overlap for their whole length.  What the early release no longer orders is ordered explicitly:
-    // program slots by completion counters the next resolve kernel of the slot waits for, scratch images by a copy per slot.
-    static const bool persist_off = [] { const char* e = getenv("FAA_PERSIST"); return e && e[0] == '0'; }();
-    const bool persist = use_chain && !persist_off;
-    size_t scratch_slot_bytes = 0;
-    if ((p->has_sg || use_mid) && !d_partner && (w & 3) == 0) {
-        scratch_slot_bytes = (size_t)n_all * img_bytes;
-        const size_t need = scratch_slot_bytes * (persist ? 2 : 1);
+    s.use_mid = s.use_split && P.stage && (w & 3) == 0 && tail->out_w == w && tail->out_h == h &&
+                P.crop_pad == 0 && ((uintptr_t)d_out % 16) == 0;
+    if (s.use_mid) R.split = 2;
+    if (s.use_split && P.octets && P.crop_pad == 0) R.allow |= 4;     // the lean gather paths exist in this launch
+    // scratch images: Sharpness -> gather programs of the cluster kernel, every Sharpness-first two-op program of the mid
+    // kernel; one per program slot in the chained schedule
+    if ((p->has_sg || s.use_mid) && !d_partner && (w & 3) == 0) {
+        s.scratch_slot_bytes = (size_t)n_all * img_bytes;
+        const size_t need = s.scratch_slot_bytes * (s.use_chain ? 2 : 1);
         if (p->d_scratch_bytes < need) {
             if (p->d_scratch) { CK(cudaStreamSynchronize(stream)); CK(cudaFree(p->d_scratch)); p->d_scratch = nullptr; p->d_scratch_bytes = 0; }
             CK(cudaMalloc(&p->d_scratch, need));
@@ -759,11 +969,9 @@ static int augment_common(faa_policy_t* p, const uint8_t* d_in_all, int n_all, i
     }
     // With the lean gathers (allow bit 2) and a scratch image (bit 1) every program of a three-way split is light or mid
     // (faa_core.cuh prog_is_light / prog_is_mid cover all class combinations; tests/test_gpu_fastpaths.py runs every ordered
-    // op pair through this schedule): the cluster kernel has nothing to do and is not launched.  FAA_HEAVY=1 launches it anyway.
-    static const bool heavy_always = [] { const char* e = getenv("FAA_HEAVY"); return e && e[0] == '1'; }();
-    const bool no_heavy = use_mid && (R.allow & 6) == 6 && P.mat_cap > 0 && !heavy_always;
-    bool use_tab = false;
-    if (tail->out_dtype != FAA_U8_HWC) { if (int e = normalisation(p, tail, P, use_tab, stream)) return e; }
+    // op pair through this schedule): the cluster kernel has nothing to do and is not launched.
+    s.no_heavy = s.use_mid && (R.allow & 6) == 6 && P.mat_cap > 0;
+    if (tail->out_dtype != FAA_U8_HWC) { if (int e = normalisation(p, tail, P, s.use_tab, stream)) return e; }
     else { for (int c = 0; c < 3; ++c) { P.scale[c] = 1.0f; P.bias[c] = 0.0f; } }      // lean paths: the byte value itself
     if (p->lighting_rgb && tail->out_dtype != FAA_U8_HWC && apply_tail) {
         // Lighting (augmentations.py:197-215): one normalisation table per image, built on the stream in torch's fp32 order
@@ -778,251 +986,28 @@ static int augment_common(faa_policy_t* p, const uint8_t* d_in_all, int n_all, i
         CK(launch_lighting_tables(p->lighting_rgb, p->d_norm_img, n_all, tail->mean, tail->std, stream));
         g_launches++;
         P.norm_tab = p->d_norm_img; P.norm_stride = 768;
-        use_tab = true;
+        s.use_tab = true;
     }
     // fused Mixup mixes the fp32 normalised values before the output rounding: the fma shortcut is only proven to round
     // like the exact value for a DIRECT fp16 / bf16 store, so two-source launches always take the exact table
-    if (d_partner) use_tab = true;
-    // Self-resolving launch (FAA_SELF=0 turns it off): a launch of tiny images is bound by kernel latencies and by the
-    // host's launch rate, not by bytes.  Thread 0 of every CTA draws its image's decisions and builds the program itself
-    // (same Philox counters, same build_prog): ONE kernel per step, no program array, no ticket - consecutive steps have
-    // no dependency left and overlap through programmatic dependent launch.
-    static const bool self_off = [] { const char* e = getenv("FAA_SELF"); return e && e[0] == '0'; }();
-    if (!use_split && !self_off && rng && !d_samples && !d_partner && (size_t)h * w <= 4096) {     // (tiny images: see below)
-        const uintptr_t in0 = (uintptr_t)d_in_all + (in_mod ? 0 : (size_t)first * img_bytes),
-                        in1 = in0 + (size_t)(in_mod ? in_mod : batch) * img_bytes;
-        const uintptr_t out0 = (uintptr_t)d_out, out1 = out0 + (size_t)batch * tail->out_h * tail->out_w * 3 * out_elem_size(tail->out_dtype);
-        auto overlap = [](uintptr_t a0, uintptr_t a1, const uintptr_t b[2]) { return a0 < b[1] && b[0] < a1; };
-        const bool overlap_ok = p->overlap_calls && p->chain_live && p->chain_stream == stream && !overlap(in0, in1, p->prev_out) &&
-                                !overlap(out0, out1, p->prev_out) && !overlap(out0, out1, p->prev_in) && !P.norm_stride;
-        AugParams Ps = P;
-        Ps.progs = nullptr; Ps.order = nullptr; Ps.n_heavy = nullptr; Ps.ready = nullptr; Ps.done = nullptr; Ps.grid_y = 0;
-        Ps.self_resolve = 1;
-        Ps.sr_ops = d_ops; Ps.sr_probs = p->d_probs; memcpy(&Ps.sr_rng, rng, sizeof(RngCfg));
-        Ps.sr_n_sub = p->n_sub; Ps.sr_n_op = p->n_op; Ps.sr_op_base = op_base; Ps.sr_apply_tail = apply_tail; Ps.sr_allow = R.allow;
-        // chain = 1: no griddepcontrol.wait (nothing of the previous kernel is consumed), dependents released once the CTA has
-        // its program; a step that touches the previous step's buffers is launched as a plain stream-ordered kernel instead
-        Ps.chain = overlap_ok ? 1 : 0; Ps.pdl = 0;
-        // Only for tiny images (CIFAR): there the one-block resolve kernel is as long as the pixel kernel; for larger images
-        // every band CTA would repeat the whole serial resolve work.
-        // Sharpness -> gather programs are evaluated lazily instead of through the scratch image - the last thing consecutive
-        // steps shared - and every CTA releases the next step at once (chain = 3).
-        Ps.sr_allow &= ~2; Ps.scratch = nullptr;
-        if (overlap_ok) Ps.chain = 3;
-        CK(launch_augment(Ps, tail->out_dtype, use_tab, 0, stream));
-        g_launches++;
-        p->ahead_valid = false;
-        p->chain_live = true; p->chain_stream = stream;
-        p->prev_in[0] = in0; p->prev_in[1] = in1; p->prev_out[0] = out0; p->prev_out[1] = out1;
-        return FAA_OK;
-    }
+    if (d_partner) s.use_tab = true;
+    // Only for tiny images (CIFAR): there the one-block resolve kernel is as long as the pixel kernel; for larger images
+    // every band CTA would repeat the whole serial resolve work.
+    if (!s.use_split && rng && !d_samples && !d_partner && (size_t)h * w <= 4096)
+        return launch_self_resolving(p, P, R, s.use_tab, tail->out_dtype, stream);
     // resolve-ahead: did the previous call already resolve exactly this batch on the side stream?
-    const bool spec_ok = allow_ahead && !ahead_off && rng && !d_samples && !d_partner;
+    s.speculate = allow_ahead && rng && !d_samples && !d_partner;
     faa_policy::AheadKey key; memset(&key, 0, sizeof key);
-    if (spec_ok) {
+    if (s.speculate) {
         key.seed = rng->seed; key.first_index = rng->first_index;
         const int32_t v[16] = {batch, n_all, first, h, w, tail->out_h, tail->out_w, op_base, apply_tail, R.allow, R.split,
-                               rng->crop_pad, rng->hflip, rng->zero_box_len, (use_order ? 1 : 0) | (in_mod << 1), (use_chain ? 1 : 0) | (P.norm_stride ? 2 : 0)};
+                               rng->crop_pad, rng->hflip, rng->zero_box_len, (s.use_order ? 1 : 0) | (in_mod << 1),
+                               (s.use_chain ? 1 : 0) | (P.norm_stride ? 2 : 0)};
         memcpy(key.v, v, sizeof v);
     }
-    auto set_mid_geometry = [&](AugParams& a) {
-        int mb = P.bands;                                   // halve the band count while a band (+ halo) stays <= 80 KB (2 CTAs / SM)
-        while (mb > 1 && band_capacity(mb / 2, h, w, tail->out_h, 0) <= 80 * 1024) mb /= 2;
-        static const int mid_bands = [] { const char* e = getenv("FAA_MID_BANDS"); return e ? atoi(e) : 0; }();
-        if (mid_bands >= 1 && mid_bands <= 8 && (mid_bands & (mid_bands - 1)) == 0 && mid_bands <= h) mb = mid_bands;
-        a.bands = mb;
-        fill_geom(a.geo[0], mb, h, w, tail->out_h, 0, true);
-        a.band_cap = a.geo[0].band_cap; a.mat_cap = 0;
-    };
-    const bool hit = spec_ok && p->ahead_valid && memcmp(&key, &p->ahead_key, sizeof key) == 0;
-    int slot = p->cur_slot;
-    if (use_chain) {
-        // ---- chained schedule -------------------------------------------------------------------------
-        // A step may only overlap the previous one if it neither reads what that step wrote nor writes what it
-        // read or wrote (and follows it on the same stream); otherwise its first kernel is a plain dependent launch.
-        const uintptr_t in0 = (uintptr_t)d_in_all + (in_mod ? 0 : (size_t)first * img_bytes),
-                        in1 = in0 + (size_t)(in_mod ? in_mod : batch) * img_bytes;
-        const uintptr_t out0 = (uintptr_t)d_out, out1 = out0 + (size_t)batch * tail->out_h * tail->out_w * 3 * out_elem_size(tail->out_dtype);
-        auto overlap = [](uintptr_t a0, uintptr_t a1, const uintptr_t b[2]) { return a0 < b[1] && b[0] < a1; };
-        // ... and only if the caller has promised that this call's inputs were complete before the previous call was issued
-        // (faa_policy_set_overlap / faa_augment_many): a kernel launched with programmatic serialization that does not execute
-        // griddepcontrol.wait has no visibility guarantee for what the kernel right in front of it wrote, and that kernel
-        // may be the producer of this batch (a gather, a copy).  Within a call every kernel only consumes what its own
-        // call's first - stream-ordered - kernel already waited for.
-        bool overlap_ok = p->overlap_calls && p->chain_live && p->chain_stream == stream && !overlap(in0, in1, p->prev_out) &&
-                          !overlap(out0, out1, p->prev_out) && !overlap(out0, out1, p->prev_in);
-        AugParams Pc = P;
-        Pc.chain = persist ? 2 : 1; Pc.pdl = 0;
-        // completion counter of a slot: the first spare word behind its order / counters / ready arrays
-        auto done_word = [&](int s) { return reinterpret_cast<uint32_t*>(reinterpret_cast<int32_t*>(p->d_order) + (size_t)s * (4 * cap_imgs + 8) + 4 * cap_imgs); };
-        auto wait_for_slot = [&](int s, ResolveParams& r) {
-            r.wait_done = persist ? done_word(s) : nullptr; r.wait_target = p->done_target[s];
-        };
-        if (hit) {
-            slot = p->ahead_slot;
-            Pc.ticket = p->ahead_ticket;
-            bind_slot(slot, R, &Pc);
-        } else {
-            bind_slot(slot, R, &Pc);
-            R.ticket = ++p->ticket; R.pdl = overlap_ok ? 1 : 0;
-            Pc.ticket = R.ticket;
-            wait_for_slot(slot, R);
-            CK(launch_resolve(R, stream));
-            g_launches++;
-            overlap_ok = true;                              // the kernels behind it may overlap IT
-        }
-        p->cur_slot = slot;
-        p->ahead_valid = false;
-        {   // speculate on the next call: same everything, first_index advanced by the stride seen so far
-            uint64_t stride = (uint64_t)batch;
-            faa_policy::AheadKey base = key; base.first_index = 0;
-            faa_policy::AheadKey lastb = p->last_key; lastb.first_index = 0;
-            if (p->have_last && memcmp(&base, &lastb, sizeof base) == 0 && rng->first_index > p->last_key.first_index)
-                stride = rng->first_index - p->last_key.first_index;
-            p->last_key = key; p->have_last = true;
-            ResolveParams R2 = R;
-            R2.rng.first_index = rng->first_index + stride;
-            bind_slot(slot ^ 1, R2, nullptr);
-            R2.ticket = ++p->ticket; R2.pdl = overlap_ok ? 1 : 0;
-            // (its slot's last readers - the step before this one - copied their programs before they let any
-            //  later kernel of the stream start, so the resolve kernel may overwrite the slot as soon as it runs;
-            //  persistent readers release their dependents at once and are waited for through the slot's counter)
-            wait_for_slot(slot ^ 1, R2);
-            CK(launch_resolve(R2, stream));
-            g_launches++;
-            p->ahead_key = key; p->ahead_key.first_index = rng->first_index + stride;
-            p->ahead_slot = slot ^ 1; p->ahead_valid = true; p->ahead_ticket = R2.ticket;
-        }
-        if (persist) {
-            if (!p->sm_count) CK(cudaDeviceGetAttribute(&p->sm_count, cudaDevAttrMultiProcessorCount, p->device));
-            Pc.done = done_word(slot);
-            if (P.scratch) Pc.scratch = P.scratch + (size_t)slot * scratch_slot_bytes;
-        }
-        AugParams Pm = Pc;                                  // the mid kernel: its own (taller) bands in bands / geo[0]
-        if (use_mid) set_mid_geometry(Pm);
-        if (persist) {
-            // one resident wave each (launch bounds: light CTAs / SM, 2 mid CTAs / SM)
-            static const int rows_l = [] { const char* e = getenv("FAA_ROWS_LIGHT"); return e ? atoi(e) : 0; }();
-            static const int rows_m = [] { const char* e = getenv("FAA_ROWS_MID"); return e ? atoi(e) : 0; }();
-            const int lb = P.geo[1].bands > 0 ? P.geo[1].bands : 1;
-            Pc.grid_y = rows_l > 0 ? rows_l : (p->sm_count * resident_ctas_per_sm(1)) / lb;
-            // (mid rows: ONE CTA per SM, so that the light CTAs that follow share the SM with it from the start)
-            Pm.grid_y = rows_m > 0 ? rows_m : p->sm_count / (Pm.bands > 0 ? Pm.bands : 1);
-            if (Pc.grid_y < 1) Pc.grid_y = 1;
-            if (Pm.grid_y < 1) Pm.grid_y = 1;
-        }
-        const int order3[3] = {chain_mode == 2 ? 1 : 0, 2, chain_mode == 2 ? 0 : 1};   // default: cluster, mid, light
-        for (int k = 0; k < 3; ++k) {
-            const int which = order3[k];
-            if (which != 0 && !use_split) continue;          // one pixel kernel
-            if (which == 2) { if (use_mid) { CK(launch_augment(Pm, tail->out_dtype, use_tab, 2, stream)); g_launches++; if (persist) p->done_target[slot] += augment_cta_count(Pm, 2); } }
-            else if (which == 0 && no_heavy) continue;
-            else {
-                AugParams Pk = Pc;
-                if (which == 0) Pk.grid_y = 0;              // the cluster kernel keeps one cluster per entry
-                CK(launch_augment(Pk, tail->out_dtype, use_tab, which, stream)); g_launches++;
-                if (persist) p->done_target[slot] += augment_cta_count(Pk, which);
-            }
-        }
-        p->chain_live = true; p->chain_stream = stream;
-        p->prev_in[0] = in0; p->prev_in[1] = in1; p->prev_out[0] = out0; p->prev_out[1] = out1;
-        return FAA_OK;
-    }
-    p->chain_live = false;
-    if (hit) {
-        slot = p->ahead_slot;
-        CK(cudaStreamWaitEvent(stream, p->ev_ahead, 0));
-        P.pdl = 0;                                          // no resolve kernel right in front of the pixel kernel
-        bind_slot(slot, R, &P);
-    } else {
-        bind_slot(slot, R, &P);
-        CK(launch_resolve(R, stream));
-        g_launches++;
-    }
-    p->cur_slot = slot;
-    p->ahead_valid = false;
-    if (P.n_heavy || spec_ok) {
-        if (!p->light_stream) {
-            {
-                int lo = 0, hi = 0;
-                CK(cudaDeviceGetStreamPriorityRange(&lo, &hi));       // hi = numerically lowest = greatest priority
-                CK(cudaStreamCreateWithPriority(&p->light_stream, cudaStreamNonBlocking, hi));
-            }
-            {
-                int lo = 0, hi = 0;
-                CK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-                CK(cudaStreamCreateWithPriority(&p->ahead_stream, cudaStreamNonBlocking, hi));   // one block: get a slot promptly
-            }
-            {
-                int lo = 0, hi = 0;
-                CK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-                CK(cudaStreamCreateWithPriority(&p->mid_stream, cudaStreamNonBlocking, hi));
-            }
-            CK(cudaEventCreateWithFlags(&p->ev_mid, cudaEventDisableTiming));
-            CK(cudaEventCreateWithFlags(&p->ev_res, cudaEventDisableTiming));
-            CK(cudaEventCreateWithFlags(&p->ev_light, cudaEventDisableTiming));
-            CK(cudaEventCreateWithFlags(&p->ev_ahead, cudaEventDisableTiming));
-        }
-        CK(cudaEventRecord(p->ev_res, stream));               // this batch's programs are ready
-    }
-    if (spec_ok) {
-        // speculate on the next call: same everything, first_index advanced by the stride seen so far
-        uint64_t stride = (uint64_t)batch;
-        faa_policy::AheadKey base = key; base.first_index = 0;
-        faa_policy::AheadKey lastb = p->last_key; lastb.first_index = 0;
-        if (p->have_last && memcmp(&base, &lastb, sizeof base) == 0 && rng->first_index > p->last_key.first_index)
-            stride = rng->first_index - p->last_key.first_index;
-        p->last_key = key; p->have_last = true;
-        ResolveParams R2 = R;
-        R2.rng.first_index = rng->first_index + stride;
-        bind_slot(slot ^ 1, R2, nullptr);
-        CK(cudaStreamWaitEvent(p->ahead_stream, p->ev_res, 0));      // the other slot's last readers are done
-        CK(launch_resolve(R2, p->ahead_stream));
-        CK(cudaEventRecord(p->ev_ahead, p->ahead_stream));
-        g_launches++;
-        p->ahead_key = key; p->ahead_key.first_index = rng->first_index + stride;
-        p->ahead_slot = slot ^ 1; p->ahead_valid = true;
-    }
-    // launch 2: pixels
-    if (P.n_heavy) {
-        // Two pixel kernels, concurrently: the light streaming kernel goes first on the caller's
-        // stream and fills the machine; the cluster kernel runs on a HIGH-PRIORITY side stream, so its
-        // clusters take the CTA slots as they free up (heavy images finish early, light work fills gaps).
-        static const bool prio_off = [] { const char* e = getenv("FAA_PRIO"); return e && e[0] == '0'; }();
-        if (prio_off) {
-            CK(cudaStreamWaitEvent(p->light_stream, p->ev_res, 0));
-            CK(launch_augment(P, tail->out_dtype, use_tab, 0, stream));
-            CK(launch_augment(P, tail->out_dtype, use_tab, 1, p->light_stream));
-            if (use_mid) { AugParams Pm = P; Pm.pdl = 0; set_mid_geometry(Pm); CK(launch_augment(Pm, tail->out_dtype, use_tab, 2, p->light_stream)); g_launches++; }
-            CK(cudaEventRecord(p->ev_light, p->light_stream));
-        } else {
-            AugParams Ph = P; Ph.pdl = 0;                           // not behind the resolve kernel in its stream
-            CK(cudaStreamWaitEvent(p->light_stream, p->ev_res, 0));
-            static const bool mid_same = [] { const char* e = getenv("FAA_MID_STREAM"); return e && e[0] == '0'; }();
-            static const int order_knob = [] { const char* e = getenv("FAA_ORDER"); return e ? atoi(e) : 0; }();
-            if (use_mid && !mid_same) CK(cudaStreamWaitEvent(p->mid_stream, p->ev_res, 0));
-            // the streaming kernel goes FIRST: it fills the machine at once; the priority streams' clusters then take
-            // the slots its CTAs free (launched first, the thousands of exiting CTAs of the cluster kernels would hold
-            // up the work distributor)
-            if (order_knob == 0) CK(launch_augment(P, tail->out_dtype, use_tab, 1, stream));
-            if (!no_heavy) CK(launch_augment(Ph, tail->out_dtype, use_tab, 0, p->light_stream)); else g_launches--;
-            if (order_knob == 1) CK(launch_augment(P, tail->out_dtype, use_tab, 1, stream));
-            if (use_mid) {                                                               // statistics / Sharpness clusters: third stream
-                AugParams Pm = Ph; set_mid_geometry(Pm);
-                CK(launch_augment(Pm, tail->out_dtype, use_tab, 2, mid_same ? p->light_stream : p->mid_stream)); g_launches++;
-                if (!mid_same) CK(cudaEventRecord(p->ev_mid, p->mid_stream));
-            }
-            if (order_knob == 2) CK(launch_augment(P, tail->out_dtype, use_tab, 1, stream));
-            CK(cudaEventRecord(p->ev_light, p->light_stream));
-            if (use_mid && !mid_same) CK(cudaStreamWaitEvent(stream, p->ev_mid, 0));
-        }
-        CK(cudaStreamWaitEvent(stream, p->ev_light, 0));
-        g_launches += 2;
-    } else {
-        CK(launch_augment(P, tail->out_dtype, use_tab, 0, stream));
-        g_launches++;
-    }
-    return FAA_OK;
+    s.hit = s.speculate && p->ahead_valid && memcmp(&key, &p->ahead_key, sizeof key) == 0;
+    if (s.use_chain) return launch_chained(p, P, R, s, key, tail->out_dtype, stream);
+    return launch_event(p, P, R, s, key, tail->out_dtype, stream);
 }
 
 int faa_augment(faa_policy_t* p, const uint8_t* d_in, void* d_out, int batch, int h, int w, const faa_tail_t* tail,

@@ -1402,8 +1402,8 @@ static __device__ __forceinline__ void cluster_kernel_body(const AugParams& P) {
 
     // Programmatic dependent launch: everything above overlaps the resolve kernel's tail; the
     // schedule and the programs it writes are only read after this point.
-    if (!P.chain) asm volatile("griddepcontrol.wait;" ::: "memory");
-    if (P.chain == 3) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // self-resolving, nothing shared between steps
+    if (P.chain == CHAIN_STREAM_ORDERED) asm volatile("griddepcontrol.wait;" ::: "memory");
+    if (P.chain == CHAIN_SELF_RESOLVING) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // nothing shared between steps
     wait_ticket(P.ready, P.ticket);
 
     // split launches: this (cluster) kernel owns the first n_heavy entries of the schedule
@@ -1438,8 +1438,10 @@ static __device__ __forceinline__ void cluster_kernel_body(const AugParams& P) {
     __syncthreads();
     // chained steps: the next kernel of the stream may start once every CTA of this one has copied its program
     // (it may overwrite the OTHER program slot only); Sharpness->gather programs also own a scratch image that
-    // the next step reuses, so they only release at exit
-    if (P.chain && P.chain != 3 && st[0].prog.cls != C_SG) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    // the next step reuses, so they only release at exit.  (A chained step is tested as "neither stream-ordered nor
+    // self-resolving": `== CHAIN_STEP` compiles to one instruction less, and the shifted code made the self-resolving
+    // CIFAR step 0.5% slower on an H100 80GB HBM3 at 400 W.)
+    if (P.chain != CHAIN_STREAM_ORDERED && P.chain != CHAIN_SELF_RESOLVING && st[0].prog.cls != C_SG) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     if (s_len) {
 #pragma unroll
         for (int s = 0; s < NSRC; ++s) mbar_wait(&s_bar[s], 0);
@@ -1547,7 +1549,7 @@ __global__ void __launch_bounds__(kMidThreadsMax, 2) faa_augment_mid_kernel(cons
     if (TAB && !P.norm_stride)
         for (int i = threadIdx.x; i < 768; i += blockDim.x) s_norm[i] = __ldg(P.norm_tab + i);
     wait_ticket(P.ready, P.ticket);
-    if (P.chain == 2) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // persistent: see count_done
+    if (P.chain == CHAIN_STEP) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // persistent: see count_done
     const int e0 = ld_sched(P.n_heavy, P.chain), n_ent = ld_sched(P.n_heavy + 1, P.chain) - e0;
     // One entry per row, or a persistent row's entries.  The body is written for ONE entry; so that the compiler does not
     // hoist its loop-invariant parts (thread-index arithmetic, peer addresses) in front of the loop, where they would live
@@ -1570,7 +1572,6 @@ __global__ void __launch_bounds__(kMidThreadsMax, 2) faa_augment_mid_kernel(cons
     if (threadIdx.x < sizeof(Prog) / 4)
         reinterpret_cast<uint32_t*>(&st.prog)[threadIdx.x] = ld_sched(reinterpret_cast<const uint32_t*>(P.progs + idx) + threadIdx.x, P.chain);
     __syncthreads();
-    if (P.chain == 1) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");     // program copied
     if (s_len) mbar_wait(&s_bar, 0);
 
     const int y0 = P.geo[0].y[band], y1 = P.geo[0].y[band + 1];
@@ -1733,7 +1734,7 @@ __global__ void __launch_bounds__(kThreads, FAA_LIGHT_CTAS) faa_augment_light_ke
     if (TAB && !P.norm_stride)
         for (int i = threadIdx.x; i < 768; i += blockDim.x) s_norm[i] = __ldg(P.norm_tab + i);
     wait_ticket(P.ready, P.ticket);
-    if (P.chain == 2) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // persistent: see count_done
+    if (P.chain == CHAIN_STEP) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // persistent: see count_done
     const int n_heavy = ld_sched(P.n_heavy + 1, P.chain);       // entries in front of the light segment (heavy + mid)
     for (int round = 0;; ++round) {                              // one entry per row, or a persistent row's entries (see the mid kernel)
     const int ent = sched_entry(round, (int)blockIdx.y, (int)gridDim.y);
@@ -1753,7 +1754,6 @@ __global__ void __launch_bounds__(kThreads, FAA_LIGHT_CTAS) faa_augment_light_ke
     if (threadIdx.x < sizeof(Prog) / 4)
         reinterpret_cast<uint32_t*>(&s_prog)[threadIdx.x] = ld_sched(reinterpret_cast<const uint32_t*>(P.progs + idx) + threadIdx.x, P.chain);
     __syncthreads();
-    if (P.chain == 1) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");     // program copied: see the cluster kernel
     const uint32_t lut_mask = s_prog.lut_mask;
     if (lut_mask) {                                   // static LUTs only (no statistics in light programs)
 #pragma unroll
@@ -2094,8 +2094,6 @@ int pick_bands(int H, int W, int out_h, int out_w) {
     long long quads = (long long)out_h * ((out_w + 3) / 4);
     int b = 1;
     while (b < 8 && quads / (b * 2) >= 1024 && b * 2 <= H && b * 2 <= out_h) b *= 2;
-    const char* e = getenv("FAA_BANDS");          // tuning knob for experiments
-    if (e && *e) { int v = atoi(e); if (v >= 1 && v <= 8) b = (v <= H && v <= out_h) ? v : b; }
     return b;
 }
 
@@ -2126,27 +2124,28 @@ uint32_t band_capacity(int bands, int H, int W, int out_h, int crop_pad) {
 
 #endif  // !FAA_TU_OUT
 
-template <int OUT, int NSRC, bool TAB>
-static cudaError_t launch_one(const AugParams& p, cudaStream_t stream) {
-    const size_t dyn = (size_t)p.geo[0].band_cap * NSRC + (size_t)p.mat_cap;
-    static size_t configured[kMaxDevices] = {};     // per instantiation AND per device (the attribute is per device)
+// raise Kernel's dynamic shared memory limit to `dyn` bytes on the current device if it is below that
+// (the attribute is per kernel AND per device)
+template <auto Kernel>
+static cudaError_t reserve_dyn_smem(size_t dyn) {
+    static size_t configured[kMaxDevices] = {};
     int dev = 0;
     if (cudaError_t e = cudaGetDevice(&dev)) return e;
     if (dev < 0 || dev >= kMaxDevices) return cudaErrorInvalidDevice;
     if (dyn > configured[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(faa_augment_kernel<OUT, NSRC, TAB>,
-                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
-        if (e != cudaSuccess) return e;
+        if (cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn)) return e;
         configured[dev] = dyn;
     }
+    return cudaSuccess;
+}
+
+template <int OUT, int NSRC, bool TAB>
+static cudaError_t launch_one(const AugParams& p, cudaStream_t stream) {
+    const size_t dyn = (size_t)p.geo[0].band_cap * NSRC + (size_t)p.mat_cap;
+    if (cudaError_t e = reserve_dyn_smem<faa_augment_kernel<OUT, NSRC, TAB>>(dyn)) return e;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)p.bands, (unsigned)p.B, 1);
-    // tiny bands (CIFAR: 1024 pixels per image): fewer threads per CTA = more resident CTAs = more per-CTA latency
-    // chains (program, TMA, first store) in flight
-    static const int small_threads = [] { const char* e = getenv("FAA_SMALL_THREADS"); int v = e ? atoi(e) : 0;
-                                          return (v == 128 || v == 256) ? v : 256; }();      // (make_lut needs 3 warps)
-    const int threads = ((int64_t)p.H * p.W <= (int64_t)p.bands * 2048) ? small_threads : kThreads;
-    cfg.blockDim = dim3((unsigned)threads, 1, 1);
+    cfg.blockDim = dim3(kThreads, 1, 1);
     cfg.dynamicSmemBytes = dyn;
     cfg.stream = stream;
     cudaLaunchAttribute attr[2];
@@ -2166,16 +2165,7 @@ static inline int rows_of(const AugParams& p) { return (p.grid_y > 0 && p.grid_y
 template <int OUT, bool TAB>
 static cudaError_t launch_light(const AugParams& p, cudaStream_t stream) {
     const size_t dyn = (size_t)p.geo[1].band_cap;
-    static size_t configured[kMaxDevices] = {};
-    int dev = 0;
-    if (cudaError_t e = cudaGetDevice(&dev)) return e;
-    if (dev < 0 || dev >= kMaxDevices) return cudaErrorInvalidDevice;
-    if (dyn > configured[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(faa_augment_light_kernel<OUT, TAB>,
-                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
-        if (e != cudaSuccess) return e;
-        configured[dev] = dyn;
-    }
+    if (cudaError_t e = reserve_dyn_smem<faa_augment_light_kernel<OUT, TAB>>(dyn)) return e;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)p.geo[1].bands, (unsigned)rows_of(p), 1);
     cfg.blockDim = dim3(kThreads, 1, 1);
@@ -2191,37 +2181,25 @@ static cudaError_t launch_light(const AugParams& p, cudaStream_t stream) {
 
 template <int OUT, bool TAB>
 static cudaError_t launch_mid(const AugParams& p, cudaStream_t stream) {
-    {
-        const size_t dyn = (size_t)p.geo[0].band_cap;
-        static size_t configured[kMaxDevices] = {};
-        int dev = 0;
-        if (cudaError_t e = cudaGetDevice(&dev)) return e;
-        if (dev < 0 || dev >= kMaxDevices) return cudaErrorInvalidDevice;
-        if (dyn > configured[dev]) {
-            cudaError_t e = cudaFuncSetAttribute(faa_augment_mid_kernel<OUT, TAB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
-            if (e != cudaSuccess) return e;
-            configured[dev] = dyn;
-        }
-        cudaLaunchConfig_t cfg = {};
-        static const int mid_threads = [] { const char* e = getenv("FAA_MID_THREADS"); int v = e ? atoi(e) : 0;
-                                            return (v == 128 || v == 256 || v == 512) ? v : 0; }();
-        // enough threads for the band: 512 for the tall bands of large images, 256 otherwise
-        const int threads = mid_threads ? mid_threads : ((size_t)p.geo[0].band_cap > 48 * 1024 ? 512 : 256);
-        cfg.gridDim = dim3((unsigned)p.bands, (unsigned)rows_of(p), 1);
-        cfg.blockDim = dim3((unsigned)threads, 1, 1);
-        cfg.dynamicSmemBytes = dyn;
-        cfg.stream = stream;
-        cudaLaunchAttribute attr[2];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = (unsigned)p.bands;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = 1;
-        attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[1].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = p.chain ? 2 : 1;
-        return cudaLaunchKernelEx(&cfg, faa_augment_mid_kernel<OUT, TAB>, p);
-    }
+    const size_t dyn = (size_t)p.geo[0].band_cap;
+    if (cudaError_t e = reserve_dyn_smem<faa_augment_mid_kernel<OUT, TAB>>(dyn)) return e;
+    cudaLaunchConfig_t cfg = {};
+    // enough threads for the band: 512 for the tall bands of large images, 256 otherwise
+    const int threads = dyn > 48 * 1024 ? 512 : 256;
+    cfg.gridDim = dim3((unsigned)p.bands, (unsigned)rows_of(p), 1);
+    cfg.blockDim = dim3((unsigned)threads, 1, 1);
+    cfg.dynamicSmemBytes = dyn;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[2];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)p.bands;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[1].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = p.chain ? 2 : 1;
+    return cudaLaunchKernelEx(&cfg, faa_augment_mid_kernel<OUT, TAB>, p);
 }
 
 template <int OUT>

@@ -41,6 +41,16 @@ struct BandGeom {
     uint32_t lo[8], len[8];     // staged byte range of the raw image per band (len 0: nothing staged)
 };
 
+// AugParams::chain: how a pixel launch is ordered against the kernel in front of it in its stream
+enum ChainMode : int32_t {
+    CHAIN_STREAM_ORDERED = 0,   // griddepcontrol.wait before the schedule is read (or no programmatic launch at all)
+    CHAIN_STEP = 1,             // chained step (resolve, pixel kernels and the next step on ONE stream, programmatic
+                                // dependent launches): no griddepcontrol.wait - the ticket orders the programs; the persistent
+                                // mid / light kernels release their dependents at once and the slot's next writer waits for
+                                // `done`; the cluster kernel releases them once its program is copied
+    CHAIN_SELF_RESOLVING = 2,   // self-resolving step: nothing is shared between steps, every CTA releases the next at once
+};
+
 // step 2 (one cluster per image): pixels
 struct AugParams {
     const uint8_t* in;          // [n_all][H][W][3] uint8
@@ -69,11 +79,7 @@ struct AugParams {
     int32_t pdl;                // launched with programmatic stream serialization
     const int32_t* ready;       // chained steps: spin until *ready == ticket before reading programs / order / n_heavy
     int32_t ticket;
-    int32_t chain;              // 1: steps are chained with programmatic dependent launches on ONE stream - no
-                                // griddepcontrol.wait (nothing of the previous kernel is consumed), trigger the
-                                // dependents once this CTA has copied its program
-                                // 2: same, with persistent mid / light kernels - the dependents are released at once and
-                                // the slot's next writer waits for `done` instead
+    int32_t chain;              // ChainMode
     int32_t grid_y;             // > 0: launch this many schedule rows (CTAs / clusters per band); each one loops over the
                                 // entries row, row + grid_y, ... of its segment.  0: one row per image (B)
     uint32_t* done;             // optional completion counter: every CTA adds 1 when it has finished (release)

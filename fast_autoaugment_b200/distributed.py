@@ -9,8 +9,8 @@ rank-local under DDP, ``train.py:55``; global pairing is an extension):
   communication);
 * every sample's partner is needed by exactly ONE sample (the pairing is a permutation), so the exchange
   is a **partner-only all-to-all** of raw uint8 images (``mixup_global``): a rank receives only the <= B/G
-  images its own samples pair with - 1/G of what a whole-pool all-gather (``mixup_global_allgather``, kept
-  as the north star's baseline) would deliver - 3 B/px on the wire: half of the fp16 output, a quarter of fp32.
+  images its own samples pair with - 1/G of what a whole-pool all-gather would deliver - 3 B/px on the wire:
+  half of the fp16 output, a quarter of fp32.
   Mixing is linear, so "augment the partner here" equals "augment there, send, mix";
 * the fused-Mixup kernel recomputes each partner's augmentation from the received raw image with the
   partner's own decisions: Philox records drawn for the GLOBAL sample indices on every rank (16 + 8 n_op
@@ -378,32 +378,3 @@ def mixup_global_peer(policy: CompiledPolicy, local_u8: torch.Tensor, targets: t
         timing["m1"] = torch.cuda.Event(enable_timing=True); timing["m1"].record()
     return out, targets, all_targets[tgt_idx_dev], lam
 
-
-def mixup_global_allgather(policy: CompiledPolicy, local_u8: torch.Tensor, targets: torch.Tensor, tail: TailSpec, alpha: float,
-                           seed: int, step: int, group=None, samples=None, boxes=None):
-    """The north star's baseline exchange: all-gather of the WHOLE raw pool (G times the bytes ``mixup_global``
-    moves), then the same fused kernel.  Same results as ``mixup_global``.
-
-    Returns ``(data, targets, partner_targets, lam)`` like reference ``mixup`` (aug_mixup.py:23).
-    Decisions: fused Philox keyed by the global sample index (default), or resolved records given
-    for the local shard (``samples``/``boxes`` numpy arrays, all-gathered as bytes).
-    """
-    rank, world = dist.get_rank(group), dist.get_world_size(group)
-    b = local_u8.shape[0]
-    n = b * world
-    perm, lam = global_pairing(n, alpha, seed, step)
-    lo, hi = shard_bounds(n, rank, world)
-    pool = gather_pool(local_u8, group)
-    all_targets = gather_pool(targets, group)
-    partner = perm[lo:hi]
-    rng = pool_s = pool_b = None
-    if samples is None:
-        rng = make_rng(seed, step * n, tail)
-    else:
-        dev = local_u8.device
-        s = torch.from_numpy(np.ascontiguousarray(samples).view(np.uint8).reshape(b, -1).copy()).to(dev)
-        bx = torch.from_numpy(np.ascontiguousarray(boxes).view(np.uint8).reshape(b, -1).copy()).to(dev)
-        pool_s, pool_b = gather_pool(s, group).reshape(-1), gather_pool(bx, group).reshape(-1)
-    data = augment_batch(policy, local_u8, tail, rng=rng, partner=partner, lam=lam, pool=pool,
-                         pool_samples=pool_s, pool_boxes=pool_b, first=lo)
-    return data, targets, all_targets[partner.to(all_targets.device)], lam
