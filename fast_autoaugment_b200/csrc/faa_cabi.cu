@@ -211,6 +211,9 @@ struct faa_policy {
     AheadKey ahead_key{}; bool ahead_valid = false; int ahead_slot = 0, cur_slot = 0;
     bool have_last = false; AheadKey last_key{};
     cudaStream_t ahead_stream = nullptr; cudaEvent_t ev_ahead = nullptr;
+    bool ahead_on_side = false;          // an event-schedule resolve-ahead on ahead_stream that no later launch waited for yet
+    cudaStream_t last_stream = nullptr; bool have_last_stream = false;   // the stream of the previous call (follow_stream)
+    cudaEvent_t ev_switch = nullptr;
     void* d_scratch = nullptr; size_t d_scratch_bytes = 0;   // Sharpness->gather scratch images
     bool overlap_calls = false;          // faa_policy_set_overlap: consecutive calls on one stream may overlap (see augment_common)
     uint32_t done_target[2] = {0, 0};    // persistent chained steps: CTAs that have been launched on each program slot so far
@@ -340,6 +343,7 @@ int faa_policy_destroy(faa_policy_t* p) {
     if (p->ev_mid) cudaEventDestroy(p->ev_mid);
     if (p->ahead_stream) cudaStreamDestroy(p->ahead_stream);
     if (p->ev_ahead) cudaEventDestroy(p->ev_ahead);
+    if (p->ev_switch) cudaEventDestroy(p->ev_switch);
     if (p->ev_res) cudaEventDestroy(p->ev_res);
     if (p->ev_light) cudaEventDestroy(p->ev_light);
     delete p;
@@ -664,6 +668,22 @@ static void record_step(faa_policy* p, const AugParams& P, int out_dtype, cudaSt
     p->chain_live = true; p->chain_stream = stream;
 }
 
+// A call on another stream than the previous call first waits for everything issued to that stream so far.  The
+// previous call's kernels may still read the program slot, scratch image and tables this call rewrites, and nothing else
+// orders them across streams: event-schedule kernels do not count themselves (a chained resolve's completion-counter wait
+// passes at once, an event-schedule resolve does not wait at all), and a chained hit would poll a ticket whose resolve
+// kernel sits in the other stream and need not have started.  Alternating streams therefore serialise; calls on one
+// stream pay nothing.
+static int follow_stream(faa_policy* p, cudaStream_t stream) {
+    if (p->have_last_stream && p->last_stream != stream) {
+        if (!p->ev_switch) CK(cudaEventCreateWithFlags(&p->ev_switch, cudaEventDisableTiming));
+        CK(cudaEventRecord(p->ev_switch, p->last_stream));
+        CK(cudaStreamWaitEvent(stream, p->ev_switch, 0));
+    }
+    p->last_stream = stream; p->have_last_stream = true;
+    return FAA_OK;
+}
+
 // Resolve-ahead: speculate that the next call is this one (`key`) with first_index advanced by the stride seen so far.
 // Returns the resolve parameters of that call; the caller binds them to the other slot, launches them and then sets
 // ahead_valid.
@@ -714,6 +734,9 @@ static int launch_self_resolving(faa_policy* p, const AugParams& P, const Resolv
 // kernel of the slot waits for, scratch images by a copy per slot.
 static int launch_chained(faa_policy* p, const AugParams& P, ResolveParams& R, const Schedule& s,
                           const faa_policy::AheadKey& key, int out_dtype, cudaStream_t stream) {
+    // an event-schedule call resolved ahead into the other slot on ahead_stream: this step's resolve-ahead rewrites that
+    // slot on `stream` (a chained step never hits an event-schedule speculation: the key differs)
+    if (p->ahead_on_side) { CK(cudaStreamWaitEvent(stream, p->ev_ahead, 0)); p->ahead_on_side = false; }
     bool overlap_ok = may_overlap_previous(p, P, out_dtype, stream);
     AugParams Pc = P;
     Pc.chain = CHAIN_STEP; Pc.pdl = 0;
@@ -776,6 +799,7 @@ static int launch_event(faa_policy* p, AugParams& P, ResolveParams& R, const Sch
     if (s.hit) {
         slot = p->ahead_slot;
         CK(cudaStreamWaitEvent(stream, p->ev_ahead, 0));
+        p->ahead_on_side = false;
         P.pdl = 0;                                          // no resolve kernel right in front of the pixel kernel
         bind_slot(p, s, P.first, slot, R, &P);
     } else {
@@ -806,7 +830,7 @@ static int launch_event(faa_policy* p, AugParams& P, ResolveParams& R, const Sch
         CK(launch_resolve(R2, p->ahead_stream));
         CK(cudaEventRecord(p->ev_ahead, p->ahead_stream));
         g_launches++;
-        p->ahead_valid = true;
+        p->ahead_valid = true; p->ahead_on_side = true;
     }
     if (!P.n_heavy) {                                       // one pixel kernel
         CK(launch_augment(P, out_dtype, s.use_tab, 0, stream));
@@ -840,7 +864,8 @@ static int launch_event(faa_policy* p, AugParams& P, ResolveParams& R, const Sch
 static int augment_common(faa_policy_t* p, const uint8_t* d_in_all, int n_all, int first, void* d_out, int batch,
                           int h, int w, const faa_tail_t* tail, const faa_sample_t* d_samples,
                           const faa_box_t* d_boxes, const faa_rng_t* rng, int op_base, const int32_t* d_partner,
-                          float lam, float oml, int apply_tail, bool allow_ahead, void* stream_v, int in_mod = 0) {
+                          float lam, float oml, int apply_tail, bool allow_ahead, void* stream_v, int in_mod = 0,
+                          bool own_stream = true) {
     if (!p || (!d_in_all && batch > 0) || (!d_out && batch > 0)) return fail(FAA_ERR_VALUE, "null argument");
     if (batch < 0 || first < 0 || first + batch > n_all) return fail(FAA_ERR_VALUE, "bad batch range");
     if (batch > 65535) return fail(FAA_ERR_UNSUPPORTED, "at most 65535 images per call (one grid row per image): split the batch");
@@ -854,6 +879,8 @@ static int augment_common(faa_policy_t* p, const uint8_t* d_in_all, int n_all, i
     if (batch == 0) return FAA_OK;
     if (int e = bind_device(p)) return e;
     cudaStream_t stream = (cudaStream_t)stream_v;
+    // (own_stream false: a chunk of faa_augment_host on one of its side streams, which that call orders itself)
+    if (own_stream) { if (int e = follow_stream(p, stream)) return e; }
     const OpRec* d_ops = nullptr;
     // resolved samples can only reference ops the host sampler validated; Philox can pick anything
     if (int e = device_table(p, h, w, d_samples == nullptr, &d_ops)) return e;
@@ -1229,6 +1256,7 @@ int faa_augment_host(faa_policy_t* p, const uint8_t* h_in, void* h_out, void* d_
     // The policy owns the device input buffer and the pinned stages: the previous call's asynchronous copies must
     // have finished before any of them is rewritten (a pageable source is memcpy'd into the stage right below)
     if (p->host_in_flight) { CK(cudaEventSynchronize(p->ev_host_done)); p->host_in_flight = false; }
+    if (int e = follow_stream(p, stream)) return e;        // (the side streams fork from `stream` below)
     if (!p->ev_host_done) CK(cudaEventCreateWithFlags(&p->ev_host_done, cudaEventDisableTiming));
     const size_t in_img = (size_t)h * w * 3;
     const size_t out_img = (size_t)tail->out_h * tail->out_w * 3 * out_elem_size(tail->out_dtype);
@@ -1276,7 +1304,7 @@ int faa_augment_host(faa_policy_t* p, const uint8_t* h_in, void* h_out, void* d_
         cudaStream_t s = p->side[c & 1];
         CK(cudaMemcpyAsync((uint8_t*)p->d_in + in_img * b0, src + in_img * b0, in_img * (b1 - b0), cudaMemcpyHostToDevice, s));
         if (int e = augment_common(p, (const uint8_t*)p->d_in, batch, b0, (uint8_t*)d_out + out_img * b0, b1 - b0, h, w,
-                                   tail, nullptr, nullptr, rng, 0, nullptr, 1.0f, 0.0f, 1, false, s)) return e;
+                                   tail, nullptr, nullptr, rng, 0, nullptr, 1.0f, 0.0f, 1, false, s, 0, false)) return e;
         if (dst) CK(cudaMemcpyAsync((uint8_t*)dst + out_img * b0, (uint8_t*)d_out + out_img * b0, out_img * (b1 - b0), cudaMemcpyDeviceToHost, s));
     }
     for (int i = 0; i < 2; ++i) {

@@ -97,6 +97,72 @@ def emu_augment(emu, pol, batch_u8, samples, boxes, tail=None, norm=None, partne
     return out
 
 
+def emu_philox_records(emu, pol, n, h, w, tail, seed, first_index):
+    """Decision records of samples [first_index, first_index + n) from the emulator's Philox sampler (the kernels'
+    sampler compiled for the host): what a fused Philox launch draws for those indices, without a GPU."""
+    from fast_autoaugment_b200 import _lib
+    from fast_autoaugment_b200.engine import make_rng
+    oh, ow = tail.out_size if tail.out_size is not None else (h, w)
+    table = np.ascontiguousarray(pol.compiled_table(h, w))
+    probs = np.ascontiguousarray(pol.probs, dtype=np.float64)
+    rng = make_rng(seed, first_index, tail)
+    samples = np.zeros(n, dtype=_lib.SAMPLE_DTYPE)
+    boxes = np.zeros((n, pol.n_op), dtype=_lib.BOX_DTYPE)
+    rc = emu.faa_emu_philox(table.ctypes.data, probs.ctypes.data, pol.n_sub, pol.n_op, C.addressof(rng), n, h, w, oh, ow,
+                            samples.ctypes.data, boxes.ctypes.data)
+    assert rc == 0
+    return samples, boxes
+
+
+def reference_output(emu, pol, batch_u8, tail, samples, boxes, lighting_rgb=None, partner=None, lam=1.0, threads=16):
+    """Host reference of one launch on resolved records: emu_augment, then the exact ToTensor+Normalize table.  Returns a
+    CPU tensor laid out like the launch's output: uint8 [B, oh, ow, 3] for uint8 tails, else [B, 3, oh, ow] in
+    tail.out_dtype - fp16 / bf16 being the fp32 value rounded once.  Lighting (lighting_rgb [B, 3]): the uint8 result,
+    then ((u / 255 + rgb) - mean) / std in torch fp32.  Images are split over threads (the emulator releases the GIL)."""
+    import concurrent.futures
+    import torch
+    from fast_autoaugment_b200.engine import TailSpec
+    B = batch_u8.shape[0]
+    u8_out = tail.out_dtype == torch.uint8 or lighting_rgb is not None
+    if lighting_rgb is not None:
+        assert tail.cutout == 0, "CutoutDefault zeroes the normalised value: not modelled together with Lighting"
+        run_tail = TailSpec(tail.out_size, tail.crop_pad, tail.hflip, tail.mean, tail.std, 0, torch.uint8)
+    else:
+        run_tail = tail
+    norm = None if u8_out else exact_norm_table(tail.mean, tail.std)
+    if partner is not None:                     # fused Mixup: the partners index the whole batch
+        out = emu_augment(emu, pol, batch_u8, samples, boxes, run_tail, norm, partner=partner, lam=lam)
+    else:
+        step = max(1, -(-B // threads))
+        parts = [(lo, min(B, lo + step)) for lo in range(0, B, step)]
+        with concurrent.futures.ThreadPoolExecutor(len(parts)) as ex:
+            outs = list(ex.map(lambda r: emu_augment(emu, pol, np.ascontiguousarray(batch_u8[r[0]:r[1]]),
+                                                     samples[r[0]:r[1]], boxes[r[0]:r[1]], run_tail, norm), parts))
+        out = np.concatenate(outs)
+    out = torch.from_numpy(out)
+    if lighting_rgb is not None:
+        t = out.permute(0, 3, 1, 2).float().div(255)
+        t = t.add(torch.as_tensor(lighting_rgb, dtype=torch.float32).cpu().view(B, 3, 1, 1).expand_as(t))
+        m = torch.tensor(tail.mean, dtype=torch.float32).view(1, 3, 1, 1)
+        s = torch.tensor(tail.std, dtype=torch.float32).view(1, 3, 1, 1)
+        return ((t - m) / s).to(tail.out_dtype)
+    return out if u8_out else out.to(tail.out_dtype)
+
+
+def philox_reference(emu, pol, batch_u8, tail, seed, first_index, replicas=1, **kw):
+    """Host reference of a fused Philox launch (FusedAugmenter, augment_batch(rng=...), run_many steps): records from
+    emu_philox_records, pixels from reference_output.  replicas > 1: a TTA launch, replica r draws the samples
+    first_index + r * B + i and the result is stacked [replicas, B, ...]."""
+    B, H, W, _ = batch_u8.shape
+    outs = [reference_output(emu, pol, batch_u8, tail,
+                             *emu_philox_records(emu, pol, B, H, W, tail, seed, first_index + r * B), **kw)
+            for r in range(replicas)]
+    if replicas == 1:
+        return outs[0]
+    import torch
+    return torch.stack(outs)
+
+
 def set_emu_sigs(emu):
     vp = C.c_void_p
     emu.faa_emu_augment.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, vp,
