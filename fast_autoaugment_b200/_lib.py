@@ -25,6 +25,8 @@ SAMPLE_DTYPE = np.dtype([("sub", "<u2"), ("gate", "u1"), ("sign", "u1"), ("crop_
                          ("zero_box", "<i2", (4,))])
 BOX_DTYPE = np.dtype([("x0", "<i2"), ("y0", "<i2"), ("x1", "<i2"), ("y1", "<i2")])
 JITTER_DTYPE = np.dtype([("alpha", "<f4", (3,)), ("order", "u1", (4,))])          # faa_jitter_t
+CROP_BOX_DTYPE = np.dtype([("x0", "<i4"), ("y0", "<i4"), ("w", "<i4"), ("h", "<i4")])  # faa_crop_box_t
+CROP_RANDOM, CROP_CENTER = 0, 1
 assert SAMPLE_DTYPE.itemsize == 16 and BOX_DTYPE.itemsize == 8
 
 
@@ -37,6 +39,12 @@ class Tail(C.Structure):          # faa_tail_t
 class Rng(C.Structure):           # faa_rng_t
     _fields_ = [("seed", C.c_uint64), ("first_index", C.c_uint64), ("crop_pad", C.c_int32),
                 ("hflip", C.c_int32), ("zero_box_len", C.c_int32), ("reserved", C.c_int32)]
+
+
+class CropCfg(C.Structure):       # faa_crop_cfg_t
+    _fields_ = [("mode", C.c_int32), ("img_size", C.c_int32), ("min_covered", C.c_double),
+                ("aspect_lo", C.c_double), ("aspect_hi", C.c_double), ("area_lo", C.c_double),
+                ("area_hi", C.c_double), ("max_attempts", C.c_int32), ("reserved", C.c_int32), ("rng", Rng)]
 
 
 def _load():
@@ -80,6 +88,8 @@ def _load():
         "faa_mix_u8_peer": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, P(Tail), f32, f32, vp]),
         "faa_color_jitter": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp]),
         "faa_policy_set_lighting": (C.c_int, [vp, vp, C.c_int]),
+        "faa_center_crop_box": (C.c_int, [C.c_int, C.c_int, C.c_int, vp]),
+        "faa_crop_resize": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, P(Tail), vp, P(CropCfg), vp]),
         "faa_launch_count": (u64, []),
     }
     for name, (res, args) in sig.items():

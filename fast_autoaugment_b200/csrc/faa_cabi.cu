@@ -1121,6 +1121,69 @@ int faa_color_jitter(const uint8_t* d_in, uint8_t* d_out, int batch, int h, int 
     return FAA_OK;
 }
 
+static_assert(sizeof(faa_crop_box_t) == sizeof(CropBox), "crop box layout");
+static_assert(sizeof(faa_crop_cfg_t) == sizeof(CropCfg) && offsetof(faa_crop_cfg_t, rng) == offsetof(CropCfg, rng),
+              "crop config layout");
+
+int faa_center_crop_box(int h, int w, int img_size, faa_crop_box_t* out) {
+    if (!out) return fail(FAA_ERR_VALUE, "null argument");
+    if (int e = check_shape(h, w)) return e;
+    if (img_size <= 0) return fail(FAA_ERR_VALUE, "img_size must be positive");
+    CropBox b = center_crop_box(h, w, img_size);
+    memcpy(out, &b, sizeof b);
+    return FAA_OK;
+}
+
+static int check_crop_cfg(const faa_crop_cfg_t* c) {
+    if (c->mode != FAA_CROP_RANDOM && c->mode != FAA_CROP_CENTER) return fail(FAA_ERR_VALUE, "bad crop mode");
+    if (c->img_size <= 0) return fail(FAA_ERR_VALUE, "img_size must be positive");
+    if (c->mode == FAA_CROP_RANDOM) {                       // the reference's asserts (data.py:269-272)
+        if (!(c->min_covered > 0.0)) return fail(FAA_ERR_MAGNITUDE, "min_covered must be positive");
+        if (!(c->aspect_lo > 0.0 && c->aspect_lo <= c->aspect_hi)) return fail(FAA_ERR_MAGNITUDE, "bad aspect_ratio_range");
+        if (!(c->area_lo > 0.0 && c->area_lo <= c->area_hi)) return fail(FAA_ERR_MAGNITUDE, "bad area_range");
+        if (c->max_attempts < 1) return fail(FAA_ERR_MAGNITUDE, "max_attempts must be >= 1");
+    }
+    return FAA_OK;
+}
+
+int faa_crop_resize(const uint8_t* d_in, void* d_out, int batch, int h, int w, const faa_tail_t* tail,
+                    const faa_crop_box_t* d_boxes, const faa_crop_cfg_t* cfg, void* stream) {
+    if (!cfg || ((!d_in || !d_out) && batch > 0)) return fail(FAA_ERR_VALUE, "null argument");
+    if (batch < 0) return fail(FAA_ERR_VALUE, "negative batch");
+    if (batch > 65535) return fail(FAA_ERR_UNSUPPORTED, "batch must be <= 65535");
+    if (int e = check_shape(h, w)) return e;
+    if (int e = check_tail(tail)) return e;
+    if (int e = check_crop_cfg(cfg)) return e;
+    if (tail->out_dtype != FAA_U8_HWC)
+        for (int c = 0; c < 3; ++c)
+            if (!(tail->std[c] != 0.0f)) return fail(FAA_ERR_VALUE, "std must be non-zero");
+    if (!d_boxes) {
+        // the device sampler's boxes lie inside the image; the center box (center mode, and the random mode's
+        // fallback after failed attempts) can be empty when img_size is small against the short side
+        CropBox b = center_crop_box(h, w, cfg->img_size);
+        if (b.w <= 0 || b.h <= 0) return fail(FAA_ERR_VALUE, "the center crop of this image is empty");
+    }
+    if (int e = ensure_device()) return e;
+    if (batch == 0) return FAA_OK;
+    if (d_boxes) {
+        std::vector<CropBox> hb((size_t)batch);
+        CK(cudaMemcpyAsync(hb.data(), d_boxes, hb.size() * sizeof(CropBox), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+        CK(cudaStreamSynchronize((cudaStream_t)stream));
+        for (int i = 0; i < batch; ++i) {
+            const CropBox& b = hb[(size_t)i];
+            if (b.w <= 0 || b.h <= 0 || b.x0 < 0 || b.y0 < 0 || b.x0 > w - b.w || b.y0 > h - b.h)
+                return fail(FAA_ERR_VALUE, "crop box " + std::to_string(i) + " is empty or not inside the image");
+        }
+    }
+    const CropResizeTile t = plan_crop_resize(h, w, tail->out_h, tail->out_w);
+    if (t.smem == 0) return fail(FAA_ERR_UNSUPPORTED, "no crop-resize tile fits in shared memory");
+    CropCfg c; memcpy(&c, cfg, sizeof c);
+    CK(launch_crop_resize(d_in, d_out, batch, h, w, tail->out_h, tail->out_w, tail->out_dtype, tail->mean, tail->std,
+                          reinterpret_cast<const CropBox*>(d_boxes), c, t, (cudaStream_t)stream));
+    g_launches++;
+    return FAA_OK;
+}
+
 int faa_mix_u8(faa_policy_t* p, const uint8_t* d_a, const uint8_t* d_b, const int32_t* d_partner, const int16_t* d_zero_box_a,
                const int16_t* d_zero_box_b, void* d_out, int batch, int h, int w, const faa_tail_t* tail, float lam,
                float one_minus_lam, void* stream) {

@@ -599,4 +599,158 @@ FAA_HD uint32_t prog_cost(const Prog& g) {
     return cost;
 }
 
+// ------------------------------------------------------- crop + bicubic resize --
+// EfficientNetRandomCrop / EfficientNetCenterCrop (data.py:267-345) followed by
+// transforms.Resize((s, s), BICUBIC) (data.py:61-62, 76-77), i.e. Pillow's ImagingResample
+// for 8-bit RGB: per axis an fp64 coefficient table, converted to 22-bit fixed point; a
+// horizontal pass into a uint8 intermediate, then a vertical pass.  A pass whose axis keeps
+// its size is the identity (Pillow skips it; the bicubic weights would be exactly 1, 0, 0 ...).
+struct CropBox { int32_t x0, y0, w, h; };                 // == faa_crop_box_t
+
+constexpr int kResPrecisionBits = 22;
+
+FAA_HD double d_div(double a, double b) {
+#if defined(__CUDA_ARCH__)
+    return __ddiv_rn(a, b);
+#else
+    volatile double r = a / b; return r;
+#endif
+}
+FAA_HD double d_sqrt(double a) {
+#if defined(__CUDA_ARCH__)
+    return __dsqrt_rn(a);
+#else
+    volatile double r = __builtin_sqrt(a); return r;
+#endif
+}
+FAA_HD double d_rint(double a) {                           // Python round() of a float: half to even
+#if defined(__CUDA_ARCH__)
+    return rint(a);
+#else
+    return __builtin_rint(a);
+#endif
+}
+
+// Pillow bicubic_filter, a = -0.5 (support 2)
+FAA_HD double bicubic_w(double x) {
+    if (x < 0.0) x = -x;
+    if (x < 1.0) return d_add(d_mul(d_mul(d_add(d_mul(1.5, x), -2.5), x), x), 1.0);
+    if (x < 2.0) return d_mul(d_add(d_mul(d_add(d_mul(d_add(x, -5.0), x), 8.0), x), -4.0), -0.5);
+    return 0.0;
+}
+
+// Taps of one axis: ksize of precompute_coeffs (an upper bound on the taps of any output index).
+FAA_HD int resize_ksize(int in, int out) {
+    const double scale = d_div((double)in, (double)out);
+    const double fs = scale > 1.0 ? scale : 1.0;
+    const double support = d_mul(2.0, fs);
+    const double c = (double)(int)support;
+    return 2 * (int)(c < support ? c + 1.0 : c) + 1;
+}
+
+// precompute_coeffs + normalize_coeffs_8bpc for output index xx: first input index and tap count, then the
+// int32 weights k[0..n).  Identity axes (in == out) give one tap of weight 1 << 22.
+FAA_HD int resize_coeffs(int in, int out, int xx, int* xmin_out, int32_t* k) {
+    if (in == out) { *xmin_out = xx; k[0] = 1 << kResPrecisionBits; return 1; }
+    const double scale = d_div((double)in, (double)out);
+    const double fs = scale > 1.0 ? scale : 1.0;
+    const double support = d_mul(2.0, fs);
+    const double ss = d_div(1.0, fs);
+    const double center = d_mul(d_add((double)xx, 0.5), scale);
+    int xmin = (int)d_add(d_add(center, -support), 0.5);
+    if (xmin < 0) xmin = 0;
+    int xmax = (int)d_add(d_add(center, support), 0.5);
+    if (xmax > in) xmax = in;
+    const int n = xmax - xmin;
+    double ww = 0.0;
+    for (int x = 0; x < n; ++x) ww = d_add(ww, bicubic_w(d_mul(d_add(d_add((double)(x + xmin), -center), 0.5), ss)));
+    for (int x = 0; x < n; ++x) {
+        double w = bicubic_w(d_mul(d_add(d_add((double)(x + xmin), -center), 0.5), ss));
+        if (ww != 0.0) w = d_div(w, ww);
+        const double f = d_mul(w, (double)(1 << kResPrecisionBits));
+        k[x] = (int32_t)(w < 0.0 ? d_add(f, -0.5) : d_add(f, 0.5));
+    }
+    *xmin_out = xmin;
+    return n;
+}
+
+// (1 << 21) + sum, shifted and clipped to a byte (Pillow clip8)
+FAA_HD uint32_t resize_clip8(int32_t ss) {
+    if (ss <= 0) return 0u;
+    if (ss >= (1 << (kResPrecisionBits + 8))) return 255u;
+    return (uint32_t)(ss >> kResPrecisionBits);
+}
+
+// EfficientNetCenterCrop (data.py:337-345) through Image.crop's int(round()) of the box
+FAA_HD CropBox center_crop_box(int H, int W, int img_size) {
+    const int short_side = W < H ? W : H;
+    const double c = d_mul(d_div((double)img_size, (double)(img_size + 32)), (double)short_side);
+    const double top = d_rint(d_div(d_add((double)H, -c), 2.0));
+    const double left = d_rint(d_div(d_add((double)W, -c), 2.0));
+    CropBox b;
+    b.x0 = (int32_t)left; b.y0 = (int32_t)top;
+    b.w = (int32_t)d_rint(d_add(left, c)) - b.x0;
+    b.h = (int32_t)d_rint(d_add(top, c)) - b.y0;
+    return b;
+}
+
+struct CropCfg {                                           // == faa_crop_cfg_t
+    int32_t mode;                                          // 0 random, 1 center
+    int32_t img_size;
+    double min_covered, aspect_lo, aspect_hi, area_lo, area_hi;
+    int32_t max_attempts, reserved;
+    RngCfg rng;
+};
+
+// One attempt of EfficientNetRandomCrop.__call__ (data.py:280-317) from its two uniforms (u_ar: the aspect
+// ratio's random(), u_h: the height's).  Returns 0 = rejected, 1 = box size accepted (w, h set; the caller then
+// draws x, y), 2 = the crop is the whole image (center-crop fallback).
+FAA_HD int crop_attempt(const CropCfg& c, int W, int H, double u_ar, double u_h, int& w_out, int& h_out) {
+    const double area = (double)((long long)W * H);
+    const double min_area = d_mul(c.area_lo, area), max_area = d_mul(c.area_hi, area);
+    const double ar = d_add(c.aspect_lo, d_mul(d_add(c.aspect_hi, -c.aspect_lo), u_ar));     // random.uniform
+    int height = (int)d_rint(d_sqrt(d_div(min_area, ar)));
+    int max_height = (int)d_rint(d_sqrt(d_div(max_area, ar)));
+    if (d_mul((double)max_height, ar) > (double)W) {
+        max_height = (int)d_div(d_add(d_add((double)W, 0.5), -1e-7), ar);
+        if (d_mul((double)max_height, ar) > (double)W) max_height -= 1;
+    }
+    if (max_height > H) max_height = H;
+    if (height >= max_height) height = max_height;
+    height = (int)d_rint(d_add((double)height, d_mul((double)(max_height - height), u_h)));
+    const int width = (int)d_rint(d_mul((double)height, ar));
+    const double a = (double)((long long)width * height);
+    if (a < min_area || a > max_area) return 0;
+    if (width > W || height > H) return 0;
+    if (a < d_mul(c.min_covered, area)) return 0;
+    if (width == W && height == H) return 2;
+    w_out = width; h_out = height;
+    return 1;
+}
+
+// Device-side crop sampler: same distributions as EfficientNetRandomCrop, drawn from Philox keyed like
+// philox_sample (seed, global sample index) in a counter subspace philox_sample never uses: w = 1, z = attempt
+// number for the two uniforms of an attempt, z = 0xFFFFFFFF for the offsets x, y.
+FAA_HD CropBox philox_crop_box(const CropCfg& c, uint64_t index, int H, int W) {
+    if (c.mode != 0) return center_crop_box(H, W, c.img_size);
+    const uint32_t k0 = (uint32_t)c.rng.seed, k1 = (uint32_t)(c.rng.seed >> 32);
+    U4 ctr; ctr.x = (uint32_t)index; ctr.y = (uint32_t)(index >> 32); ctr.w = 1u;
+    for (int t = 0; t < c.max_attempts; ++t) {
+        ctr.z = (uint32_t)t;
+        const U4 b = philox4x32_10(ctr, k0, k1);
+        int w = 0, h = 0;
+        const int r = crop_attempt(c, W, H, (double)b.x * (1.0 / 4294967296.0), (double)b.y * (1.0 / 4294967296.0), w, h);
+        if (r == 0) continue;
+        if (r == 2) break;
+        ctr.z = 0xFFFFFFFFu;
+        const U4 o = philox4x32_10(ctr, k0, k1);
+        CropBox bx;
+        bx.x0 = (int32_t)umulhi32(o.x, (uint32_t)(W - w + 1));      // random.randint(0, W - w)
+        bx.y0 = (int32_t)umulhi32(o.y, (uint32_t)(H - h + 1));
+        bx.w = w; bx.h = h;
+        return bx;
+    }
+    return center_crop_box(H, W, c.img_size);
+}
+
 }  // namespace faa

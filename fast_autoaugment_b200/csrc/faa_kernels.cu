@@ -31,6 +31,7 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
+#include <cassert>
 #include <cstdlib>
 #include <type_traits>
 #include <cstring>
@@ -1979,6 +1980,184 @@ cudaError_t launch_lighting_tables(const float* rgb, float* tabs, int n, const f
     if (n <= 0) return cudaSuccess;
     faa_lighting_tables_kernel<<<(unsigned)((n * 768 + 255) / 256), 256, 0, stream>>>(rgb, tabs, n, mean[0], mean[1], mean[2], std[0], std[1], std[2]);
     return cudaGetLastError();
+}
+
+// ---------------------------------------------------------------------------------------
+// EfficientNet crop + Pillow bicubic Resize (data.py:61-62, 76-77, 267-345; faa_core.cuh crop_attempt /
+// resize_coeffs).  One CTA per (tile_w x tile_h) output tile of one image, no whole-image state: thread 0 fixes the
+// crop box (given, or drawn with philox_crop_box), the CTA builds the horizontal coefficients of its tile's columns
+// and the vertical ones of its rows in shared memory, runs the horizontal pass over exactly the crop rows its rows
+// read into a uint8 intermediate (one packed RGB word per pixel), then the vertical pass from there, and writes
+// uint8 HWC or ToTensor + Normalize (exact fp32 table, then one rounding to fp16 / bf16) NCHW.
+struct CropResizeParams {
+    const uint8_t* in;           // [B][H][W][3]
+    void* out;                   // [B][out_h][out_w][3] uint8 or [B][3][out_h][out_w]
+    const CropBox* boxes;        // [B] or nullptr: draw with cfg
+    CropCfg cfg;
+    int32_t H, W, out_h, out_w;
+    int32_t tile_w, tile_h, tw_shift;   // tile_w = 1 << tw_shift
+    int32_t kx_cap, ky_cap, rows_cap;   // taps per column / row and intermediate rows a CTA can hold
+    float mean[3], std[3];
+};
+
+// (not inlined: the fp64 division / sqrt slow paths inside would otherwise make the kernel spill)
+__device__ __noinline__ CropBox draw_crop_box(const CropCfg* c, uint64_t index, int H, int W) {
+    return philox_crop_box(*c, index, H, W);
+}
+
+template <int OUT>
+__global__ void __launch_bounds__(256, 4) faa_crop_resize_kernel(const __grid_constant__ CropResizeParams P) {
+    extern __shared__ int32_t cr_smem[];
+    __shared__ float s_norm[OUT == OUT_U8_HWC ? 1 : 768];
+    __shared__ CropBox s_box;
+    const int img = blockIdx.z, tid = threadIdx.x;
+    const int ox0 = blockIdx.x * P.tile_w, oy0 = blockIdx.y * P.tile_h;
+    const int ncols = min(P.tile_w, P.out_w - ox0), nrows = min(P.tile_h, P.out_h - oy0);
+    int32_t* hk = cr_smem;                                   // [tile_w][kx_cap]
+    int32_t* hmin = hk + P.tile_w * P.kx_cap;                // [tile_w]
+    int32_t* hn = hmin + P.tile_w;
+    int32_t* vk = hn + P.tile_w;                             // [tile_h][ky_cap]
+    int32_t* vmin = vk + P.tile_h * P.ky_cap;
+    int32_t* vn = vmin + P.tile_h;
+    uint32_t* inter = reinterpret_cast<uint32_t*>(vn + P.tile_h);   // [rows_cap][tile_w]
+    if (tid == 0) s_box = P.boxes ? P.boxes[img] : draw_crop_box(&P.cfg, P.cfg.rng.first_index + (uint64_t)img, P.H, P.W);
+    if (OUT != OUT_U8_HWC) {                                 // data.py:76-78: x = u8 / 255 ; (x - mean) / std in fp32
+        for (int i = tid; i < 768; i += blockDim.x) {
+            const int ch = i >> 8;
+            s_norm[i] = __fdiv_rn(__fadd_rn(__fdiv_rn((float)(i & 255), 255.0f), -P.mean[ch]), P.std[ch]);
+        }
+    }
+    __syncthreads();
+    const CropBox b = s_box;
+    if (tid < ncols) {
+        int xm;
+        hn[tid] = resize_coeffs(b.w, P.out_w, ox0 + tid, &xm, hk + tid * P.kx_cap);
+        hmin[tid] = xm;
+    } else if (tid >= 128 && tid - 128 < nrows) {
+        const int r = tid - 128;
+        int ym;
+        vn[r] = resize_coeffs(b.h, P.out_h, oy0 + r, &ym, vk + r * P.ky_cap);
+        vmin[r] = ym;
+    }
+    __syncthreads();
+    const int r0 = vmin[0];
+    // crop rows this tile reads: at most (tile_h - 1) * scale_y + taps + 1 <= rows_cap (plan_crop_resize bounds them
+    // for every crop of the source, with one row to spare)
+    const int rows = vmin[nrows - 1] + vn[nrows - 1] - r0;
+    assert(rows <= P.rows_cap);
+    // horizontal pass: crop rows [r0, r0 + rows) x this tile's columns -> inter
+    const size_t img_base = (size_t)img * P.H * P.W * 3u;
+    const int tmask = P.tile_w - 1;
+    for (int i = tid; i < (rows << P.tw_shift); i += blockDim.x) {
+        const int r = i >> P.tw_shift, c = i & tmask;
+        if (c >= ncols) continue;
+        const uint8_t* src = P.in + img_base + ((size_t)(b.y0 + r0 + r) * P.W + (size_t)(b.x0 + hmin[c])) * 3u;
+        const int32_t* k = hk + c * P.kx_cap;
+        const int n = hn[c];
+        int32_t s0 = 1 << (kResPrecisionBits - 1), s1 = s0, s2 = s0;
+        for (int t = 0; t < n; ++t) {
+            const int32_t w = k[t];
+            s0 += (int32_t)__ldg(src + 3 * t) * w;
+            s1 += (int32_t)__ldg(src + 3 * t + 1) * w;
+            s2 += (int32_t)__ldg(src + 3 * t + 2) * w;
+        }
+        inter[(r << P.tw_shift) + c] = resize_clip8(s0) | (resize_clip8(s1) << 8) | (resize_clip8(s2) << 16);
+    }
+    __syncthreads();
+    // vertical pass: inter -> output
+    for (int i = tid; i < (nrows << P.tw_shift); i += blockDim.x) {
+        const int r = i >> P.tw_shift, c = i & tmask;
+        if (c >= ncols) continue;
+        const uint32_t* col = inter + ((vmin[r] - r0) << P.tw_shift) + c;
+        const int32_t* k = vk + r * P.ky_cap;
+        const int n = vn[r];
+        int32_t s0 = 1 << (kResPrecisionBits - 1), s1 = s0, s2 = s0;
+        for (int t = 0; t < n; ++t) {
+            const int32_t w = k[t];
+            const uint32_t p = col[t << P.tw_shift];
+            s0 += (int32_t)(p & 255u) * w;
+            s1 += (int32_t)((p >> 8) & 255u) * w;
+            s2 += (int32_t)((p >> 16) & 255u) * w;
+        }
+        const uint32_t v0 = resize_clip8(s0), v1 = resize_clip8(s1), v2 = resize_clip8(s2);
+        const int oy = oy0 + r, ox = ox0 + c;
+        if constexpr (OUT == OUT_U8_HWC) {
+            uint8_t* o = reinterpret_cast<uint8_t*>(P.out) + (((size_t)img * P.out_h + oy) * P.out_w + ox) * 3u;
+            o[0] = (uint8_t)v0; o[1] = (uint8_t)v1; o[2] = (uint8_t)v2;
+        } else {
+            const size_t plane = (size_t)P.out_h * P.out_w;
+            const size_t off = (size_t)img * 3u * plane + (size_t)oy * P.out_w + ox;
+            const float f0 = s_norm[v0], f1 = s_norm[256 + v1], f2 = s_norm[512 + v2];
+            if constexpr (OUT == OUT_F32) {
+                float* o = reinterpret_cast<float*>(P.out) + off;
+                o[0] = f0; o[plane] = f1; o[2 * plane] = f2;
+            } else if constexpr (OUT == OUT_F16) {
+                __half* o = reinterpret_cast<__half*>(P.out) + off;
+                o[0] = __float2half_rn(f0); o[plane] = __float2half_rn(f1); o[2 * plane] = __float2half_rn(f2);
+            } else {
+                __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(P.out) + off;
+                o[0] = __float2bfloat16_rn(f0); o[plane] = __float2bfloat16_rn(f1); o[2 * plane] = __float2bfloat16_rn(f2);
+            }
+        }
+    }
+}
+
+// Tile of a crop-resize launch: the largest tile whose coefficients and intermediate fit, for ANY crop of the
+// h x w source (a crop's scale, taps and rows are bounded by the full image's).  Prefers <= 48 KB (several CTAs
+// per SM); the 1 x 1 tile of an 8192 x 8192 source needs ~96 KB, so every valid size has a tile.
+CropResizeTile plan_crop_resize(int H, int W, int out_h, int out_w) {
+    const int kx = min(W, resize_ksize(W, out_w)), ky = min(H, resize_ksize(H, out_h));
+    const double sy = (double)H / out_h > 1.0 ? (double)H / out_h : 1.0;
+    int tw0 = 1, shift0 = 0;
+    while (tw0 < 32 && tw0 < out_w) { tw0 *= 2; ++shift0; }
+    CropResizeTile best; best.smem = 0;
+    for (int pass = 0; pass < 2 && best.smem == 0; ++pass) {
+        const size_t limit = pass == 0 ? 48u * 1024u : 220u * 1024u;
+        for (int tw = tw0, sh = shift0; tw >= 1 && best.smem == 0; tw /= 2, --sh)
+            for (int th = 32; th >= 1; th /= 2) {
+                if (th > 1 && th / 2 >= out_h) continue;
+                const int rows = min(H, (int)ceil((th - 1) * sy) + ky + 2);
+                const size_t smem = 4u * ((size_t)tw * (kx + 2) + (size_t)th * (ky + 2) + (size_t)rows * tw);
+                if (smem <= limit) {
+                    best.tile_w = tw; best.tile_h = th; best.tw_shift = sh; best.kx_cap = kx; best.ky_cap = ky;
+                    best.rows_cap = rows; best.smem = smem;
+                    break;
+                }
+            }
+    }
+    return best;
+}
+
+template <auto Kernel> static cudaError_t reserve_dyn_smem(size_t dyn);     // (defined below)
+
+// The dynamic shared memory limit is always raised to the plan's size: the kernel's static shared memory (the
+// normalisation table) counts against the default 48 KB too, so a plan just under 48 KB of dynamic memory would not
+// launch without it.
+template <int OUT>
+static cudaError_t launch_crop_resize_as(const CropResizeParams& P, dim3 grid, size_t smem, cudaStream_t stream) {
+    if (cudaError_t e = reserve_dyn_smem<faa_crop_resize_kernel<OUT>>(smem)) return e;
+    faa_crop_resize_kernel<OUT><<<grid, 256, smem, stream>>>(P);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_crop_resize(const uint8_t* in, void* out, int batch, int H, int W, int out_h, int out_w, int out_type,
+                               const float mean[3], const float std[3], const CropBox* boxes, const CropCfg& cfg,
+                               const CropResizeTile& t, cudaStream_t stream) {
+    if (batch <= 0) return cudaSuccess;
+    CropResizeParams P;
+    P.in = in; P.out = out; P.boxes = boxes; P.cfg = cfg;
+    P.H = H; P.W = W; P.out_h = out_h; P.out_w = out_w;
+    P.tile_w = t.tile_w; P.tile_h = t.tile_h; P.tw_shift = t.tw_shift;
+    P.kx_cap = t.kx_cap; P.ky_cap = t.ky_cap; P.rows_cap = t.rows_cap;
+    for (int c = 0; c < 3; ++c) { P.mean[c] = mean[c]; P.std[c] = std[c]; }
+    const dim3 grid((unsigned)((out_w + t.tile_w - 1) / t.tile_w), (unsigned)((out_h + t.tile_h - 1) / t.tile_h), (unsigned)batch);
+    switch (out_type) {
+    case OUT_F16:    return launch_crop_resize_as<OUT_F16>(P, grid, t.smem, stream);
+    case OUT_BF16:   return launch_crop_resize_as<OUT_BF16>(P, grid, t.smem, stream);
+    case OUT_F32:    return launch_crop_resize_as<OUT_F32>(P, grid, t.smem, stream);
+    case OUT_U8_HWC: return launch_crop_resize_as<OUT_U8_HWC>(P, grid, t.smem, stream);
+    default: return cudaErrorInvalidValue;
+    }
 }
 
 // ---------------------------------------------------------------------------------------

@@ -105,6 +105,12 @@ cudaError_t launch_mix_u8(const uint8_t* a, const uint8_t* b, const int32_t* par
                           cudaStream_t stream, const uint8_t* const* b_ptrs = nullptr);
 
 cudaError_t launch_color_jitter(const uint8_t* in, uint8_t* out, const void* recs, int batch, int H, int W, cudaStream_t stream);
+// EfficientNet crop + bicubic resize (faa_crop_resize_kernel): output tile and shared-memory plan
+struct CropResizeTile { int32_t tile_w, tile_h, tw_shift, kx_cap, ky_cap, rows_cap; size_t smem; };
+CropResizeTile plan_crop_resize(int H, int W, int out_h, int out_w);     // smem == 0: nothing fits
+cudaError_t launch_crop_resize(const uint8_t* in, void* out, int batch, int H, int W, int out_h, int out_w, int out_type,
+                               const float mean[3], const float std[3], const CropBox* boxes, const CropCfg& cfg,
+                               const CropResizeTile& t, cudaStream_t stream);
 cudaError_t launch_lighting_tables(const float* rgb, float* tabs, int n, const float mean[3], const float std[3], cudaStream_t stream);
 
 int pick_bands(int H, int W, int out_h, int out_w);

@@ -13,6 +13,7 @@ from __future__ import annotations
 
 import math
 import os
+import random
 
 import numpy as np
 import PIL.Image
@@ -22,7 +23,7 @@ from torch.utils.data import Sampler, SubsetRandomSampler
 from . import _lib, archive
 from .conf import Config as C
 from .engine import (CIFAR_MEAN, CIFAR_STD, IMAGENET_MEAN, IMAGENET_STD, CompiledPolicy, TailSpec,
-                     augment_batch, make_rng)
+                     augment_batch, center_crop_box, crop_cfg, crop_resize, make_rng)
 
 
 class Augmentation(object):
@@ -154,6 +155,214 @@ class ColorJitter(object):
         return out
 
 
+class EfficientNetCenterCrop(object):
+    """Drop-in for reference ``EfficientNetCenterCrop`` (data.py:323-345): the square of side
+    ``imgsize / (imgsize + 32) * short side`` in the middle of the image.  Batched: ``cfg()`` for ``crop_resize``."""
+
+    def __init__(self, imgsize):
+        self.imgsize = imgsize
+
+    def box(self, h, w):
+        """(x0, y0, w, h) after Image.crop's rounding of the box"""
+        return center_crop_box(h, w, self.imgsize)
+
+    def __call__(self, img):
+        x0, y0, w, h = self.box(img.size[1], img.size[0])
+        return img.crop((x0, y0, x0 + w, y0 + h))
+
+    def sample_parity(self, n, h, w):
+        """[n] boxes (``_lib.CROP_BOX_DTYPE``); draws nothing"""
+        b = np.zeros(n, dtype=_lib.CROP_BOX_DTYPE)
+        b["x0"], b["y0"], b["w"], b["h"] = self.box(h, w)
+        return b
+
+    def cfg(self, seed=0, first_index=0):
+        return crop_cfg(self.imgsize, center=True, seed=seed, first_index=first_index)
+
+
+class EfficientNetRandomCrop(object):
+    """Drop-in for reference ``EfficientNetRandomCrop`` (data.py:267-320): up to ``max_attempts`` draws of an aspect
+    ratio and a height from Python's ``random``, then ``random.randint`` for x and y; the whole image or ten failed
+    attempts fall back to the center crop.  ``__call__`` and ``sample_parity`` consume ``random`` exactly like the
+    reference; ``cfg(seed, first_index)`` lets the kernel draw the boxes instead (Philox: same distributions, not the
+    reference's stream)."""
+
+    def __init__(self, imgsize, min_covered=0.1, aspect_ratio_range=(3. / 4, 4. / 3), area_range=(0.08, 1.0),
+                 max_attempts=10):
+        assert 0.0 < min_covered
+        assert 0 < aspect_ratio_range[0] <= aspect_ratio_range[1]
+        assert 0 < area_range[0] <= area_range[1]
+        assert 1 <= max_attempts
+        self.imgsize = imgsize
+        self.min_covered = min_covered
+        self.aspect_ratio_range = aspect_ratio_range
+        self.area_range = area_range
+        self.max_attempts = max_attempts
+        self._fallback = EfficientNetCenterCrop(imgsize)
+
+    def box(self, h, w):
+        """one draw: (x0, y0, w, h) of the crop of an h x w image"""
+        W, H = w, h
+        min_area = self.area_range[0] * (W * H)
+        max_area = self.area_range[1] * (W * H)
+        for _ in range(self.max_attempts):
+            aspect_ratio = random.uniform(*self.aspect_ratio_range)
+            height = int(round(math.sqrt(min_area / aspect_ratio)))
+            max_height = int(round(math.sqrt(max_area / aspect_ratio)))
+            if max_height * aspect_ratio > W:
+                max_height = int((W + 0.5 - 1e-7) / aspect_ratio)
+                if max_height * aspect_ratio > W:
+                    max_height -= 1
+            if max_height > H:
+                max_height = H
+            if height >= max_height:
+                height = max_height
+            height = int(round(random.uniform(height, max_height)))
+            width = int(round(height * aspect_ratio))
+            area = width * height
+            if area < min_area or area > max_area:
+                continue
+            if width > W or height > H:
+                continue
+            if area < self.min_covered * (W * H):
+                continue
+            if width == W and height == H:
+                return self._fallback.box(h, w)
+            x = random.randint(0, W - width)
+            y = random.randint(0, H - height)
+            return x, y, width, height
+        return self._fallback.box(h, w)
+
+    def __call__(self, img):
+        x0, y0, w, h = self.box(img.size[1], img.size[0])
+        return img.crop((x0, y0, x0 + w, y0 + h))
+
+    def sample_parity(self, n, h, w):
+        """[n] boxes (``_lib.CROP_BOX_DTYPE``) drawn one image after another from ``random``"""
+        b = np.zeros(n, dtype=_lib.CROP_BOX_DTYPE)
+        for i in range(n):
+            b[i] = self.box(h, w)
+        return b
+
+    def cfg(self, seed=0, first_index=0):
+        return crop_cfg(self.imgsize, False, self.min_covered, self.aspect_ratio_range, self.area_range,
+                        self.max_attempts, seed, first_index)
+
+
+# EfficientNet input resolutions, reference networks/efficientnet_pytorch/utils.py:174-181 (the `res` coefficient)
+EFFICIENTNET_SIZES = {"efficientnet-b0": 224, "efficientnet-b1": 240, "efficientnet-b2": 260, "efficientnet-b3": 300,
+                      "efficientnet-b4": 380, "efficientnet-b5": 456, "efficientnet-b6": 528, "efficientnet-b7": 600}
+
+
+def imagenet_input_size(model_type):
+    """data.py:50-55: 224, or the EfficientNet resolution when the model is an EfficientNet"""
+    model_type = str(model_type or "")
+    if "efficientnet" in model_type:
+        return EFFICIENTNET_SIZES[model_type]
+    return 224
+
+
+class ImageNetChain(object):
+    """The reference's ImageNet transforms (data.py:60-80) on uint8 [B,H,W,3] CUDA batches of full-size images.
+
+    ``train``: ``Augmentation(policy)`` at source size (uint8) -> ``EfficientNetRandomCrop`` + ``Resize(BICUBIC)``
+    (``faa_crop_resize``, uint8) -> ``ColorJitter(0.4, 0.4, 0.4)`` in place -> one launch of the identity policy with
+    ``RandomHorizontalFlip`` + ``ToTensor`` + ``Lighting(0.1)`` + ``Normalize``.  The flip runs after the jitter here:
+    the jitter is per-pixel with a whole-image mean, so the order does not change a value.
+    ``test``: ``EfficientNetCenterCrop`` + ``Resize`` + ``ToTensor`` + ``Normalize`` in one launch.
+
+    ``parity=True`` draws like the reference's per-image loop (a ``num_workers=0`` DataLoader), image after image:
+    policy (``random``, ``numpy``), crop (``random``), flip (``torch.rand``), jitter (``randperm(4)`` + three
+    uniforms), Lighting (three normals).  Otherwise the policy, crop and flip are drawn by the kernels (Philox keyed by
+    (seed, first_index + i)) and the jitter / Lighting records by vectorised torch calls on the device."""
+
+    _EIGVAL = _IMAGENET_PCA["eigval"]
+    _EIGVEC = _IMAGENET_PCA["eigvec"]
+
+    def __init__(self, policies, input_size=224, out_dtype=torch.float32):
+        self.input_size = int(input_size)
+        self.crop = EfficientNetRandomCrop(self.input_size)
+        self.center = EfficientNetCenterCrop(self.input_size)
+        self.jitter = ColorJitter(0.4, 0.4, 0.4)
+        self.lighting = Lighting(0.1)
+        self.aug = Augmentation(policies) if policies is not None else None
+        self.flip_policy = CompiledPolicy([[("Invert", -1.0, 0.0)]])       # a slot that never fires and draws nothing
+        self.tail = TailSpec(None, 0, True, IMAGENET_MEAN, IMAGENET_STD, 0, out_dtype)
+        self.test_tail = TailSpec(None, 0, False, IMAGENET_MEAN, IMAGENET_STD, 0, out_dtype)
+
+    def sample_parity(self, n, h, w):
+        """per-image records in the reference's draw order: (policy samples, policy boxes or None, crop boxes,
+        flip samples of the identity policy, jitter records, Lighting offsets [n, 3])"""
+        pol = self.aug.compiled if self.aug is not None else None
+        samples, boxes = [], []
+        crops = np.zeros(n, dtype=_lib.CROP_BOX_DTYPE)
+        flips = np.zeros(n, dtype=_lib.SAMPLE_DTYPE)
+        jit = np.zeros(n, dtype=_lib.JITTER_DTYPE)
+        rgb = torch.zeros(n, 3)
+        for i in range(n):
+            if pol is not None:
+                s, b = pol.sample_parity(1, h, w, TailSpec.raw_u8())
+                samples.append(s)
+                boxes.append(b)
+            crops[i] = self.crop.box(h, w)
+            flips[i]["flip"] = 1 if bool(torch.rand(1) < 0.5) else 0
+            jit[i] = self.jitter.sample_parity(1)[0]
+            if self.lighting.alphastd != 0:
+                rgb[i] = self.lighting._rgb(torch.empty(0))
+        if pol is None:
+            return None, None, crops, flips, jit, rgb
+        return np.concatenate(samples), np.concatenate(boxes), crops, flips, jit, rgb
+
+    def _device_records(self, n, dev, seed, first_index):
+        g = torch.Generator(device=dev)
+        g.manual_seed((int(seed) * 1000003 + int(first_index)) & 0x7FFFFFFFFFFFFFFF)
+        order = torch.argsort(torch.rand(n, 4, device=dev, generator=g), dim=1).to(torch.int32)   # randperm(4) per image
+        alpha = torch.empty(n, 3, device=dev)
+        for j, r in enumerate(self.jitter.ranges):
+            if r is None:
+                alpha[:, j] = 1.0
+            else:
+                alpha[:, j].uniform_(r[0], r[1], generator=g)
+        present = torch.tensor([r is not None for r in self.jitter.ranges] + [False], device=dev)
+        order = torch.where(present[order.long()], order, torch.full_like(order, 3))
+        packed = order[:, 0] | (order[:, 1] << 8) | (order[:, 2] << 16) | (order[:, 3] << 24)
+        recs = torch.cat([alpha.view(torch.int32), packed[:, None]], dim=1).contiguous()
+        a = torch.randn(n, 3, device=dev, generator=g) * float(self.lighting.alphastd)
+        eigvec = torch.tensor(self._EIGVEC, device=dev)
+        eigval = torch.tensor(self._EIGVAL, device=dev)
+        rgb = (eigvec[None] * a[:, None, :] * eigval[None, None, :]).sum(2)
+        return recs, rgb
+
+    def train(self, batch_u8, parity=False, seed=0, first_index=0, records=None):
+        """uint8 [B,H,W,3] CUDA -> [B, 3, s, s] ``out_dtype``.  ``records``: the tuple of ``sample_parity`` (drawn
+        here when ``parity`` and not given)."""
+        b, h, w, _ = batch_u8.shape
+        dev = batch_u8.device
+        if parity and records is None:
+            records = self.sample_parity(b, h, w)
+        if records is not None:
+            samples, boxes, crops, flips, jit, rgb = records
+            x = batch_u8 if self.aug is None else augment_batch(self.aug.compiled, batch_u8, TailSpec.raw_u8(), samples, boxes)
+            y = crop_resize(x, self.input_size, boxes=crops)
+            self.jitter.jitter_batch(y, jit, out=y)
+            zb = np.zeros((b, 1), dtype=_lib.BOX_DTYPE)
+            return augment_batch(self.flip_policy, y, self.tail, flips, zb, lighting_rgb=rgb)
+        raw = TailSpec.raw_u8()
+        x = batch_u8 if self.aug is None else augment_batch(self.aug.compiled, batch_u8, raw,
+                                                            rng=make_rng(seed, first_index, raw))
+        y = crop_resize(x, self.input_size, rng=self.crop.cfg(seed, first_index))
+        recs, rgb = self._device_records(b, dev, seed, first_index)
+        with torch.cuda.device(dev):
+            import ctypes as C
+            _lib.check(_lib.lib.faa_color_jitter(y.data_ptr(), y.data_ptr(), b, self.input_size, self.input_size,
+                                                 recs.data_ptr(), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+        return augment_batch(self.flip_policy, y, self.tail, rng=make_rng(seed, first_index, self.tail), lighting_rgb=rgb)
+
+    def test(self, batch_u8, out=None):
+        """uint8 [B,H,W,3] CUDA -> [B, 3, s, s]: center crop + resize + ToTensor + Normalize, one launch"""
+        return crop_resize(batch_u8, self.input_size, rng=self.center.cfg(), tail=self.test_tail, out=out)
+
+
 def policy_by_conf_name(aug):
     """conf['aug'] -> policy list, with the reference's error behaviour (data.py:85-109)."""
     if isinstance(aug, list):
@@ -217,13 +426,16 @@ class GpuAugmentedLoader:
     """
 
     def __init__(self, dataset: DeviceDataset, batch, policies, tail: TailSpec, sampler=None, shuffle=False,
-                 drop_last=False, seed=None, parity=False):
+                 drop_last=False, seed=None, parity=False, chain=None, chain_mode="train"):
+        """``chain``: an ``ImageNetChain`` that transforms the batches instead of the fused policy launch
+        (``chain_mode`` 'train' or 'test')."""
         if not torch.cuda.is_available():
             raise _lib.FaaRuntimeError("fast_autoaugment_b200 needs a CUDA device (no CPU fallback)")
         self.dataset, self.batch_size, self.tail = dataset, int(batch), tail
         self.sampler, self.shuffle, self.drop_last, self.parity = sampler, shuffle, drop_last, parity
         self.aug = Augmentation(policies) if policies is not None else Augmentation([[("Invert", 0.0, 0.0)]])
         self.seed = int(torch.initial_seed() if seed is None else seed) & 0x7FFFFFFFFFFFFFFF
+        self.chain, self.chain_mode = chain, chain_mode
         self._drawn = 0                   # samples drawn so far: the Philox counter never repeats across epochs
 
     def _n(self):
@@ -246,7 +458,12 @@ class GpuAugmentedLoader:
             idx = idx_all[k * self.batch_size:(k + 1) * self.batch_size]
             t = torch.as_tensor(idx, dtype=torch.int64).to(dev, non_blocking=True)
             raw = self.dataset.images.index_select(0, t)
-            data = self.aug.augment_batch(raw, self.tail, seed=self.seed, first_index=self._drawn, parity=self.parity)
+            if self.chain is None:
+                data = self.aug.augment_batch(raw, self.tail, seed=self.seed, first_index=self._drawn, parity=self.parity)
+            elif self.chain_mode == "test":
+                data = self.chain.test(raw)
+            else:
+                data = self.chain.train(raw, parity=self.parity, seed=self.seed, first_index=self._drawn)
             self._drawn += len(idx)
             yield data, self.dataset.labels.index_select(0, t)
 
@@ -294,7 +511,11 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
     DataLoader workers is replaced by one fused kernel launch per batch.
 
     Extra conf keys (optional): ``faa_out_dtype`` ('float32' default - what the reference yields -, 'float16',
-    'bfloat16'), ``faa_parity`` (replay the reference's global RNG draws per sample; tests)."""
+    'bfloat16'), ``faa_parity`` (replay the reference's global RNG draws per sample; tests), ``faa_crop_resize``
+    (ImageNet: the stored images are uncropped sources of one size and the loaders run the reference's full chains,
+    ``ImageNetChain``: train / valid = policy -> EfficientNetRandomCrop + bicubic Resize -> ColorJitter -> HFlip +
+    Lighting + Normalize, test = EfficientNetCenterCrop + Resize + Normalize, at 224 or the EfficientNet size of
+    ``conf['model']['type']``; without it ImageNet images must already have the network's size)."""
     from sklearn.model_selection import StratifiedShuffleSplit
     import torch.distributed as dist
 
@@ -345,6 +566,16 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
                 range(len(total_trainset)), num_replicas=dist.get_world_size(), rank=dist.get_rank())
 
     parity = bool(conf.get("faa_parity", False))
+    if "imagenet" in dataset and conf.get("faa_crop_resize", False):      # data.py:49-80, 217-224
+        model_type = (conf.get("model") or {}).get("type", "")
+        chain = ImageNetChain(policies, imagenet_input_size(model_type), out_dtype)
+        trainloader = GpuAugmentedLoader(total_trainset, batch, policies, tail, sampler=train_sampler,
+                                         shuffle=train_sampler is None, drop_last=True, parity=parity, chain=chain)
+        validloader = GpuAugmentedLoader(total_trainset, batch, policies, tail, sampler=valid_sampler,
+                                         shuffle=False, drop_last=False, parity=parity, chain=chain)
+        testloader = GpuAugmentedLoader(testset, batch, None, test_tail, shuffle=False, drop_last=False,
+                                        chain=chain, chain_mode="test")
+        return train_sampler, trainloader, validloader, testloader
     trainloader = GpuAugmentedLoader(total_trainset, batch, policies, tail, sampler=train_sampler,
                                      shuffle=train_sampler is None, drop_last=True, parity=parity)       # data.py:214-216
     validloader = GpuAugmentedLoader(total_trainset, batch, policies, tail, sampler=valid_sampler,

@@ -417,3 +417,68 @@ def augment_tta(policy: CompiledPolicy, batch_u8: torch.Tensor, tail: TailSpec, 
         check(lib.faa_augment_tta(policy.handle, batch_u8.data_ptr(), out.data_ptr(), B, int(replicas), H, W, C.byref(t),
                                   C.byref(rng), _stream_ptr(batch_u8.device)))
     return out
+
+
+def crop_cfg(img_size, center=False, min_covered=0.1, aspect_ratio_range=(3. / 4, 4. / 3), area_range=(0.08, 1.0),
+             max_attempts=10, seed=0, first_index=0):
+    """``faa_crop_cfg_t`` of EfficientNetRandomCrop / EfficientNetCenterCrop(img_size) (reference data.py:267-345);
+    ``seed`` / ``first_index`` key the device crop sampler (Philox, global sample index first_index + i)."""
+    c = _lib.CropCfg()
+    c.mode = _lib.CROP_CENTER if center else _lib.CROP_RANDOM
+    c.img_size = int(img_size)
+    c.min_covered = float(min_covered)
+    c.aspect_lo, c.aspect_hi = float(aspect_ratio_range[0]), float(aspect_ratio_range[1])
+    c.area_lo, c.area_hi = float(area_range[0]), float(area_range[1])
+    c.max_attempts = int(max_attempts)
+    c.rng = make_rng(seed, first_index)
+    return c
+
+
+def center_crop_box(h, w, img_size):
+    """(x0, y0, w, h) of EfficientNetCenterCrop(img_size) on an h x w image (C ABI ``faa_center_crop_box``)."""
+    b = np.zeros(1, dtype=_lib.CROP_BOX_DTYPE)
+    check(lib.faa_center_crop_box(int(h), int(w), int(img_size), b.ctypes.data))
+    return tuple(int(v) for v in b[0])
+
+
+def crop_resize(batch_u8: torch.Tensor, size, boxes=None, rng=None, tail: TailSpec | None = None, out=None):
+    """EfficientNet crop + ``Resize((s, s), BICUBIC)`` of a uint8 [B,H,W,3] CUDA batch in ONE launch (C ABI
+    ``faa_crop_resize``), bit-exact with Pillow's ``crop`` + ``resize``.
+
+    ``size``: output size (int or (h, w)).  ``boxes``: per-image crop boxes ([B] ``CROP_BOX_DTYPE`` array, or an
+    int32 [B, 4] array / tensor of x0, y0, w, h); otherwise ``rng`` is a ``crop_cfg`` and the kernel draws (random
+    mode) or computes (center mode) the boxes.  ``tail``: None or a uint8 ``TailSpec`` -> uint8 [B, s, s, 3]; a float
+    ``TailSpec`` -> ToTensor + Normalize fused in, [B, 3, s, s] of ``tail.out_dtype`` (its crop / flip / Cutout fields
+    are not used here)."""
+    _require_cuda(batch_u8, "batch")
+    if batch_u8.dtype != torch.uint8 or batch_u8.dim() != 4 or batch_u8.shape[-1] != 3:
+        raise ValueError("batch must be uint8 [B, H, W, 3]")
+    if (boxes is None) == (rng is None):
+        raise ValueError("give exactly one of boxes= and rng=")
+    batch_u8 = batch_u8.contiguous()
+    dev = batch_u8.device
+    B, H, W, _ = batch_u8.shape
+    oh, ow = (size, size) if isinstance(size, int) else (int(size[0]), int(size[1]))
+    tail = tail or TailSpec.raw_u8()
+    t = tail.c_struct(H, W)
+    t.out_h, t.out_w = oh, ow
+    shape = (B, oh, ow, 3) if tail.out_dtype == torch.uint8 else (B, 3, oh, ow)
+    if out is None:
+        out = torch.empty(shape, dtype=tail.out_dtype, device=dev)
+    elif tuple(out.shape) != shape or out.dtype != tail.out_dtype or not out.is_contiguous() or out.device != dev:
+        raise ValueError("out must be a contiguous %s tensor %s on %s" % (tail.out_dtype, shape, dev))
+    d_boxes = None
+    if boxes is not None:
+        if isinstance(boxes, torch.Tensor):
+            d_boxes = boxes.to(device=dev, dtype=torch.int32).contiguous().reshape(-1)
+        else:
+            a = np.ascontiguousarray(boxes)
+            a = a.view(np.int32) if a.dtype == _lib.CROP_BOX_DTYPE else a.astype(np.int32)
+            d_boxes = torch.from_numpy(np.ascontiguousarray(a).reshape(-1).copy()).to(dev)
+        if d_boxes.numel() != 4 * B:
+            raise ValueError("need one box (x0, y0, w, h) per image")
+    cfg = rng if rng is not None else crop_cfg(oh)
+    with torch.cuda.device(dev):
+        check(lib.faa_crop_resize(batch_u8.data_ptr(), out.data_ptr(), B, H, W, C.byref(t),
+                                  d_boxes.data_ptr() if d_boxes is not None else None, C.byref(cfg), _stream_ptr(dev)))
+    return out

@@ -242,6 +242,37 @@ int faa_color_jitter(const uint8_t* d_in, uint8_t* d_out, int batch, int h, int 
  * fp32 operation order.  NULL switches it off again.  The array must stay valid until those launches ran. */
 int faa_policy_set_lighting(faa_policy_t* p, const float* d_rgb, int n);
 
+/* ---- EfficientNet crops + bicubic resize: the geometry of the ImageNet chains (data.py:61-62, 76-77, 267-345)
+ * EfficientNetRandomCrop(img_size) / EfficientNetCenterCrop(img_size), then transforms.Resize((s, s), BICUBIC),
+ * i.e. Pillow's Image.crop (box rounded half to even) and ImagingResample (8-bit, bicubic a = -0.5, 22-bit fixed
+ * point, horizontal pass into a uint8 intermediate, then the vertical pass), bit-exact. */
+typedef struct faa_crop_box { int32_t x0, y0, w, h; } faa_crop_box_t;   /* crop = rows [y0, y0+h) x columns [x0, x0+w) */
+
+enum faa_crop_mode { FAA_CROP_RANDOM = 0, FAA_CROP_CENTER = 1 };
+
+typedef struct faa_crop_cfg {
+    int32_t   mode;                   /* enum faa_crop_mode                                            */
+    int32_t   img_size;               /* EfficientNet*Crop(imgsize): the center crop is s/(s+32) of the short side */
+    double    min_covered;            /* EfficientNetRandomCrop(min_covered=0.1,                          */
+    double    aspect_lo, aspect_hi;   /*     aspect_ratio_range=(3/4, 4/3),                               */
+    double    area_lo, area_hi;       /*     area_range=(0.08, 1.0),                                      */
+    int32_t   max_attempts;           /*     max_attempts=10)                                             */
+    int32_t   reserved;
+    faa_rng_t rng;                    /* seed / first_index of the device crop sampler (other fields unused) */
+} faa_crop_cfg_t;
+
+/* host helper: the box EfficientNetCenterCrop(img_size) cuts from an h x w image */
+int faa_center_crop_box(int h, int w, int img_size, faa_crop_box_t* out);
+
+/* d_in : uint8 [batch][h][w][3] (device).  d_out: [batch][tail->out_h][tail->out_w][3] uint8 when tail->out_dtype is
+ * FAA_U8_HWC (the train chain continues with faa_color_jitter), else [batch][3][out_h][out_w] with ToTensor + Normalize
+ * (tail->mean / std) fused in: the same values faa_augment writes for the same uint8 image.  d_boxes: one box per image
+ * (device memory; checked against the image on the host, which waits for the stream), or NULL: the kernel draws
+ * them itself (cfg->mode; random boxes from Philox keyed by (cfg->rng.seed, cfg->rng.first_index + i): the reference's
+ * distributions, not its stream).  An ordinary stream-ordered launch.  tail->use_zero_box and crop_pad are ignored. */
+int faa_crop_resize(const uint8_t* d_in, void* d_out, int batch, int h, int w, const faa_tail_t* tail,
+                    const faa_crop_box_t* d_boxes, const faa_crop_cfg_t* cfg, void* stream);
+
 /* number of kernels this library has launched since load (bench bookkeeping) */
 uint64_t faa_launch_count(void);
 
