@@ -570,6 +570,23 @@ static int check_tail(const faa_tail_t* tail) {
     return FAA_OK;
 }
 
+// The policy kernels move whole quads of pixels as words whenever rows hold whole quads: the input as 32-bit words
+// (load12, W % 4 == 0) and each output plane as one 16-byte (fp32), 8-byte (fp16 / bf16) or three 32-bit (uint8 HWC)
+// stores (store_plane4, emit_quad, out_w % 4 == 0).  Image, plane and row offsets are multiples of those sizes then, so
+// the buffers' bases decide.  (The 16-byte paths - TMA staging, octets, the mid kernel - test their own alignment and
+// are simply not taken.)  A contiguous view at an offset into a larger allocation can miss these alignments.
+static int check_alignment(const void* d_in, const void* d_out, int w, const faa_tail_t* tail) {
+    if ((w & 3) == 0 && ((uintptr_t)d_in & 3))
+        return fail(FAA_ERR_UNSUPPORTED, "the input must be 4-byte aligned when W % 4 == 0 (32-bit loads)");
+    if ((tail->out_w & 3) == 0) {
+        const uintptr_t need = tail->out_dtype == FAA_F32 ? 16 : tail->out_dtype == FAA_U8_HWC ? 4 : 8;
+        if ((uintptr_t)d_out & (need - 1))
+            return fail(FAA_ERR_UNSUPPORTED, "the output must be " + std::to_string(need) +
+                                             "-byte aligned when its width is a multiple of 4 (vector stores)");
+    }
+    return FAA_OK;
+}
+
 int faa_sample_philox(faa_policy_t* p, int batch, int h, int w, const faa_tail_t* tail, const faa_rng_t* rng,
                       faa_sample_t* d_samples, faa_box_t* d_boxes, void* stream) {
     if (!p || !rng || !d_samples || !d_boxes) return fail(FAA_ERR_VALUE, "null argument");
@@ -875,6 +892,7 @@ static int augment_common(faa_policy_t* p, const uint8_t* d_in_all, int n_all, i
     if (rng && !d_samples && apply_tail) { if (int e = check_crop(h, w, tail, rng->crop_pad > 0 ? rng->crop_pad : 0)) return e; }
     if (op_base < 0 || op_base >= p->n_op) return fail(FAA_ERR_VALUE, "op_base out of range");
     if (tail->out_dtype == FAA_U8_HWC && d_partner) return fail(FAA_ERR_UNSUPPORTED, "mixup needs a float output");
+    if (batch > 0) { if (int e = check_alignment(d_in_all, d_out, w, tail)) return e; }
     if (int e = ensure_device()) return e;
     if (batch == 0) return FAA_OK;
     if (int e = bind_device(p)) return e;
@@ -1062,6 +1080,10 @@ int faa_augment_many(faa_policy_t* p, int n_steps, const uint8_t* const* d_in, v
     if (!p || !rng || !d_in || !d_out) return fail(FAA_ERR_VALUE, "null argument");
     if (n_steps < 0) return fail(FAA_ERR_VALUE, "bad step count");
     if (p->n_op > FAA_MAX_FUSED_OPS) return fail(FAA_ERR_UNSUPPORTED, "multi-step launches support policies of at most 2 ops");
+    if (batch > 0) {                                    // refuse before the first step is issued
+        if (int e = check_tail(tail)) return e;
+        for (int k = 0; k < n_steps; ++k) { if (int e = check_alignment(d_in[k], d_out[k], w, tail)) return e; }
+    }
     std::lock_guard<std::mutex> call_lk(p->call_mu);
     faa_rng_t r = *rng;
     const bool saved = p->overlap_calls;
@@ -1311,6 +1333,9 @@ int faa_augment_host(faa_policy_t* p, const uint8_t* h_in, void* h_out, void* d_
     if (p->n_op > FAA_MAX_FUSED_OPS) return fail(FAA_ERR_UNSUPPORTED, "host-buffer entry supports policies of at most 2 ops");
     if (int e = check_shape(h, w)) return e;
     if (int e = check_tail(tail)) return e;
+    // (the device input is the policy's own allocation; a caller-owned device output is checked up front, before any
+    //  chunk is issued)
+    if (d_out_keep && batch > 0) { if (int e = check_alignment(nullptr, d_out_keep, w, tail)) return e; }
     if (int e = ensure_device()) return e;
     if (batch <= 0) return FAA_OK;
     if (int e = bind_device(p)) return e;

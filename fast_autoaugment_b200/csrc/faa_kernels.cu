@@ -1457,7 +1457,11 @@ static __device__ __forceinline__ void cluster_kernel_body(const AugParams& P) {
 
     if constexpr (NSRC == 1) {
         const int cls = st[0].prog.cls;
-        const Ctx c = make_ctx(P, raw0, s_dyn, s_lo, s_len, P.H, P.W, st[0], cls != C_PLAIN && cls != C_LUT);
+        // C_PLAIN / C_LUT final passes only read the composed LUT; but a C_LUT program with slot-1 statistics (Contrast
+        // behind a LUT op, in a launch without a materialisation chunk) takes them lazily through Level<1>, which
+        // evaluates op 0 from the records
+        const bool full = (cls != C_PLAIN && cls != C_LUT) || (st[0].prog.stat_mask & 2u);
+        const Ctx c = make_ctx(P, raw0, s_dyn, s_lo, s_len, P.H, P.W, st[0], full);
         if (cls == C_MAT) {
             any_stats = run_materialised<OUT, TAB>(P, s_norm, st[0], c, s_dyn + P.band_cap, out_img, band, cluster);
         } else if (cls == C_SG) {

@@ -145,7 +145,10 @@ int faa_sample_philox(faa_policy_t* p, int batch, int h, int w, const faa_tail_t
  *      d_out: [batch][3][out_h][out_w] of tail->out_dtype (or uint8 HWC)
  *      d_samples / d_boxes: resolved decisions; if d_samples == NULL the kernel draws them
  *      itself from `rng` (fused Philox mode).  op_base selects which FAA_MAX_FUSED_OPS-wide
- *      window of the sub-policy this launch applies (chained launches for n_op > 2). */
+ *      window of the sub-policy this launch applies (chained launches for n_op > 2).
+ *      Alignment (all policy entries): d_in 4-byte aligned when w % 4 == 0; d_out 16-byte (fp32),
+ *      8-byte (fp16 / bf16) or 4-byte (uint8 HWC) aligned when out_w % 4 == 0; else
+ *      FAA_ERR_UNSUPPORTED. */
 int faa_augment(faa_policy_t* p, const uint8_t* d_in, void* d_out, int batch, int h, int w,
                 const faa_tail_t* tail, const faa_sample_t* d_samples, const faa_box_t* d_boxes,
                 const faa_rng_t* rng, int op_base, void* stream);
