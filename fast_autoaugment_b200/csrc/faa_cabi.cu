@@ -7,6 +7,7 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <atomic>
 #include <cmath>
 #include <cstdio>
@@ -607,16 +608,10 @@ int faa_sample_philox(faa_policy_t* p, int batch, int h, int w, const faa_tail_t
     return FAA_OK;
 }
 
-// What augment_common decided for one call: which kernels run, on which schedule, and how their buffers are bound.
-struct Schedule {
-    bool use_order;             // the resolve kernel writes a cost-sorted schedule (order / n_heavy)
-    bool use_split;             // the light streaming kernel (and the mid kernel) take the programs they cover
-    bool use_mid;               // three-way split: statistics-LUT and Sharpness programs run in the mid kernel
-    bool use_chain;             // chained schedule (else the event schedule)
-    bool no_heavy;              // every program is light or mid: the cluster kernel is not launched
+// What augment_common decided for one call: the launch plan, and what this call adds to it.
+struct Schedule : LaunchPlan {
     bool use_tab;               // exact normalisation table instead of one fma
-    bool speculate;             // resolve the next call's batch ahead (resolve-ahead)
-    bool hit;                   // ... and the previous call already resolved exactly this one
+    bool hit;                   // the previous call already resolved exactly this batch (resolve-ahead)
     size_t scratch_slot_bytes;  // scratch images per program slot
 };
 
@@ -644,14 +639,9 @@ static void bind_slot(const faa_policy* p, const Schedule& s, int first, int slo
     }
 }
 
-// the mid kernel's launch: its own (taller) bands in bands / geo[0] - the band count is halved while a band (+ halo)
-// stays <= 80 KB (2 CTAs / SM)
-static AugParams mid_params(AugParams a) {
-    int mb = a.bands;
-    while (mb > 1 && band_capacity(mb / 2, a.H, a.W, a.out_h, 0) <= 80 * 1024) mb /= 2;
-    a.bands = mb;
-    fill_geom(a.geo[0], mb, a.H, a.W, a.out_h, 0, true);
-    a.band_cap = a.geo[0].band_cap; a.mat_cap = 0;
+// the mid kernel's launch: its own (taller) bands in bands / geo[0]
+static AugParams mid_params(AugParams a, const BandGeom& mid) {
+    a.bands = mid.bands; a.geo[0] = mid; a.band_cap = mid.band_cap; a.mat_cap = 0;
     return a;
 }
 
@@ -780,7 +770,7 @@ static int launch_chained(faa_policy* p, const AugParams& P, ResolveParams& R, c
     p->ahead_valid = true; p->ahead_ticket = R2.ticket;
 
     if (!p->sm_count) CK(cudaDeviceGetAttribute(&p->sm_count, cudaDevAttrMultiProcessorCount, p->device));
-    AugParams Pm = s.use_mid ? mid_params(Pc) : Pc;
+    AugParams Pm = s.use_mid ? mid_params(Pc, s.mid) : Pc;
     // one resident wave each (launch bounds: light CTAs / SM; mid rows: ONE CTA per SM, so that the light CTAs that
     // follow share the SM with it from the start)
     const int lb = P.geo[1].bands > 0 ? P.geo[1].bands : 1;
@@ -868,7 +858,7 @@ static int launch_event(faa_policy* p, AugParams& P, ResolveParams& R, const Sch
         g_launches++;
     }
     if (s.use_mid) {
-        CK(launch_augment(mid_params(Ph), out_dtype, s.use_tab, 2, p->mid_stream));
+        CK(launch_augment(mid_params(Ph, s.mid), out_dtype, s.use_tab, 2, p->mid_stream));
         g_launches++;
         CK(cudaEventRecord(p->ev_mid, p->mid_stream));
     }
@@ -878,33 +868,45 @@ static int launch_event(faa_policy* p, AugParams& P, ResolveParams& R, const Sch
     return FAA_OK;
 }
 
-static int augment_common(faa_policy_t* p, const uint8_t* d_in_all, int n_all, int first, void* d_out, int batch,
-                          int h, int w, const faa_tail_t* tail, const faa_sample_t* d_samples,
-                          const faa_box_t* d_boxes, const faa_rng_t* rng, int op_base, const int32_t* d_partner,
-                          float lam, float oml, int apply_tail, bool allow_ahead, void* stream_v, int in_mod = 0,
-                          bool own_stream = true) {
-    if (!p || (!d_in_all && batch > 0) || (!d_out && batch > 0)) return fail(FAA_ERR_VALUE, "null argument");
-    if (batch < 0 || first < 0 || first + batch > n_all) return fail(FAA_ERR_VALUE, "bad batch range");
+// One policy launch as an entry point describes it: images [first, first + batch) of the n_all images at `in`, with
+// resolved decisions (samples / boxes) or decisions drawn by `rng`.
+struct AugRequest {
+    const uint8_t* in = nullptr; void* out = nullptr;
+    int n_all = 0, first = 0, batch = 0, h = 0, w = 0;
+    const faa_tail_t* tail = nullptr; void* stream = nullptr;
+    const faa_sample_t* samples = nullptr; const faa_box_t* boxes = nullptr; const faa_rng_t* rng = nullptr;
+    int op_base = 0, apply_tail = 1;                // apply_tail: the final window of the policy
+    const int32_t* partner = nullptr; float lam = 1.0f, one_minus_lam = 0.0f;    // fused Mixup
+    bool allow_ahead = false;                       // the next call's batch may be resolved ahead
+    int in_mod = 0;                                 // > 0: replicated launch (TTA), entry v reads input image v % in_mod
+    bool own_stream = true;                         // false: a chunk of faa_augment_host on one of its side streams,
+                                                    // which that call orders itself
+};
+
+static int augment_common(faa_policy_t* p, const AugRequest& q) {
+    const faa_tail_t* tail = q.tail;
+    const int batch = q.batch, h = q.h, w = q.w;
+    if (!p || (!q.in && batch > 0) || (!q.out && batch > 0)) return fail(FAA_ERR_VALUE, "null argument");
+    if (batch < 0 || q.first < 0 || q.first + batch > q.n_all) return fail(FAA_ERR_VALUE, "bad batch range");
     if (batch > 65535) return fail(FAA_ERR_UNSUPPORTED, "at most 65535 images per call (one grid row per image): split the batch");
     if (int e = check_shape(h, w)) return e;
     if (int e = check_tail(tail)) return e;
-    if (!d_samples && !rng) return fail(FAA_ERR_VALUE, "need either resolved samples or an rng config");
-    if (rng && !d_samples && apply_tail) { if (int e = check_crop(h, w, tail, rng->crop_pad > 0 ? rng->crop_pad : 0)) return e; }
-    if (op_base < 0 || op_base >= p->n_op) return fail(FAA_ERR_VALUE, "op_base out of range");
-    if (tail->out_dtype == FAA_U8_HWC && d_partner) return fail(FAA_ERR_UNSUPPORTED, "mixup needs a float output");
-    if (batch > 0) { if (int e = check_alignment(d_in_all, d_out, w, tail)) return e; }
+    if (!q.samples && !q.rng) return fail(FAA_ERR_VALUE, "need either resolved samples or an rng config");
+    if (q.rng && !q.samples && q.apply_tail) { if (int e = check_crop(h, w, tail, q.rng->crop_pad > 0 ? q.rng->crop_pad : 0)) return e; }
+    if (q.op_base < 0 || q.op_base >= p->n_op) return fail(FAA_ERR_VALUE, "op_base out of range");
+    if (tail->out_dtype == FAA_U8_HWC && q.partner) return fail(FAA_ERR_UNSUPPORTED, "mixup needs a float output");
+    if (batch > 0) { if (int e = check_alignment(q.in, q.out, w, tail)) return e; }
     if (int e = ensure_device()) return e;
     if (batch == 0) return FAA_OK;
     if (int e = bind_device(p)) return e;
-    cudaStream_t stream = (cudaStream_t)stream_v;
-    // (own_stream false: a chunk of faa_augment_host on one of its side streams, which that call orders itself)
-    if (own_stream) { if (int e = follow_stream(p, stream)) return e; }
+    cudaStream_t stream = (cudaStream_t)q.stream;
+    if (q.own_stream) { if (int e = follow_stream(p, stream)) return e; }
     const OpRec* d_ops = nullptr;
     // resolved samples can only reference ops the host sampler validated; Philox can pick anything
-    if (int e = device_table(p, h, w, d_samples == nullptr, &d_ops)) return e;
+    if (int e = device_table(p, h, w, q.samples == nullptr, &d_ops)) return e;
     {   // per-image program buffer (grown, never shrunk; stream-ordered reuse)
         std::lock_guard<std::mutex> lk(p->mu);
-        size_t need = (size_t)n_all * sizeof(Prog);
+        size_t need = (size_t)q.n_all * sizeof(Prog);
         if (p->d_progs_bytes < need) {
             if (p->d_progs) {
                 CK(cudaStreamSynchronize(stream));
@@ -921,88 +923,38 @@ static int augment_common(faa_policy_t* p, const uint8_t* d_in_all, int n_all, i
             p->done_target[0] = p->done_target[1] = 0;      // (the completion counters live in d_order and start at zero)
         }
     }
-    // geometry of the pixel launch (needed by the resolve step: allow_mat)
+    PlanInput in = {};
+    in.H = h; in.W = w; in.out_h = tail->out_h; in.out_w = tail->out_w; in.out_u8 = tail->out_dtype == FAA_U8_HWC;
+    in.batch = batch; in.crop_pad = std::min(h, std::max({0, tail->crop_pad, q.rng ? q.rng->crop_pad : 0}));
+    in.in_mod16 = (uint32_t)((uintptr_t)q.in % 16); in.out_mod16 = (uint32_t)((uintptr_t)q.out % 16);
+    in.two_src = q.partner != nullptr; in.apply_tail = q.apply_tail != 0; in.has_sg = p->has_sg;
+    in.split_min = kSplitMin;
+    if (const char* e = getenv("FAA_SPLIT_MIN")) in.split_min = strtoull(e, nullptr, 10);   // tests: force either path
+    in.philox = q.rng && !q.samples; in.allow_ahead = q.allow_ahead;
+    Schedule s{plan_launch(in)};
     AugParams P; memset(&P, 0, sizeof P);
-    P.in = d_in_all; P.out = d_out;
-    P.partner = d_partner;
-    P.B = batch; P.H = h; P.W = w; P.out_h = tail->out_h; P.out_w = tail->out_w; P.first = first; P.in_mod = in_mod;
-    P.use_zero_box = (tail->use_zero_box && apply_tail) ? 1 : 0;
-    P.lam = lam; P.one_minus_lam = oml;
-    P.bands = pick_bands(h, w, tail->out_h, tail->out_w);
-    // TMA band staging needs 16-byte aligned image bases and a band that fits shared memory
-    // (crop_pad only sizes the staged band; rows outside it are read from global memory)
-    P.crop_pad = tail->crop_pad > 0 ? tail->crop_pad : 0;
-    if (rng && rng->crop_pad > P.crop_pad) P.crop_pad = rng->crop_pad;
-    if (P.crop_pad > h) P.crop_pad = h;
-    P.band_cap = (int32_t)band_capacity(P.bands, h, w, tail->out_h, P.crop_pad);
-    const size_t img_bytes = (size_t)h * w * 3;
-    const int nsrc = d_partner ? 2 : 1;
-    P.stage = (img_bytes % 16 == 0 && ((uintptr_t)d_in_all % 16) == 0 && (size_t)P.band_cap * nsrc <= 150 * 1024) ? 1 : 0;
-    if (!P.stage) P.band_cap = 0;
-    {   // per-kernel band geometry and fastdiv reciprocals (host side: no divisions in the kernels)
-        fill_geom(P.geo[0], P.bands, h, w, tail->out_h, P.crop_pad, P.stage != 0);
-        int lb = P.bands;
-        if (P.bands == 8) {
-            // the light kernel needs no cluster, so any band count works: take the one in 5..8 whose
-            // quads-per-CTA fills whole 256-thread iterations best (224x224: 7 bands = exactly 7 iterations)
-            const int qpr = (tail->out_w + 3) / 4;
-            double best = -1.0;
-            for (int b = 8; b >= 5; --b) {
-                const int rows = (tail->out_h + b - 1) / b;
-                const int quads = rows * qpr, iters = (quads + 255) / 256;
-                const double eff = (double)quads / (iters * 256.0) * ((double)tail->out_h / (rows * b));
-                if (eff > best + 0.02) { best = eff; lb = b; }
-            }
-        }
-        fill_geom(P.geo[1], lb, h, w, tail->out_h, P.crop_pad, P.stage != 0 && (size_t)band_capacity(lb, h, w, tail->out_h, P.crop_pad) <= 100 * 1024);
-        auto rcp = [](uint32_t d) { return d <= 1 ? 0u : (uint32_t)((0x100000000ull + d - 1) / d); };
-        P.rcp_out_qpr = rcp((uint32_t)(tail->out_w + 3) / 4); P.rcp_w = rcp((uint32_t)w); P.rcp_wq = rcp((uint32_t)w / 4);
-        P.rcp_opr = (w & 7) ? 0u : rcp((uint32_t)w / 8);
-        P.octets = ((w & 7) == 0 && tail->out_w == w && tail->out_h == h &&
-                    ((uintptr_t)d_out % 16) == 0 && P.stage) ? 1 : 0;          // (uint8 HWC included: 24-byte octets, 8-byte aligned)
-    }
-    // materialisation chunk: as many rows as fit ~16 KB, at least 3 (single-source launches only)
-    {
-        // big enough to keep a whole band (+ halo, + crop slack) resident when that is <= 24 KB, else ~16 KB chunks
-        const int pitch = w * 3;
-        const int band_rows = (h + P.bands - 1) / P.bands + 2 + 2 * P.crop_pad;
-        int rows = (band_rows * pitch <= 24576) ? band_rows : 16384 / pitch;
-        if (rows > h + 2) rows = h + 2;
-        P.mat_cap = (!d_partner && rows >= 3) ? ((rows * pitch + 32 + 15) & ~15) : 0;   // + 2 guard bands
-    }
+    P.in = q.in; P.out = q.out; P.partner = q.partner;
+    P.B = batch; P.H = h; P.W = w; P.out_h = tail->out_h; P.out_w = tail->out_w; P.first = q.first; P.in_mod = q.in_mod;
+    P.use_zero_box = (tail->use_zero_box && q.apply_tail) ? 1 : 0;
+    P.lam = q.lam; P.one_minus_lam = q.one_minus_lam;
+    P.bands = s.geo[0].bands; P.geo[0] = s.geo[0]; P.geo[1] = s.geo[1];
+    P.stage = s.stage; P.band_cap = s.geo[0].band_cap; P.crop_pad = in.crop_pad; P.octets = s.octets; P.mat_cap = s.mat_cap;
+    // fastdiv reciprocals (host side: no divisions in the kernels)
+    auto rcp = [](uint32_t d) { return d <= 1 ? 0u : (uint32_t)((0x100000000ull + d - 1) / d); };
+    P.rcp_out_qpr = rcp((uint32_t)(tail->out_w + 3) / 4); P.rcp_w = rcp((uint32_t)w); P.rcp_wq = rcp((uint32_t)w / 4);
+    P.rcp_opr = (w & 7) ? 0u : rcp((uint32_t)w / 8);
     P.pdl = 1;
     // launch 1: decisions -> programs (the whole pool when partners may be anywhere in it)
     ResolveParams R; memset(&R, 0, sizeof R);
     R.ops = d_ops; R.probs = p->d_probs;
-    R.samples = reinterpret_cast<const Sample*>(d_samples); R.boxes = reinterpret_cast<const Box*>(d_boxes);
-    if (rng) memcpy(&R.rng, rng, sizeof(RngCfg));
-    R.first = d_partner ? 0 : first; R.n = d_partner ? n_all : batch;
+    R.samples = reinterpret_cast<const Sample*>(q.samples); R.boxes = reinterpret_cast<const Box*>(q.boxes);
+    if (q.rng) memcpy(&R.rng, q.rng, sizeof(RngCfg));
+    R.first = q.partner ? 0 : q.first; R.n = q.partner ? q.n_all : batch;
     R.H = h; R.W = w; R.out_h = tail->out_h; R.out_w = tail->out_w;
-    R.n_sub = p->n_sub; R.n_op = p->n_op; R.op_base = op_base; R.apply_tail = apply_tail;
-    R.allow = P.mat_cap > 0 ? 1 : 0;
-    Schedule s{};
-    s.use_order = !d_partner;
-    // (small launches are launch-latency bound: one pixel kernel is faster there)
-    size_t split_min = (size_t)4 << 20;                   // pixels per launch from which two pixel kernels pay off
-    if (const char* e = getenv("FAA_SPLIT_MIN")) split_min = (size_t)strtoull(e, nullptr, 10);   // tests: force either path
-    // (uint8 HWC output - the Mixup exchange format - splits when the lean octet paths can write it)
-    s.use_split = s.use_order && (tail->out_dtype != FAA_U8_HWC || (P.octets && P.crop_pad == 0 && apply_tail)) &&
-                  (size_t)batch * h * w >= split_min;
-    R.split = s.use_split ? 1 : 0;
-    // Chained steps need the Philox sampler on the device and a caller that allows the next batch to be resolved ahead.
-    // Launches too small to split are chained as well (resolve(N+1), cluster(N)): their step is bound by kernel latencies,
-    // which only overlap across steps on one stream; uint8 output of one pixel kernel stays on the event schedule.
-    s.use_chain = (s.use_split || tail->out_dtype != FAA_U8_HWC) && allow_ahead && rng && !d_samples && !d_partner;
-    // Three-way split: statistics-LUT and Sharpness programs run in the lean mid kernel.
-    // Needs the geometry its paths assume: float planes of the image's own size, no crop, W % 4 == 0, staged bands.
-    s.use_mid = s.use_split && P.stage && (w & 3) == 0 && tail->out_w == w && tail->out_h == h &&
-                P.crop_pad == 0 && ((uintptr_t)d_out % 16) == 0;
-    if (s.use_mid) R.split = 2;
-    if (s.use_split && P.octets && P.crop_pad == 0) R.allow |= 4;     // the lean gather paths exist in this launch
-    // scratch images: Sharpness -> gather programs of the cluster kernel, every Sharpness-first two-op program of the mid
-    // kernel; one per program slot in the chained schedule
-    if ((p->has_sg || s.use_mid) && !d_partner && (w & 3) == 0) {
-        s.scratch_slot_bytes = (size_t)n_all * img_bytes;
+    R.n_sub = p->n_sub; R.n_op = p->n_op; R.op_base = q.op_base; R.apply_tail = q.apply_tail;
+    R.allow = s.allow; R.split = s.split;
+    if (s.scratch) {            // one scratch image per image, per program slot in the chained schedule
+        s.scratch_slot_bytes = (size_t)q.n_all * h * w * 3;
         const size_t need = s.scratch_slot_bytes * (s.use_chain ? 2 : 1);
         if (p->d_scratch_bytes < need) {
             if (p->d_scratch) { CK(cudaStreamSynchronize(stream)); CK(cudaFree(p->d_scratch)); p->d_scratch = nullptr; p->d_scratch_bytes = 0; }
@@ -1010,44 +962,35 @@ static int augment_common(faa_policy_t* p, const uint8_t* d_in_all, int n_all, i
             p->d_scratch_bytes = need;
         }
         P.scratch = (uint8_t*)p->d_scratch;
-        R.allow |= 2;
     }
-    // With the lean gathers (allow bit 2) and a scratch image (bit 1) every program of a three-way split is light or mid
-    // (faa_core.cuh prog_is_light / prog_is_mid cover all class combinations; tests/test_gpu_fastpaths.py runs every ordered
-    // op pair through this schedule): the cluster kernel has nothing to do and is not launched.
-    s.no_heavy = s.use_mid && (R.allow & 6) == 6 && P.mat_cap > 0;
     if (tail->out_dtype != FAA_U8_HWC) { if (int e = normalisation(p, tail, P, s.use_tab, stream)) return e; }
     else { for (int c = 0; c < 3; ++c) { P.scale[c] = 1.0f; P.bias[c] = 0.0f; } }      // lean paths: the byte value itself
-    if (p->lighting_rgb && tail->out_dtype != FAA_U8_HWC && apply_tail) {
+    if (p->lighting_rgb && tail->out_dtype != FAA_U8_HWC && q.apply_tail) {
         // Lighting (augmentations.py:197-215): one normalisation table per image, built on the stream in torch's fp32 order
-        if (d_partner) return fail(FAA_ERR_UNSUPPORTED, "Lighting together with fused Mixup is not supported");
-        if (p->lighting_n != n_all) return fail(FAA_ERR_VALUE, "faa_policy_set_lighting was given a different number of images");
-        const size_t need = (size_t)n_all * 768 * sizeof(float);
+        if (q.partner) return fail(FAA_ERR_UNSUPPORTED, "Lighting together with fused Mixup is not supported");
+        if (p->lighting_n != q.n_all) return fail(FAA_ERR_VALUE, "faa_policy_set_lighting was given a different number of images");
+        const size_t need = (size_t)q.n_all * 768 * sizeof(float);
         if (p->d_norm_img_bytes < need) {
             if (p->d_norm_img) { CK(cudaStreamSynchronize(stream)); CK(cudaFree(p->d_norm_img)); p->d_norm_img = nullptr; p->d_norm_img_bytes = 0; }
             CK(cudaMalloc(&p->d_norm_img, need));
             p->d_norm_img_bytes = need;
         }
-        CK(launch_lighting_tables(p->lighting_rgb, p->d_norm_img, n_all, tail->mean, tail->std, stream));
+        CK(launch_lighting_tables(p->lighting_rgb, p->d_norm_img, q.n_all, tail->mean, tail->std, stream));
         g_launches++;
         P.norm_tab = p->d_norm_img; P.norm_stride = 768;
         s.use_tab = true;
     }
     // fused Mixup mixes the fp32 normalised values before the output rounding: the fma shortcut is only proven to round
     // like the exact value for a DIRECT fp16 / bf16 store, so two-source launches always take the exact table
-    if (d_partner) s.use_tab = true;
-    // Only for tiny images (CIFAR): there the one-block resolve kernel is as long as the pixel kernel; for larger images
-    // every band CTA would repeat the whole serial resolve work.
-    if (!s.use_split && rng && !d_samples && !d_partner && (size_t)h * w <= 4096)
-        return launch_self_resolving(p, P, R, s.use_tab, tail->out_dtype, stream);
+    if (q.partner) s.use_tab = true;
+    if (s.self_resolving) return launch_self_resolving(p, P, R, s.use_tab, tail->out_dtype, stream);
     // resolve-ahead: did the previous call already resolve exactly this batch on the side stream?
-    s.speculate = allow_ahead && rng && !d_samples && !d_partner;
     faa_policy::AheadKey key; memset(&key, 0, sizeof key);
     if (s.speculate) {
-        key.seed = rng->seed; key.first_index = rng->first_index;
-        const int32_t v[16] = {batch, n_all, first, h, w, tail->out_h, tail->out_w, op_base, apply_tail, R.allow, R.split,
-                               rng->crop_pad, rng->hflip, rng->zero_box_len, (s.use_order ? 1 : 0) | (in_mod << 1),
-                               (s.use_chain ? 1 : 0) | (P.norm_stride ? 2 : 0)};
+        key.seed = q.rng->seed; key.first_index = q.rng->first_index;
+        const int32_t v[16] = {batch, q.n_all, q.first, h, w, tail->out_h, tail->out_w, q.op_base, q.apply_tail, R.allow,
+                               R.split, q.rng->crop_pad, q.rng->hflip, q.rng->zero_box_len,
+                               (s.use_order ? 1 : 0) | (q.in_mod << 1), (s.use_chain ? 1 : 0) | (P.norm_stride ? 2 : 0)};
         memcpy(key.v, v, sizeof v);
     }
     s.hit = s.speculate && p->ahead_valid && memcmp(&key, &p->ahead_key, sizeof key) == 0;
@@ -1064,8 +1007,11 @@ int faa_augment(faa_policy_t* p, const uint8_t* d_in, void* d_out, int batch, in
     int apply_tail = (op_base + FAA_MAX_FUSED_OPS >= p->n_op) ? 1 : 0;
     if (!apply_tail && tail && (tail->out_dtype != FAA_U8_HWC || tail->out_h != h || tail->out_w != w))
         return fail(FAA_ERR_VALUE, "intermediate launches of a chained policy must write uint8 HWC at the input size");
-    return augment_common(p, d_in, batch, 0, d_out, batch, h, w, tail, d_samples, d_boxes, rng, op_base, nullptr,
-                          1.0f, 0.0f, apply_tail, p->n_op <= FAA_MAX_FUSED_OPS, stream);
+    AugRequest q;
+    q.in = d_in; q.out = d_out; q.n_all = q.batch = batch; q.h = h; q.w = w; q.tail = tail;
+    q.samples = d_samples; q.boxes = d_boxes; q.rng = rng; q.op_base = op_base; q.apply_tail = apply_tail;
+    q.allow_ahead = p->n_op <= FAA_MAX_FUSED_OPS; q.stream = stream;
+    return augment_common(p, q);
 }
 
 int faa_policy_set_overlap(faa_policy_t* p, int on) {
@@ -1086,14 +1032,16 @@ int faa_augment_many(faa_policy_t* p, int n_steps, const uint8_t* const* d_in, v
     }
     std::lock_guard<std::mutex> call_lk(p->call_mu);
     faa_rng_t r = *rng;
+    AugRequest q;
+    q.n_all = q.batch = batch; q.h = h; q.w = w; q.tail = tail; q.rng = &r; q.allow_ahead = true; q.stream = stream;
     const bool saved = p->overlap_calls;
     int rc = FAA_OK;
     for (int k = 0; k < n_steps && rc == FAA_OK; ++k) {
         // every input exists before this call: steps 2.. may overlap their predecessor; step 1 follows whatever the caller
         // issued before (stream order) unless the caller made the promise for whole calls too
         p->overlap_calls = k > 0 ? true : saved;
-        rc = augment_common(p, d_in[k], batch, 0, d_out[k], batch, h, w, tail, nullptr, nullptr, &r, 0, nullptr,
-                            1.0f, 0.0f, 1, true, stream);
+        q.in = d_in[k]; q.out = d_out[k];
+        rc = augment_common(p, q);
         r.first_index += index_stride;
     }
     p->overlap_calls = saved;
@@ -1109,8 +1057,10 @@ int faa_augment_tta(faa_policy_t* p, const uint8_t* d_in, void* d_out, int batch
     std::lock_guard<std::mutex> call_lk(p->call_mu);
     // one launch over batch * replicas schedule entries; entry v = r * batch + i reads image i and draws the decisions of
     // global sample first_index + v: replica r equals a plain launch with first_index + r * batch
-    return augment_common(p, d_in, batch * replicas, 0, d_out, batch * replicas, h, w, tail, nullptr, nullptr, rng, 0, nullptr,
-                          1.0f, 0.0f, 1, true, stream, replicas > 1 ? batch : 0);
+    AugRequest q;
+    q.in = d_in; q.out = d_out; q.n_all = q.batch = batch * replicas; q.h = h; q.w = w; q.tail = tail; q.rng = rng;
+    q.allow_ahead = true; q.stream = stream; q.in_mod = replicas > 1 ? batch : 0;
+    return augment_common(p, q);
 }
 
 int faa_augment_mixup(faa_policy_t* p, const uint8_t* d_in_all, int n_all, int first, void* d_out, int batch, int h,
@@ -1120,8 +1070,11 @@ int faa_augment_mixup(faa_policy_t* p, const uint8_t* d_in_all, int n_all, int f
     if (p->n_op > FAA_MAX_FUSED_OPS) return fail(FAA_ERR_UNSUPPORTED, "fused mixup supports policies of at most 2 ops");
     if (!(lam >= 0.0f && lam <= 1.0f)) return fail(FAA_ERR_MAGNITUDE, "lam must be in [0, 1]");   // aug_mixup.py:20
     std::lock_guard<std::mutex> call_lk(p->call_mu);
-    return augment_common(p, d_in_all, n_all, first, d_out, batch, h, w, tail, d_samples_all, d_boxes_all, rng, 0,
-                          d_partner, lam, one_minus_lam, 1, false, stream);
+    AugRequest q;
+    q.in = d_in_all; q.out = d_out; q.n_all = n_all; q.first = first; q.batch = batch; q.h = h; q.w = w; q.tail = tail;
+    q.samples = d_samples_all; q.boxes = d_boxes_all; q.rng = rng; q.stream = stream;
+    q.partner = d_partner; q.lam = lam; q.one_minus_lam = one_minus_lam;
+    return augment_common(p, q);
 }
 
 int faa_policy_set_lighting(faa_policy_t* p, const float* d_rgb, int n) {
@@ -1386,13 +1339,15 @@ int faa_augment_host(faa_policy_t* p, const uint8_t* h_in, void* h_out, void* d_
     CK(cudaEventRecord(p->ev_fork, stream));
     CK(cudaStreamWaitEvent(p->side[0], p->ev_fork, 0));
     CK(cudaStreamWaitEvent(p->side[1], p->ev_fork, 0));
+    AugRequest q;
+    q.in = (const uint8_t*)p->d_in; q.n_all = batch; q.h = h; q.w = w; q.tail = tail; q.rng = rng; q.own_stream = false;
     for (int c = 0; c < chunks; ++c) {
         int b0 = (int)((long long)batch * c / chunks), b1 = (int)((long long)batch * (c + 1) / chunks);
         if (b1 <= b0) continue;
         cudaStream_t s = p->side[c & 1];
         CK(cudaMemcpyAsync((uint8_t*)p->d_in + in_img * b0, src + in_img * b0, in_img * (b1 - b0), cudaMemcpyHostToDevice, s));
-        if (int e = augment_common(p, (const uint8_t*)p->d_in, batch, b0, (uint8_t*)d_out + out_img * b0, b1 - b0, h, w,
-                                   tail, nullptr, nullptr, rng, 0, nullptr, 1.0f, 0.0f, 1, false, s, 0, false)) return e;
+        q.out = (uint8_t*)d_out + out_img * b0; q.first = b0; q.batch = b1 - b0; q.stream = s;
+        if (int e = augment_common(p, q)) return e;
         if (dst) CK(cudaMemcpyAsync((uint8_t*)dst + out_img * b0, (uint8_t*)d_out + out_img * b0, out_img * (b1 - b0), cudaMemcpyDeviceToHost, s));
     }
     for (int i = 0; i < 2; ++i) {

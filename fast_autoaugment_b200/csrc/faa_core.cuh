@@ -753,4 +753,167 @@ FAA_HD CropBox philox_crop_box(const CropCfg& c, uint64_t index, int H, int W) {
     return center_crop_box(H, W, c.img_size);
 }
 
+// ------------------------------------------------- launch planner (host only) --
+// Which code each kernel of a policy launch runs, decided from the launch's sizes and buffer addresses alone - no
+// device, no allocation.  faa_cabi.cu launches what plan_launch returns; the host build (tests/emu) exports the same
+// function, so the CPU tests check the launch-geometry case table against the planner itself.
+
+// row-band geometry of a pixel launch, precomputed on the host (no divisions in the kernels)
+struct BandGeom {
+    int32_t bands;              // CTAs per image
+    int32_t band_cap;           // bytes of dynamic shared memory per staged band (0: staging off)
+    int32_t y[9];               // band b owns image rows [y[b], y[b+1]) for whole-image statistics
+    int32_t oy[9];              // ... and output rows [oy[b], oy[b+1])
+    uint32_t lo[8], len[8];     // staged byte range of the raw image per band (len 0: nothing staged)
+};
+
+// the byte range of image rows a CTA may touch through the band-local paths
+inline void band_range(int band, int bands, int H, int W, int out_h, int crop_pad, uint32_t img_bytes, uint32_t& lo,
+                       uint32_t& len) {
+    const int y0 = (int)((uint32_t)(band * H) / (uint32_t)bands), y1 = (int)((uint32_t)((band + 1) * H) / (uint32_t)bands);
+    const int oy0 = (int)((uint32_t)(band * out_h) / (uint32_t)bands), oy1 = (int)((uint32_t)((band + 1) * out_h) / (uint32_t)bands);
+    int r0 = (y0 < oy0 - crop_pad ? y0 : oy0 - crop_pad) - 1;
+    int r1 = (y1 > oy1 + crop_pad ? y1 : oy1 + crop_pad) + 1;
+    if (r0 < 0) r0 = 0;
+    if (r1 > H) r1 = H;
+    if (r1 <= r0) { lo = 0; len = 0; return; }
+    const uint32_t row = (uint32_t)W * 3u;
+    lo = ((uint32_t)r0 * row) & ~15u;
+    uint32_t hi = ((uint32_t)r1 * row + 15u) & ~15u;
+    if (hi > img_bytes) hi = img_bytes;
+    len = hi - lo;
+}
+
+inline int pick_bands(int H, int out_h, int out_w) {
+    // aim for >= ~1024 output quads per CTA; cluster size must be a power of two <= 8
+    long long quads = (long long)out_h * ((out_w + 3) / 4);
+    int b = 1;
+    while (b < 8 && quads / (b * 2) >= 1024 && b * 2 <= H && b * 2 <= out_h) b *= 2;
+    return b;
+}
+
+inline void fill_geom(BandGeom& g, int bands, int H, int W, int out_h, int crop_pad, bool stage) {
+    g = BandGeom{}; g.bands = bands;
+    uint32_t cap = 0;
+    for (int b = 0; b <= bands; ++b) {
+        g.y[b] = (int32_t)((uint32_t)(b * H) / (uint32_t)bands);
+        g.oy[b] = (int32_t)((uint32_t)(b * out_h) / (uint32_t)bands);
+    }
+    for (int b = 0; b < bands && stage; ++b) {
+        band_range(b, bands, H, W, out_h, crop_pad, (uint32_t)H * (uint32_t)W * 3u, g.lo[b], g.len[b]);
+        if (g.len[b] > cap) cap = g.len[b];
+    }
+    g.band_cap = (int32_t)((cap + 127u) & ~127u);
+}
+
+// the largest band of `bands`, rounded up to 128 bytes
+inline uint32_t band_capacity(int bands, int H, int W, int out_h, int crop_pad) {
+    BandGeom g;
+    fill_geom(g, bands, H, W, out_h, crop_pad, true);
+    return (uint32_t)g.band_cap;
+}
+
+// the mid kernel runs enough threads for its band: 512 for the tall bands of large images, 256 otherwise
+inline int mid_kernel_threads(uint32_t band_cap) { return band_cap > 48 * 1024 ? 512 : 256; }
+
+constexpr uint64_t kSplitMin = (uint64_t)4 << 20;     // pixels per launch from which two pixel kernels pay off
+
+struct PlanInput {
+    int32_t H, W, out_h, out_w, batch;
+    int32_t crop_pad;               // the larger of the tail's and the rng's, clamped to H
+    bool out_u8;                    // uint8 HWC output (else fp32 / fp16 / bf16 planes)
+    uint32_t in_mod16, out_mod16;   // the input's and the output's base address mod 16
+    // fused Mixup (a partner image per output); the final window of the policy; some program is Sharpness -> gather
+    bool two_src, apply_tail, has_sg;
+    uint64_t split_min;             // pixels per launch from which the light (+ mid) kernels take part of the work
+    // decisions drawn on the device (else resolved samples); the caller lets the next batch be resolved ahead
+    bool philox, allow_ahead;
+};
+
+struct LaunchPlan {
+    BandGeom geo[2];            // [0] cluster kernel (band_cap 0: no TMA staging), [1] light streaming kernel
+    BandGeom mid;               // the mid kernel's own (taller) bands, when use_mid
+    int32_t mid_threads;        // ... and its threads per CTA
+    bool stage;                 // TMA-stage the cluster kernel's band
+    bool octets;                // the 8-pixel fast paths
+    int32_t mat_cap;            // bytes of the materialisation chunk (0: none)
+    bool use_order;             // the resolve kernel writes a cost-sorted schedule (order / n_heavy)
+    bool use_split;             // the light streaming kernel (and the mid kernel) take the programs they cover
+    bool use_mid;               // three-way split: statistics-LUT and Sharpness programs run in the mid kernel
+    int32_t split;              // ResolveParams::split
+    int32_t allow;              // ResolveParams::allow: bit 0 chunk, bit 1 scratch image, bit 2 lean gathers
+    bool scratch;               // a scratch image per image (Sharpness -> gather)
+    bool no_heavy;              // every program is light or mid: the cluster kernel is not launched
+    bool self_resolving;        // one kernel that draws and builds its programs itself
+    bool use_chain;             // chained schedule (else the event schedule), unless self-resolving
+    bool speculate;             // resolve the next call's batch ahead (resolve-ahead)
+};
+
+inline LaunchPlan plan_launch(const PlanInput& in) {
+    LaunchPlan L = {};
+    const int h = in.H, w = in.W;
+    const bool same_size = in.out_w == w && in.out_h == h;
+    // TMA band staging needs 16-byte aligned image bases and a band that fits shared memory
+    // (crop_pad only sizes the staged band; rows outside it are read from global memory)
+    const int bands = pick_bands(h, in.out_h, in.out_w);
+    const uint32_t cap = band_capacity(bands, h, w, in.out_h, in.crop_pad);
+    L.stage = ((size_t)h * w * 3) % 16 == 0 && in.in_mod16 == 0 && (size_t)cap * (in.two_src ? 2 : 1) <= 150 * 1024;
+    fill_geom(L.geo[0], bands, h, w, in.out_h, in.crop_pad, L.stage);
+    int lb = bands;
+    if (bands == 8) {
+        // the light kernel needs no cluster, so any band count works: take the one in 5..8 whose
+        // quads-per-CTA fills whole 256-thread iterations best (224x224: 7 bands = exactly 7 iterations)
+        const int qpr = (in.out_w + 3) / 4;
+        double best = -1.0;
+        for (int b = 8; b >= 5; --b) {
+            const int rows = (in.out_h + b - 1) / b;
+            const int quads = rows * qpr, iters = (quads + 255) / 256;
+            const double eff = (double)quads / (iters * 256.0) * ((double)in.out_h / (rows * b));
+            if (eff > best + 0.02) { best = eff; lb = b; }
+        }
+    }
+    fill_geom(L.geo[1], lb, h, w, in.out_h, in.crop_pad, L.stage && band_capacity(lb, h, w, in.out_h, in.crop_pad) <= 100 * 1024);
+    L.octets = (w & 7) == 0 && same_size && in.out_mod16 == 0 && L.stage;    // (uint8 HWC included: 24-byte octets)
+    // materialisation chunk: a whole band (+ halo, + crop slack) when that is <= 24 KB, else ~16 KB; >= 3 rows
+    const int pitch = w * 3;
+    const int band_rows = (h + bands - 1) / bands + 2 + 2 * in.crop_pad;
+    int mat_rows = band_rows * pitch <= 24576 ? band_rows : 16384 / pitch;
+    if (mat_rows > h + 2) mat_rows = h + 2;
+    L.mat_cap = (!in.two_src && mat_rows >= 3) ? ((mat_rows * pitch + 32 + 15) & ~15) : 0;   // + 2 guard bands
+    L.use_order = !in.two_src;
+    // (small launches are launch-latency bound: one pixel kernel is faster there; uint8 HWC output - the Mixup exchange
+    //  format - splits when the lean octet paths can write it)
+    L.use_split = L.use_order && (!in.out_u8 || (L.octets && in.crop_pad == 0 && in.apply_tail)) &&
+                  (uint64_t)in.batch * h * w >= in.split_min;
+    // Three-way split: statistics-LUT and Sharpness programs run in the lean mid kernel.
+    // Needs the geometry its paths assume: float planes of the image's own size, no crop, W % 4 == 0, staged bands.
+    L.use_mid = L.use_split && L.stage && (w & 3) == 0 && same_size && in.crop_pad == 0 && in.out_mod16 == 0;
+    L.split = L.use_mid ? 2 : L.use_split ? 1 : 0;
+    if (L.use_mid) {            // halve the band count while a band (+ halo) stays <= 80 KB (2 CTAs / SM)
+        int mb = bands;
+        while (mb > 1 && band_capacity(mb / 2, h, w, in.out_h, 0) <= 80 * 1024) mb /= 2;
+        fill_geom(L.mid, mb, h, w, in.out_h, 0, true);
+        L.mid_threads = mid_kernel_threads((uint32_t)L.mid.band_cap);
+    }
+    // scratch images: Sharpness -> gather programs of the cluster kernel, every Sharpness-first two-op program of the mid
+    // kernel
+    L.scratch = (in.has_sg || L.use_mid) && !in.two_src && (w & 3) == 0;
+    // allow bit 0: the chunk, bit 1: a scratch image, bit 2: the lean gather paths exist in this launch
+    L.allow = (L.mat_cap > 0 ? 1 : 0) | (L.scratch ? 2 : 0) | (L.use_split && L.octets && in.crop_pad == 0 ? 4 : 0);
+    // With the lean gathers (allow bit 2) and a scratch image (bit 1) every program of a three-way split is light or mid
+    // (prog_is_light / prog_is_mid cover all class combinations; tests/test_gpu_fastpaths.py runs every ordered op pair
+    // through this schedule): the cluster kernel has nothing to do and is not launched.
+    L.no_heavy = L.use_mid && (L.allow & 6) == 6 && L.mat_cap > 0;
+    const bool ahead = in.philox && !in.two_src;
+    // Only for tiny images (CIFAR): there the one-block resolve kernel is as long as the pixel kernel; for larger images
+    // every band CTA would repeat the whole serial resolve work.
+    L.self_resolving = !L.use_split && ahead && (size_t)h * w <= 4096;
+    // Chained steps need the Philox sampler on the device and a caller that allows the next batch to be resolved ahead.
+    // Launches too small to split are chained as well (resolve(N+1), cluster(N)): their step is bound by kernel latencies,
+    // which only overlap across steps on one stream; uint8 output of one pixel kernel stays on the event schedule.
+    L.use_chain = (L.use_split || !in.out_u8) && in.allow_ahead && ahead;
+    L.speculate = in.allow_ahead && ahead;
+    return L;
+}
+
 }  // namespace faa

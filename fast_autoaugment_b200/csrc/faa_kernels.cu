@@ -220,23 +220,6 @@ __device__ __forceinline__ void count_done(uint32_t* done) {
     if (threadIdx.x == 0) asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(done) : "memory");
 }
 
-// the byte range of image rows a CTA may touch through the band-local paths
-__host__ __device__ inline void band_range(int band, int bands, int H, int W, int out_h, int crop_pad,
-                                            uint32_t img_bytes, uint32_t& lo, uint32_t& len) {
-    const int y0 = (int)((uint32_t)(band * H) / (uint32_t)bands), y1 = (int)((uint32_t)((band + 1) * H) / (uint32_t)bands);
-    const int oy0 = (int)((uint32_t)(band * out_h) / (uint32_t)bands), oy1 = (int)((uint32_t)((band + 1) * out_h) / (uint32_t)bands);
-    int r0 = (y0 < oy0 - crop_pad ? y0 : oy0 - crop_pad) - 1;
-    int r1 = (y1 > oy1 + crop_pad ? y1 : oy1 + crop_pad) + 1;
-    if (r0 < 0) r0 = 0;
-    if (r1 > H) r1 = H;
-    if (r1 <= r0) { lo = 0; len = 0; return; }
-    const uint32_t row = (uint32_t)W * 3u;
-    lo = ((uint32_t)r0 * row) & ~15u;
-    uint32_t hi = ((uint32_t)r1 * row + 15u) & ~15u;
-    if (hi > img_bytes) hi = img_bytes;
-    len = hi - lo;
-}
-
 // ---------------------------------------------------------------------------------------
 __device__ __forceinline__ Ctx make_ctx(const AugParams& P, const uint8_t* raw, const uint8_t* sraw, uint32_t s_lo, uint32_t s_len,
                                         int H, int W, const ImgState& st, bool full) {
@@ -2271,40 +2254,6 @@ cudaError_t launch_mix_u8(const uint8_t* a, const uint8_t* b, const int32_t* par
     return cudaGetLastError();
 }
 
-// ---------------------------------------------------------------------------------------
-int pick_bands(int H, int W, int out_h, int out_w) {
-    // aim for >= ~1024 output quads per CTA; cluster size must be a power of two <= 8
-    long long quads = (long long)out_h * ((out_w + 3) / 4);
-    int b = 1;
-    while (b < 8 && quads / (b * 2) >= 1024 && b * 2 <= H && b * 2 <= out_h) b *= 2;
-    return b;
-}
-
-void fill_geom(BandGeom& g, int bands, int H, int W, int out_h, int crop_pad, bool stage) {
-    memset(&g, 0, sizeof g);
-    g.bands = bands;
-    uint32_t cap = 0;
-    for (int b = 0; b <= bands; ++b) {
-        g.y[b] = (int32_t)((uint32_t)(b * H) / (uint32_t)bands);
-        g.oy[b] = (int32_t)((uint32_t)(b * out_h) / (uint32_t)bands);
-    }
-    for (int b = 0; b < bands && stage; ++b) {
-        band_range(b, bands, H, W, out_h, crop_pad, (uint32_t)H * (uint32_t)W * 3u, g.lo[b], g.len[b]);
-        if (g.len[b] > cap) cap = g.len[b];
-    }
-    g.band_cap = (int32_t)((cap + 127u) & ~127u);
-}
-
-uint32_t band_capacity(int bands, int H, int W, int out_h, int crop_pad) {
-    uint32_t cap = 0;
-    for (int b = 0; b < bands; ++b) {
-        uint32_t lo, len;
-        band_range(b, bands, H, W, out_h, crop_pad, (uint32_t)H * (uint32_t)W * 3u, lo, len);
-        if (len > cap) cap = len;
-    }
-    return (cap + 127u) & ~127u;
-}
-
 #endif  // !FAA_TU_OUT
 
 // raise Kernel's dynamic shared memory limit to `dyn` bytes on the current device if it is below that
@@ -2367,10 +2316,8 @@ static cudaError_t launch_mid(const AugParams& p, cudaStream_t stream) {
     const size_t dyn = (size_t)p.geo[0].band_cap;
     if (cudaError_t e = reserve_dyn_smem<faa_augment_mid_kernel<OUT, TAB>>(dyn)) return e;
     cudaLaunchConfig_t cfg = {};
-    // enough threads for the band: 512 for the tall bands of large images, 256 otherwise
-    const int threads = dyn > 48 * 1024 ? 512 : 256;
     cfg.gridDim = dim3((unsigned)p.bands, (unsigned)rows_of(p), 1);
-    cfg.blockDim = dim3((unsigned)threads, 1, 1);
+    cfg.blockDim = dim3((unsigned)mid_kernel_threads((uint32_t)dyn), 1, 1);
     cfg.dynamicSmemBytes = dyn;
     cfg.stream = stream;
     cudaLaunchAttribute attr[2];

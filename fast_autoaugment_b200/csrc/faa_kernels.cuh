@@ -32,15 +32,6 @@ struct ResolveParams {
 };
 cudaError_t launch_resolve(const ResolveParams& p, cudaStream_t stream);
 
-// row-band geometry of a pixel launch, precomputed on the host (no divisions in the kernels)
-struct BandGeom {
-    int32_t bands;              // CTAs per image
-    int32_t band_cap;           // bytes of dynamic shared memory per staged band (0: staging off)
-    int32_t y[9];               // band b owns image rows [y[b], y[b+1]) for whole-image statistics
-    int32_t oy[9];              // ... and output rows [oy[b], oy[b+1])
-    uint32_t lo[8], len[8];     // staged byte range of the raw image per band (len 0: nothing staged)
-};
-
 // AugParams::chain: how a pixel launch is ordered against the kernel in front of it in its stream
 enum ChainMode : int32_t {
     CHAIN_STREAM_ORDERED = 0,   // griddepcontrol.wait before the schedule is read (or no programmatic launch at all)
@@ -112,9 +103,5 @@ cudaError_t launch_crop_resize(const uint8_t* in, void* out, int batch, int H, i
                                const float mean[3], const float std[3], const CropBox* boxes, const CropCfg& cfg,
                                const CropResizeTile& t, cudaStream_t stream);
 cudaError_t launch_lighting_tables(const float* rgb, float* tabs, int n, const float mean[3], const float std[3], cudaStream_t stream);
-
-int pick_bands(int H, int W, int out_h, int out_w);
-void fill_geom(BandGeom& g, int bands, int H, int W, int out_h, int crop_pad, bool stage);
-uint32_t band_capacity(int bands, int H, int W, int out_h, int crop_pad);
 
 }  // namespace faa

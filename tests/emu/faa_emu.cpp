@@ -255,7 +255,7 @@ int faa_emu_classes(const void* ops_v, int n_op, const void* samples_v, const vo
 }
 
 // weight class of every image's program in a three-way split launch (faa_resolve_kernel): 2 light, 1 mid, 0 heavy.
-// `allow`: bit 0 materialisation chunk, bit 1 scratch image, bit 2 lean octet gathers (faa_cabi.cu sets 7 for the
+// `allow`: bit 0 materialisation chunk, bit 1 scratch image, bit 2 lean octet gathers (plan_launch sets 7 for the
 // headline geometry and then does NOT launch the cluster kernel: no program may be heavy)
 int faa_emu_weight_classes(const void* ops_v, int n_op, const void* samples_v, const void* boxes_v, int B, int H, int W,
                            int out_w, int apply_tail, int allow, uint8_t* wc_out, uint8_t* cls_out) {
@@ -283,6 +283,25 @@ int faa_emu_philox(const void* ops_v, const double* probs, int n_sub, int n_op, 
         for (int j = 0; j < n_op; ++j) boxes[(size_t)i * n_op + j] = bx[j];
     }
     return 0;
+}
+
+// The launch planner's decisions (plan_launch) as int32 values, in the order faa_emu_plan_fields names them; returns
+// their count.  split_min < 0: the library's default.
+const char* faa_emu_plan_fields() {
+    return "bands band_cap stage light_bands light_staged octets mat_cap use_order use_split use_mid split mid_bands "
+           "mid_threads allow scratch no_heavy self_resolving use_chain speculate";
+}
+
+int faa_emu_plan(int H, int W, int out_h, int out_w, int batch, int crop_pad, int out_u8, int in_mod16, int out_mod16,
+                 int two_src, int apply_tail, int has_sg, long long split_min, int philox, int allow_ahead, int32_t* out) {
+    const LaunchPlan L = plan_launch({H, W, out_h, out_w, batch, crop_pad, out_u8 != 0, (uint32_t)in_mod16,
+                                      (uint32_t)out_mod16, two_src != 0, apply_tail != 0, has_sg != 0,
+                                      split_min < 0 ? kSplitMin : (uint64_t)split_min, philox != 0, allow_ahead != 0});
+    const int32_t v[] = {L.geo[0].bands, L.geo[0].band_cap, L.stage, L.geo[1].bands, L.geo[1].band_cap > 0, L.octets,
+                         L.mat_cap, L.use_order, L.use_split, L.use_mid, L.split, L.mid.bands, L.mid_threads, L.allow,
+                         L.scratch, L.no_heavy, L.self_resolving, L.use_chain, L.speculate};
+    memcpy(out, v, sizeof v);
+    return (int)(sizeof v / sizeof v[0]);
 }
 
 // raw Philox4x32-10 block, for the known-answer test

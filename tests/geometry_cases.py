@@ -1,131 +1,57 @@
-"""Launch geometries of the policy kernels: one case per planner regime, and a restatement of the planner.
+"""Launch geometries of the policy kernels: one case per planner regime.
 
-`augment_common` (csrc/faa_cabi.cu) picks, separately for each kernel of a launch, which code runs: whether the band
-is staged into shared memory by TMA, whether the light kernel's (narrower) band is, whether the materialisation chunk
-exists, whether the octet paths and the lean gathers exist, whether the mid kernel runs and with which bands, and
-whether the cluster kernel is launched at all (`no_heavy`).  Those choices depend on the image size and on the buffers'
-addresses, so every regime is a separate thing to test.
+The launch planner (`plan_launch`, csrc/faa_core.cuh) picks, separately for each kernel of a launch, which code runs:
+whether the band is staged into shared memory by TMA, whether the light kernel's (narrower) band is, whether the
+materialisation chunk exists, whether the octet paths and the lean gathers exist, whether the mid kernel runs and with
+which bands, and whether the cluster kernel is launched at all (`no_heavy`).  Those choices depend on the image size
+and on the buffers' addresses, so every regime is a separate thing to test.
 
-`plan()` below is a RESTATEMENT of those decisions in Python, written from the C++ and citing it; it is not shared
-with the library.  tests/test_geometry_plan.py checks that every case of CASES is in the regime it claims and that
-every regime has a case; tests/test_gpu_geometries.py runs every case on the device against the oracle and asserts
-the planner's launch count, which cross-checks this restatement against the real planner.
+`plan()` below asks the planner itself, through the host build of faa_core.cuh (tests/emu).
+tests/test_geometry_plan.py checks that every case of CASES is in the regime it claims and that every regime has a
+case; tests/test_gpu_geometries.py runs every case on the device against the oracle and asserts the launch count.
 """
+import ctypes as C
 from dataclasses import dataclass
-
-SPLIT_MIN = 4 << 20            # faa_cabi.cu:968: pixels per launch from which the split kernels run
-
-
-# ---- csrc/faa_kernels.cu:2271-2302 and :224-238 ------------------------------------------------------------------
-def pick_bands(H, W, out_h, out_w):
-    """faa_kernels.cu:2271: >= ~1024 output quads per CTA, a power of two <= 8"""
-    quads = out_h * ((out_w + 3) // 4)
-    b = 1
-    while b < 8 and quads // (b * 2) >= 1024 and b * 2 <= H and b * 2 <= out_h:
-        b *= 2
-    return b
-
-
-def band_range(band, bands, H, W, out_h, crop_pad):
-    """faa_kernels.cu:224: byte range [lo, lo + len) of the rows band `band` may touch"""
-    img_bytes = H * W * 3
-    y0, y1 = band * H // bands, (band + 1) * H // bands
-    oy0, oy1 = band * out_h // bands, (band + 1) * out_h // bands
-    r0 = min(y0, oy0 - crop_pad) - 1
-    r1 = max(y1, oy1 + crop_pad) + 1
-    r0, r1 = max(r0, 0), min(r1, H)
-    if r1 <= r0:
-        return 0, 0
-    row = W * 3
-    lo = (r0 * row) & ~15
-    hi = min((r1 * row + 15) & ~15, img_bytes)
-    return lo, hi - lo
-
-
-def band_capacity(bands, H, W, out_h, crop_pad):
-    """faa_kernels.cu:2294: the largest band, rounded up to 128 bytes"""
-    cap = max(band_range(b, bands, H, W, out_h, crop_pad)[1] for b in range(bands))
-    return (cap + 127) & ~127
-
-
-def light_bands(bands, out_h, out_w):
-    """faa_cabi.cu:926-938: the light kernel takes the band count in 5..8 that fills 256-thread iterations best"""
-    if bands != 8:
-        return bands
-    qpr = (out_w + 3) // 4
-    best, lb = -1.0, bands
-    for b in range(8, 4, -1):
-        rows = (out_h + b - 1) // b
-        quads = rows * qpr
-        iters = (quads + 255) // 256
-        eff = quads / (iters * 256.0) * (out_h / (rows * b))
-        if eff > best + 0.02:
-            best, lb = eff, b
-    return lb
 
 
 @dataclass
 class Plan:
     W: int
     bands: int
-    stage: bool               # :922 TMA staging of the cluster kernel's band
-    stage_off: str            # why not: "size" (H*W*3 % 16), "base" (input address), "band" (> 150 KB), "" if staged
+    stage: bool               # TMA staging of the cluster kernel's band
+    stage_off: str            # why not: "size" (H*W*3 % 16), "base" (input address), "band" (too large), "" if staged
     light_bands: int
-    light_staged: bool        # :939 the light kernel's band is staged (<= 100 KB)
-    octets: bool              # :943 the 8-pixel paths
-    mat: bool                 # :947-954 the materialisation chunk (>= 3 rows)
-    split: bool               # :971 light (+ mid) kernels take the programs they cover
-    use_mid: bool             # :980 the mid kernel runs
-    mid_bands: int            # :632 mid_params
-    mid_threads: int          # faa_kernels.cu:2367: 512 threads when a mid band is > 48 KB
-    no_heavy: bool            # :1000 the cluster kernel is not launched
+    light_staged: bool        # the light kernel's band is staged
+    octets: bool              # the 8-pixel paths
+    mat: bool                 # the materialisation chunk (>= 3 rows)
+    split: bool               # light (+ mid) kernels take the programs they cover
+    use_mid: bool             # the mid kernel runs
+    mid_bands: int
+    mid_threads: int
+    no_heavy: bool            # the cluster kernel is not launched
     allow: int                # resolve-kernel allow bits: 1 chunk, 2 scratch, 4 lean gathers
 
     def launches(self):
-        """kernels of one call on resolved records (event schedule, faa_cabi.cu:795-861): the resolve kernel, then
+        """kernels of one call on resolved records (event schedule, faa_cabi.cu launch_event): the resolve kernel, then
         either the cluster kernel alone or light + (mid) + (cluster unless no_heavy)"""
         if not self.split:
             return 2
         return 2 + int(self.use_mid) + int(not self.no_heavy)
 
 
-def plan(H, W, batch, u8=False, in_off=0, out_off=0, split_min=SPLIT_MIN, has_sg=True):
-    """faa_cabi.cu:906-1000 for a single-source launch of the image's own size, no crop, final window (apply_tail),
-    input and output at `in_off` / `out_off` bytes from a 256-byte aligned allocation"""
-    out_h, out_w, crop_pad = H, W, 0
-    bands = pick_bands(H, W, out_h, out_w)
-    cap = band_capacity(bands, H, W, out_h, crop_pad)
-    if (H * W * 3) % 16:
-        stage_off = "size"
-    elif in_off % 16:
-        stage_off = "base"
-    elif cap > 150 * 1024:
-        stage_off = "band"
-    else:
-        stage_off = ""
-    stage = stage_off == ""
-    lb = light_bands(bands, out_h, out_w)
-    light_staged = stage and band_capacity(lb, H, W, out_h, crop_pad) <= 100 * 1024
-    octets = W % 8 == 0 and out_off % 16 == 0 and stage
-    pitch = W * 3
-    band_rows = (H + bands - 1) // bands + 2 + 2 * crop_pad
-    rows = band_rows if band_rows * pitch <= 24576 else 16384 // pitch
-    rows = min(rows, H + 2)
-    mat = rows >= 3
-    allow = 1 if mat else 0
-    split = (not u8 or octets) and batch * H * W >= split_min
-    use_mid = split and stage and W % 4 == 0 and out_off % 16 == 0
-    if split and octets:
-        allow |= 4
-    if (has_sg or use_mid) and W % 4 == 0:
-        allow |= 2
-    no_heavy = use_mid and (allow & 6) == 6 and mat
-    mb = bands
-    while mb > 1 and band_capacity(mb // 2, H, W, out_h, 0) <= 80 * 1024:
-        mb //= 2
-    mid_threads = 512 if band_capacity(mb, H, W, out_h, 0) > 48 * 1024 else 256
-    return Plan(W, bands, stage, stage_off, lb, light_staged, octets, mat, split, use_mid, mb if use_mid else 0,
-                mid_threads if use_mid else 0, no_heavy, allow)
+def plan(emu, H, W, batch, u8=False, in_off=0, out_off=0, split_min=-1, has_sg=True):
+    """the planner's decisions for a single-source launch on resolved records, of the image's own size, no crop, final
+    window (apply_tail), input and output at `in_off` / `out_off` bytes from a 256-byte aligned allocation
+    (split_min -1: the library's default)"""
+    names = emu.faa_emu_plan_fields().decode().split()
+    out = (C.c_int32 * len(names))()
+    assert emu.faa_emu_plan(H, W, H, W, batch, 0, int(u8), in_off % 16, out_off % 16, 0, 1, int(has_sg), split_min, 0, 0,
+                            out) == len(names)
+    d = dict(zip(names, out))
+    stage_off = "" if d["stage"] else "size" if (H * W * 3) % 16 else "base" if in_off % 16 else "band"
+    return Plan(W, d["bands"], bool(d["stage"]), stage_off, d["light_bands"], bool(d["light_staged"]), bool(d["octets"]),
+                d["mat_cap"] > 0, bool(d["use_split"]), bool(d["use_mid"]), d["mid_bands"], d["mid_threads"],
+                bool(d["no_heavy"]), d["allow"])
 
 
 def regime(p: Plan):

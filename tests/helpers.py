@@ -173,6 +173,8 @@ def set_emu_sigs(emu):
     emu.faa_emu_philox.restype = C.c_int
     emu.faa_emu_philox_block.argtypes = [vp, vp, vp]
     emu.faa_emu_philox_block.restype = None
+    emu.faa_emu_plan_fields.restype = C.c_char_p
+    emu.faa_emu_plan.argtypes = [C.c_int] * 12 + [C.c_longlong, C.c_int, C.c_int, vp]     # returns the field count
     return emu
 
 

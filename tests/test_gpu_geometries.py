@@ -112,8 +112,8 @@ def _bad(got, want):
 class _Run:
     """all output types of one case through both launch paths, against one uint8 reference"""
 
-    def __init__(self, case, pol, x, samples, boxes, want_u8, monkeypatch):
-        self.case, self.pol, self.x, self.samples, self.boxes = case, pol, x, samples, boxes
+    def __init__(self, emu, case, pol, x, samples, boxes, want_u8, monkeypatch):
+        self.emu, self.case, self.pol, self.x, self.samples, self.boxes = emu, case, pol, x, samples, boxes
         self.want_u8 = want_u8                                          # [n, H, W, 3] uint8 on the device
         self.mp = monkeypatch
         tab = torch.from_numpy(exact_norm_table(MEAN, STD)).cuda()
@@ -126,7 +126,7 @@ class _Run:
         if path == "cluster":
             return 2
         if u8:           # uint8 output splits only through the octet paths
-            return G.plan(H, W, n, u8=True, in_off=self.case.in_off, split_min=0).launches()
+            return G.plan(self.emu, H, W, n, u8=True, in_off=self.case.in_off, split_min=0).launches()
         return self.case.launches
 
     def call(self, path, tail, samples, out=None):
@@ -185,7 +185,7 @@ def _dtypes(case):
 
 
 @pytest.mark.parametrize("case", [c for c in G.CASES if not c.big], ids=lambda c: c.id)
-def test_policy_kernels_match_the_oracle(case, monkeypatch):
+def test_policy_kernels_match_the_oracle(case, emu, monkeypatch):
     H, W = case.shape
     policies = _policies()
     n = len(policies)
@@ -194,7 +194,7 @@ def test_policy_kernels_match_the_oracle(case, monkeypatch):
     want_u8 = torch.from_numpy(np.stack([want[i] for i in range(n)])).cuda()
     x = _device_input(batch, case.in_off)
     del batch, want
-    run = _Run(case, CompiledPolicy(policies), x, samples, boxes, want_u8, monkeypatch)
+    run = _Run(emu, case, CompiledPolicy(policies), x, samples, boxes, want_u8, monkeypatch)
     run.check(_dtypes(case), cutout=not case.out_off, u8=not case.out_off)
 
 
@@ -217,12 +217,12 @@ def test_policy_kernels_match_the_host_build_at_large_sizes(case, emu, monkeypat
         assert np.array_equal(ref[i].numpy(), oracle[i]), (case.id, i, policies[i])
     x = _device_input(batch, case.in_off)
     del batch
-    run = _Run(case, pol, x, samples, boxes, ref.cuda(), monkeypatch)
+    run = _Run(emu, case, pol, x, samples, boxes, ref.cuda(), monkeypatch)
     limit = case.shape in G.LIMIT_SHAPES
     run.check((torch.float16,) if limit else _dtypes(case), cutout=not limit)
 
 
-def test_statistics_ops_over_67_million_pixels(monkeypatch):
+def test_statistics_ops_over_67_million_pixels(emu, monkeypatch):
     """four 8192 x 8192 images (the header's limit) per launch, single ops: the histogram and luma-sum ops on ramp and
     constant images put 67 M pixels into one histogram; uint8 and fp16 output against the oracle"""
     H = W = 8192
@@ -234,7 +234,7 @@ def test_statistics_ops_over_67_million_pixels(monkeypatch):
         samples, boxes, want = _records(policies, batch, range(4))
         want_u8 = torch.from_numpy(np.stack([want[i] for i in range(4)])).cuda()
         del want
-        run = _Run(case, CompiledPolicy(policies), torch.from_numpy(batch).cuda(), samples, boxes, want_u8, monkeypatch)
+        run = _Run(emu, case, CompiledPolicy(policies), torch.from_numpy(batch).cuda(), samples, boxes, want_u8, monkeypatch)
         run.check((torch.float16,), cutout=False)
         del run, want_u8
         torch.cuda.empty_cache()
@@ -254,7 +254,7 @@ def test_production_philox_calls_back_to_back(shape, B, dtype, emu, monkeypatch)
     xs = [synth_batch(B, shape, seed=40 + k) for k in range(3)]
     xd = [torch.from_numpy(x).cuda() for x in xs]
     outs = [aug.empty_out(B) for _ in range(3)]
-    pixel = G.plan(H, W, B, u8=dtype == torch.uint8).launches() - 1    # pixel kernels per call
+    pixel = G.plan(emu, H, W, B, u8=dtype == torch.uint8).launches() - 1    # pixel kernels per call
     counts = []
     for k in range(3):
         n0 = _launches()

@@ -1,4 +1,4 @@
-"""The three-way split never launches the cluster kernel for the headline geometry (faa_cabi.cu: `no_heavy`), so the
+"""The three-way split never launches the cluster kernel for the headline geometry (faa_core.cuh: `no_heavy`), so the
 program builder must sort EVERY program into the light or the mid kernel there - a heavy program would simply not be
 written.  Checked on the host through the emulation build of faa_core.cuh (the same source the resolve kernel compiles):
 every single op and every ordered op pair, every gate / sign combination, with and without Cutout boxes and flips - at
@@ -6,6 +6,7 @@ every image size of tests/geometry_cases.py where the planner sets `no_heavy` (c
 import ctypes as C
 import itertools
 import random
+import re
 
 import numpy as np
 import pytest
@@ -30,9 +31,9 @@ def _classes(emu, pol, samples, boxes, H, W, allow):
     return wc, cls
 
 
-# the image sizes of tests/geometry_cases.py where the planner sets `no_heavy`, besides the headline 224 x 224
-_LEAN_SHAPES = sorted({c.shape for c in G.CASES
-                       if G.plan(*c.shape, 64, in_off=c.in_off, out_off=c.out_off, split_min=0).no_heavy})
+# the image sizes of tests/geometry_cases.py where the planner sets `no_heavy` (the regimes with a mid kernel and no
+# cluster kernel), besides the headline 224 x 224
+_LEAN_SHAPES = sorted({c.shape for c in G.CASES if re.search(r"mid \d+ bands", c.regime) and "cluster kernel" not in c.regime})
 
 
 def _check_lean(emu, H, W):
@@ -62,10 +63,13 @@ def test_every_program_is_light_or_mid_in_a_lean_launch(emu):
     _check_lean(emu, 224, 224)
 
 
-def test_the_lean_shapes_are_the_no_heavy_cases():
+def test_the_lean_shapes_are_the_no_heavy_cases(emu):
     assert len(_LEAN_SHAPES) >= 8 and (8192, 8) in _LEAN_SHAPES and (600, 600) in _LEAN_SHAPES
+    no_heavy = {c.shape for c in G.CASES
+                if G.plan(emu, *c.shape, 64, in_off=c.in_off, out_off=c.out_off, split_min=0).no_heavy}
+    assert no_heavy == set(_LEAN_SHAPES), {"missing": no_heavy - set(_LEAN_SHAPES), "extra": set(_LEAN_SHAPES) - no_heavy}
     for shape in [(224, 224)] + _LEAN_SHAPES:
-        p = G.plan(*shape, 512 if shape == (224, 224) else 64, split_min=0)
+        p = G.plan(emu, *shape, 512 if shape == (224, 224) else 64, split_min=0)
         assert p.no_heavy and p.allow == 7, (shape, p)
 
 
