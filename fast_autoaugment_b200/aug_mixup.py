@@ -18,7 +18,11 @@ _DT = {torch.float16: _lib.F16, torch.bfloat16: _lib.BF16, torch.float32: _lib.F
 
 
 def mixup_resolved(data: torch.Tensor, indices: torch.Tensor, lam: float, out=None):
-    """``data*lam + data[indices]*(1-lam)`` (reference aug_mixup.py:21) on a CUDA tensor."""
+    """``data*lam + data[indices]*(1-lam)`` (reference aug_mixup.py:21) on a CUDA tensor.
+
+    ``out`` (optional) must not overlap ``data``: mixing in place would let one sample be overwritten while another
+    still reads it as its partner, so an overlapping ``out`` raises ``ValueError`` before anything is launched.  At
+    most 65535 samples per call."""
     if not data.is_cuda:
         raise _lib.FaaRuntimeError("mixup needs a CUDA tensor (no CPU fallback)")
     if data.dtype not in _DT:
@@ -28,6 +32,8 @@ def mixup_resolved(data: torch.Tensor, indices: torch.Tensor, lam: float, out=No
     n_per = data.numel() // max(b, 1)
     if out is None:
         out = torch.empty_like(data)
+    elif out.shape != data.shape or out.dtype != data.dtype or out.device != data.device or not out.is_contiguous():
+        raise ValueError("out must be a contiguous tensor of data's shape, dtype and device")
     perm = indices.to(device=data.device, dtype=torch.int64).contiguous()
     with torch.cuda.device(data.device):
         stream = C.c_void_p(torch.cuda.current_stream(data.device).cuda_stream)

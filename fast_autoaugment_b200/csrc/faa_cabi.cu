@@ -1254,6 +1254,12 @@ int faa_mixup(const void* d_data, void* d_out, const int64_t* d_perm, int batch,
     if (batch < 0 || n_per_sample < 0) return fail(FAA_ERR_VALUE, "negative size");
     if (dtype < 0 || dtype > FAA_F32) return fail(FAA_ERR_VALUE, "bad dtype");
     if (int e = ensure_device()) return e;
+    if (batch > 65535) return fail(FAA_ERR_UNSUPPORTED, "at most 65535 images per call (one grid row per image): split the batch");
+    // a CTA may still be reading a sample as another CTA's partner when its own output is written: no in-place mixing
+    const uintptr_t bytes = (uintptr_t)batch * (uintptr_t)n_per_sample * (dtype == FAA_F32 ? 4u : 2u);
+    const uintptr_t lo_in = (uintptr_t)d_data, lo_out = (uintptr_t)d_out;
+    if (bytes > 0 && lo_out < lo_in + bytes && lo_in < lo_out + bytes)
+        return fail(FAA_ERR_VALUE, "out overlaps data: a sample would be overwritten while another reads it as its partner");
     CK(launch_mixup(d_data, d_out, d_perm, batch, n_per_sample, dtype, lam, one_minus_lam, (cudaStream_t)stream));
     if (batch > 0 && n_per_sample > 0) g_launches++;
     return FAA_OK;

@@ -199,7 +199,9 @@ int faa_augment_host(faa_policy_t* p, const uint8_t* h_in, void* h_out, void* d_
 
 /* ---- standalone Mixup on already-augmented device tensors: replaces mixup()
  *      (aug_mixup.py:13-23) given the resolved permutation and lambda.
- *      out[i] = data[i]*lam + data[perm[i]]*(1-lam), fp32 math, n_per_sample elements each. */
+ *      out[i] = data[i]*lam + data[perm[i]]*(1-lam), fp32 math, n_per_sample elements each.
+ *      d_out must not overlap d_data (FAA_ERR_VALUE: a sample would be overwritten while another
+ *      reads it as its partner); batch <= 65535 (FAA_ERR_UNSUPPORTED). */
 int faa_mixup(const void* d_data, void* d_out, const int64_t* d_perm, int batch,
               int64_t n_per_sample, int dtype, float lam, float one_minus_lam, void* stream);
 

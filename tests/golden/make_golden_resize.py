@@ -11,6 +11,9 @@ Imports the reference read-only like make_golden.py and writes only golden_resiz
 * ``test_<H>x<W>`` / ``train_<H>x<W>`` (+ ``in_<H>x<W>``, digests of the inputs ``chain_input`` regenerates): per-image sha256 digests (first 16 hex digits) of the fp32 output of
   the reference ``transform_test`` and ``transform_train`` with ``fa_resnet50_rimagenet`` (data.py:60-80, 94-95) on
   seeded inputs, under ``random.seed / np.random.seed / torch.manual_seed(3)``, one image after another.
+* ``test_s<s>_<H>x<W>`` / ``train_s<s>_<H>x<W>`` (+ ``in_s<s>_<H>x<W>``): the same digests for the EfficientNet input
+  sizes ``EFFNET_CHAIN_CASES`` (data.py:53-55): ``EfficientNetRandomCrop(s)`` / ``EfficientNetCenterCrop(s)`` and
+  ``Resize((s, s))``, inputs from ``np.random.default_rng(s)``.
 
 Environment that produced the committed file: Pillow 12.2.0, numpy 2.3.5, torch 2.11.0, torchvision 0.26.0.
 """
@@ -28,6 +31,7 @@ BOX_CASES = ((224, 375, 500), (224, 256, 256), (224, 333, 500), (380, 500, 375),
              (224, 3, 4), (224, 2, 2))        # (tiny images: whole-image and failed-attempt fallbacks)
 N_BOXES = 200
 CHAIN_CASES = ((256, 256, 64), (375, 500, 32))
+EFFNET_CHAIN_CASES = ((380, 375, 500, 8), (600, 375, 500, 8))      # (s, H, W, N)
 
 
 def coord_image(h, w):
@@ -44,6 +48,32 @@ def chain_input(rng, i, h, w):
 
 def digest(a) -> str:
     return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()[:16]
+
+
+def effnet_chain_inputs(s, h, w, n):
+    rng = np.random.default_rng(s)
+    return np.stack([chain_input(rng, i, h, w) for i in range(n)])
+
+
+def reference_transforms(aug, archive, data, s):
+    """the reference's transform_train / transform_test at input size s, as data.py:60-80 and 94-95 build them"""
+    from torchvision.transforms import transforms as T
+    norm = T.Normalize(mean=[0.485, 0.456, 0.406], std=[0.229, 0.224, 0.225])
+    train = T.Compose([
+        data.EfficientNetRandomCrop(s), T.Resize((s, s), interpolation=PIL.Image.BICUBIC), T.RandomHorizontalFlip(),
+        T.ColorJitter(brightness=0.4, contrast=0.4, saturation=0.4), T.ToTensor(),
+        aug.Lighting(0.1, data._IMAGENET_PCA["eigval"], data._IMAGENET_PCA["eigvec"]), norm])
+    train.transforms.insert(0, data.Augmentation(archive.fa_resnet50_rimagenet()))
+    test = T.Compose([data.EfficientNetCenterCrop(s), T.Resize((s, s), interpolation=PIL.Image.BICUBIC), T.ToTensor(), norm])
+    return {"train": train, "test": test}
+
+
+def chain_digests(tf, batch):
+    """digests of tf on each image, under the seeds of the committed digests, one image after another"""
+    random.seed(3)
+    np.random.seed(3)
+    torch.manual_seed(3)
+    return np.array([digest(tf(PIL.Image.fromarray(a)).numpy()) for a in batch])
 
 
 def main(ref):
@@ -81,6 +111,12 @@ def main(ref):
             np.random.seed(3)
             torch.manual_seed(3)
             out["%s_%s" % (name, tag)] = np.array([digest(tf(PIL.Image.fromarray(a)).numpy()) for a in batch])
+    for s, h, w, n in EFFNET_CHAIN_CASES:
+        tag = "s%d_%dx%d" % (s, h, w)
+        batch = effnet_chain_inputs(s, h, w, n)
+        out["in_" + tag] = np.array([digest(a) for a in batch])
+        for name, tf in reference_transforms(aug, archive, data, s).items():
+            out["%s_%s" % (name, tag)] = chain_digests(tf, batch)
     np.savez_compressed(os.path.join(HERE, "golden_resize.npz"), **out)
     print("wrote golden_resize.npz:", os.path.getsize(os.path.join(HERE, "golden_resize.npz")), "bytes")
 
