@@ -9,9 +9,15 @@ and on the buffers' addresses, so every regime is a separate thing to test.
 `plan()` below asks the planner itself, through the host build of faa_core.cuh (tests/emu).
 tests/test_geometry_plan.py checks that every case of CASES is in the regime it claims and that every regime has a
 case; tests/test_gpu_geometries.py runs every case on the device against the oracle and asserts the launch count.
+CROP_CASES (RandomCrop: crop_pad and outputs smaller than the image) and MIX_CASES (fused Mixup, two sources) do the
+same for the other two inputs of the planner that change what the kernels run; tests/test_gpu_crop_mix_geometries.py
+runs them on the device.
 """
 import ctypes as C
 from dataclasses import dataclass
+
+
+STAGE_LIMIT = 150 * 1024     # bytes of staged band(s) per cluster-kernel CTA (both sources' together)
 
 
 @dataclass
@@ -19,7 +25,8 @@ class Plan:
     W: int
     bands: int
     stage: bool               # TMA staging of the cluster kernel's band
-    stage_off: str            # why not: "size" (H*W*3 % 16), "base" (input address), "band" (too large), "" if staged
+    stage_off: str            # why not: "size" (H*W*3 % 16), "base" (input address), "band" (too large), "" if staged;
+                              # two sources: "doubled band" when one source's band would stage but two do not fit
     light_bands: int
     light_staged: bool        # the light kernel's band is staged
     octets: bool              # the 8-pixel paths
@@ -30,32 +37,52 @@ class Plan:
     mid_threads: int
     no_heavy: bool            # the cluster kernel is not launched
     allow: int                # resolve-kernel allow bits: 1 chunk, 2 scratch, 4 lean gathers
+    band_cap: int = 0         # bytes of one source's staged cluster-kernel band (0: unstaged)
+    crop: bool = False        # RandomCrop: crop_pad > 0 or an output smaller than the image
+    smaller: bool = False     # the output is smaller than the image
+    two_src: bool = False     # fused Mixup
+    self_resolving: bool = False
+    use_chain: bool = False   # chained schedule (Philox records, resolve-ahead allowed)
 
     def launches(self):
         """kernels of one call on resolved records (event schedule, faa_cabi.cu launch_event): the resolve kernel, then
-        either the cluster kernel alone or light + (mid) + (cluster unless no_heavy)"""
+        either the cluster kernel alone or light + (mid) + (cluster unless no_heavy); a self-resolving launch is one
+        kernel"""
+        if self.self_resolving:
+            return 1
         if not self.split:
             return 2
         return 2 + int(self.use_mid) + int(not self.no_heavy)
 
 
-def plan(emu, H, W, batch, u8=False, in_off=0, out_off=0, split_min=-1, has_sg=True):
-    """the planner's decisions for a single-source launch on resolved records, of the image's own size, no crop, final
-    window (apply_tail), input and output at `in_off` / `out_off` bytes from a 256-byte aligned allocation
-    (split_min -1: the library's default)"""
+def plan(emu, H, W, batch, u8=False, in_off=0, out_off=0, split_min=-1, has_sg=True, out_h=None, out_w=None, crop_pad=0,
+         two_src=False, philox=False, allow_ahead=False):
+    """the planner's decisions for a launch of the final window (apply_tail), input and output at `in_off` / `out_off`
+    bytes from a 256-byte aligned allocation (split_min -1: the library's default).  By default a single-source launch
+    on resolved records, of the image's own size, no crop; out_h / out_w / crop_pad: RandomCrop; two_src: fused Mixup;
+    philox / allow_ahead: records drawn on the device, the next batch may be resolved ahead"""
+    out_h, out_w = H if out_h is None else out_h, W if out_w is None else out_w
     names = emu.faa_emu_plan_fields().decode().split()
     out = (C.c_int32 * len(names))()
-    assert emu.faa_emu_plan(H, W, H, W, batch, 0, int(u8), in_off % 16, out_off % 16, 0, 1, int(has_sg), split_min, 0, 0,
-                            out) == len(names)
+    assert emu.faa_emu_plan(H, W, out_h, out_w, batch, crop_pad, int(u8), in_off % 16, out_off % 16, int(two_src), 1,
+                            int(has_sg), split_min, int(philox), int(allow_ahead), out) == len(names)
     d = dict(zip(names, out))
     stage_off = "" if d["stage"] else "size" if (H * W * 3) % 16 else "base" if in_off % 16 else "band"
+    if stage_off == "band" and two_src and plan(emu, H, W, batch, u8, in_off, out_off, split_min, has_sg, out_h, out_w,
+                                                 crop_pad).stage:
+        stage_off = "doubled band"
     return Plan(W, d["bands"], bool(d["stage"]), stage_off, d["light_bands"], bool(d["light_staged"]), bool(d["octets"]),
                 d["mat_cap"] > 0, bool(d["use_split"]), bool(d["use_mid"]), d["mid_bands"], d["mid_threads"],
-                bool(d["no_heavy"]), d["allow"])
+                bool(d["no_heavy"]), d["allow"], d["band_cap"], crop_pad > 0 or (out_h, out_w) != (H, W),
+                (out_h, out_w) != (H, W), two_src, bool(d["self_resolving"]), bool(d["use_chain"]))
 
 
 def regime(p: Plan):
     """the regime names of the case table (the code a split float launch runs)"""
+    if p.two_src:       # fused Mixup: the cluster kernel alone, no chunk, no scratch image
+        return "mix%s, %s" % (" with a crop" if p.crop else "", "staged" if p.stage else "unstaged (%s)" % p.stage_off)
+    if p.crop:
+        return _crop_regime(p)
     if not p.split:
         return "one pixel kernel"
     if p.use_mid:
@@ -69,6 +96,22 @@ def regime(p: Plan):
     if not p.mat:
         return "unstaged (%s), no chunk" % p.stage_off
     return "unstaged (%s)" % p.stage_off
+
+
+def _crop_regime(p: Plan):
+    """RandomCrop launches: no mid kernel (crop_pad > 0 or a smaller output), so a split launch runs the light and the
+    cluster kernel on bands that include the crop slack; uint8 output with a crop does not split"""
+    if not p.split:
+        return "crop, one pixel kernel"
+    if not p.stage:
+        return "crop, unstaged (%s)%s" % (p.stage_off, "" if p.mat else ", no chunk")
+    if p.band_cap + 4096 > STAGE_LIMIT:          # within 4 KB of the limit
+        return "crop, band at the limit%s" % ("" if p.light_staged else ", light band unstaged")
+    if not p.light_staged:
+        return "crop, staged, light band unstaged"
+    if p.smaller:
+        return "crop to a smaller output, staged"
+    return "crop, staged, %s" % ("octets" if p.octets else "no octets")
 
 
 @dataclass
@@ -144,3 +187,105 @@ REGIMES = [
 PHOTO_SHAPES = [(375, 500), (500, 375), (333, 500), (480, 640), (640, 480), (427, 640), (768, 1024), (1200, 1600),
                 (2048, 1536), (1536, 2048), (3000, 4000)]
 LIMIT_SHAPES = [(8, 8192), (8192, 8), (2, 8192), (8192, 2), (8192, 8192)]
+
+
+@dataclass
+class TailCase:
+    """a RandomCrop launch (CROP_CASES) or a fused Mixup launch (MIX_CASES): the input shape, the output size and the
+    tail's crop padding (a hint: records may reach further, the rows outside the staged band come from global memory)"""
+    shape: tuple
+    out: tuple
+    pad: int
+    regime: str
+    launches: int             # kernels per float call on resolved records with FAA_SPLIT_MIN 0 (the unsplit path: 2)
+    why: str
+    in_off: int = 0           # input byte offset (4-byte aligned)
+    u8: bool = False          # uint8 HWC output
+    two_src: bool = False
+    big: bool = False         # reduced program list, emulator reference + an oracle sample
+
+    def plan(self, emu, batch=64, split_min=0):
+        return plan(emu, *self.shape, batch, u8=self.u8, in_off=self.in_off, split_min=split_min, out_h=self.out[0],
+                    out_w=self.out[1], crop_pad=self.pad, two_src=self.two_src)
+
+    @property
+    def id(self):
+        s = ("mix_" if self.two_src else "crop_") + "%dx%d" % self.shape
+        return (s + ("_to%dx%d" % self.out if self.out != self.shape else "") + ("_pad%d" % self.pad if self.pad else "") +
+                ("_in%d" % self.in_off if self.in_off else "") + ("_u8" if self.u8 else ""))
+
+
+# A split crop launch is resolve + light + cluster kernel (3): the mid kernel needs the image's own geometry.  A crop moves
+# the octet paths to the images at offset (0, 0) and makes the pointwise programs of the others C_GENERIC when crop_dx % 4
+# != 0 (build_prog): those go to the cluster kernel.
+CROP_CASES = [
+    TailCase((32, 32), (32, 32), 4, "crop, staged, octets", 3, "CIFAR: one band of 3 KB; images at (0, 0) take the octets"),
+    TailCase((224, 224), (224, 224), 4, "crop, staged, octets", 3, "8 bands of 25 KB, the light kernel 7"),
+    TailCase((224, 224), (224, 224), 16, "crop, staged, octets", 3, "bands of 41 KB (16 rows of crop slack on each side)"),
+    TailCase((8192, 8), (8192, 8), 4, "crop, staged, octets", 3, "header limit: 24-byte rows, bands of 24 KB", big=True),
+    TailCase((300, 300), (300, 300), 4, "crop, staged, no octets", 3, "W % 8 == 4: no octets; bands of 42 KB"),
+    TailCase((224, 224), (224, 224), 127, "crop, band at the limit, light band unstaged", 3,
+             "127 rows of slack: every band is the whole image, 150528 B <= 150 KB; the light kernel's 7 bands are too "
+             "(> 100 KB) and read global memory"),
+    TailCase((380, 380), (380, 380), 32, "crop, staged, light band unstaged", 3, "bands of 127 KB: staged for the "
+             "cluster kernel, over 100 KB for the light kernel"),
+    TailCase((224, 224), (200, 200), 0, "crop to a smaller output, staged", 3, "output rows != image rows, no padding: "
+             "offsets in [0, 24]; output bands of 25 rows against image bands of 28; no octets; light kernel 8 bands"),
+    TailCase((256, 256), (224, 224), 8, "crop to a smaller output, staged", 3, "offsets in [-8, 40]; bands of 52 KB"),
+    TailCase((240, 240), (224, 224), 8, "crop to a smaller output, staged", 3, "offsets in [-8, 24]; bands of 37 KB"),
+    TailCase((456, 456), (456, 456), 64, "crop, unstaged (band)", 3, "bands of 57 + 2 * 64 rows + halo: 250 KB > 150 KB"),
+    TailCase((600, 600), (600, 600), 127, "crop, unstaged (band)", 3, "bands of 75 + 2 * 127 rows + halo: 582 KB"),
+    TailCase((375, 500), (368, 496), 4, "crop, unstaged (size)", 3, "375 * 500 * 3 % 16 == 4; light kernel 5 bands"),
+    TailCase((224, 224), (224, 224), 4, "crop, unstaged (base)", 3, "input 4 bytes past a 16-byte boundary", in_off=4),
+    TailCase((1536, 2048), (1536, 2048), 8, "crop, unstaged (band), no chunk", 3,
+             "pitch 6144 B: a chunk of band + 2 * 8 rows > 24 KB, 16384 / pitch = 2 rows < 3", big=True),
+    TailCase((8, 8192), (8, 8192), 4, "crop, unstaged (band), no chunk", 3, "header limit: 8 one-row bands + 4 rows of "
+             "slack on each side = the whole 192 KB image", big=True),
+    TailCase((224, 224), (224, 224), 4, "crop, one pixel kernel", 2, "uint8 HWC output splits only through the octet "
+             "paths without a crop: the cluster kernel alone", u8=True),
+]
+
+# Fused Mixup (NSRC = 2) never splits: resolve + cluster kernel (2), no materialisation chunk and no scratch image, so
+# two-op programs run the lazy C_GENERIC path and Sharpness -> gather programs are evaluated lazily.  Both sources' bands
+# are staged together, within 150 KB.
+MIX_CASES = [
+    TailCase((224, 224), (224, 224), 0, "mix, staged", 2, "2 x 20 KB", two_src=True),
+    TailCase((256, 256), (256, 256), 0, "mix, staged", 2, "2 x 26 KB", two_src=True),
+    TailCase((380, 380), (380, 380), 0, "mix, staged", 2, "2 x 56 KB", two_src=True),
+    TailCase((8, 8192), (8, 8192), 0, "mix, staged", 2, "2 x 72 KB: the closest to the limit", two_src=True, big=True),
+    TailCase((2, 8192), (2, 8192), 0, "mix, staged", 2, "2 one-row bands of 48 KB", two_src=True, big=True),
+    TailCase((8192, 2), (8192, 2), 0, "mix, staged", 2, "W % 4 == 2: C_GENERIC only; 2 x 6 KB", two_src=True, big=True),
+    TailCase((456, 456), (456, 456), 0, "mix, unstaged (doubled band)", 2, "2 x 79 KB > 150 KB; a single source stages",
+             two_src=True),
+    TailCase((600, 600), (600, 600), 0, "mix, unstaged (doubled band)", 2, "2 x 135 KB", two_src=True),
+    TailCase((375, 500), (375, 500), 0, "mix, unstaged (size)", 2, "375 * 500 * 3 % 16 == 4", two_src=True),
+    TailCase((224, 224), (224, 224), 0, "mix, unstaged (base)", 2, "input 4 bytes past a 16-byte boundary", in_off=4,
+             two_src=True),
+    TailCase((768, 1024), (768, 1024), 0, "mix, unstaged (band)", 2, "one source's band is already 294 KB",
+             two_src=True, big=True),
+    TailCase((224, 224), (224, 224), 16, "mix with a crop, staged", 2, "2 x 41 KB", two_src=True),
+    TailCase((380, 380), (380, 380), 32, "mix with a crop, unstaged (doubled band)", 2, "2 x 127 KB", two_src=True),
+]
+
+# every regime of the crop and Mixup tables
+CROP_REGIMES = [
+    "crop, staged, octets",
+    "crop, staged, no octets",
+    "crop, band at the limit, light band unstaged",
+    "crop, staged, light band unstaged",
+    "crop to a smaller output, staged",
+    "crop, unstaged (band)",
+    "crop, unstaged (size)",
+    "crop, unstaged (base)",
+    "crop, unstaged (band), no chunk",
+    "crop, one pixel kernel",
+]
+MIX_REGIMES = [
+    "mix, staged",
+    "mix, unstaged (doubled band)",
+    "mix, unstaged (size)",
+    "mix, unstaged (base)",
+    "mix, unstaged (band)",
+    "mix with a crop, staged",
+    "mix with a crop, unstaged (doubled band)",
+]
