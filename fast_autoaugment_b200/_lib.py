@@ -26,8 +26,9 @@ SAMPLE_DTYPE = np.dtype([("sub", "<u2"), ("gate", "u1"), ("sign", "u1"), ("crop_
 BOX_DTYPE = np.dtype([("x0", "<i2"), ("y0", "<i2"), ("x1", "<i2"), ("y1", "<i2")])
 JITTER_DTYPE = np.dtype([("alpha", "<f4", (3,)), ("order", "u1", (4,))])          # faa_jitter_t
 CROP_BOX_DTYPE = np.dtype([("x0", "<i4"), ("y0", "<i4"), ("w", "<i4"), ("h", "<i4")])  # faa_crop_box_t
+IMAGE_DTYPE = np.dtype([("data", "<u8"), ("h", "<i4"), ("w", "<i4")])              # faa_image_t
 CROP_RANDOM, CROP_CENTER = 0, 1
-assert SAMPLE_DTYPE.itemsize == 16 and BOX_DTYPE.itemsize == 8
+assert SAMPLE_DTYPE.itemsize == 16 and BOX_DTYPE.itemsize == 8 and IMAGE_DTYPE.itemsize == 16
 
 
 class Tail(C.Structure):          # faa_tail_t
@@ -71,6 +72,8 @@ def _load():
         "faa_cutout_box": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, f64, f64, vp]),
         "faa_sample_policy_mt": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]),
         "faa_sample_philox": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, P(Tail), P(Rng), vp, vp, vp]),
+        "faa_sample_philox_at": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, P(Tail), P(Rng), vp, vp, vp, vp]),
+        "faa_policy_cached_tables": (C.c_int, [vp, P(C.c_int), P(u64)]),
         "faa_augment": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, P(Tail), vp, vp, P(Rng), C.c_int, vp]),
         "faa_policy_set_overlap": (C.c_int, [vp, C.c_int]),
         "faa_augment_many": (C.c_int, [vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, P(Tail), P(Rng), C.c_uint64, vp]),
@@ -90,6 +93,7 @@ def _load():
         "faa_policy_set_lighting": (C.c_int, [vp, vp, C.c_int]),
         "faa_center_crop_box": (C.c_int, [C.c_int, C.c_int, C.c_int, vp]),
         "faa_crop_resize": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, P(Tail), vp, P(CropCfg), vp]),
+        "faa_crop_resize_ragged": (C.c_int, [vp, vp, C.c_int, vp, P(Tail), vp, P(CropCfg), vp]),
         "faa_launch_count": (u64, []),
     }
     for name, (res, args) in sig.items():

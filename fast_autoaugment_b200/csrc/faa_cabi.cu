@@ -590,6 +590,19 @@ static int check_alignment(const void* d_in, const void* d_out, int w, const faa
 
 int faa_sample_philox(faa_policy_t* p, int batch, int h, int w, const faa_tail_t* tail, const faa_rng_t* rng,
                       faa_sample_t* d_samples, faa_box_t* d_boxes, void* stream) {
+    return faa_sample_philox_at(p, batch, h, w, tail, rng, nullptr, d_samples, d_boxes, stream);
+}
+
+int faa_policy_cached_tables(faa_policy_t* p, int* n_tables, uint64_t* bytes) {
+    if (!p || !n_tables || !bytes) return fail(FAA_ERR_VALUE, "null argument");
+    std::lock_guard<std::mutex> lk(p->mu);
+    *n_tables = (int)p->dev_tables.size();
+    *bytes = (uint64_t)p->dev_tables.size() * p->n_sub * p->n_op * 2u * sizeof(OpRec);
+    return FAA_OK;
+}
+
+int faa_sample_philox_at(faa_policy_t* p, int batch, int h, int w, const faa_tail_t* tail, const faa_rng_t* rng,
+                         const int32_t* d_pos, faa_sample_t* d_samples, faa_box_t* d_boxes, void* stream) {
     if (!p || !rng || !d_samples || !d_boxes) return fail(FAA_ERR_VALUE, "null argument");
     if (int e = check_shape(h, w)) return e;
     if (int e = check_tail(tail)) return e;
@@ -601,7 +614,7 @@ int faa_sample_philox(faa_policy_t* p, int batch, int h, int w, const faa_tail_t
     ResolveParams R; memset(&R, 0, sizeof R);
     R.ops = d_ops; R.probs = p->d_probs; memcpy(&R.rng, rng, sizeof(RngCfg));
     R.samples_out = reinterpret_cast<Sample*>(d_samples); R.boxes_out = reinterpret_cast<Box*>(d_boxes);
-    R.first = 0; R.n = batch; R.H = h; R.W = w; R.out_h = tail->out_h; R.out_w = tail->out_w;
+    R.pos = d_pos; R.first = 0; R.n = batch; R.H = h; R.W = w; R.out_h = tail->out_h; R.out_w = tail->out_w;
     R.n_sub = p->n_sub; R.n_op = p->n_op; R.op_base = 0; R.apply_tail = 1;
     CK(launch_resolve(R, (cudaStream_t)stream));
     if (batch > 0) g_launches++;
@@ -1121,40 +1134,90 @@ static int check_crop_cfg(const faa_crop_cfg_t* c) {
     return FAA_OK;
 }
 
+// the output and crop configuration of a crop-resize call
+static int check_crop_resize(const faa_tail_t* tail, const faa_crop_cfg_t* cfg) {
+    if (int e = check_tail(tail)) return e;
+    if (int e = check_crop_cfg(cfg)) return e;
+    if (tail->out_dtype != FAA_U8_HWC)
+        for (int c = 0; c < 3; ++c)
+            if (!(tail->std[c] != 0.0f)) return fail(FAA_ERR_VALUE, "std must be non-zero");
+    return FAA_OK;
+}
+
+// Boxes the kernel draws: the device sampler's boxes lie inside the image; the center box (center mode, and the random
+// mode's fallback after failed attempts) can be empty when img_size is small against the short side.
+static bool center_box_empty(int h, int w, const faa_crop_cfg_t* cfg) {
+    const CropBox b = center_crop_box(h, w, cfg->img_size);
+    return b.w <= 0 || b.h <= 0;
+}
+
+// Given boxes (device memory): copied back and checked against image i's own size (images[i], or h x w for every image
+// when images is null); the host waits for the stream.
+static int check_given_boxes(const faa_crop_box_t* d_boxes, int batch, const faa_image_t* images, int h, int w,
+                             cudaStream_t stream) {
+    std::vector<CropBox> hb((size_t)batch);
+    CK(cudaMemcpyAsync(hb.data(), d_boxes, hb.size() * sizeof(CropBox), cudaMemcpyDeviceToHost, stream));
+    CK(cudaStreamSynchronize(stream));
+    for (int i = 0; i < batch; ++i) {
+        const CropBox& b = hb[(size_t)i];
+        const int ih = images ? (int)images[i].h : h, iw = images ? (int)images[i].w : w;
+        if (b.w <= 0 || b.h <= 0 || b.x0 < 0 || b.y0 < 0 || b.x0 > iw - b.w || b.y0 > ih - b.h)
+            return fail(FAA_ERR_VALUE, "crop box " + std::to_string(i) + " is empty or not inside the image");
+    }
+    return FAA_OK;
+}
+
 int faa_crop_resize(const uint8_t* d_in, void* d_out, int batch, int h, int w, const faa_tail_t* tail,
                     const faa_crop_box_t* d_boxes, const faa_crop_cfg_t* cfg, void* stream) {
     if (!cfg || ((!d_in || !d_out) && batch > 0)) return fail(FAA_ERR_VALUE, "null argument");
     if (batch < 0) return fail(FAA_ERR_VALUE, "negative batch");
     if (batch > 65535) return fail(FAA_ERR_UNSUPPORTED, "batch must be <= 65535");
     if (int e = check_shape(h, w)) return e;
-    if (int e = check_tail(tail)) return e;
-    if (int e = check_crop_cfg(cfg)) return e;
-    if (tail->out_dtype != FAA_U8_HWC)
-        for (int c = 0; c < 3; ++c)
-            if (!(tail->std[c] != 0.0f)) return fail(FAA_ERR_VALUE, "std must be non-zero");
-    if (!d_boxes) {
-        // the device sampler's boxes lie inside the image; the center box (center mode, and the random mode's
-        // fallback after failed attempts) can be empty when img_size is small against the short side
-        CropBox b = center_crop_box(h, w, cfg->img_size);
-        if (b.w <= 0 || b.h <= 0) return fail(FAA_ERR_VALUE, "the center crop of this image is empty");
-    }
+    if (int e = check_crop_resize(tail, cfg)) return e;
+    if (!d_boxes && center_box_empty(h, w, cfg)) return fail(FAA_ERR_VALUE, "the center crop of this image is empty");
     if (int e = ensure_device()) return e;
     if (batch == 0) return FAA_OK;
-    if (d_boxes) {
-        std::vector<CropBox> hb((size_t)batch);
-        CK(cudaMemcpyAsync(hb.data(), d_boxes, hb.size() * sizeof(CropBox), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-        CK(cudaStreamSynchronize((cudaStream_t)stream));
-        for (int i = 0; i < batch; ++i) {
-            const CropBox& b = hb[(size_t)i];
-            if (b.w <= 0 || b.h <= 0 || b.x0 < 0 || b.y0 < 0 || b.x0 > w - b.w || b.y0 > h - b.h)
-                return fail(FAA_ERR_VALUE, "crop box " + std::to_string(i) + " is empty or not inside the image");
-        }
-    }
+    if (d_boxes)
+        if (int e = check_given_boxes(d_boxes, batch, nullptr, h, w, (cudaStream_t)stream))
+            return e;
     const CropResizeTile t = plan_crop_resize(h, w, tail->out_h, tail->out_w);
     if (t.smem == 0) return fail(FAA_ERR_UNSUPPORTED, "no crop-resize tile fits in shared memory");
     CropCfg c; memcpy(&c, cfg, sizeof c);
-    CK(launch_crop_resize(d_in, d_out, batch, h, w, tail->out_h, tail->out_w, tail->out_dtype, tail->mean, tail->std,
-                          reinterpret_cast<const CropBox*>(d_boxes), c, t, (cudaStream_t)stream));
+    CK(launch_crop_resize(d_in, nullptr, d_out, batch, h, w, tail->out_h, tail->out_w, tail->out_dtype, tail->mean,
+                          tail->std, reinterpret_cast<const CropBox*>(d_boxes), c, t, (cudaStream_t)stream));
+    g_launches++;
+    return FAA_OK;
+}
+
+static_assert(sizeof(faa_image_t) == 16 && sizeof(CropImage) == 16 && offsetof(faa_image_t, h) == offsetof(CropImage, h),
+              "image descriptor layout");
+
+int faa_crop_resize_ragged(const faa_image_t* h_images, const faa_image_t* d_images, int batch, void* d_out,
+                           const faa_tail_t* tail, const faa_crop_box_t* d_boxes, const faa_crop_cfg_t* cfg, void* stream) {
+    if (!cfg || ((!h_images || !d_images || !d_out) && batch > 0)) return fail(FAA_ERR_VALUE, "null argument");
+    if (batch < 0) return fail(FAA_ERR_VALUE, "negative batch");
+    if (batch > 65535) return fail(FAA_ERR_UNSUPPORTED, "batch must be <= 65535");
+    if (int e = check_crop_resize(tail, cfg)) return e;
+    int max_h = 1, max_w = 1;
+    for (int i = 0; i < batch; ++i) {
+        const faa_image_t& m = h_images[i];
+        if (!m.data) return fail(FAA_ERR_VALUE, "image " + std::to_string(i) + " has no data");
+        if (int e = check_shape(m.h, m.w)) return e;
+        if (!d_boxes && center_box_empty(m.h, m.w, cfg))
+            return fail(FAA_ERR_VALUE, "the center crop of image " + std::to_string(i) + " is empty");
+        max_h = std::max(max_h, (int)m.h); max_w = std::max(max_w, (int)m.w);
+    }
+    if (int e = ensure_device()) return e;
+    if (batch == 0) return FAA_OK;
+    if (d_boxes)
+        if (int e = check_given_boxes(d_boxes, batch, h_images, 0, 0, (cudaStream_t)stream))
+            return e;
+    const CropResizeTile t = plan_crop_resize(max_h, max_w, tail->out_h, tail->out_w);
+    if (t.smem == 0) return fail(FAA_ERR_UNSUPPORTED, "no crop-resize tile fits in shared memory");
+    CropCfg c; memcpy(&c, cfg, sizeof c);
+    CK(launch_crop_resize(nullptr, reinterpret_cast<const CropImage*>(d_images), d_out, batch, max_h, max_w, tail->out_h,
+                          tail->out_w, tail->out_dtype, tail->mean, tail->std, reinterpret_cast<const CropBox*>(d_boxes), c,
+                          t, (cudaStream_t)stream));
     g_launches++;
     return FAA_OK;
 }

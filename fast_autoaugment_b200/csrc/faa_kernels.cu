@@ -118,7 +118,8 @@ __global__ void __launch_bounds__(1024) faa_resolve_kernel(const __grid_constant
                 else { bx[j].x0 = bx[j].y0 = 0; bx[j].x1 = bx[j].y1 = -1; }
             }
         } else {
-            philox_sample(P.rng, P.rng.first_index + (uint64_t)i, P.ops, P.probs, P.n_sub, P.n_op, P.H, P.W,
+            const uint64_t at = P.pos != nullptr ? (uint64_t)(uint32_t)P.pos[i] : (uint64_t)i;
+            philox_sample(P.rng, P.rng.first_index + at, P.ops, P.probs, P.n_sub, P.n_op, P.H, P.W,
                           P.out_h, P.out_w, s, bx);
         }
         if (P.progs != nullptr) {
@@ -1976,12 +1977,16 @@ cudaError_t launch_lighting_tables(const float* rgb, float* tabs, int n, const f
 // and the vertical ones of its rows in shared memory, runs the horizontal pass over exactly the crop rows its rows
 // read into a uint8 intermediate (one packed RGB word per pixel), then the vertical pass from there, and writes
 // uint8 HWC or ToTensor + Normalize (exact fp32 table, then one rounding to fp16 / bf16) NCHW.
+// A ragged batch (images != nullptr) differs only in where thread 0 finds the image and its size: every per-image
+// quantity (box, coefficients, rows) already derives from the box, and the plan is made for the batch's largest height
+// and largest width (see launch_crop_resize).
 struct CropResizeParams {
-    const uint8_t* in;           // [B][H][W][3]
+    const uint8_t* in;           // [B][H][W][3] (uniform batch)
+    const CropImage* images;     // [B] descriptors (ragged batch) or nullptr
     void* out;                   // [B][out_h][out_w][3] uint8 or [B][3][out_h][out_w]
     const CropBox* boxes;        // [B] or nullptr: draw with cfg
     CropCfg cfg;
-    int32_t H, W, out_h, out_w;
+    int32_t H, W, out_h, out_w;  // H x W: every image's size (uniform) or the largest height / width (ragged)
     int32_t tile_w, tile_h, tw_shift;   // tile_w = 1 << tw_shift
     int32_t kx_cap, ky_cap, rows_cap;   // taps per column / row and intermediate rows a CTA can hold
     float mean[3], std[3];
@@ -1997,6 +2002,8 @@ __global__ void __launch_bounds__(256, 4) faa_crop_resize_kernel(const __grid_co
     extern __shared__ int32_t cr_smem[];
     __shared__ float s_norm[OUT == OUT_U8_HWC ? 1 : 768];
     __shared__ CropBox s_box;
+    __shared__ const uint8_t* s_src;
+    __shared__ int32_t s_src_w;
     const int img = blockIdx.z, tid = threadIdx.x;
     const int ox0 = blockIdx.x * P.tile_w, oy0 = blockIdx.y * P.tile_h;
     const int ncols = min(P.tile_w, P.out_w - ox0), nrows = min(P.tile_h, P.out_h - oy0);
@@ -2007,7 +2014,13 @@ __global__ void __launch_bounds__(256, 4) faa_crop_resize_kernel(const __grid_co
     int32_t* vmin = vk + P.tile_h * P.ky_cap;
     int32_t* vn = vmin + P.tile_h;
     uint32_t* inter = reinterpret_cast<uint32_t*>(vn + P.tile_h);   // [rows_cap][tile_w]
-    if (tid == 0) s_box = P.boxes ? P.boxes[img] : draw_crop_box(&P.cfg, P.cfg.rng.first_index + (uint64_t)img, P.H, P.W);
+    if (tid == 0) {
+        CropImage d;
+        if (P.images != nullptr) d = P.images[img];
+        else { d.data = P.in + (size_t)img * P.H * P.W * 3u; d.h = P.H; d.w = P.W; }
+        s_src = d.data; s_src_w = d.w;
+        s_box = P.boxes ? P.boxes[img] : draw_crop_box(&P.cfg, P.cfg.rng.first_index + (uint64_t)img, d.h, d.w);
+    }
     if (OUT != OUT_U8_HWC) {                                 // data.py:76-78: x = u8 / 255 ; (x - mean) / std in fp32
         for (int i = tid; i < 768; i += blockDim.x) {
             const int ch = i >> 8;
@@ -2033,12 +2046,13 @@ __global__ void __launch_bounds__(256, 4) faa_crop_resize_kernel(const __grid_co
     const int rows = vmin[nrows - 1] + vn[nrows - 1] - r0;
     assert(rows <= P.rows_cap);
     // horizontal pass: crop rows [r0, r0 + rows) x this tile's columns -> inter
-    const size_t img_base = (size_t)img * P.H * P.W * 3u;
+    const uint8_t* const img_src = s_src;
+    const size_t pitch = (size_t)s_src_w * 3u;
     const int tmask = P.tile_w - 1;
     for (int i = tid; i < (rows << P.tw_shift); i += blockDim.x) {
         const int r = i >> P.tw_shift, c = i & tmask;
         if (c >= ncols) continue;
-        const uint8_t* src = P.in + img_base + ((size_t)(b.y0 + r0 + r) * P.W + (size_t)(b.x0 + hmin[c])) * 3u;
+        const uint8_t* src = img_src + (size_t)(b.y0 + r0 + r) * pitch + (size_t)(b.x0 + hmin[c]) * 3u;
         const int32_t* k = hk + c * P.kx_cap;
         const int n = hn[c];
         int32_t s0 = 1 << (kResPrecisionBits - 1), s1 = s0, s2 = s0;
@@ -2092,6 +2106,11 @@ __global__ void __launch_bounds__(256, 4) faa_crop_resize_kernel(const __grid_co
 // Tile of a crop-resize launch: the largest tile whose coefficients and intermediate fit, for ANY crop of the
 // h x w source (a crop's scale, taps and rows are bounded by the full image's).  Prefers <= 48 KB (several CTAs
 // per SM); the 1 x 1 tile of an 8192 x 8192 source needs ~96 KB, so every valid size has a tile.
+// A ragged batch is planned at (largest height, largest width), which may come from two different images.  That plan
+// holds every image h x w with h <= H and w <= W: its crop box is at most w wide and h high, resize_ksize is
+// non-decreasing in the input size (scale, support and their ceiling all grow with it), so the taps of a column are at
+// most min(w, ksize(w)) <= kx and those of a row at most ky; the vertical scale is box_h / out_h <= H / out_h, so the
+// rows a tile reads are at most min(h, ceil((th - 1) * sy) + ky + 2) <= rows.  The kernel's assert keeps checking it.
 CropResizeTile plan_crop_resize(int H, int W, int out_h, int out_w) {
     const int kx = min(W, resize_ksize(W, out_w)), ky = min(H, resize_ksize(H, out_h));
     const double sy = (double)H / out_h > 1.0 ? (double)H / out_h : 1.0;
@@ -2127,12 +2146,12 @@ static cudaError_t launch_crop_resize_as(const CropResizeParams& P, dim3 grid, s
     return cudaGetLastError();
 }
 
-cudaError_t launch_crop_resize(const uint8_t* in, void* out, int batch, int H, int W, int out_h, int out_w, int out_type,
-                               const float mean[3], const float std[3], const CropBox* boxes, const CropCfg& cfg,
-                               const CropResizeTile& t, cudaStream_t stream) {
+cudaError_t launch_crop_resize(const uint8_t* in, const CropImage* images, void* out, int batch, int H, int W, int out_h,
+                               int out_w, int out_type, const float mean[3], const float std[3], const CropBox* boxes,
+                               const CropCfg& cfg, const CropResizeTile& t, cudaStream_t stream) {
     if (batch <= 0) return cudaSuccess;
     CropResizeParams P;
-    P.in = in; P.out = out; P.boxes = boxes; P.cfg = cfg;
+    P.in = in; P.images = images; P.out = out; P.boxes = boxes; P.cfg = cfg;
     P.H = H; P.W = W; P.out_h = out_h; P.out_w = out_w;
     P.tile_w = t.tile_w; P.tile_h = t.tile_h; P.tw_shift = t.tw_shift;
     P.kx_cap = t.kx_cap; P.ky_cap = t.ky_cap; P.rows_cap = t.rows_cap;

@@ -21,6 +21,7 @@ struct ResolveParams {
     Sample* samples_out;        // optional [n]
     Box* boxes_out;             // optional [n][n_op]
     RngCfg rng;
+    const int32_t* pos;         // Philox: record t draws global sample rng.first_index + pos[t] (nullptr: + t)
     int32_t first, n;           // images [first, first+n) of the arrays above
     int32_t H, W, out_h, out_w, n_sub, n_op, op_base, apply_tail;
     int32_t allow;              // bit 0: the pixel kernel has a materialisation chunk, bit 1: a global scratch image
@@ -98,10 +99,12 @@ cudaError_t launch_mix_u8(const uint8_t* a, const uint8_t* b, const int32_t* par
 cudaError_t launch_color_jitter(const uint8_t* in, uint8_t* out, const void* recs, int batch, int H, int W, cudaStream_t stream);
 // EfficientNet crop + bicubic resize (faa_crop_resize_kernel): output tile and shared-memory plan
 struct CropResizeTile { int32_t tile_w, tile_h, tw_shift, kx_cap, ky_cap, rows_cap; size_t smem; };
+struct CropImage { const uint8_t* data; int32_t h, w; };               // == faa_image_t: one image of a ragged batch
 CropResizeTile plan_crop_resize(int H, int W, int out_h, int out_w);     // smem == 0: nothing fits
-cudaError_t launch_crop_resize(const uint8_t* in, void* out, int batch, int H, int W, int out_h, int out_w, int out_type,
-                               const float mean[3], const float std[3], const CropBox* boxes, const CropCfg& cfg,
-                               const CropResizeTile& t, cudaStream_t stream);
+// images == nullptr: `in` is [batch][H][W][3]; else image i is images[i] (device array) and H x W is only the plan's size
+cudaError_t launch_crop_resize(const uint8_t* in, const CropImage* images, void* out, int batch, int H, int W, int out_h,
+                               int out_w, int out_type, const float mean[3], const float std[3], const CropBox* boxes,
+                               const CropCfg& cfg, const CropResizeTile& t, cudaStream_t stream);
 cudaError_t launch_lighting_tables(const float* rgb, float* tabs, int n, const float mean[3], const float std[3], cudaStream_t stream);
 
 }  // namespace faa

@@ -22,8 +22,8 @@ from torch.utils.data import Sampler, SubsetRandomSampler
 
 from . import _lib, archive
 from .conf import Config as C
-from .engine import (CIFAR_MEAN, CIFAR_STD, IMAGENET_MEAN, IMAGENET_STD, CompiledPolicy, TailSpec,
-                     augment_batch, center_crop_box, crop_cfg, crop_resize, make_rng)
+from .engine import (CIFAR_MEAN, CIFAR_STD, IMAGENET_MEAN, IMAGENET_STD, CompiledPolicy, RaggedImages, TailSpec,
+                     augment_batch, center_crop_box, crop_cfg, crop_resize, make_rng, sample_philox_at)
 
 
 class Augmentation(object):
@@ -274,7 +274,14 @@ class ImageNetChain(object):
     ``parity=True`` draws like the reference's per-image loop (a ``num_workers=0`` DataLoader), image after image:
     policy (``random``, ``numpy``), crop (``random``), flip (``torch.rand``), jitter (``randperm(4)`` + three
     uniforms), Lighting (three normals).  Otherwise the policy, crop and flip are drawn by the kernels (Philox keyed by
-    (seed, first_index + i)) and the jitter / Lighting records by vectorised torch calls on the device."""
+    (seed, first_index + i)) and the jitter / Lighting records by vectorised torch calls on the device.
+
+    Both also take a ``RaggedImages`` batch of differently sized sources (the reference transforms one PIL image at a
+    time, so every image is cropped at its own size).  ``test`` is then one ragged crop-resize launch.  ``train`` runs
+    the policy once per distinct source size (the images of that size gathered, each with the decisions of its batch
+    position: ``faa_sample_philox_at``, or its parity records) into a packed uint8 intermediate, then one ragged
+    crop-resize, and the same jitter and flip + Lighting + Normalize launches as a uniform batch.  A batch of one size
+    gives the bytes of the uniform chain.  The policy handle keeps one compiled table per source size it has seen."""
 
     _EIGVAL = _IMAGENET_PCA["eigval"]
     _EIGVEC = _IMAGENET_PCA["eigvec"]
@@ -290,16 +297,21 @@ class ImageNetChain(object):
         self.tail = TailSpec(None, 0, True, IMAGENET_MEAN, IMAGENET_STD, 0, out_dtype)
         self.test_tail = TailSpec(None, 0, False, IMAGENET_MEAN, IMAGENET_STD, 0, out_dtype)
 
-    def sample_parity(self, n, h, w):
+    def sample_parity(self, n, h=None, w=None, sizes=None):
         """per-image records in the reference's draw order: (policy samples, policy boxes or None, crop boxes,
-        flip samples of the identity policy, jitter records, Lighting offsets [n, 3])"""
+        flip samples of the identity policy, jitter records, Lighting offsets [n, 3]).  ``sizes``: [n] (h, w) of each
+        image (a ragged batch) instead of one h x w for all."""
         pol = self.aug.compiled if self.aug is not None else None
+        sizes = [(h, w)] * n if sizes is None else [(int(a), int(b)) for a, b in np.asarray(sizes).reshape(-1, 2)]
+        if len(sizes) != n:
+            raise ValueError("need one size per image")
         samples, boxes = [], []
         crops = np.zeros(n, dtype=_lib.CROP_BOX_DTYPE)
         flips = np.zeros(n, dtype=_lib.SAMPLE_DTYPE)
         jit = np.zeros(n, dtype=_lib.JITTER_DTYPE)
         rgb = torch.zeros(n, 3)
         for i in range(n):
+            h, w = sizes[i]
             if pol is not None:
                 s, b = pol.sample_parity(1, h, w, TailSpec.raw_u8())
                 samples.append(s)
@@ -334,8 +346,10 @@ class ImageNetChain(object):
         return recs, rgb
 
     def train(self, batch_u8, parity=False, seed=0, first_index=0, records=None):
-        """uint8 [B,H,W,3] CUDA -> [B, 3, s, s] ``out_dtype``.  ``records``: the tuple of ``sample_parity`` (drawn
-        here when ``parity`` and not given)."""
+        """uint8 [B,H,W,3] CUDA (or ``RaggedImages``) -> [B, 3, s, s] ``out_dtype``.  ``records``: the tuple of
+        ``sample_parity`` (drawn here when ``parity`` and not given)."""
+        if isinstance(batch_u8, RaggedImages):
+            return self._train_ragged(batch_u8, parity, seed, first_index, records)
         b, h, w, _ = batch_u8.shape
         dev = batch_u8.device
         if parity and records is None:
@@ -358,8 +372,59 @@ class ImageNetChain(object):
                                                  recs.data_ptr(), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
         return augment_batch(self.flip_policy, y, self.tail, rng=make_rng(seed, first_index, self.tail), lighting_rgb=rgb)
 
+    def _policy_ragged(self, batch, records, seed, first_index):
+        """the policy at source size, one launch group per distinct size -> RaggedImages of the results (batch order).
+        Each group's images are one contiguous [n, h, w, 3] starting on a 16-byte boundary: the policy kernels' word
+        loads and stores need the alignment of a fresh allocation."""
+        pol = self.aug.compiled
+        raw = TailSpec.raw_u8()
+        groups = batch.groups()
+        slab = [(-(-len(pos) * h * w * 3 // 16)) * 16 for (h, w), pos in groups]
+        inter = torch.empty(int(sum(slab)), dtype=torch.uint8, device=batch.device)
+        offsets = np.zeros(len(batch), np.int64)
+        at = 0
+        for ((h, w), pos), size in zip(groups, slab):
+            n = len(pos)
+            src_off = batch.offsets[pos]
+            if (int(src_off[0]) + batch.storage.data_ptr()) % 16 == 0 and \
+                    np.array_equal(src_off, src_off[0] + np.arange(n) * h * w * 3):      # already packed in batch order
+                x = batch.storage[int(src_off[0]):int(src_off[0]) + n * h * w * 3].view(n, h, w, 3)
+            else:
+                x = torch.stack([batch.image(int(i)) for i in pos])
+            out = inter[at:at + n * h * w * 3].view(n, h, w, 3)
+            if records is not None:
+                samples, boxes = records[0][pos], records[1][pos]
+            else:
+                samples, boxes = sample_philox_at(pol, pos, h, w, raw, make_rng(seed, first_index, raw), batch.device)
+            augment_batch(pol, x, raw, samples, boxes, out=out)
+            offsets[pos] = at + np.arange(n) * h * w * 3
+            at += size
+        return RaggedImages(inter, offsets, batch.sizes)
+
+    def _train_ragged(self, batch, parity, seed, first_index, records):
+        b = len(batch)
+        dev = batch.device
+        if parity and records is None:
+            records = self.sample_parity(b, sizes=batch.sizes)
+        x = batch if self.aug is None else self._policy_ragged(batch, records, seed, first_index)
+        s = self.input_size
+        if records is not None:
+            _, _, crops, flips, jit, rgb = records
+            y = crop_resize(x, s, boxes=crops)
+            self.jitter.jitter_batch(y, jit, out=y)
+            zb = np.zeros((b, 1), dtype=_lib.BOX_DTYPE)
+            return augment_batch(self.flip_policy, y, self.tail, flips, zb, lighting_rgb=rgb)
+        y = crop_resize(x, s, rng=self.crop.cfg(seed, first_index))
+        recs, rgb = self._device_records(b, dev, seed, first_index)
+        with torch.cuda.device(dev):
+            import ctypes as C
+            _lib.check(_lib.lib.faa_color_jitter(y.data_ptr(), y.data_ptr(), b, s, s, recs.data_ptr(),
+                                                 C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+        return augment_batch(self.flip_policy, y, self.tail, rng=make_rng(seed, first_index, self.tail), lighting_rgb=rgb)
+
     def test(self, batch_u8, out=None):
-        """uint8 [B,H,W,3] CUDA -> [B, 3, s, s]: center crop + resize + ToTensor + Normalize, one launch"""
+        """uint8 [B,H,W,3] CUDA (or ``RaggedImages``) -> [B, 3, s, s]: center crop + resize + ToTensor + Normalize, one
+        launch"""
         return crop_resize(batch_u8, self.input_size, rng=self.center.cfg(), tail=self.test_tail, out=out)
 
 
@@ -413,6 +478,32 @@ class DeviceDataset:
         return d
 
 
+class RaggedDeviceDataset:
+    """``DeviceDataset`` of differently sized uint8 images (``RaggedImages`` on the device) + int64 targets: the
+    ImageNet sources of the ``faa_crop_resize`` loaders."""
+
+    def __init__(self, images, targets, device="cuda"):
+        if isinstance(images, RaggedImages):
+            self.images = RaggedImages(images.storage.to(device), images.offsets, images.sizes)
+        else:
+            self.images = RaggedImages.from_list(images, device)
+        self.targets = [int(t) for t in targets]
+        if len(self.targets) != len(self.images):
+            raise ValueError("need one target per image")
+        self.labels = torch.as_tensor(self.targets, dtype=torch.int64, device=device)
+
+    def __len__(self):
+        return len(self.images)
+
+    def subset(self, idx):
+        idx = [int(i) for i in idx]
+        d = RaggedDeviceDataset.__new__(RaggedDeviceDataset)
+        d.images = self.images.select(idx)
+        d.targets = [self.targets[i] for i in idx]
+        d.labels = self.labels.index_select(0, torch.as_tensor(idx, dtype=torch.int64, device=self.labels.device))
+        return d
+
+
 class GpuAugmentedLoader:
     """What ``get_dataloaders`` hands to ``train.py:47`` / ``search.py:101`` instead of a torch ``DataLoader``:
     an iterable of ``(data, label)`` whose ``data`` is the augmented, normalised CUDA batch (``.cuda()`` at
@@ -425,10 +516,10 @@ class GpuAugmentedLoader:
     torch generators (a ``num_workers=0`` DataLoader); the default draws on the device with Philox.
     """
 
-    def __init__(self, dataset: DeviceDataset, batch, policies, tail: TailSpec, sampler=None, shuffle=False,
+    def __init__(self, dataset: DeviceDataset | RaggedDeviceDataset, batch, policies, tail: TailSpec, sampler=None, shuffle=False,
                  drop_last=False, seed=None, parity=False, chain=None, chain_mode="train"):
         """``chain``: an ``ImageNetChain`` that transforms the batches instead of the fused policy launch
-        (``chain_mode`` 'train' or 'test')."""
+        (``chain_mode`` 'train' or 'test'); a ``RaggedDeviceDataset`` needs one."""
         if not torch.cuda.is_available():
             raise _lib.FaaRuntimeError("fast_autoaugment_b200 needs a CUDA device (no CPU fallback)")
         self.dataset, self.batch_size, self.tail = dataset, int(batch), tail
@@ -436,6 +527,8 @@ class GpuAugmentedLoader:
         self.aug = Augmentation(policies) if policies is not None else Augmentation([[("Invert", 0.0, 0.0)]])
         self.seed = int(torch.initial_seed() if seed is None else seed) & 0x7FFFFFFFFFFFFFFF
         self.chain, self.chain_mode = chain, chain_mode
+        if isinstance(dataset, RaggedDeviceDataset) and chain is None:
+            raise ValueError("images of different sizes need an ImageNetChain (conf['faa_crop_resize'])")
         self._drawn = 0                   # samples drawn so far: the Philox counter never repeats across epochs
 
     def _n(self):
@@ -457,7 +550,10 @@ class GpuAugmentedLoader:
         for k in range(len(self)):
             idx = idx_all[k * self.batch_size:(k + 1) * self.batch_size]
             t = torch.as_tensor(idx, dtype=torch.int64).to(dev, non_blocking=True)
-            raw = self.dataset.images.index_select(0, t)
+            if isinstance(self.dataset, RaggedDeviceDataset):
+                raw = self.dataset.images.select(idx)            # descriptors into the dataset's storage: no pixel copy
+            else:
+                raw = self.dataset.images.index_select(0, t)
             if self.chain is None:
                 data = self.aug.augment_batch(raw, self.tail, seed=self.seed, first_index=self._drawn, parity=self.parity)
             elif self.chain_mode == "test":
@@ -475,15 +571,35 @@ def _load_arrays(dataset, dataroot):
     ``dataroot`` is the reference's dataset directory (torchvision layout, read with ``download=False`` - the
     build and GPU boxes have no network), or a directory holding ``<dataset>_train.npz`` / ``<dataset>_test.npz``
     (arrays ``data`` [N,H,W,3] uint8 and ``targets``), or - for in-memory injection (tests, synthetic benchmarks) -
-    a mapping ``{"train": (images, targets), "test": (images, targets)}``."""
+    a mapping ``{"train": (images, targets), "test": (images, targets)}``.
+
+    ImageNet sources may differ in size: a mapping whose images are a list of uint8 HWC arrays of different sizes, or
+    an .npz whose ``data`` is the images' bytes packed back to back with their ``sizes`` [N, 2] (h, w).  Those images
+    come back as a list of arrays."""
     base = dataset.replace("reduced_", "")
+    ragged_ok = "imagenet" in dataset
+
+    def images(x):
+        if ragged_ok and isinstance(x, (list, tuple)) and len({np.shape(a) for a in x}) > 1:
+            return [np.asarray(a) for a in x]
+        return np.asarray(x)
+
+    def npz_images(z):
+        if ragged_ok and "sizes" in z.files:
+            sizes = np.asarray(z["sizes"], np.int64).reshape(-1, 2)
+            ends = np.cumsum(sizes[:, 0] * sizes[:, 1] * 3)
+            flat = np.asarray(z["data"], np.uint8).reshape(-1)
+            if len(ends) and ends[-1] != flat.size:
+                raise ValueError("packed data does not match sizes")
+            return [p.reshape(h, w, 3) for p, (h, w) in zip(np.split(flat, ends[:-1]), sizes)]
+        return z["data"]
     if isinstance(dataroot, dict):
         tr, te = dataroot["train"], dataroot.get("test", dataroot["train"])
-        return np.asarray(tr[0]), list(tr[1]), np.asarray(te[0]), list(te[1])
+        return images(tr[0]), list(tr[1]), images(te[0]), list(te[1])
     npz = [os.path.join(str(dataroot), "%s_%s.npz" % (base, s)) for s in ("train", "test")]
     if all(os.path.exists(p) for p in npz):
         a, b = np.load(npz[0]), np.load(npz[1])
-        return a["data"], list(a["targets"]), b["data"], list(b["targets"])
+        return npz_images(a), list(a["targets"]), npz_images(b), list(b["targets"])
     import torchvision
     if base in ("cifar10", "cifar100"):
         cls = torchvision.datasets.CIFAR10 if base == "cifar10" else torchvision.datasets.CIFAR100
@@ -512,7 +628,7 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
 
     Extra conf keys (optional): ``faa_out_dtype`` ('float32' default - what the reference yields -, 'float16',
     'bfloat16'), ``faa_parity`` (replay the reference's global RNG draws per sample; tests), ``faa_crop_resize``
-    (ImageNet: the stored images are uncropped sources of one size and the loaders run the reference's full chains,
+    (ImageNet: the stored images are uncropped sources, of one size or of many, and the loaders run the reference's full chains,
     ``ImageNetChain``: train / valid = policy -> EfficientNetRandomCrop + bicubic Resize -> ColorJitter -> HFlip +
     Lighting + Normalize, test = EfficientNetCenterCrop + Resize + Normalize, at 224 or the EfficientNet size of
     ``conf['model']['type']``; without it ImageNet images must already have the network's size)."""
@@ -534,8 +650,15 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
     policies = policy_by_conf_name(conf["aug"])                 # data.py:85-109 (ValueError on an unknown name)
 
     tr_x, tr_y, te_x, te_y = _load_arrays(dataset, dataroot)
+    ragged = isinstance(tr_x, list) or isinstance(te_x, list)
+    if ragged and not conf.get("faa_crop_resize", False):
+        raise ValueError("ImageNet images of different sizes need conf['faa_crop_resize']: without it the images are "
+                         "augmented at one fixed size")
+
+    def device_dataset(x, y):
+        return RaggedDeviceDataset(x, y) if isinstance(x, list) else DeviceDataset(x, y)
     if dataset in ("cifar10", "cifar100", "svhn", "imagenet"):
-        total_trainset, testset = DeviceDataset(tr_x, tr_y), DeviceDataset(te_x, te_y)
+        total_trainset, testset = device_dataset(tr_x, tr_y), device_dataset(te_x, te_y)
     elif dataset in ("reduced_cifar10", "reduced_svhn"):        # data.py:117-126, 136-146
         test_size = 46000 if dataset == "reduced_cifar10" else 73257 - 1000
         sss = StratifiedShuffleSplit(n_splits=1, test_size=test_size, random_state=0)

@@ -441,23 +441,108 @@ def center_crop_box(h, w, img_size):
     return tuple(int(v) for v in b[0])
 
 
-def crop_resize(batch_u8: torch.Tensor, size, boxes=None, rng=None, tail: TailSpec | None = None, out=None):
+class RaggedImages:
+    """A batch or dataset of differently sized uint8 HWC images in one byte buffer (on the device for every launch).
+
+    ``storage``: 1-D uint8 tensor; image i is ``sizes[i] = (h, w)`` rows of ``w * 3`` bytes starting at byte
+    ``offsets[i]`` (host int64 [N]; ``sizes`` host int32 [N, 2]).  Several descriptors may share bytes or leave gaps:
+    ``select`` makes new descriptors into the same storage without copying a pixel."""
+
+    def __init__(self, storage: torch.Tensor, offsets, sizes):
+        if not isinstance(storage, torch.Tensor) or storage.dtype != torch.uint8 or storage.dim() != 1 \
+                or not storage.is_contiguous():
+            raise ValueError("storage must be a contiguous 1-D uint8 tensor")
+        self.storage = storage
+        self.offsets = np.ascontiguousarray(offsets, dtype=np.int64).reshape(-1)
+        self.sizes = np.ascontiguousarray(sizes, dtype=np.int32).reshape(-1, 2)
+        if len(self.offsets) != len(self.sizes):
+            raise ValueError("need one offset per size")
+        if len(self.sizes) and (int(self.sizes.min()) < 1 or int(self.offsets.min()) < 0 or
+                                int((self.offsets + self.nbytes()).max()) > storage.numel()):
+            raise ValueError("every image must be at least 1 x 1 and lie inside the storage")
+        self._desc = None
+
+    @staticmethod
+    def from_list(images, device="cuda"):
+        """uint8 HWC images (NumPy arrays or CUDA tensors), packed back to back with one copy."""
+        sizes = np.array([tuple(int(v) for v in a.shape[:2]) for a in images], dtype=np.int32).reshape(-1, 2)
+        for a in images:
+            u8 = a.dtype == torch.uint8 if isinstance(a, torch.Tensor) else np.asarray(a).dtype == np.uint8
+            if not u8 or a.ndim != 3 or a.shape[2] != 3:
+                raise ValueError("every image must be uint8 [H, W, 3]")
+        n = sizes[:, 0].astype(np.int64) * sizes[:, 1] * 3
+        offsets = np.concatenate([[0], np.cumsum(n)[:-1]]).astype(np.int64)
+        if len(images) and all(isinstance(a, torch.Tensor) and a.device == torch.device(device) for a in images):
+            storage = torch.cat([a.reshape(-1) for a in images]).to(device)
+        else:
+            host = np.empty(int(n.sum()), np.uint8)
+            for a, o, k in zip(images, offsets, n):
+                host[o:o + k] = (a.cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)).reshape(-1)
+            storage = torch.from_numpy(host).to(device)
+        return RaggedImages(storage, offsets, sizes)
+
+    def __len__(self):
+        return len(self.sizes)
+
+    @property
+    def device(self):
+        return self.storage.device
+
+    def nbytes(self):
+        """bytes of each image, int64 [N]"""
+        return self.sizes[:, 0].astype(np.int64) * self.sizes[:, 1] * 3
+
+    def select(self, idx):
+        idx = np.asarray(idx, dtype=np.int64).reshape(-1)
+        return RaggedImages(self.storage, self.offsets[idx], self.sizes[idx])
+
+    def image(self, i):
+        """uint8 [h, w, 3] view of image i"""
+        h, w = (int(v) for v in self.sizes[i])
+        o = int(self.offsets[i])
+        return self.storage[o:o + h * w * 3].view(h, w, 3)
+
+    def groups(self):
+        """[((h, w), positions)]: the batch positions of each distinct size, in batch order, sizes in order of their first
+        image"""
+        out = {}
+        for i, (h, w) in enumerate(self.sizes.tolist()):
+            out.setdefault((h, w), []).append(i)
+        return [(k, np.array(v, dtype=np.int64)) for k, v in out.items()]
+
+    def descriptors(self):
+        """(host ``IMAGE_DTYPE`` [N], device uint8 copy of it): the ``faa_image_t`` arrays of ``faa_crop_resize_ragged``"""
+        if self._desc is None:
+            d = np.zeros(len(self), dtype=_lib.IMAGE_DTYPE)
+            d["data"] = self.storage.data_ptr() + self.offsets.astype(np.uint64)
+            d["h"], d["w"] = self.sizes[:, 0], self.sizes[:, 1]
+            self._desc = (d, torch.from_numpy(d.view(np.uint8).copy()).to(self.device))
+        return self._desc
+
+
+def crop_resize(batch_u8, size, boxes=None, rng=None, tail: TailSpec | None = None, out=None):
     """EfficientNet crop + ``Resize((s, s), BICUBIC)`` of a uint8 [B,H,W,3] CUDA batch in ONE launch (C ABI
-    ``faa_crop_resize``), bit-exact with Pillow's ``crop`` + ``resize``.
+    ``faa_crop_resize``), bit-exact with Pillow's ``crop`` + ``resize``.  A ``RaggedImages`` batch runs the same in one
+    launch too (``faa_crop_resize_ragged``), each image cropped at its own size.
 
     ``size``: output size (int or (h, w)).  ``boxes``: per-image crop boxes ([B] ``CROP_BOX_DTYPE`` array, or an
     int32 [B, 4] array / tensor of x0, y0, w, h); otherwise ``rng`` is a ``crop_cfg`` and the kernel draws (random
     mode) or computes (center mode) the boxes.  ``tail``: None or a uint8 ``TailSpec`` -> uint8 [B, s, s, 3]; a float
     ``TailSpec`` -> ToTensor + Normalize fused in, [B, 3, s, s] of ``tail.out_dtype`` (its crop / flip / Cutout fields
     are not used here)."""
-    _require_cuda(batch_u8, "batch")
-    if batch_u8.dtype != torch.uint8 or batch_u8.dim() != 4 or batch_u8.shape[-1] != 3:
-        raise ValueError("batch must be uint8 [B, H, W, 3]")
+    ragged = isinstance(batch_u8, RaggedImages)
+    _require_cuda(batch_u8.storage if ragged else batch_u8, "batch")
+    if not ragged:
+        if batch_u8.dtype != torch.uint8 or batch_u8.dim() != 4 or batch_u8.shape[-1] != 3:
+            raise ValueError("batch must be uint8 [B, H, W, 3]")
     if (boxes is None) == (rng is None):
         raise ValueError("give exactly one of boxes= and rng=")
-    batch_u8 = batch_u8.contiguous()
-    dev = batch_u8.device
-    B, H, W, _ = batch_u8.shape
+    if ragged:
+        dev, B, H, W = batch_u8.device, len(batch_u8), 1, 1
+    else:
+        batch_u8 = batch_u8.contiguous()
+        dev = batch_u8.device
+        B, H, W, _ = batch_u8.shape
     oh, ow = (size, size) if isinstance(size, int) else (int(size[0]), int(size[1]))
     tail = tail or TailSpec.raw_u8()
     t = tail.c_struct(H, W)
@@ -479,6 +564,33 @@ def crop_resize(batch_u8: torch.Tensor, size, boxes=None, rng=None, tail: TailSp
             raise ValueError("need one box (x0, y0, w, h) per image")
     cfg = rng if rng is not None else crop_cfg(oh)
     with torch.cuda.device(dev):
-        check(lib.faa_crop_resize(batch_u8.data_ptr(), out.data_ptr(), B, H, W, C.byref(t),
-                                  d_boxes.data_ptr() if d_boxes is not None else None, C.byref(cfg), _stream_ptr(dev)))
+        if ragged:
+            h_desc, d_desc = batch_u8.descriptors()
+            check(lib.faa_crop_resize_ragged(h_desc.ctypes.data, d_desc.data_ptr(), B, out.data_ptr(), C.byref(t),
+                                             d_boxes.data_ptr() if d_boxes is not None else None, C.byref(cfg),
+                                             _stream_ptr(dev)))
+        else:
+            check(lib.faa_crop_resize(batch_u8.data_ptr(), out.data_ptr(), B, H, W, C.byref(t),
+                                      d_boxes.data_ptr() if d_boxes is not None else None, C.byref(cfg), _stream_ptr(dev)))
     return out
+
+
+def sample_philox_at(policy: CompiledPolicy, positions, h, w, tail: TailSpec, rng, device):
+    """Decisions of the global samples ``rng.first_index + positions[k]`` for h x w images, drawn on the device (C ABI
+    ``faa_sample_philox_at``): (samples, boxes) as CUDA uint8 tensors for ``augment_batch``."""
+    pos = torch.as_tensor(np.asarray(positions, dtype=np.int32), device=device)
+    n = int(pos.numel())
+    d_s = torch.empty(n * 16, dtype=torch.uint8, device=device)
+    d_b = torch.empty(max(1, n * policy.n_op * 8), dtype=torch.uint8, device=device)
+    t = tail.c_struct(h, w)
+    with torch.cuda.device(device):
+        check(lib.faa_sample_philox_at(policy.handle, n, int(h), int(w), C.byref(t), C.byref(rng), pos.data_ptr(),
+                                       d_s.data_ptr(), d_b.data_ptr(), _stream_ptr(device)))
+    return d_s, d_b
+
+
+def cached_tables(policy: CompiledPolicy):
+    """(number, bytes) of the per-size device tables of compiled ops the handle holds (C ABI ``faa_policy_cached_tables``)"""
+    n, b = C.c_int(), C.c_uint64()
+    check(lib.faa_policy_cached_tables(policy.handle, C.byref(n), C.byref(b)))
+    return int(n.value), int(b.value)

@@ -136,6 +136,17 @@ int faa_sample_policy_mt(const faa_policy_t* p, int batch, int h, int w,
 int faa_sample_philox(faa_policy_t* p, int batch, int h, int w, const faa_tail_t* tail,
                       const faa_rng_t* rng, faa_sample_t* d_samples, faa_box_t* d_boxes,
                       void* stream);
+/* the same sampler at given positions: record k (k < n) holds the decisions of global sample
+ * rng->first_index + d_pos[k] (d_pos: n non-negative int32 on the device; NULL = 0..n-1, which is
+ * faa_sample_philox), drawn for an h x w image.  The per-image Augmentation(policy) draws of the
+ * ImageNet train chain (data.py:60, 257-264) on a batch of mixed source sizes: the images of one
+ * size are augmented together, each with the decisions of its position in the batch. */
+int faa_sample_philox_at(faa_policy_t* p, int n, int h, int w, const faa_tail_t* tail,
+                         const faa_rng_t* rng, const int32_t* d_pos, faa_sample_t* d_samples,
+                         faa_box_t* d_boxes, void* stream);
+/* how many per-size device tables of compiled ops the handle holds, and their bytes (one per image
+ * size it has augmented or sampled; they live as long as the handle) */
+int faa_policy_cached_tables(faa_policy_t* p, int* n_tables, uint64_t* bytes);
 
 /* ---- the hot path: replaces, for a whole batch, Augmentation.__call__ (data.py:257-264)
  *      -> apply_augment (augmentations.py:192-194) -> the 19 ops (augmentations.py:13-144)
@@ -277,6 +288,17 @@ int faa_center_crop_box(int h, int w, int img_size, faa_crop_box_t* out);
  * distributions, not its stream).  An ordinary stream-ordered launch.  tail->use_zero_box and crop_pad are ignored. */
 int faa_crop_resize(const uint8_t* d_in, void* d_out, int batch, int h, int w, const faa_tail_t* tail,
                     const faa_crop_box_t* d_boxes, const faa_crop_cfg_t* cfg, void* stream);
+
+/* ---- the same crop + resize over a batch of differently sized images (data.py:61-62, 76-77, 267-345 run on one
+ * PIL image at a time, so each image is cropped at its own size): image i is h_images[i].h x h_images[i].w uint8 HWC
+ * at h_images[i].data (device memory, rows packed, any byte offset).  h_images is the host copy, used to validate and
+ * plan without waiting for the device; d_images is a device copy with the same contents, which the kernel reads.
+ * Boxes are drawn (or checked) against each image's own size, with the same Philox keys as faa_crop_resize, so a
+ * batch of equal sizes gives the same bytes as faa_crop_resize.  One launch. */
+typedef struct faa_image { const uint8_t* data; int32_t h, w; } faa_image_t;             /* 16 bytes */
+int faa_crop_resize_ragged(const faa_image_t* h_images, const faa_image_t* d_images, int batch, void* d_out,
+                           const faa_tail_t* tail, const faa_crop_box_t* d_boxes, const faa_crop_cfg_t* cfg,
+                           void* stream);
 
 /* number of kernels this library has launched since load (bench bookkeeping) */
 uint64_t faa_launch_count(void);
