@@ -94,6 +94,7 @@ def _load():
         "faa_center_crop_box": (C.c_int, [C.c_int, C.c_int, C.c_int, vp]),
         "faa_crop_resize": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, P(Tail), vp, P(CropCfg), vp]),
         "faa_crop_resize_ragged": (C.c_int, [vp, vp, C.c_int, vp, P(Tail), vp, P(CropCfg), vp]),
+        "faa_augment_ragged": (C.c_int, [vp, vp, vp, C.c_int, vp, vp, vp, vp, P(Rng), C.c_int, vp]),
         "faa_launch_count": (u64, []),
     }
     for name, (res, args) in sig.items():

@@ -237,6 +237,12 @@ struct faa_policy {
     int32_t ahead_ticket = 0;
     cudaStream_t chain_stream = nullptr; bool chain_live = false;   // the previous call was a chained step on this stream
     uintptr_t prev_out[2] = {0, 0}, prev_in[2] = {0, 0};            // byte ranges the previous chained step wrote / read
+    // faa_augment_ragged: per-call tables (per-size AugParams, RaggedImg, launch lists, copy jobs), programs, scratch
+    // images and re-aligned input copies (grown, never shrunk; stream-ordered reuse)
+    void* d_rg_tab = nullptr; size_t d_rg_tab_bytes = 0;
+    void* d_rg_progs = nullptr; size_t d_rg_progs_bytes = 0;
+    void* d_rg_scratch = nullptr; size_t d_rg_scratch_bytes = 0;
+    void* d_rg_copy = nullptr; size_t d_rg_copy_bytes = 0;
 };
 
 // All device state of a policy handle lives on ONE device: the one current at its first device call.
@@ -331,6 +337,7 @@ int faa_policy_destroy(faa_policy_t* p) {
     if (p->d_norm_img) cudaFree(p->d_norm_img);
     if (p->d_in) cudaFree(p->d_in);
     if (p->d_out) cudaFree(p->d_out);
+    for (void* b : {p->d_rg_tab, p->d_rg_progs, p->d_rg_scratch, p->d_rg_copy}) if (b) cudaFree(b);
     if (p->h_in_stage) cudaFreeHost(p->h_in_stage);
     if (p->h_out_stage) cudaFreeHost(p->h_out_stage);
     for (int i = 0; i < 2; ++i) {
@@ -1219,6 +1226,135 @@ int faa_crop_resize_ragged(const faa_image_t* h_images, const faa_image_t* d_ima
                           tail->out_w, tail->out_dtype, tail->mean, tail->std, reinterpret_cast<const CropBox*>(d_boxes), c,
                           t, (cudaStream_t)stream));
     g_launches++;
+    return FAA_OK;
+}
+
+// grows one of the handle's ragged-launch buffers; earlier calls' kernels that may still use it are ordered on `stream`
+// (follow_stream), so waiting for it before the free is enough
+static int grow_on_stream(void** ptr, size_t* have, size_t need, cudaStream_t stream) {
+    if (*have >= need) return FAA_OK;
+    if (*ptr) { CK(cudaStreamSynchronize(stream)); CK(cudaFree(*ptr)); *ptr = nullptr; *have = 0; }
+    need = std::max(need, (size_t)65536);
+    CK(cudaMalloc(ptr, need));
+    *have = need;
+    return FAA_OK;
+}
+
+static size_t align16(size_t v) { return (v + 15) & ~(size_t)15; }
+
+int faa_augment_ragged(faa_policy_t* p, const faa_image_t* h_in, const faa_image_t* d_in, int batch,
+                       const faa_image_t* h_out, const faa_image_t* d_out, const faa_sample_t* d_samples,
+                       const faa_box_t* d_boxes, const faa_rng_t* rng, int op_base, void* stream_v) {
+    if (!p || ((!h_in || !d_in || !h_out || !d_out) && batch > 0)) return fail(FAA_ERR_VALUE, "null argument");
+    if (batch < 0) return fail(FAA_ERR_VALUE, "negative batch");
+    if (batch > 65535) return fail(FAA_ERR_UNSUPPORTED, "at most 65535 images per call (one grid row per image): split the batch");
+    if (!d_samples && !rng) return fail(FAA_ERR_VALUE, "need either resolved samples or an rng config");
+    if (rng && !d_samples && (rng->crop_pad != 0 || rng->hflip != 0 || rng->zero_box_len != 0))
+        return fail(FAA_ERR_VALUE, "a ragged launch writes every image at its own size: the rng must have no crop_pad, hflip or "
+                                   "zero_box_len");
+    if (op_base < 0 || op_base >= p->n_op) return fail(FAA_ERR_VALUE, "op_base out of range");
+    std::vector<RaggedImageIn> ins((size_t)batch);
+    for (int i = 0; i < batch; ++i) {
+        const faa_image_t& a = h_in[i];
+        const faa_image_t& o = h_out[i];
+        const std::string who = "image " + std::to_string(i);
+        if (!a.data || !o.data) return fail(FAA_ERR_VALUE, who + " has no data");
+        if (check_shape(a.h, a.w)) return fail(FAA_ERR_VALUE, who + " has a size out of range");
+        if (o.h != a.h || o.w != a.w) return fail(FAA_ERR_VALUE, "output " + who + " is not the size of its input");
+        if ((a.w & 3) == 0 && ((uintptr_t)o.data & 3))
+            return fail(FAA_ERR_UNSUPPORTED, "output " + who + " must be 4-byte aligned when its width is a multiple of 4 "
+                                             "(vector stores)");
+        ins[(size_t)i] = {a.h, a.w, (uint32_t)((uintptr_t)a.data % 16), (uint32_t)((uintptr_t)o.data % 16)};
+    }
+    if (int e = ensure_device()) return e;
+    if (batch == 0) return FAA_OK;
+    if (int e = bind_device(p)) return e;
+    std::lock_guard<std::mutex> call_lk(p->call_mu);
+    cudaStream_t stream = (cudaStream_t)stream_v;
+    if (int e = follow_stream(p, stream)) return e;
+    const RaggedPlan plan = plan_ragged(ins.data(), batch, p->has_sg);
+
+    // per-size launch parameters (in / out / progs / scratch are patched in per image by the kernel)
+    const size_t n_geo = plan.geoms.size();
+    std::vector<const OpRec*> geo_ops(n_geo);
+    std::vector<AugParams> geo(n_geo);
+    for (size_t k = 0; k < n_geo; ++k) {
+        const RaggedGeom& g = plan.geoms[k];
+        // resolved samples can only reference ops the host sampler validated; Philox can pick anything
+        if (int e = device_table(p, g.H, g.W, d_samples == nullptr, &geo_ops[k])) return e;
+        AugParams& a = geo[k];
+        memset(&a, 0, sizeof a);
+        a.B = 1; a.H = a.out_h = g.H; a.W = a.out_w = g.W;
+        a.bands = g.plan.geo[0].bands; a.geo[0] = g.plan.geo[0]; a.geo[1] = g.plan.geo[1];
+        a.stage = g.plan.stage; a.band_cap = g.plan.geo[0].band_cap; a.octets = g.plan.octets; a.mat_cap = g.plan.mat_cap;
+        a.rcp_out_qpr = g.rcp_out_qpr; a.rcp_w = g.rcp_w; a.rcp_wq = g.rcp_wq; a.rcp_opr = g.rcp_opr;
+        for (int c = 0; c < 3; ++c) { a.scale[c] = 1.0f; a.bias[c] = 0.0f; }      // uint8 output: the byte value itself
+    }
+    // per image: scratch images (Sharpness -> gather) and re-aligned copies of inputs whose base breaks the 32-bit loads
+    // of W % 4 == 0 images, as byte offsets into the handle's buffers
+    std::vector<int64_t> scratch_at((size_t)batch, -1), copy_at((size_t)batch, -1);
+    size_t scratch_bytes = 0, copy_bytes = 0;
+    int n_copy = 0;
+    for (int i = 0; i < batch; ++i) {
+        const RaggedGeom& g = plan.geoms[(size_t)plan.geom_of[(size_t)i]];
+        const size_t bytes = (size_t)g.H * g.W * 3;
+        if (g.plan.scratch) { scratch_at[(size_t)i] = (int64_t)scratch_bytes; scratch_bytes += align16(bytes); }
+        if ((g.W & 3) == 0 && ((uintptr_t)h_in[i].data & 3)) { copy_at[(size_t)i] = (int64_t)copy_bytes; copy_bytes += align16(bytes); ++n_copy; }
+    }
+    const size_t off_img = align16(n_geo * sizeof(AugParams));
+    const size_t off_list = off_img + align16((size_t)batch * sizeof(RaggedImg));
+    const size_t off_copy = off_list + align16((size_t)batch * sizeof(int32_t));
+    const size_t tab_bytes = off_copy + (size_t)n_copy * sizeof(RaggedCopy);
+    if (int e = grow_on_stream(&p->d_rg_tab, &p->d_rg_tab_bytes, tab_bytes, stream)) return e;
+    if (int e = grow_on_stream(&p->d_rg_progs, &p->d_rg_progs_bytes, (size_t)batch * sizeof(Prog), stream)) return e;
+    if (scratch_bytes) { if (int e = grow_on_stream(&p->d_rg_scratch, &p->d_rg_scratch_bytes, scratch_bytes, stream)) return e; }
+    if (copy_bytes) { if (int e = grow_on_stream(&p->d_rg_copy, &p->d_rg_copy_bytes, copy_bytes, stream)) return e; }
+    uint8_t* d_tab = (uint8_t*)p->d_rg_tab;
+    std::vector<uint8_t> host(tab_bytes, 0);
+    memcpy(host.data(), geo.data(), n_geo * sizeof(AugParams));
+    RaggedImg* imgs = reinterpret_cast<RaggedImg*>(host.data() + off_img);
+    RaggedCopy* copies = reinterpret_cast<RaggedCopy*>(host.data() + off_copy);
+    for (int i = 0, c = 0; i < batch; ++i) {
+        const int k = plan.geom_of[(size_t)i];
+        RaggedImg& m = imgs[i];
+        m.ops = geo_ops[(size_t)k]; m.H = plan.geoms[(size_t)k].H; m.W = plan.geoms[(size_t)k].W;
+        m.allow = plan.geoms[(size_t)k].plan.allow; m.geom = k;
+        m.scratch = scratch_at[(size_t)i] < 0 ? nullptr : (uint8_t*)p->d_rg_scratch + scratch_at[(size_t)i];
+        m.realigned = nullptr;
+        if (copy_at[(size_t)i] >= 0) {
+            uint8_t* dst = (uint8_t*)p->d_rg_copy + copy_at[(size_t)i];
+            copies[c++] = {h_in[i].data, dst, (uint64_t)m.H * m.W * 3};
+            m.realigned = dst;
+        }
+    }
+    memcpy(host.data() + off_list, plan.order.data(), (size_t)batch * sizeof(int32_t));
+    CK(cudaMemcpyAsync(d_tab, host.data(), tab_bytes, cudaMemcpyHostToDevice, stream));   // (pageable: staged at once)
+    const RaggedImg* d_imgs = reinterpret_cast<const RaggedImg*>(d_tab + off_img);
+    if (n_copy) {
+        CK(launch_realign(reinterpret_cast<const RaggedCopy*>(d_tab + off_copy), n_copy, stream));
+        g_launches++;
+    }
+    // decisions -> programs, each image at its own size (Philox: global sample first_index + batch position)
+    ResolveParams R; memset(&R, 0, sizeof R);
+    R.probs = p->d_probs;
+    R.samples = reinterpret_cast<const Sample*>(d_samples); R.boxes = reinterpret_cast<const Box*>(d_boxes);
+    if (rng) memcpy(&R.rng, rng, sizeof(RngCfg));
+    R.progs = reinterpret_cast<Prog*>(p->d_rg_progs); R.first = 0; R.n = batch;
+    R.n_sub = p->n_sub; R.n_op = p->n_op; R.op_base = op_base;
+    R.apply_tail = (op_base + FAA_MAX_FUSED_OPS >= p->n_op) ? 1 : 0;
+    CK(launch_resolve_ragged(R, d_imgs, stream));
+    g_launches++;
+    // pixels: one cluster-kernel launch per band count, largest images first
+    for (const RaggedLaunch& L : plan.launches) {
+        RaggedParams rp;
+        rp.geoms = reinterpret_cast<const AugParams*>(d_tab); rp.imgs = d_imgs;
+        rp.in = reinterpret_cast<const CropImage*>(d_in); rp.out = reinterpret_cast<const CropImage*>(d_out);
+        rp.progs = reinterpret_cast<const Prog*>(p->d_rg_progs);
+        rp.list = reinterpret_cast<const int32_t*>(d_tab + off_list) + L.first;
+        CK(launch_augment_ragged(rp, L.bands, L.count, L.smem, stream));
+        g_launches++;
+    }
+    p->chain_live = false;                  // the next chained step follows this call in stream order
     return FAA_OK;
 }
 

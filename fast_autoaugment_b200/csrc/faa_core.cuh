@@ -18,6 +18,9 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <algorithm>
+#include <vector>
+
 #if defined(__CUDACC__)
 #define FAA_HD __host__ __device__ __forceinline__
 #else
@@ -914,6 +917,79 @@ inline LaunchPlan plan_launch(const PlanInput& in) {
     L.use_chain = (L.use_split || !in.out_u8) && in.allow_ahead && ahead;
     L.speculate = in.allow_ahead && ahead;
     return L;
+}
+
+// ---- ragged policy launches: one launch over images of many sizes, uint8 HWC out at each image's own size ----------
+// Each image runs the cluster kernel with the geometry plan_launch gives a uniform uint8 launch of that size alone (its
+// bands, staged band, chunk, octets, allow bits).  The cluster size is a launch attribute, so the images are grouped
+// into one pixel launch per band count present (1, 2, 4 or 8 CTAs per image).
+struct RaggedImageIn { int32_t H, W; uint32_t in_mod16, out_mod16; };   // an image's size and its buffers' bases mod 16
+
+struct RaggedGeom {                 // one distinct (size, staging, octets) of the batch
+    int32_t H, W;
+    LaunchPlan plan;                // plan_launch of a uniform uint8 launch of this size at these bases (unsplit)
+    uint32_t rcp_out_qpr, rcp_w, rcp_wq, rcp_opr;    // fastdiv reciprocals (AugParams)
+};
+
+struct RaggedLaunch { int32_t bands, first, count; uint32_t smem; };   // images order[first, first + count)
+
+struct RaggedPlan {
+    std::vector<RaggedGeom> geoms;
+    std::vector<int32_t> geom_of;   // [n] image -> geoms index
+    std::vector<int32_t> order;     // [n] image indices, launch by launch; each launch's images largest first
+    std::vector<RaggedLaunch> launches;   // largest first (by their first image): the large images start first
+};
+
+inline uint32_t fastdiv_rcp(uint32_t d) { return d <= 1 ? 0u : (uint32_t)((0x100000000ull + d - 1) / d); }
+
+inline RaggedPlan plan_ragged(const RaggedImageIn* imgs, int n, bool has_sg) {
+    RaggedPlan R;
+    R.geom_of.resize((size_t)n);
+    for (int i = 0; i < n; ++i) {
+        const RaggedImageIn& m = imgs[i];
+        PlanInput in = {};
+        in.H = m.H; in.W = m.W; in.out_h = m.H; in.out_w = m.W; in.batch = 1; in.out_u8 = true;
+        in.in_mod16 = m.in_mod16; in.out_mod16 = m.out_mod16; in.apply_tail = true; in.has_sg = has_sg;
+        in.split_min = UINT64_MAX;                        // the cluster kernel alone
+        const LaunchPlan L = plan_launch(in);
+        int k = 0;
+        while (k < (int)R.geoms.size() && !(R.geoms[k].H == m.H && R.geoms[k].W == m.W && R.geoms[k].plan.stage == L.stage &&
+                                            R.geoms[k].plan.octets == L.octets)) ++k;
+        if (k == (int)R.geoms.size()) {
+            RaggedGeom g;
+            g.H = m.H; g.W = m.W; g.plan = L;
+            g.rcp_out_qpr = fastdiv_rcp((uint32_t)(m.W + 3) / 4); g.rcp_w = fastdiv_rcp((uint32_t)m.W);
+            g.rcp_wq = fastdiv_rcp((uint32_t)m.W / 4); g.rcp_opr = (m.W & 7) ? 0u : fastdiv_rcp((uint32_t)m.W / 8);
+            R.geoms.push_back(g);
+        }
+        R.geom_of[(size_t)i] = k;
+    }
+    // largest first (pixels, then batch position): the order of the launches and of the images inside each
+    std::vector<int32_t> by_size((size_t)n);
+    for (int i = 0; i < n; ++i) by_size[(size_t)i] = i;
+    std::stable_sort(by_size.begin(), by_size.end(), [&](int32_t a, int32_t b) {
+        return (int64_t)imgs[a].H * imgs[a].W > (int64_t)imgs[b].H * imgs[b].W;
+    });
+    for (int32_t i : by_size) {
+        const RaggedGeom& g = R.geoms[(size_t)R.geom_of[(size_t)i]];
+        const int32_t bands = g.plan.geo[0].bands;
+        size_t l = 0;
+        while (l < R.launches.size() && R.launches[l].bands != bands) ++l;
+        if (l == R.launches.size()) R.launches.push_back({bands, 0, 0, 0u});
+        RaggedLaunch& L = R.launches[l];
+        ++L.count;
+        const uint32_t smem = (uint32_t)g.plan.geo[0].band_cap + (uint32_t)g.plan.mat_cap;
+        if (smem > L.smem) L.smem = smem;
+    }
+    int32_t at = 0;
+    for (RaggedLaunch& L : R.launches) { L.first = at; at += L.count; L.count = 0; }
+    R.order.resize((size_t)n);
+    for (int32_t i : by_size) {
+        size_t l = 0;
+        while (R.launches[l].bands != R.geoms[(size_t)R.geom_of[(size_t)i]].plan.geo[0].bands) ++l;
+        R.order[(size_t)(R.launches[l].first + R.launches[l].count++)] = i;
+    }
+    return R;
 }
 
 }  // namespace faa

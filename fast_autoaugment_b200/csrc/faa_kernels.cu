@@ -163,6 +163,40 @@ __global__ void __launch_bounds__(1024) faa_resolve_kernel(const __grid_constant
     }
 }
 
+// ragged launch (faa_augment_ragged): the same decisions -> program step, image i at its own size with its own op
+// table and allow bits (imgs[i]); Philox draws global sample rng.first_index + i.  No schedule: the host orders the images.
+__global__ void __launch_bounds__(1024) faa_resolve_ragged_kernel(const __grid_constant__ ResolveParams P, const RaggedImg* imgs) {
+    for (int i = threadIdx.x; i < P.n; i += blockDim.x) {
+        const RaggedImg m = imgs[i];
+        Sample s;
+        Box bx[8];
+        if (P.samples != nullptr) {
+            s = P.samples[i];
+            for (int j = 0; j < P.n_op; ++j) {
+                if (P.boxes != nullptr) bx[j] = P.boxes[(size_t)i * P.n_op + j];
+                else { bx[j].x0 = bx[j].y0 = 0; bx[j].x1 = bx[j].y1 = -1; }
+            }
+        } else {
+            philox_sample(P.rng, P.rng.first_index + (uint64_t)i, m.ops, P.probs, P.n_sub, P.n_op, m.H, m.W, m.H, m.W, s, bx);
+        }
+        Prog g;
+        build_prog(s, bx, m.ops, P.n_op, P.op_base, P.apply_tail, m.H, m.W, m.W, m.allow, g);
+        g.bucket = 0;
+        P.progs[i] = g;
+    }
+}
+
+// the library's aligned copies of ragged inputs whose base breaks the word loads: job blockIdx.y, 4 bytes per thread
+// and step (the byte count of an image with W % 4 == 0 is a multiple of 12)
+__global__ void __launch_bounds__(256) faa_realign_kernel(const RaggedCopy* jobs) {
+    const RaggedCopy j = jobs[blockIdx.y];
+    uint32_t* dst = reinterpret_cast<uint32_t*>(j.dst);
+    for (uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; k < j.bytes / 4; k += (uint64_t)gridDim.x * blockDim.x) {
+        const uint8_t* s = j.src + 4 * k;
+        dst[k] = (uint32_t)__ldg(s) | ((uint32_t)__ldg(s + 1) << 8) | ((uint32_t)__ldg(s + 2) << 16) | ((uint32_t)__ldg(s + 3) << 24);
+    }
+}
+
 #endif  // !FAA_TU_OUT
 
 // ---------------------------------------------------------------------------------------
@@ -1371,8 +1405,9 @@ static __device__ __noinline__ void self_resolve_prog(const AugParams& P, int i,
     *dst = g;
 }
 
+// entry: this cluster's schedule row (blockIdx.y of a uniform launch)
 template <int OUT, int NSRC, bool TAB>
-static __device__ __forceinline__ void cluster_kernel_body(const AugParams& P) {
+static __device__ __forceinline__ void cluster_kernel_body(const AugParams& P, int entry) {
     extern __shared__ __align__(128) uint8_t s_dyn[];           // NSRC staged row bands [+ materialisation chunk]
     cg::cluster_group cluster = cg::this_cluster();
     __shared__ ImgState st[NSRC];
@@ -1392,9 +1427,9 @@ static __device__ __forceinline__ void cluster_kernel_body(const AugParams& P) {
     wait_ticket(P.ready, P.ticket);
 
     // split launches: this (cluster) kernel owns the first n_heavy entries of the schedule
-    if (P.n_heavy != nullptr && (int)blockIdx.y >= ld_sched(P.n_heavy, P.chain)) return;      // cluster-uniform
+    if (P.n_heavy != nullptr && entry >= ld_sched(P.n_heavy, P.chain)) return;      // cluster-uniform
     // LPT schedule entry: a uniform load per warp (no shared-memory hand-off, no barrier)
-    const int img = P.order ? ld_sched(P.order + P.first + blockIdx.y, P.chain) : (int)blockIdx.y;
+    const int img = P.order ? ld_sched(P.order + P.first + entry, P.chain) : entry;
     int src_idx[NSRC];
     src_idx[0] = P.first + img;
     if constexpr (NSRC == 2) src_idx[1] = P.partner[img];
@@ -1513,9 +1548,31 @@ __device__ __forceinline__ void inplace_pointwise(const AugParams& P, uint8_t* b
 
 template <int OUT, int NSRC, bool TAB>
 __global__ void __launch_bounds__(kThreads, (NSRC == 1 ? FAA_MIN_CTAS : 2)) faa_augment_kernel(const __grid_constant__ AugParams P) {
-    cluster_kernel_body<OUT, NSRC, TAB>(P);
+    cluster_kernel_body<OUT, NSRC, TAB>(P, (int)blockIdx.y);
     count_done(P.done);                                          // (CTAs without an entry included)
 }
+
+#if defined(FAA_TU_OUT) && FAA_TU_OUT == 3   // OUT_U8_HWC
+// Ragged policy launch (faa_augment_ragged): cluster blockIdx.y runs image list[blockIdx.y] at its own size.  The
+// image's per-size launch parameters are copied into shared memory once per CTA and its pointers patched in; the body
+// is the uniform cluster kernel's, reading them from there (no order, no split, no chaining, uint8 HWC, one source).
+__global__ void __launch_bounds__(kThreads, FAA_MIN_CTAS) faa_augment_ragged_kernel(const __grid_constant__ RaggedParams R) {
+    __shared__ AugParams sP;
+    const int i = __ldg(R.list + blockIdx.y);
+    const RaggedImg& m = R.imgs[i];
+    const uint32_t* src = reinterpret_cast<const uint32_t*>(R.geoms + m.geom);
+    for (int k = threadIdx.x; k < (int)(sizeof(AugParams) / 4); k += blockDim.x) reinterpret_cast<uint32_t*>(&sP)[k] = __ldg(src + k);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        sP.in = m.realigned ? m.realigned : R.in[i].data;
+        sP.out = const_cast<uint8_t*>(R.out[i].data);
+        sP.scratch = m.scratch;
+        sP.progs = R.progs + i;
+    }
+    __syncthreads();
+    cluster_kernel_body<OUT_U8_HWC, 1, false>(sP, 0);
+}
+#endif
 
 // ---------------------------------------------------------------------------------------
 // launch 2b: the "mid" kernel of a three-way split: statistics -> per-channel LUT programs (AutoContrast, Equalize,
@@ -2311,6 +2368,26 @@ static cudaError_t launch_one(const AugParams& p, cudaStream_t stream) {
     return cudaLaunchKernelEx(&cfg, faa_augment_kernel<OUT, NSRC, TAB>, p);
 }
 
+#if defined(FAA_TU_OUT) && FAA_TU_OUT == 3   // OUT_U8_HWC
+cudaError_t launch_augment_ragged(const RaggedParams& r, int bands, int count, size_t smem, cudaStream_t stream) {
+    if (count <= 0) return cudaSuccess;
+    if (cudaError_t e = reserve_dyn_smem<faa_augment_ragged_kernel>(smem)) return e;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)bands, (unsigned)count, 1);
+    cfg.blockDim = dim3(kThreads, 1, 1);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)bands;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, faa_augment_ragged_kernel, r);
+}
+#endif
+
 static inline int rows_of(const AugParams& p) { return (p.grid_y > 0 && p.grid_y < p.B) ? p.grid_y : p.B; }
 
 template <int OUT, bool TAB>
@@ -2407,6 +2484,19 @@ cudaError_t launch_resolve(const ResolveParams& p, cudaStream_t stream) {
     cfg.attrs = attr;
     cfg.numAttrs = p.pdl ? 1 : 0;
     return cudaLaunchKernelEx(&cfg, faa_resolve_kernel, p);
+}
+
+cudaError_t launch_resolve_ragged(const ResolveParams& p, const RaggedImg* imgs, cudaStream_t stream) {
+    if (p.n <= 0) return cudaSuccess;
+    const int threads = p.n >= 1024 ? 1024 : ((p.n + 31) / 32) * 32;
+    faa_resolve_ragged_kernel<<<1, threads, 0, stream>>>(p, imgs);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_realign(const RaggedCopy* jobs, int n, cudaStream_t stream) {
+    if (n <= 0) return cudaSuccess;
+    faa_realign_kernel<<<dim3(64, (unsigned)n, 1), 256, 0, stream>>>(jobs);
+    return cudaGetLastError();
 }
 
 cudaError_t launch_mixup(const void* data, void* out, const int64_t* perm, int batch, int64_t n_per_sample,

@@ -89,6 +89,32 @@ unsigned augment_cta_count(const AugParams& p, int which);
 int resident_ctas_per_sm(int which);     // the launch bounds of the light (1) / mid (2) / cluster (0) kernel
 cudaError_t launch_augment(const AugParams& p, int out_type, bool use_tab, int which, cudaStream_t stream);   // which: 0 cluster, 1 light, 2 mid
 
+struct CropImage { const uint8_t* data; int32_t h, w; };               // == faa_image_t: one image of a ragged batch
+
+// ragged policy launch (faa_augment_ragged): what the resolve and cluster kernels need per image, by batch position
+struct RaggedImg {
+    const uint8_t* realigned;   // the library's 4-byte aligned copy of the input, or nullptr: the caller's descriptor
+    uint8_t* scratch;           // scratch image of the image's own size for Sharpness -> gather programs, or nullptr
+    const OpRec* ops;           // compiled table of the image's size [n_sub][n_op][2]
+    int32_t H, W;
+    int32_t allow;              // ResolveParams::allow of the image's geometry
+    int32_t geom;               // index of the image's per-size AugParams
+};
+// one launch of the cluster kernel over images list[0, count) of a ragged batch (grid (bands, count))
+struct RaggedParams {
+    const AugParams* geoms;     // per-size launch parameters (in / out / progs / scratch are per image)
+    const RaggedImg* imgs;      // [batch]
+    const CropImage* in;        // [batch] the caller's device descriptors
+    const CropImage* out;
+    const Prog* progs;          // [batch]
+    const int32_t* list;        // this launch's images, largest first
+};
+cudaError_t launch_resolve_ragged(const ResolveParams& p, const RaggedImg* imgs, cudaStream_t stream);
+cudaError_t launch_augment_ragged(const RaggedParams& r, int bands, int count, size_t smem, cudaStream_t stream);
+// copies n images to 4-byte aligned buffers: src[k] -> dst[k], bytes[k] (device arrays) in one launch
+struct RaggedCopy { const uint8_t* src; uint8_t* dst; uint64_t bytes; };
+cudaError_t launch_realign(const RaggedCopy* jobs, int n, cudaStream_t stream);
+
 cudaError_t launch_mixup(const void* data, void* out, const int64_t* perm, int batch, int64_t n_per_sample,
                          int dtype, float lam, float one_minus_lam, cudaStream_t stream);
 
@@ -99,7 +125,6 @@ cudaError_t launch_mix_u8(const uint8_t* a, const uint8_t* b, const int32_t* par
 cudaError_t launch_color_jitter(const uint8_t* in, uint8_t* out, const void* recs, int batch, int H, int W, cudaStream_t stream);
 // EfficientNet crop + bicubic resize (faa_crop_resize_kernel): output tile and shared-memory plan
 struct CropResizeTile { int32_t tile_w, tile_h, tw_shift, kx_cap, ky_cap, rows_cap; size_t smem; };
-struct CropImage { const uint8_t* data; int32_t h, w; };               // == faa_image_t: one image of a ragged batch
 CropResizeTile plan_crop_resize(int H, int W, int out_h, int out_w);     // smem == 0: nothing fits
 // images == nullptr: `in` is [batch][H][W][3]; else image i is images[i] (device array) and H x W is only the plan's size
 cudaError_t launch_crop_resize(const uint8_t* in, const CropImage* images, void* out, int batch, int H, int W, int out_h,

@@ -54,8 +54,19 @@ class Augmentation(object):
                       out=None):
         """uint8 [B,H,W,3] CUDA tensor -> augmented batch.  ``parity=True`` replays the global
         generators like the reference's per-sample loop; otherwise the kernel draws with Philox
-        keyed by (``seed``, ``first_index`` + i)."""
+        keyed by (``seed``, ``first_index`` + i).  A ``RaggedImages`` batch is augmented image by image at its own
+        size (uint8, ``tail`` raw) into a ``RaggedImages``; with ``parity`` each image's draws are made at its size,
+        in batch order, as calling this object on the images one after another would."""
         tail = tail or TailSpec.raw_u8()
+        if isinstance(batch_u8, RaggedImages):
+            if parity:
+                recs = [self.compiled.sample_parity(1, int(h), int(w), tail) for h, w in batch_u8.sizes]
+                samples = np.concatenate([s for s, _ in recs]) if recs else np.zeros(0, _lib.SAMPLE_DTYPE)
+                boxes = np.concatenate([b for _, b in recs]) if recs else np.zeros((0, self.compiled.n_op), _lib.BOX_DTYPE)
+                return augment_batch(self.compiled, batch_u8, tail, samples, boxes, out=out)
+            if seed is None:
+                seed = int(torch.randint(0, 2 ** 62, (1,)).item())
+            return augment_batch(self.compiled, batch_u8, tail, rng=make_rng(seed, first_index, tail), out=out)
         b, h, w, _ = batch_u8.shape
         if parity:
             samples, boxes = self.compiled.sample_parity(b, h, w, tail)

@@ -228,7 +228,16 @@ def augment_batch(policy: CompiledPolicy, batch_u8: torch.Tensor, tail: TailSpec
     mode; or rng (``make_rng``) - fused Philox mode.  partner/lam: fused Mixup; ``pool`` is the
     array partner indexes into (defaults to ``batch_u8`` itself), ``first`` the position of this
     batch inside the pool (multi-GPU global pairing).
+
+    A ``RaggedImages`` batch (differently sized images) is augmented image by image at its own size in one launch group
+    (C ABI ``faa_augment_ragged``) and returned as a ``RaggedImages`` of the same sizes: ``tail`` must be
+    ``TailSpec.raw_u8()``; ``out`` may be a ``RaggedImages`` of the same sizes; record i / global sample
+    ``rng.first_index + i`` belongs to image i, drawn at its size.  No ``partner``, ``pool`` or ``lighting_rgb``.
     """
+    if isinstance(batch_u8, RaggedImages):
+        if partner is not None or pool is not None or lighting_rgb is not None:
+            raise ValueError("a ragged batch takes no partner, pool or lighting_rgb: it is augmented at source size into uint8")
+        return _augment_ragged(policy, batch_u8, tail, samples, boxes, rng, out)
     _require_cuda(batch_u8, "batch")
     if batch_u8.dtype != torch.uint8 or batch_u8.dim() != 4 or batch_u8.shape[-1] != 3:
         raise ValueError("batch must be uint8 [B, H, W, 3]")
@@ -481,6 +490,14 @@ class RaggedImages:
             storage = torch.from_numpy(host).to(device)
         return RaggedImages(storage, offsets, sizes)
 
+    @staticmethod
+    def empty(sizes, device="cuda"):
+        """uninitialised images of the given (h, w) sizes, each starting on a 16-byte boundary of a fresh allocation"""
+        sizes = np.ascontiguousarray(sizes, dtype=np.int32).reshape(-1, 2)
+        slot = (sizes[:, 0].astype(np.int64) * sizes[:, 1] * 3 + 15) // 16 * 16
+        storage = torch.empty(int(slot.sum()), dtype=torch.uint8, device=device)
+        return RaggedImages(storage, np.cumsum(slot) - slot, sizes)
+
     def __len__(self):
         return len(self.sizes)
 
@@ -518,6 +535,47 @@ class RaggedImages:
             d["h"], d["w"] = self.sizes[:, 0], self.sizes[:, 1]
             self._desc = (d, torch.from_numpy(d.view(np.uint8).copy()).to(self.device))
         return self._desc
+
+
+def _augment_ragged(policy, batch: RaggedImages, tail, samples, boxes, rng, out):
+    """augment_batch on a RaggedImages batch (C ABI ``faa_augment_ragged``); policies of more than two ops run window
+    by window through uint8 intermediates, as ``_augment_launch`` does"""
+    raw = TailSpec.raw_u8()
+    if (tail.out_size, tail.crop_pad, tail.hflip, tail.cutout, tail.out_dtype) != \
+            (raw.out_size, raw.crop_pad, raw.hflip, raw.cutout, raw.out_dtype):
+        raise ValueError("a ragged batch is augmented at each image's own size into uint8: the tail must be TailSpec.raw_u8()")
+    if (samples is None) == (rng is None):
+        raise ValueError("give either samples (and boxes) or rng")
+    _require_cuda(batch.storage, "batch")
+    dev = batch.device
+    if out is None:
+        out = RaggedImages.empty(batch.sizes, dev)
+    elif not isinstance(out, RaggedImages) or not np.array_equal(out.sizes, batch.sizes) or out.device != dev:
+        raise ValueError("out must be a RaggedImages of the batch's sizes on its device")
+    if len(batch) == 0:
+        return out
+
+    def to_dev(a):
+        if a is None or isinstance(a, torch.Tensor):
+            if a is not None:
+                _require_cuda(a, "records")
+            return a
+        return torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1).copy()).to(dev)
+
+    d_s, d_b = to_dev(samples), to_dev(boxes)
+    rng_p = C.byref(rng) if rng is not None else None
+    B = len(batch)
+    with torch.cuda.device(dev):
+        stream = _stream_ptr(dev)
+        cur = batch
+        for base in range(0, policy.n_op, _lib.MAX_FUSED_OPS):
+            nxt = out if base + _lib.MAX_FUSED_OPS >= policy.n_op else RaggedImages.empty(batch.sizes, dev)
+            (h_in, d_in), (h_out, d_out) = cur.descriptors(), nxt.descriptors()
+            check(lib.faa_augment_ragged(policy.handle, h_in.ctypes.data, d_in.data_ptr(), B, h_out.ctypes.data,
+                                         d_out.data_ptr(), d_s.data_ptr() if d_s is not None else None,
+                                         d_b.data_ptr() if d_b is not None else None, rng_p, base, stream))
+            cur = nxt
+    return out
 
 
 def crop_resize(batch_u8, size, boxes=None, rng=None, tail: TailSpec | None = None, out=None):

@@ -300,6 +300,22 @@ int faa_crop_resize_ragged(const faa_image_t* h_images, const faa_image_t* d_ima
                            const faa_tail_t* tail, const faa_crop_box_t* d_boxes, const faa_crop_cfg_t* cfg,
                            void* stream);
 
+/* ---- the policy over a batch of differently sized images (data.py:253-264 Augmentation, called on one PIL image of
+ * any size at a time): image i (h_in[i].h x h_in[i].w uint8 HWC at h_in[i].data, device memory, rows packed, any byte
+ * offset) is augmented at its own size into h_out[i] (same size, uint8 HWC).  h_in / h_out are host copies, used to
+ * validate and plan without waiting for the device; d_in / d_out are device copies with the same contents, which the
+ * kernels read.  Output i equals faa_augment on image i alone with a uint8 HWC tail of its size:
+ *   d_samples == NULL: the decisions of global sample rng->first_index + i drawn for an h_i x w_i image (the records of
+ *                      faa_sample_philox_at at position i); the rng has no crop_pad, hflip or zero_box_len;
+ *   else             : d_samples[i] and d_boxes[i][n_op], drawn for image i's own size.
+ * op_base selects the FAA_MAX_FUSED_OPS-wide window as in faa_augment; every window writes uint8.  One resolve launch and
+ * one pixel launch per cluster size present (at most four), plus one copy launch when some image with w % 4 == 0 starts
+ * off a 4-byte boundary (the library re-aligns those inputs).  Output alignment: h_out[i].data 4-byte aligned when
+ * w % 4 == 0, else FAA_ERR_UNSUPPORTED.  batch <= 65535. */
+int faa_augment_ragged(faa_policy_t* p, const faa_image_t* h_in, const faa_image_t* d_in, int batch,
+                       const faa_image_t* h_out, const faa_image_t* d_out, const faa_sample_t* d_samples,
+                       const faa_box_t* d_boxes, const faa_rng_t* rng, int op_base, void* stream);
+
 /* number of kernels this library has launched since load (bench bookkeeping) */
 uint64_t faa_launch_count(void);
 

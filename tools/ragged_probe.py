@@ -10,6 +10,9 @@
    gathered images), the ragged crop-resize, ColorJitter, the jitter / Lighting records and HFlip + Lighting + Normalize;
    then the whole ``ImageNetChain.train`` call.  Also: policy groups per batch, and the per-size policy tables the
    handle has cached after the run.
+4. The ragged policy launch (``augment_batch`` on ``RaggedImages``) against the per-size groups on the same mixture
+   (packed back to back and 16-byte aligned), and against the uniform launch on b256 batches of one size (375x500, which
+   the uniform launch runs in the cluster kernel, and 480x640, which it splits into the light / mid kernels).
 
 Prints the card's name and power limit from the same run."""
 import argparse
@@ -137,6 +140,32 @@ def main():
     n_tab, nbytes = engine.cached_tables(pol)
     print("\n3. per-size policy tables cached by the handle after the run: %d tables, %.1f KB (%.1f KB each; never evicted)"
           % (n_tab, nbytes / 1024, nbytes / 1024 / max(1, n_tab)))
+
+    print("\n4. the ragged policy launch (faa_augment_ragged, uint8 at source size, Philox), alternated call by call")
+    rng_raw = engine.make_rng(1, 0, raw)
+    xa = RaggedImages.empty(x.sizes)                      # the same images, every one on a 16-byte boundary
+    for i in range(bb):
+        xa.image(i).copy_(x.image(i))
+    for name, src in (("packed back to back (from_list; W % 4 == 0 images re-aligned)", x), ("16-byte aligned images", xa)):
+        out = RaggedImages.empty(x.sizes)
+        want = chain._policy_ragged(src, None, 1, 0)
+        n0 = _lib.lib.faa_launch_count()
+        engine.augment_batch(pol, src, raw, rng=rng_raw, out=out)
+        torch.cuda.synchronize()
+        n_launch = _lib.lib.faa_launch_count() - n0
+        assert all(torch.equal(out.image(i), want.image(i)) for i in range(bb))
+        grp, rag = alternated([lambda: chain._policy_ragged(src, None, 1, 0),
+                               lambda: engine.augment_batch(pol, src, raw, rng=rng_raw, out=out)], args.iters)
+        print("  b256 mixture, %-62s per-size groups %8.1f us   ragged %8.1f us (%d launches)" % (name, grp, rag, n_launch))
+    for h, w in ((375, 500), (480, 640)):
+        xu = torch.from_numpy(rng.integers(0, 256, (bb, h, w, 3), dtype=np.uint8)).cuda()
+        r = RaggedImages(xu.view(-1), np.arange(bb, dtype=np.int64) * h * w * 3, [(h, w)] * bb)
+        ou, orag = torch.empty_like(xu), RaggedImages.empty(r.sizes)
+        uni, rag = alternated([lambda: engine.augment_batch(pol, xu, raw, rng=rng_raw, out=ou),
+                               lambda: engine.augment_batch(pol, r, raw, rng=rng_raw, out=orag)], args.iters)
+        assert all(torch.equal(orag.image(i), ou[i]) for i in range(bb))
+        print("  b256 of one size %dx%d: uniform augment_batch %8.1f us   ragged %8.1f us   (%+.1f %%)"
+              % (h, w, uni, rag, 100.0 * (rag / uni - 1)))
 
 
 if __name__ == "__main__":
