@@ -12,9 +12,19 @@ case; tests/test_gpu_geometries.py runs every case on the device against the ora
 CROP_CASES (RandomCrop: crop_pad and outputs smaller than the image) and MIX_CASES (fused Mixup, two sources) do the
 same for the other two inputs of the planner that change what the kernels run; tests/test_gpu_crop_mix_geometries.py
 runs them on the device.
+
+RAGGED_CASES does it for the ragged policy launch (`faa_augment_ragged`, planned by `plan_ragged`): one image per
+per-image geometry, named by `ragged_regime()`, and RAGGED_MIXES, the calls tests/test_gpu_ragged_geometries.py makes
+of them with the pixel launches each one claims.
 """
 import ctypes as C
+import os
+import subprocess
 from dataclasses import dataclass
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 STAGE_LIMIT = 150 * 1024     # bytes of staged band(s) per cluster-kernel CTA (both sources' together)
@@ -289,3 +299,168 @@ MIX_REGIMES = [
     "mix with a crop, staged",
     "mix with a crop, unstaged (doubled band)",
 ]
+
+
+# ------------------------------------------------------------------------------------- ragged policy launches --
+# `faa_augment_ragged` gives every image the cluster-kernel geometry `plan_launch` picks for a uniform uint8 launch of
+# that image alone (`plan_ragged`, csrc/faa_core.cuh) and groups the images into one pixel launch per cluster size; the
+# launch's dynamic shared memory is the largest band + chunk among its images.  A W % 4 == 0 image whose input does not
+# start on a 4-byte boundary is first copied to an aligned buffer (one more launch for the whole call).
+def load_emu_ragged_plan():
+    """the host build of `plan_ragged` (tests/emu/faa_emu_ragged_plan.cpp), built on demand with g++"""
+    so = os.path.join(ROOT, "tests", "emu", "libfaa_emu_ragged_plan.so")
+    src = os.path.join(ROOT, "tests", "emu", "faa_emu_ragged_plan.cpp")
+    core = os.path.join(ROOT, "fast_autoaugment_b200", "csrc", "faa_core.cuh")
+    if not os.path.exists(so) or os.path.getmtime(so) < max(os.path.getmtime(src), os.path.getmtime(core)):
+        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-o", so, src])
+    lib = C.CDLL(so)
+    vp = C.c_void_p
+    lib.faa_emu_ragged_geom_fields.restype = C.c_char_p
+    lib.faa_emu_plan_ragged.argtypes = [C.c_int, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp]
+    lib.faa_emu_plan_ragged.restype = C.c_int
+    return lib
+
+
+def plan_ragged(lib, sizes, in_mod16=None, out_mod16=None, has_sg=True):
+    """(geom_of [n], order [n], launches [(bands, first, count, smem)], geoms [dict]) of plan_ragged"""
+    n = len(sizes)
+    hw = np.ascontiguousarray(np.array(sizes, np.int32).reshape(-1, 2))
+    im = np.ascontiguousarray(np.zeros(n, np.int32) if in_mod16 is None else np.array(in_mod16, np.int32) % 16)
+    om = np.ascontiguousarray(np.zeros(n, np.int32) if out_mod16 is None else np.array(out_mod16, np.int32) % 16)
+    names = lib.faa_emu_ragged_geom_fields().decode().split()
+    geom_of, order = np.zeros(n, np.int32), np.zeros(n, np.int32)
+    launches = np.zeros((4, 4), np.int32)
+    geoms = np.zeros((max(n, 1), len(names)), np.int32)
+    ng = C.c_int32()
+    nl = lib.faa_emu_plan_ragged(n, hw.ctypes.data, im.ctypes.data, om.ctypes.data, int(has_sg), geom_of.ctypes.data,
+                                 order.ctypes.data, launches.ctypes.data, geoms.ctypes.data, C.byref(ng))
+    return geom_of, order, [tuple(int(v) for v in launches[k]) for k in range(nl)], \
+        [dict(zip(names, (int(v) for v in geoms[k]))) for k in range(ng.value)]
+
+
+def ragged_copied(W, in_off):
+    """the library re-aligns the input first (faa_cabi.cu faa_augment_ragged): the kernel's 32-bit loads of W % 4 == 0
+    rows need a 4-byte aligned base"""
+    return W % 4 == 0 and in_off % 4 != 0
+
+
+def ragged_regime(g, in_off=0, out_off=0):
+    """an image's regime in a ragged launch, from its `plan_ragged` geometry `g` and its input / output byte offsets
+    mod 16: (CTAs per image, staging, octets, chunk, scratch image).  Staging: "staged" (TMA), else why not, in the
+    planner's order - "base + copy" (read from the re-aligned copy), "size" (H * W * 3 % 16), "base" (input address),
+    "band" (over 150 KB).  Octets: the 8-pixel paths, else why not - W % 8, the output address, or an unstaged band."""
+    H, W = g["H"], g["W"]
+    if g["stage"]:
+        staging = "staged"
+    elif ragged_copied(W, in_off):
+        staging = "base + copy"
+    elif (H * W * 3) % 16:
+        staging = "size"
+    elif in_off % 16:
+        staging = "base"
+    else:
+        staging = "band"
+    if g["octets"]:
+        octets = "octets"
+    else:
+        octets = "no octets (%s)" % ("W % 8" if W % 8 else "output address" if out_off % 16 else "unstaged")
+    return (g["bands"], staging, octets, "chunk" if g["mat_cap"] else "no chunk",
+            "scratch" if g["scratch"] else "no scratch")
+
+
+# the values of each dimension of ragged_regime() the table must cover
+RAGGED_DIMENSIONS = [
+    (1, 2, 4, 8),
+    ("staged", "base + copy", "size", "base", "band"),
+    ("octets", "no octets (W % 8)", "no octets (output address)", "no octets (unstaged)"),
+    ("chunk", "no chunk"),
+    ("scratch", "no scratch"),
+]
+
+
+@dataclass
+class RaggedCase:
+    """one image of a ragged launch: its size, the byte offsets mod 16 of its input and output, and the regime it claims
+    (ragged_regime) under a policy with a Sharpness -> gather program"""
+    shape: tuple
+    regime: tuple
+    why: str
+    in_off: int = 0           # 0, 4, or odd (a W % 4 == 0 image is then copied first)
+    out_off: int = 0          # 0 or 4 (uint8 outputs of W % 4 == 0 images must be 4-byte aligned)
+
+    @property
+    def id(self):
+        s = "%dx%d" % self.shape
+        return s + ("_in%d" % self.in_off if self.in_off else "") + ("_out%d" % self.out_off if self.out_off else "")
+
+    @property
+    def big(self):
+        return max(self.shape) > 640
+
+
+def _rc(shape, bands, staging, octets, chunk, scratch, why, in_off=0, out_off=0):
+    return RaggedCase(shape, (bands, staging, octets, chunk, scratch), why, in_off, out_off)
+
+
+ST, COPY, SIZE, BASE, BAND = "staged", "base + copy", "size", "base", "band"
+OCT, W8, OUTA, UNST = "octets", "no octets (W % 8)", "no octets (output address)", "no octets (unstaged)"
+CH, NOCH, SCR, NOSCR = "chunk", "no chunk", "scratch", "no scratch"
+
+# Band and chunk sizes are bytes of dynamic shared memory; a launch takes the largest band + chunk of its images.
+RAGGED_CASES = [
+    _rc((128, 160), 4, ST, OCT, CH, SCR, "20480 quads: 4 CTAs of 32 rows; band 16384 B + chunk 16352 B"),
+    _rc((128, 164), 4, ST, W8, CH, SCR, "W % 8 == 4: no octets; band 16768 B"),
+    _rc((128, 160), 4, ST, OUTA, CH, SCR, "output 4 bytes past 16: no octets", out_off=4),
+    _rc((128, 160), 4, BASE, UNST, CH, SCR, "input 4 bytes past 16: no TMA staging, the chunk only", in_off=4),
+    _rc((128, 160), 4, COPY, UNST, CH, SCR, "odd input byte offset: re-aligned copy, planned unstaged", in_off=1),
+    _rc((8, 4000), 4, ST, OCT, NOCH, SCR, "2-row bands of 48000 B; pitch 12000 B: 16384 / pitch = 1 row, no chunk"),
+    _rc((8, 4000), 4, COPY, UNST, NOCH, SCR, "copied, no chunk: the lazy statistics from global memory", in_off=1),
+    _rc((5, 7620), 4, SIZE, W8, NOCH, SCR, "5 * 7620 * 3 % 16 == 4; W % 8 == 4; pitch 22860 B: no chunk"),
+    _rc((6, 3679), 4, SIZE, W8, NOCH, NOSCR, "W % 4 == 3: C_GENERIC only, no scratch image; no chunk"),
+    _rc((31, 600), 4, SIZE, UNST, CH, SCR, "31 * 600 * 3 % 16 == 8; W % 8 == 0 but unstaged: no octets"),
+    _rc((624, 640), 8, ST, OCT, CH, SCR, "78 + 2 halo rows of 1920 B: a staged band of exactly 153600 B, the limit; "
+        "+ chunk 15392 B = 168992 B of dynamic shared memory"),
+    _rc((632, 640), 8, BAND, UNST, CH, SCR, "79 + 2 rows: 155520 B > 150 KB, unstaged; chunk 15392 B"),
+    _rc((2048, 1536), 8, BAND, UNST, CH, SCR, "pitch 4608 B: a chunk of 3 rows"),
+    _rc((3000, 4000), 8, BAND, UNST, NOCH, SCR, "pitch 12000 B: 1 row, no chunk; no dynamic shared memory at all"),
+    _rc((17, 2048), 8, ST, OCT, NOCH, SCR, "3-row bands of 18432 B + halo; pitch 6144 B: 2 rows, no chunk"),
+    _rc((768, 1024), 8, COPY, UNST, CH, SCR, "a copied photo: 2.4 MB re-aligned", in_off=1),
+    _rc((8, 1024), 2, ST, OCT, CH, SCR, "2048 quads: 2 CTAs of 4 rows"),
+    _rc((3000, 2), 2, ST, W8, CH, NOSCR, "3000 quads; W % 4 == 2: no scratch image"),
+    _rc((2, 8192), 2, BASE, UNST, NOCH, SCR, "header limit: 2 one-row bands, input 4 bytes past 16; no chunk", in_off=4),
+    _rc((1, 1), 1, SIZE, W8, CH, NOSCR, "one pixel"),
+    _rc((64, 2), 1, ST, W8, CH, NOSCR, "32 quads: one CTA, a staged band of 384 B"),
+    _rc((3, 4), 1, COPY, W8, CH, SCR, "copied though 36 bytes would not stage anyway", in_off=1),
+    _rc((1, 8192), 1, ST, OCT, NOCH, SCR, "one row: one CTA, a staged band, pitch 24576 B: no chunk"),
+    _rc((8, 8192), 8, ST, OCT, NOCH, SCR, "header limit: 8 one-row bands of 73728 B, no chunk"),
+    _rc((8192, 8), 8, ST, OCT, CH, SCR, "header limit: 24-byte rows, bands of 24704 B"),
+    _rc((2, 8192), 2, ST, OCT, NOCH, SCR, "header limit: 2 one-row bands"),
+    _rc((8192, 2), 8, ST, W8, CH, NOSCR, "header limit: 6-byte rows, W % 4 == 2"),
+]
+
+# the header's largest image, its own GPU test (67 M pixels per histogram)
+RAGGED_HUGE = _rc((8192, 8192), 8, BAND, UNST, NOCH, SCR, "header limit: bands of 24 MB, no chunk")
+
+
+def ragged_case(case_id):
+    return next(c for c in RAGGED_CASES + [RAGGED_HUGE] if c.id == case_id)
+
+
+# The calls of tests/test_gpu_ragged_geometries.py, one image per case in this order, and the pixel launches plan_ragged
+# gives them: (CTAs per image, first, count, dynamic shared memory), largest images first.  Each call holds staged,
+# unstaged, chunk-less and copied images together; the first two have all four cluster sizes (four pixel launches, the
+# most a call can have).  Shared memory set by an image other than the launch's first: four_cluster_sizes - 624x640
+# behind 632x640 (8 CTAs), 8x4000 behind 5x7620 (4 CTAs); photos_and_limits - 8x8192 behind 2048x1536 and 768x1024;
+# smem_from_the_second_image - 624x640 behind 3000x4000, which needs none.
+RAGGED_MIXES = {
+    "four_cluster_sizes": (
+        ["632x640", "128x160", "128x164", "128x160_out4", "128x160_in4", "128x160_in1", "8x4000", "8x4000_in1", "5x7620",
+         "6x3679", "31x600", "624x640", "17x2048", "8x1024", "3000x2", "2x8192_in4", "1x1", "64x2", "3x4_in1", "1x8192"],
+        [(8, 0, 3, 168992), (4, 3, 10, 48000), (2, 13, 3, 33824), (1, 16, 4, 24576)]),
+    "photos_and_limits": (
+        ["2048x1536", "768x1024_in1", "8x8192", "8192x8", "2x8192", "8192x2", "128x160_in1", "3x4_in1"],
+        [(8, 0, 5, 73728), (4, 5, 1, 16352), (2, 6, 1, 49152), (1, 7, 1, 96)]),
+    "smem_from_the_second_image": (
+        ["3000x4000", "624x640", "128x160", "3x4_in1"],
+        [(8, 0, 2, 168992), (4, 2, 1, 32736), (1, 3, 1, 96)]),
+}

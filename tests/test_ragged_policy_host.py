@@ -2,54 +2,21 @@
 (tests/emu/faa_emu_ragged_plan.cpp) - every image covered once, each size's geometry that of a uniform uint8 launch of
 that size, one pixel launch per cluster size, largest first - and the C ABI's refusals before any device work."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
-from geometry_cases import LIMIT_SHAPES, PHOTO_SHAPES, plan
-from helpers import ROOT
+import geometry_cases as G
+from geometry_cases import LIMIT_SHAPES, PHOTO_SHAPES, load_emu_ragged_plan, plan, plan_ragged
 
 from fast_autoaugment_b200 import _lib, archive, engine
 from fast_autoaugment_b200.engine import RaggedImages, TailSpec
 
 
-def load_emu_ragged_plan():
-    so = os.path.join(ROOT, "tests", "emu", "libfaa_emu_ragged_plan.so")
-    src = os.path.join(ROOT, "tests", "emu", "faa_emu_ragged_plan.cpp")
-    core = os.path.join(ROOT, "fast_autoaugment_b200", "csrc", "faa_core.cuh")
-    if not os.path.exists(so) or os.path.getmtime(so) < max(os.path.getmtime(src), os.path.getmtime(core)):
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-o", so, src])
-    lib = C.CDLL(so)
-    vp = C.c_void_p
-    lib.faa_emu_ragged_geom_fields.restype = C.c_char_p
-    lib.faa_emu_plan_ragged.argtypes = [C.c_int, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp]
-    lib.faa_emu_plan_ragged.restype = C.c_int
-    return lib
-
-
 @pytest.fixture(scope="module")
 def emu_rp():
     return load_emu_ragged_plan()
-
-
-def plan_ragged(lib, sizes, in_mod16=None, out_mod16=None, has_sg=True):
-    """(geom_of [n], order [n], launches [(bands, first, count, smem)], geoms [dict]) of plan_ragged"""
-    n = len(sizes)
-    hw = np.ascontiguousarray(np.array(sizes, np.int32).reshape(-1, 2))
-    im = np.ascontiguousarray(np.zeros(n, np.int32) if in_mod16 is None else np.array(in_mod16, np.int32))
-    om = np.ascontiguousarray(np.zeros(n, np.int32) if out_mod16 is None else np.array(out_mod16, np.int32))
-    names = lib.faa_emu_ragged_geom_fields().decode().split()
-    geom_of, order = np.zeros(n, np.int32), np.zeros(n, np.int32)
-    launches = np.zeros((4, 4), np.int32)
-    geoms = np.zeros((max(n, 1), len(names)), np.int32)
-    ng = C.c_int32()
-    nl = lib.faa_emu_plan_ragged(n, hw.ctypes.data, im.ctypes.data, om.ctypes.data, int(has_sg), geom_of.ctypes.data,
-                                 order.ctypes.data, launches.ctypes.data, geoms.ctypes.data, C.byref(ng))
-    return geom_of, order, [tuple(int(v) for v in launches[k]) for k in range(nl)], \
-        [dict(zip(names, (int(v) for v in geoms[k]))) for k in range(ng.value)]
 
 
 def rcp(d):
@@ -129,6 +96,73 @@ def test_planner_groups_alignment_variants_of_one_size(emu_rp):
 def test_planner_empty_batch(emu_rp):
     geom_of, order, launches, geoms = plan_ragged(emu_rp, [])
     assert launches == [] and geoms == []
+
+
+# ------------------------------------------------------------------------- the ragged geometry table --
+@pytest.mark.parametrize("case", G.RAGGED_CASES + [G.RAGGED_HUGE], ids=lambda c: c.id)
+def test_every_ragged_case_is_in_the_regime_it_claims(emu_rp, case):
+    _, _, launches, geoms = plan_ragged(emu_rp, [case.shape], [case.in_off], [case.out_off])
+    assert G.ragged_regime(geoms[0], case.in_off, case.out_off) == case.regime, (case.id, geoms[0])
+    assert launches == [(case.regime[0], 0, 1, geoms[0]["band_cap"] + geoms[0]["mat_cap"])]
+    # only offsets the library accepts, each a different reason: aligned, 4 past 16 (no TMA base / no octets), odd
+    assert case.in_off in (0, 4) or case.in_off % 2 == 1
+    assert case.out_off in (0, 4)
+    # the same image without a Sharpness -> gather program: no scratch image, no allow bit 1
+    _, _, _, g = plan_ragged(emu_rp, [case.shape], [case.in_off], [case.out_off], has_sg=False)
+    assert not g[0]["scratch"] and g[0]["allow"] & 2 == 0
+    assert g[0]["allow"] == geoms[0]["allow"] & ~2
+    assert G.ragged_regime(g[0], case.in_off, case.out_off)[:4] == case.regime[:4]
+
+
+def test_every_value_of_every_ragged_dimension_has_a_case():
+    ids = [c.id for c in G.RAGGED_CASES]
+    assert len(ids) == len(set(ids))
+    for dim, values in enumerate(G.RAGGED_DIMENSIONS):
+        seen = {c.regime[dim] for c in G.RAGGED_CASES}
+        assert seen == set(values), (dim, {"without a case": set(values) - seen, "unlisted": seen - set(values)})
+    # the header limits are in the table (8192 x 8192 is its own GPU test)
+    assert {c.shape for c in G.RAGGED_CASES if not c.in_off and not c.out_off} >= set(LIMIT_SHAPES) - {(8192, 8192)}
+    assert G.RAGGED_HUGE.shape == (8192, 8192)
+
+
+def test_a_band_at_the_stage_limit_is_staged_and_one_row_more_is_not(emu_rp):
+    _, _, launches, g = plan_ragged(emu_rp, [(624, 640), (632, 640)])
+    assert [x["band_cap"] for x in g] == [G.STAGE_LIMIT, 0] and g[0]["stage"] and not g[1]["stage"]
+    assert launches == [(8, 0, 2, G.STAGE_LIMIT + g[0]["mat_cap"])] and g[0]["mat_cap"] == g[1]["mat_cap"] > 0
+
+
+@pytest.mark.parametrize("name", list(G.RAGGED_MIXES))
+def test_every_ragged_mixture_plans_the_launches_it_claims(emu_rp, name):
+    ids, want = G.RAGGED_MIXES[name]
+    cases = [G.ragged_case(i) for i in ids]
+    geom_of, order, launches, geoms = plan_ragged(emu_rp, [c.shape for c in cases], [c.in_off for c in cases],
+                                                  [c.out_off for c in cases])
+    assert launches == want, name
+    # each image keeps the geometry it has alone
+    for i, c in enumerate(cases):
+        assert G.ragged_regime(geoms[geom_of[i]], c.in_off, c.out_off) == c.regime, (name, c.id)
+    # a call mixes staged, unstaged, chunk-less and copied images
+    regimes = [c.regime for c in cases]
+    assert {"staged", "base + copy"} <= {r[1] for r in regimes} and len({r[1] for r in regimes}) >= 2
+    assert {"chunk", "no chunk"} == {r[3] for r in regimes}
+
+
+def test_the_ragged_mixtures_reach_every_case_and_launch_shape(emu_rp):
+    """every case runs in some mixture; some call has all four cluster sizes (four pixel launches, the most there can
+    be); some 8-CTA launch takes its shared memory from an image that is not its first"""
+    in_mixes = {i for ids, _ in G.RAGGED_MIXES.values() for i in ids}
+    assert in_mixes == {c.id for c in G.RAGGED_CASES}
+    assert any(len(want) == 4 for _, want in G.RAGGED_MIXES.values())
+    not_first = []
+    for name, (ids, want) in G.RAGGED_MIXES.items():
+        cases = [G.ragged_case(i) for i in ids]
+        geom_of, order, launches, geoms = plan_ragged(emu_rp, [c.shape for c in cases], [c.in_off for c in cases],
+                                                      [c.out_off for c in cases])
+        for bands, first, count, smem in launches:
+            g = geoms[geom_of[order[first]]]
+            if g["band_cap"] + g["mat_cap"] < smem:
+                not_first.append((name, bands))
+    assert ("four_cluster_sizes", 8) in not_first and ("smem_from_the_second_image", 8) in not_first, not_first
 
 
 # ------------------------------------------------------------------------------------------------------ C ABI --
