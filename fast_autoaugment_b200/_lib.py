@@ -28,7 +28,14 @@ JITTER_DTYPE = np.dtype([("alpha", "<f4", (3,)), ("order", "u1", (4,))])        
 CROP_BOX_DTYPE = np.dtype([("x0", "<i4"), ("y0", "<i4"), ("w", "<i4"), ("h", "<i4")])  # faa_crop_box_t
 IMAGE_DTYPE = np.dtype([("data", "<u8"), ("h", "<i4"), ("w", "<i4")])              # faa_image_t
 CROP_RANDOM, CROP_CENTER = 0, 1
+JPEG_HEADER_DTYPE = np.dtype([("offset", "<i8"), ("len", "<i8"), ("scan_off", "<i8"), ("scan_len", "<i8"),
+                              ("h", "<i4"), ("w", "<i4"), ("ncomp", "<i4"), ("hs", "<i4"), ("vs", "<i4"),
+                              ("restart", "<i4"), ("mcu_x", "<i4"), ("mcu_y", "<i4"), ("table_at", "<i4", (9,)),
+                              ("pool", "<i4", (9,)), ("qprec", "<i4"), ("reserved", "<i4")])   # faa_jpeg_header_t
+JPEG_TABLE_DTYPE = np.dtype([("q", "<u2", (64,)), ("bits", "u1", (16,)), ("vals", "u1", (256,))])   # faa_jpeg_table_t
+JPEG_TRUNCATED, JPEG_BAD_CODE, JPEG_BAD_COEF, JPEG_BAD_RESTART = 1, 2, 4, 8                       # faa_jpeg_status
 assert SAMPLE_DTYPE.itemsize == 16 and BOX_DTYPE.itemsize == 8 and IMAGE_DTYPE.itemsize == 16
+assert JPEG_HEADER_DTYPE.itemsize == 144 and JPEG_TABLE_DTYPE.itemsize == 400
 
 
 class Tail(C.Structure):          # faa_tail_t
@@ -95,6 +102,11 @@ def _load():
         "faa_crop_resize": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, P(Tail), vp, P(CropCfg), vp]),
         "faa_crop_resize_ragged": (C.c_int, [vp, vp, C.c_int, vp, P(Tail), vp, P(CropCfg), vp]),
         "faa_augment_ragged": (C.c_int, [vp, vp, vp, C.c_int, vp, vp, vp, vp, P(Rng), C.c_int, vp]),
+        "faa_jpeg_parse": (C.c_int, [C.c_char_p, C.c_size_t, vp]),
+        "faa_jpeg_tables": (C.c_int, [C.c_char_p, C.c_size_t, vp, vp]),
+        "faa_jpeg_decoder_create": (C.c_int, [P(vp)]),
+        "faa_jpeg_decoder_destroy": (C.c_int, [vp]),
+        "faa_jpeg_decode": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp]),
         "faa_launch_count": (u64, []),
     }
     for name, (res, args) in sig.items():

@@ -1569,3 +1569,153 @@ int faa_augment_host(faa_policy_t* p, const uint8_t* h_in, void* h_out, void* d_
 }
 
 }  // extern "C"
+
+// ------------------------------------------------------------------ JPEG decode --
+static_assert(sizeof(faa_jpeg_header_t) == sizeof(JpegHeader) && sizeof(JpegHeader) == 144 &&
+              offsetof(faa_jpeg_header_t, pool) == offsetof(JpegHeader, pool), "JPEG header layout");
+static_assert(sizeof(faa_jpeg_table_t) == sizeof(JpegTable), "JPEG table layout");
+
+struct faa_jpeg_decoder {
+    std::mutex mu;
+    int device = -1;                      // bound at the first decode, like a policy handle
+    void* d_coef = nullptr; size_t coef_bytes = 0;      // int16 coefficients of a call's images
+    void* d_segs = nullptr; size_t segs_bytes = 0;      // restart-segment starts
+    void* d_jobs = nullptr; size_t jobs_bytes = 0;      // per-call JpegJob table
+    cudaStream_t last_stream = nullptr; bool have_last_stream = false;
+    cudaEvent_t ev_switch = nullptr;
+};
+
+// grows a decoder buffer in stream order: the old one is released behind the work already queued on `stream`, so the
+// host never waits
+static int grow_async(void** ptr, size_t* have, size_t need, cudaStream_t stream) {
+    if (*have >= need) return FAA_OK;
+    if (*ptr) { CK(cudaFreeAsync(*ptr, stream)); *ptr = nullptr; *have = 0; }
+    need = std::max(need + need / 4, (size_t)65536);
+    CK(cudaMallocAsync(ptr, need, stream));
+    *have = need;
+    return FAA_OK;
+}
+
+static int check_jpeg_header(const JpegHeader& h, int n_tables, const std::string& who) {
+    if (h.ncomp != 1 && h.ncomp != 3) return fail(FAA_ERR_VALUE, who + ": component count must be 1 or 3");
+    if (check_shape(h.h, h.w)) return fail(FAA_ERR_VALUE, who + ": size out of range");
+    const bool samp = h.ncomp == 1 ? (h.hs == 1 && h.vs == 1)
+                                   : ((h.hs == 1 && h.vs == 1) || (h.hs == 2 && h.vs == 1) || (h.hs == 2 && h.vs == 2));
+    if (!samp) return fail(FAA_ERR_VALUE, who + ": unsupported sampling factors");
+    if (h.mcu_x != (h.w + 8 * h.hs - 1) / (8 * h.hs) || h.mcu_y != (h.h + 8 * h.vs - 1) / (8 * h.vs))
+        return fail(FAA_ERR_VALUE, who + ": MCU counts do not match the size");
+    if (h.restart < 0 || h.offset < 0 || h.len < 0 || h.scan_off < 0 || h.scan_len < 0 || h.scan_off + h.scan_len > h.len)
+        return fail(FAA_ERR_VALUE, who + ": restart interval or byte ranges out of range");
+    for (int c = 0; c < h.ncomp; ++c)
+        for (int k = 0; k < 3; ++k)
+            if (h.pool[3 * k + c] < 0 || h.pool[3 * k + c] >= n_tables)
+                return fail(FAA_ERR_VALUE, who + ": table pool index out of range");
+    return FAA_OK;
+}
+
+extern "C" {
+
+int faa_jpeg_parse(const uint8_t* bytes, size_t len, faa_jpeg_header_t* out) {
+    if (!bytes || !out) return fail(FAA_ERR_VALUE, "null argument");
+    JpegHeader h;
+    const char* why = "";
+    const int e = parse_jpeg(bytes, len, h, &why);
+    memcpy(out, &h, sizeof h);
+    if (e == JPARSE_UNSUPPORTED) return fail(FAA_ERR_UNSUPPORTED, std::string("unsupported JPEG: ") + why);
+    if (e == JPARSE_MALFORMED) return fail(FAA_ERR_VALUE, std::string("malformed JPEG: ") + why);
+    return FAA_OK;
+}
+
+int faa_jpeg_tables(const uint8_t* bytes, size_t len, const faa_jpeg_header_t* hdr, faa_jpeg_table_t out[9]) {
+    if (!bytes || !hdr || !out) return fail(FAA_ERR_VALUE, "null argument");
+    JpegHeader h; memcpy(&h, hdr, sizeof h);
+    if (h.ncomp != 1 && h.ncomp != 3) return fail(FAA_ERR_VALUE, "header has no 1 or 3 components");
+    for (int c = 0; c < h.ncomp; ++c) {
+        const size_t qbytes = (h.qprec >> c & 1) ? 128 : 64;
+        if (h.table_at[c] < 0 || (size_t)h.table_at[c] + qbytes > len) return fail(FAA_ERR_VALUE, "quantisation table outside the file");
+        for (int t = 1; t < 3; ++t) {
+            const int32_t at = h.table_at[3 * t + c];
+            if (at < 0 || (size_t)at + 16 > len) return fail(FAA_ERR_VALUE, "Huffman table outside the file");
+            size_t total = 0;
+            for (int l = 0; l < 16; ++l) total += bytes[at + l];
+            if (total > 256 || (size_t)at + 16 + total > len) return fail(FAA_ERR_VALUE, "Huffman table outside the file");
+        }
+    }
+    jpeg_tables(bytes, h, reinterpret_cast<JpegTable*>(out));
+    return FAA_OK;
+}
+
+int faa_jpeg_decoder_create(faa_jpeg_decoder_t** out) {
+    if (!out) return fail(FAA_ERR_VALUE, "null argument");
+    *out = new faa_jpeg_decoder();
+    return FAA_OK;
+}
+
+int faa_jpeg_decoder_destroy(faa_jpeg_decoder_t* d) {
+    if (!d) return FAA_OK;
+    for (void* b : {d->d_coef, d->d_segs, d->d_jobs}) if (b) cudaFree(b);      // (waits for the work that uses them)
+    if (d->ev_switch) cudaEventDestroy(d->ev_switch);
+    delete d;
+    return FAA_OK;
+}
+
+int faa_jpeg_decode(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
+                    const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
+                    const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status, void* stream_v) {
+    if (!d || ((!h_headers || !d_headers || !d_tables || !d_src || !h_out || !d_out || !d_status) && batch > 0))
+        return fail(FAA_ERR_VALUE, "null argument");
+    if (batch < 0) return fail(FAA_ERR_VALUE, "negative batch");
+    if (batch > 65535) return fail(FAA_ERR_UNSUPPORTED, "at most 65535 images per call: split the batch");
+    std::vector<JpegJob> jobs((size_t)batch + 1);
+    int64_t blocks = 0, segs = 0, tiles = 0;
+    for (int i = 0; i < batch; ++i) {
+        JpegHeader h; memcpy(&h, &h_headers[i], sizeof h);
+        const std::string who = "image " + std::to_string(i);
+        if (int e = check_jpeg_header(h, n_tables, who)) return e;
+        if (!h_out[i].data) return fail(FAA_ERR_VALUE, "output " + who + " has no data");
+        if (h_out[i].h != h.h || h_out[i].w != h.w) return fail(FAA_ERR_VALUE, "output " + who + " is not the size of its JPEG");
+        jobs[(size_t)i] = {blocks, (int32_t)segs, (int32_t)tiles};
+        blocks += jpeg_image_blocks(h);
+        segs += jpeg_segments(h);
+        tiles += (int64_t)((h.w + kJpegTileW - 1) / kJpegTileW) * ((h.h + kJpegTileH - 1) / kJpegTileH);
+        if (segs > INT32_MAX || tiles > INT32_MAX) return fail(FAA_ERR_UNSUPPORTED, "batch too large: split it");
+    }
+    jobs[(size_t)batch] = {blocks, (int32_t)segs, (int32_t)tiles};
+    if (int e = ensure_device()) return e;
+    if (batch == 0) return FAA_OK;
+    int dev = -1;
+    if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); return fail(FAA_ERR_NO_DEVICE, "no current CUDA device"); }
+    std::lock_guard<std::mutex> lk(d->mu);
+    if (d->device < 0) d->device = dev;
+    if (d->device != dev)
+        return fail(FAA_ERR_VALUE, "JPEG decoder is bound to device " + std::to_string(d->device) + " but the current device is " +
+                    std::to_string(dev) + ": create one decoder per device");
+    cudaStream_t stream = (cudaStream_t)stream_v;
+    if (d->have_last_stream && d->last_stream != stream) {          // buffers are reused in the order of the calls
+        if (!d->ev_switch) CK(cudaEventCreateWithFlags(&d->ev_switch, cudaEventDisableTiming));
+        CK(cudaEventRecord(d->ev_switch, d->last_stream));
+        CK(cudaStreamWaitEvent(stream, d->ev_switch, 0));
+    }
+    d->last_stream = stream; d->have_last_stream = true;
+    if (int e = grow_async(&d->d_coef, &d->coef_bytes, (size_t)blocks * 128, stream)) return e;
+    if (int e = grow_async(&d->d_segs, &d->segs_bytes, (size_t)segs * sizeof(int32_t), stream)) return e;
+    if (int e = grow_async(&d->d_jobs, &d->jobs_bytes, jobs.size() * sizeof(JpegJob), stream)) return e;
+    CK(cudaMemcpyAsync(d->d_jobs, jobs.data(), jobs.size() * sizeof(JpegJob), cudaMemcpyHostToDevice, stream));  // (pageable: staged at once)
+    JpegDecodeParams P;
+    P.hdrs = reinterpret_cast<const JpegHeader*>(d_headers);
+    P.pool = reinterpret_cast<const JpegTable*>(d_tables);
+    P.src = d_src;
+    P.jobs = reinterpret_cast<const JpegJob*>(d->d_jobs);
+    P.out = reinterpret_cast<const CropImage*>(d_out);
+    P.coef = reinterpret_cast<int16_t*>(d->d_coef);
+    P.segs = reinterpret_cast<int32_t*>(d->d_segs);
+    P.status = d_status;
+    P.batch = batch;
+    CK(launch_jpeg_entropy(P, stream));
+    g_launches++;
+    CK(launch_jpeg_reconstruct(P, (int)tiles, stream));
+    g_launches++;
+    return FAA_OK;
+}
+
+}  // extern "C"

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include "faa_core.cuh"
+#include "faa_jpeg.cuh"
 
 namespace faa {
 
@@ -131,5 +132,26 @@ cudaError_t launch_crop_resize(const uint8_t* in, const CropImage* images, void*
                                int out_w, int out_type, const float mean[3], const float std[3], const CropBox* boxes,
                                const CropCfg& cfg, const CropResizeTile& t, cudaStream_t stream);
 cudaError_t launch_lighting_tables(const float* rgb, float* tabs, int n, const float mean[3], const float std[3], cudaStream_t stream);
+
+// baseline JPEG decode (faa_jpeg.cu): what one faa_jpeg_decode call hands its two kernels
+struct JpegJob {                // per image of the call, plus one sentinel entry holding the total tile count
+    int64_t coef;               // first block of the image's coefficient planes in `coef`
+    int32_t seg;                // first entry of the image's restart-segment starts in `segs`
+    int32_t tile0;              // first reconstruct CTA of the image
+};
+struct JpegDecodeParams {
+    const JpegHeader* hdrs;     // [batch] (device copy)
+    const JpegTable* pool;      // table pool the headers index
+    const uint8_t* src;         // file i is bytes [hdrs[i].offset, + hdrs[i].len)
+    const JpegJob* jobs;        // [batch + 1]
+    const CropImage* out;       // [batch] uint8 HWC destinations
+    int16_t* coef;              // coefficient buffer (the decoder handle's)
+    int32_t* segs;              // restart-segment starts, relative to each scan (-1: marker not found)
+    int32_t* status;            // [batch] JpegStatus bits
+    int32_t batch;
+};
+constexpr int kJpegTileW = 64, kJpegTileH = 32;    // output pixels of one reconstruct CTA
+cudaError_t launch_jpeg_entropy(const JpegDecodeParams& p, cudaStream_t stream);
+cudaError_t launch_jpeg_reconstruct(const JpegDecodeParams& p, int n_tiles, cudaStream_t stream);
 
 }  // namespace faa

@@ -22,8 +22,9 @@ from torch.utils.data import Sampler, SubsetRandomSampler
 
 from . import _lib, archive
 from .conf import Config as C
-from .engine import (CIFAR_MEAN, CIFAR_STD, IMAGENET_MEAN, IMAGENET_STD, CompiledPolicy, RaggedImages, TailSpec,
-                     augment_batch, center_crop_box, crop_cfg, crop_resize, make_rng, sample_philox_at)
+from .engine import (CIFAR_MEAN, CIFAR_STD, IMAGENET_MEAN, IMAGENET_STD, CompiledPolicy, EncodedImages, RaggedImages,
+                     TailSpec, augment_batch, center_crop_box, crop_cfg, crop_resize, decode_jpeg, make_rng,
+                     sample_philox_at)
 
 
 class Augmentation(object):
@@ -292,7 +293,10 @@ class ImageNetChain(object):
     the policy once per distinct source size (the images of that size gathered, each with the decisions of its batch
     position: ``faa_sample_philox_at``, or its parity records) into a packed uint8 intermediate, then one ragged
     crop-resize, and the same jitter and flip + Lighting + Normalize launches as a uniform batch.  A batch of one size
-    gives the bytes of the uniform chain.  The policy handle keeps one compiled table per source size it has seen."""
+    gives the bytes of the uniform chain.  The policy handle keeps one compiled table per source size it has seen.
+
+    An ``EncodedImages`` batch (JPEG files) is decoded on the device first (``decode_jpeg``, bit-exact with the reference's
+    Pillow loader) and then runs the ragged path; the decode status of its images is left in ``last_status``."""
 
     _EIGVAL = _IMAGENET_PCA["eigval"]
     _EIGVEC = _IMAGENET_PCA["eigvec"]
@@ -307,6 +311,12 @@ class ImageNetChain(object):
         self.flip_policy = CompiledPolicy([[("Invert", -1.0, 0.0)]])       # a slot that never fires and draws nothing
         self.tail = TailSpec(None, 0, True, IMAGENET_MEAN, IMAGENET_STD, 0, out_dtype)
         self.test_tail = TailSpec(None, 0, False, IMAGENET_MEAN, IMAGENET_STD, 0, out_dtype)
+        self.last_status = None
+
+    def _decoded(self, batch):
+        if isinstance(batch, EncodedImages):
+            batch, self.last_status = decode_jpeg(batch)
+        return batch
 
     def sample_parity(self, n, h=None, w=None, sizes=None):
         """per-image records in the reference's draw order: (policy samples, policy boxes or None, crop boxes,
@@ -359,6 +369,7 @@ class ImageNetChain(object):
     def train(self, batch_u8, parity=False, seed=0, first_index=0, records=None):
         """uint8 [B,H,W,3] CUDA (or ``RaggedImages``) -> [B, 3, s, s] ``out_dtype``.  ``records``: the tuple of
         ``sample_parity`` (drawn here when ``parity`` and not given)."""
+        batch_u8 = self._decoded(batch_u8)
         if isinstance(batch_u8, RaggedImages):
             return self._train_ragged(batch_u8, parity, seed, first_index, records)
         b, h, w, _ = batch_u8.shape
@@ -435,8 +446,8 @@ class ImageNetChain(object):
 
     def test(self, batch_u8, out=None):
         """uint8 [B,H,W,3] CUDA (or ``RaggedImages``) -> [B, 3, s, s]: center crop + resize + ToTensor + Normalize, one
-        launch"""
-        return crop_resize(batch_u8, self.input_size, rng=self.center.cfg(), tail=self.test_tail, out=out)
+        launch (an ``EncodedImages`` batch is decoded first)"""
+        return crop_resize(self._decoded(batch_u8), self.input_size, rng=self.center.cfg(), tail=self.test_tail, out=out)
 
 
 def policy_by_conf_name(aug):
@@ -515,6 +526,29 @@ class RaggedDeviceDataset:
         return d
 
 
+class EncodedDeviceDataset:
+    """``RaggedDeviceDataset`` of JPEG files: the files' bytes stay on the device (``EncodedImages``, headers parsed
+    once here) and every batch is decoded on the device before its chain runs."""
+
+    def __init__(self, files, targets, device="cuda"):
+        self.images = files if isinstance(files, EncodedImages) else EncodedImages.from_bytes(files, device)
+        self.targets = [int(t) for t in targets]
+        if len(self.targets) != len(self.images):
+            raise ValueError("need one target per image")
+        self.labels = torch.as_tensor(self.targets, dtype=torch.int64, device=device)
+
+    def __len__(self):
+        return len(self.images)
+
+    def subset(self, idx):
+        idx = [int(i) for i in idx]
+        d = EncodedDeviceDataset.__new__(EncodedDeviceDataset)
+        d.images = self.images.select(idx)
+        d.targets = [self.targets[i] for i in idx]
+        d.labels = self.labels.index_select(0, torch.as_tensor(idx, dtype=torch.int64, device=self.labels.device))
+        return d
+
+
 class GpuAugmentedLoader:
     """What ``get_dataloaders`` hands to ``train.py:47`` / ``search.py:101`` instead of a torch ``DataLoader``:
     an iterable of ``(data, label)`` whose ``data`` is the augmented, normalised CUDA batch (``.cuda()`` at
@@ -527,10 +561,10 @@ class GpuAugmentedLoader:
     torch generators (a ``num_workers=0`` DataLoader); the default draws on the device with Philox.
     """
 
-    def __init__(self, dataset: DeviceDataset | RaggedDeviceDataset, batch, policies, tail: TailSpec, sampler=None, shuffle=False,
+    def __init__(self, dataset: DeviceDataset | RaggedDeviceDataset | EncodedDeviceDataset, batch, policies, tail: TailSpec, sampler=None, shuffle=False,
                  drop_last=False, seed=None, parity=False, chain=None, chain_mode="train"):
         """``chain``: an ``ImageNetChain`` that transforms the batches instead of the fused policy launch
-        (``chain_mode`` 'train' or 'test'); a ``RaggedDeviceDataset`` needs one."""
+        (``chain_mode`` 'train' or 'test'); a ``RaggedDeviceDataset`` or ``EncodedDeviceDataset`` needs one."""
         if not torch.cuda.is_available():
             raise _lib.FaaRuntimeError("fast_autoaugment_b200 needs a CUDA device (no CPU fallback)")
         self.dataset, self.batch_size, self.tail = dataset, int(batch), tail
@@ -538,7 +572,7 @@ class GpuAugmentedLoader:
         self.aug = Augmentation(policies) if policies is not None else Augmentation([[("Invert", 0.0, 0.0)]])
         self.seed = int(torch.initial_seed() if seed is None else seed) & 0x7FFFFFFFFFFFFFFF
         self.chain, self.chain_mode = chain, chain_mode
-        if isinstance(dataset, RaggedDeviceDataset) and chain is None:
+        if isinstance(dataset, (RaggedDeviceDataset, EncodedDeviceDataset)) and chain is None:
             raise ValueError("images of different sizes need an ImageNetChain (conf['faa_crop_resize'])")
         self._drawn = 0                   # samples drawn so far: the Philox counter never repeats across epochs
 
@@ -561,7 +595,7 @@ class GpuAugmentedLoader:
         for k in range(len(self)):
             idx = idx_all[k * self.batch_size:(k + 1) * self.batch_size]
             t = torch.as_tensor(idx, dtype=torch.int64).to(dev, non_blocking=True)
-            if isinstance(self.dataset, RaggedDeviceDataset):
+            if isinstance(self.dataset, (RaggedDeviceDataset, EncodedDeviceDataset)):
                 raw = self.dataset.images.select(idx)            # descriptors into the dataset's storage: no pixel copy
             else:
                 raw = self.dataset.images.index_select(0, t)
@@ -586,16 +620,27 @@ def _load_arrays(dataset, dataroot):
 
     ImageNet sources may differ in size: a mapping whose images are a list of uint8 HWC arrays of different sizes, or
     an .npz whose ``data`` is the images' bytes packed back to back with their ``sizes`` [N, 2] (h, w).  Those images
-    come back as a list of arrays."""
+    come back as a list of arrays.  ImageNet sources may also be JPEG files: a mapping whose images are a list of
+    ``bytes``, or an .npz with ``jpeg`` (the files packed back to back), ``lengths`` and ``targets``; they come back as a
+    list of ``bytes``, decoded on the device batch by batch."""
     base = dataset.replace("reduced_", "")
     ragged_ok = "imagenet" in dataset
 
     def images(x):
+        if ragged_ok and isinstance(x, (list, tuple)) and len(x) and all(isinstance(a, (bytes, bytearray)) for a in x):
+            return [bytes(a) for a in x]
         if ragged_ok and isinstance(x, (list, tuple)) and len({np.shape(a) for a in x}) > 1:
             return [np.asarray(a) for a in x]
         return np.asarray(x)
 
     def npz_images(z):
+        if ragged_ok and "jpeg" in z.files:
+            lengths = np.asarray(z["lengths"], np.int64).reshape(-1)
+            flat = np.asarray(z["jpeg"], np.uint8).reshape(-1)
+            if int(lengths.sum()) != flat.size:
+                raise ValueError("packed jpeg bytes do not match lengths")
+            ends = np.cumsum(lengths)
+            return [flat[e - n:e].tobytes() for e, n in zip(ends, lengths)]
         if ragged_ok and "sizes" in z.files:
             sizes = np.asarray(z["sizes"], np.int64).reshape(-1, 2)
             ends = np.cumsum(sizes[:, 0] * sizes[:, 1] * 3)
@@ -663,10 +708,12 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
     tr_x, tr_y, te_x, te_y = _load_arrays(dataset, dataroot)
     ragged = isinstance(tr_x, list) or isinstance(te_x, list)
     if ragged and not conf.get("faa_crop_resize", False):
-        raise ValueError("ImageNet images of different sizes need conf['faa_crop_resize']: without it the images are "
-                         "augmented at one fixed size")
+        raise ValueError("ImageNet images of different sizes (or JPEG files) need conf['faa_crop_resize']: without it the "
+                         "images are augmented at one fixed size")
 
     def device_dataset(x, y):
+        if isinstance(x, list) and len(x) and isinstance(x[0], bytes):
+            return EncodedDeviceDataset(x, y)
         return RaggedDeviceDataset(x, y) if isinstance(x, list) else DeviceDataset(x, y)
     if dataset in ("cifar10", "cifar100", "svhn", "imagenet"):
         total_trainset, testset = device_dataset(tr_x, tr_y), device_dataset(te_x, te_y)

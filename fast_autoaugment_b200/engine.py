@@ -537,6 +537,134 @@ class RaggedImages:
         return self._desc
 
 
+class EncodedImages:
+    """A batch or dataset of JPEG files: their bytes packed back to back in one device buffer, their headers parsed once
+    on the host (C ABI ``faa_jpeg_parse``), and the quantisation and Huffman tables they use deduplicated into one table
+    pool.  ``headers`` (host ``JPEG_HEADER_DTYPE`` [N]) is what ``decode_jpeg`` validates and plans from; their device
+    copy and the pool's are made on first use.  ``select`` makes a batch of some of the files without copying a byte of
+    them."""
+
+    def __init__(self, storage: torch.Tensor, headers, pool, _d_pool=None):
+        if not isinstance(storage, torch.Tensor) or storage.dtype != torch.uint8 or storage.dim() != 1 \
+                or not storage.is_contiguous():
+            raise ValueError("storage must be a contiguous 1-D uint8 tensor")
+        self.storage = storage
+        self.headers = np.ascontiguousarray(headers, dtype=_lib.JPEG_HEADER_DTYPE).reshape(-1)
+        self.pool = np.ascontiguousarray(pool, dtype=_lib.JPEG_TABLE_DTYPE).reshape(-1)
+        h = self.headers
+        if len(h) and (int(h["offset"].min()) < 0 or int((h["offset"] + h["len"]).max()) > storage.numel()):
+            raise ValueError("every file must lie inside the storage")
+        self._d_pool = _d_pool
+        self._d_headers = None
+
+    @staticmethod
+    def from_bytes(files, device="cuda"):
+        """JPEG files (``bytes``) -> EncodedImages on ``device``.  Raises ValueError naming every file the decoder
+        does not take (progressive, arithmetic, 12-bit, CMYK, other sampling, malformed ...) and why."""
+        files = [bytes(f) for f in files]
+        headers = np.zeros(len(files), dtype=_lib.JPEG_HEADER_DTYPE)
+        tabs = np.zeros(9, dtype=_lib.JPEG_TABLE_DTYPE)
+        pool, index, refused = [], {}, []
+        for i, f in enumerate(files):
+            hdr = headers[i:i + 1]
+            st = lib.faa_jpeg_parse(f, len(f), hdr.ctypes.data)
+            if st != _lib.OK:
+                refused.append("%d: %s" % (i, (lib.faa_last_error() or b"").decode()))
+                continue
+            check(lib.faa_jpeg_tables(f, len(f), hdr.ctypes.data, tabs.ctypes.data))
+            for slot in range(9):
+                if slot % 3 >= int(hdr["ncomp"][0]):
+                    continue
+                key = tabs[slot].tobytes()
+                if key not in index:
+                    index[key] = len(pool)
+                    pool.append(tabs[slot].copy())
+                headers["pool"][i, slot] = index[key]
+        if refused:
+            raise ValueError("JPEG files the decoder does not take: " + "; ".join(refused))
+        lengths = np.array([len(f) for f in files], dtype=np.int64)
+        headers["offset"] = np.cumsum(lengths) - lengths
+        packed = np.frombuffer(b"".join(files), dtype=np.uint8)
+        storage = torch.from_numpy(packed.copy()).to(device) if packed.size else torch.zeros(1, dtype=torch.uint8,
+                                                                                              device=device)
+        return EncodedImages(storage, headers, np.array(pool, dtype=_lib.JPEG_TABLE_DTYPE).reshape(-1))
+
+    def __len__(self):
+        return len(self.headers)
+
+    @property
+    def device(self):
+        return self.storage.device
+
+    @property
+    def sizes(self):
+        """(h, w) of every image, int32 [N, 2]"""
+        return np.stack([self.headers["h"], self.headers["w"]], axis=1).astype(np.int32).reshape(-1, 2)
+
+    def select(self, idx):
+        idx = np.asarray(idx, dtype=np.int64).reshape(-1)
+        return EncodedImages(self.storage, self.headers[idx], self.pool, self.device_pool())
+
+    def device_pool(self):
+        """the table pool on the device (shared by every ``select`` of this set)"""
+        if self._d_pool is None:
+            flat = self.pool.view(np.uint8).reshape(-1)
+            self._d_pool = torch.from_numpy(flat.copy() if flat.size else np.zeros(1, np.uint8)).to(self.device)
+        return self._d_pool
+
+    def device_headers(self):
+        if self._d_headers is None:
+            flat = self.headers.view(np.uint8).reshape(-1)
+            self._d_headers = torch.from_numpy(flat.copy() if flat.size else np.zeros(1, np.uint8)).to(self.device)
+        return self._d_headers
+
+
+class _JpegDecoder:
+    """C-ABI decoder handle (scratch of the decode calls); one per device"""
+
+    def __init__(self):
+        h = C.c_void_p()
+        check(lib.faa_jpeg_decoder_create(C.byref(h)))
+        self.handle = h
+
+    def __del__(self):
+        if getattr(self, "handle", None):
+            try:
+                lib.faa_jpeg_decoder_destroy(self.handle)
+            except Exception:
+                pass
+            self.handle = None
+
+
+_DECODERS = {}
+
+
+def decode_jpeg(encoded: EncodedImages, out: RaggedImages | None = None):
+    """Decode every file of ``encoded`` on its device (C ABI ``faa_jpeg_decode``: two launches, no host wait), bit-exact
+    with ``Image.open(f).convert('RGB')`` (reference imagenet.py:80).  Returns ``(images, status)``: a ``RaggedImages``
+    (``out``, by default ``RaggedImages.empty(encoded.sizes)``) and an int32 CUDA tensor of ``faa_jpeg_status`` bits per
+    image, 0 where the scan decoded completely; a corrupt image still gets defined pixels."""
+    _require_cuda(encoded.storage, "encoded")
+    dev = encoded.device
+    if out is None:
+        out = RaggedImages.empty(encoded.sizes, dev)
+    elif not isinstance(out, RaggedImages) or not np.array_equal(out.sizes, encoded.sizes) or out.device != dev:
+        raise ValueError("out must be a RaggedImages of the files' sizes on their device")
+    B = len(encoded)
+    status = torch.empty(max(B, 1), dtype=torch.int32, device=dev)[:B]
+    if B == 0:
+        return out, status
+    h_out, d_out = out.descriptors()
+    with torch.cuda.device(dev):
+        dec = _DECODERS.get(dev.index)
+        if dec is None:
+            dec = _DECODERS[dev.index] = _JpegDecoder()
+        check(lib.faa_jpeg_decode(dec.handle, encoded.headers.ctypes.data, encoded.device_headers().data_ptr(),
+                                  encoded.device_pool().data_ptr(), len(encoded.pool), encoded.storage.data_ptr(), B,
+                                  h_out.ctypes.data, d_out.data_ptr(), status.data_ptr(), _stream_ptr(dev)))
+    return out, status
+
+
 def _augment_ragged(policy, batch: RaggedImages, tail, samples, boxes, rng, out):
     """augment_batch on a RaggedImages batch (C ABI ``faa_augment_ragged``); policies of more than two ops run window
     by window through uint8 intermediates, as ``_augment_launch`` does"""

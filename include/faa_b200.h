@@ -316,6 +316,65 @@ int faa_augment_ragged(faa_policy_t* p, const faa_image_t* h_in, const faa_image
                        const faa_image_t* h_out, const faa_image_t* d_out, const faa_sample_t* d_samples,
                        const faa_box_t* d_boxes, const faa_rng_t* rng, int op_base, void* stream);
 
+/* ---- baseline JPEG decode: replaces torchvision's default_loader (imagenet.py:80, `Image.open(f).convert('RGB')`, Pillow
+ * on libjpeg-turbo with its default islow IDCT, fancy upsampling and fixed-point YCbCr->RGB) for a batch of files, bit-exact.
+ * Supported: SOF0 / SOF1 Huffman, 8-bit, one interleaved scan, 1 component (written R = G = B) or 3 in YCbCr (JFIF, or no
+ * Adobe transform 0) with luma sampling 1x1, 2x1 or 2x2 and chroma 1x1, any restart interval, up to FAA_MAX_DIM a side.
+ * Headers are parsed once on the host (when a dataset is built); the tables they use go into a caller-owned pool of
+ * faa_jpeg_table_t (deduplicated by the caller), which the headers index. */
+typedef struct faa_jpeg_header {
+    int64_t offset;           /* the file is bytes [offset, offset + len) of the decode call's d_src (parse: 0)       */
+    int64_t len;
+    int64_t scan_off;         /* entropy-coded data: bytes [scan_off, scan_off + scan_len) of the file               */
+    int64_t scan_len;
+    int32_t h, w;             /* image size                                                                          */
+    int32_t ncomp;            /* 1 (grayscale) or 3 (YCbCr)                                                          */
+    int32_t hs, vs;           /* luma sampling factors (chroma 1x1); 1, 1 for grayscale                              */
+    int32_t restart;          /* restart interval in MCUs, 0 = none                                                  */
+    int32_t mcu_x, mcu_y;     /* MCUs per row / per column                                                           */
+    int32_t table_at[9];      /* file offsets of the tables of components 0..2: quantisation [0..2], DC Huffman
+                                 [3..5], AC Huffman [6..8]; -1 for absent components                                 */
+    int32_t pool[9];          /* the same tables as indices into the caller's faa_jpeg_table_t pool (parse: -1)      */
+    int32_t qprec;            /* bit c: component c's quantisation table has 16-bit entries                          */
+    int32_t reserved;
+} faa_jpeg_header_t;          /* 144 bytes */
+
+typedef struct faa_jpeg_table {
+    uint16_t q[64];           /* quantisation table, natural (row-major) order; zero in a Huffman entry             */
+    uint8_t  bits[16];        /* Huffman table: number of codes of each length 1..16; zero in a quantisation entry  */
+    uint8_t  vals[256];       /*                symbols in code order                                                */
+} faa_jpeg_table_t;           /* 400 bytes */
+
+/* per-image status bits of faa_jpeg_decode (0 = the scan decoded completely) */
+enum faa_jpeg_status {
+    FAA_JPEG_TRUNCATED = 1,    /* the scan ended, or met a marker, before its last MCU; the rest of the image is zeros */
+    FAA_JPEG_BAD_CODE = 2,     /* a bit pattern that is no Huffman code                                              */
+    FAA_JPEG_BAD_COEF = 4,     /* a run past coefficient 63                                                          */
+    FAA_JPEG_BAD_RESTART = 8   /* not one restart marker per interval boundary                                       */
+};
+
+/* host only: parse one file's markers.  FAA_OK, FAA_ERR_UNSUPPORTED (progressive, arithmetic, lossless, 12-bit, Adobe
+ * RGB / CMYK / YCCK, other sampling, multi-scan; reason in faa_last_error()) or FAA_ERR_VALUE (malformed header). */
+int faa_jpeg_parse(const uint8_t* bytes, size_t len, faa_jpeg_header_t* out);
+/* host only: the 9 tables a parsed header refers to (table_at), in pool form; slots of absent components are zeroed */
+int faa_jpeg_tables(const uint8_t* bytes, size_t len, const faa_jpeg_header_t* hdr, faa_jpeg_table_t out[9]);
+
+/* a decoder handle owns the scratch of its calls (coefficients, restart-segment starts, per-call table), grown on demand
+ * in stream order; it is bound to the device current at its first decode, like a policy handle */
+typedef struct faa_jpeg_decoder faa_jpeg_decoder_t;
+int faa_jpeg_decoder_create(faa_jpeg_decoder_t** out);
+int faa_jpeg_decoder_destroy(faa_jpeg_decoder_t* dec);
+
+/* decodes `batch` files into uint8 HWC images.  h_headers / d_headers: host and device copies of the same headers (the
+ * host copy validates and plans without waiting for the device); d_tables: the pool of n_tables entries; d_src: the
+ * device bytes the headers' offsets point into; h_out / d_out: host and device copies of the destinations, each of its
+ * header's size (rows packed, any byte offset); d_status: [batch] int32 (device), enum faa_jpeg_status bits.  A corrupt
+ * scan never faults: its image gets a status and defined pixels.  Two launches (entropy decode, reconstruct), one
+ * cudaMemcpyAsync of the per-call table, no host wait. */
+int faa_jpeg_decode(faa_jpeg_decoder_t* dec, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
+                    const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
+                    const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status, void* stream);
+
 /* number of kernels this library has launched since load (bench bookkeeping) */
 uint64_t faa_launch_count(void);
 
