@@ -1635,6 +1635,7 @@ int faa_jpeg_tables(const uint8_t* bytes, size_t len, const faa_jpeg_header_t* h
         if (h.table_at[c] < 0 || (size_t)h.table_at[c] + qbytes > len) return fail(FAA_ERR_VALUE, "quantisation table outside the file");
         for (int t = 1; t < 3; ++t) {
             const int32_t at = h.table_at[3 * t + c];
+            if (jpeg_std_huff(at)) continue;                 // a standard table, not in the file
             if (at < 0 || (size_t)at + 16 > len) return fail(FAA_ERR_VALUE, "Huffman table outside the file");
             size_t total = 0;
             for (int l = 0; l < 16; ++l) total += bytes[at + l];

@@ -72,9 +72,6 @@ __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_entropy_kernel(const
     if (tid == 0) P.status[img] = s_status;
 }
 
-// component c's blocks [bx0, bx0 + nbx) x [by0, by0 + nby) cover what the tile reads of its plane
-struct TilePlane { int32_t bx0, by0, nbx, nby, first; };
-
 __global__ void __launch_bounds__(kReconThreads) faa_jpeg_reconstruct_kernel(const __grid_constant__ JpegDecodeParams P) {
     __shared__ uint16_t s_q[3][64];
     __shared__ int32_t s_ws[kReconMaxBlocks][64];
@@ -95,21 +92,13 @@ __global__ void __launch_bounds__(kReconThreads) faa_jpeg_reconstruct_kernel(con
     const int x0 = (t % tiles_x) * kJpegTileW, y0 = (t / tiles_x) * kJpegTileH;
     const int x1 = min(x0 + kJpegTileW, h.w), y1 = min(y0 + kJpegTileH, h.h);
     const int cw = jpeg_chroma_w(h), ch = jpeg_chroma_h(h);
-    TilePlane pl[3];
+    JpegTileWindow pl[3];
+    const int n_blocks = jpeg_tile_windows(h, x0, y0, x1, y1, pl);
     int64_t plane_base[3];
     int grid_w[3];
-    int n_blocks = 0;
     int64_t base = 0;
     for (int c = 0; c < 3; ++c) {
-        if (c >= h.ncomp) { pl[c] = {0, 0, 0, 0, n_blocks}; plane_base[c] = 0; grid_w[c] = 1; continue; }
-        int px0 = x0, px1 = x1 - 1, py0 = y0, py1 = y1 - 1;
-        if (c > 0) {
-            const int fx = h.hs == 2 ? 1 : 0, fy = h.vs == 2 ? 1 : 0;
-            px0 = max(0, x0 / h.hs - fx); px1 = min(cw - 1, (x1 - 1) / h.hs + fx);
-            py0 = max(0, y0 / h.vs - fy); py1 = min(ch - 1, (y1 - 1) / h.vs + fy);
-        }
-        pl[c] = {px0 >> 3, py0 >> 3, (px1 >> 3) - (px0 >> 3) + 1, (py1 >> 3) - (py0 >> 3) + 1, n_blocks};
-        n_blocks += pl[c].nbx * pl[c].nby;
+        if (c >= h.ncomp) { plane_base[c] = 0; grid_w[c] = 1; continue; }
         plane_base[c] = base;
         grid_w[c] = h.mcu_x * (c == 0 ? h.hs : 1);
         base += jpeg_plane_blocks(h, c);

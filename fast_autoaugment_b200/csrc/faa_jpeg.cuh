@@ -5,14 +5,17 @@
 // `Image.open(f).convert('RGB')`), i.e. Pillow on libjpeg-turbo with libjpeg's default decompression parameters:
 //   * Huffman decoding of a sequential scan (ITU T.81 F.2.2), DC prediction, de-zigzag;
 //   * JDCT_ISLOW: the integer separable IDCT of Loeffler, Ligtenberg and Moschytz with 13-bit constants, two extra
-//     bits of precision between the column and the row pass, descaling with round-half-up, and the range-limit
-//     table that adds +128 and clamps (indexed modulo 1024, as libjpeg's table is);
+//     bits of precision between the column and the row pass, descaling with round-half-up, and the range limit
+//     that adds +128 and saturates to 0..255, as libjpeg-turbo's SIMD islow IDCT on x86-64 does (libjpeg's C table
+//     wraps modulo 1024 instead; the two differ only on IDCT outputs outside [-512, 511]);
 //   * fancy upsampling (triangle filter) of 2x1 and 2x2 subsampled chroma, with its alternating rounding biases
 //     (+1/+2 horizontally, +8/+7 in 2-D) and the replication of the edge column / row of the downsampled plane;
 //     planes no more than two samples wide are replicated instead, as libjpeg does;
 //   * YCbCr -> RGB in 16-bit fixed point (R = Y + 1.402 Cr', G = Y - 0.34414 Cb' - 0.71414 Cr', B = Y + 1.772 Cb').
-// Every shift and bias below is part of that specification; tests/test_jpeg_host.py compares the result with Pillow
-// byte for byte.
+// Every shift and bias below is part of that specification; tests/test_jpeg_host.py and
+// tests/test_jpeg_streams_host.py compare the result with Pillow byte for byte.  It is exact for every stream whose
+// dequantised coefficients stay within what a forward DCT of 8-bit samples can produce (|coef * q| <= 1023 for AC,
+// <= 1024 for DC); beyond that libjpeg-turbo's SIMD IDCT wraps and saturates 16-bit lanes, which is not modelled.
 //
 // Streams: SOF0 / SOF1, 8-bit, one interleaved scan, 1 component or 3 components in YCbCr with luma sampling 1x1,
 // 2x1 or 2x2 and chroma 1x1, any restart interval.  Everything else is refused by parse_jpeg with a reason.
@@ -37,6 +40,7 @@ struct JpegHeader {
     int64_t scan_off, scan_len;       // entropy-coded data, relative to the file
     int32_t h, w, ncomp, hs, vs, restart, mcu_x, mcu_y;
     int32_t table_at[9];              // file offsets of the table payloads: quant c0..c2, DC c0..c2, AC c0..c2
+                                      // (a Huffman table no DHT defines: kJpegStdAt - k, standard table k)
     int32_t pool[9];                  // the same tables as indices into a JpegTable pool
     int32_t qprec;                    // bit c: component c's quantisation table has 16-bit entries
     int32_t reserved;
@@ -79,6 +83,39 @@ FAA_JHD int jpeg_zigzag(int k) {
 // ------------------------------------------------------------------------------------------------ header parsing --
 FAA_JHD int jpeg_u16(const uint8_t* p) { return (p[0] << 8) | p[1]; }
 
+// The Huffman tables of ITU T.81 K.3 (BITS, then HUFFVAL): DC 0, DC 1, AC 0, AC 1.  A scan whose table 0 or 1 no DHT
+// defines uses these, as libjpeg-turbo does (Motion-JPEG frames leave them out); its header's table_at then holds
+// kJpegStdAt - k for table k instead of a file offset.
+constexpr int32_t kJpegStdAt = -2;
+static const uint8_t kJpegStdHuff[4][16 + 162] = {
+    {0, 1, 5, 1, 1, 1, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11},
+    {0, 3, 1, 1, 1, 1, 1, 1, 1, 1, 1, 0, 0, 0, 0, 0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11},
+    {0, 2, 1, 3, 3, 2, 4, 3, 5, 5, 4, 4, 0, 0, 1, 125,
+     0x01, 0x02, 0x03, 0x00, 0x04, 0x11, 0x05, 0x12, 0x21, 0x31, 0x41, 0x06, 0x13, 0x51, 0x61, 0x07, 0x22, 0x71, 0x14,
+     0x32, 0x81, 0x91, 0xa1, 0x08, 0x23, 0x42, 0xb1, 0xc1, 0x15, 0x52, 0xd1, 0xf0, 0x24, 0x33, 0x62, 0x72, 0x82, 0x09,
+     0x0a, 0x16, 0x17, 0x18, 0x19, 0x1a, 0x25, 0x26, 0x27, 0x28, 0x29, 0x2a, 0x34, 0x35, 0x36, 0x37, 0x38, 0x39, 0x3a,
+     0x43, 0x44, 0x45, 0x46, 0x47, 0x48, 0x49, 0x4a, 0x53, 0x54, 0x55, 0x56, 0x57, 0x58, 0x59, 0x5a, 0x63, 0x64, 0x65,
+     0x66, 0x67, 0x68, 0x69, 0x6a, 0x73, 0x74, 0x75, 0x76, 0x77, 0x78, 0x79, 0x7a, 0x83, 0x84, 0x85, 0x86, 0x87, 0x88,
+     0x89, 0x8a, 0x92, 0x93, 0x94, 0x95, 0x96, 0x97, 0x98, 0x99, 0x9a, 0xa2, 0xa3, 0xa4, 0xa5, 0xa6, 0xa7, 0xa8, 0xa9,
+     0xaa, 0xb2, 0xb3, 0xb4, 0xb5, 0xb6, 0xb7, 0xb8, 0xb9, 0xba, 0xc2, 0xc3, 0xc4, 0xc5, 0xc6, 0xc7, 0xc8, 0xc9, 0xca,
+     0xd2, 0xd3, 0xd4, 0xd5, 0xd6, 0xd7, 0xd8, 0xd9, 0xda, 0xe1, 0xe2, 0xe3, 0xe4, 0xe5, 0xe6, 0xe7, 0xe8, 0xe9, 0xea,
+     0xf1, 0xf2, 0xf3, 0xf4, 0xf5, 0xf6, 0xf7, 0xf8, 0xf9, 0xfa},
+    {0, 2, 1, 2, 4, 4, 3, 4, 7, 5, 4, 4, 0, 1, 2, 119,
+     0x00, 0x01, 0x02, 0x03, 0x11, 0x04, 0x05, 0x21, 0x31, 0x06, 0x12, 0x41, 0x51, 0x07, 0x61, 0x71, 0x13, 0x22, 0x32,
+     0x81, 0x08, 0x14, 0x42, 0x91, 0xa1, 0xb1, 0xc1, 0x09, 0x23, 0x33, 0x52, 0xf0, 0x15, 0x62, 0x72, 0xd1, 0x0a, 0x16,
+     0x24, 0x34, 0xe1, 0x25, 0xf1, 0x17, 0x18, 0x19, 0x1a, 0x26, 0x27, 0x28, 0x29, 0x2a, 0x35, 0x36, 0x37, 0x38, 0x39,
+     0x3a, 0x43, 0x44, 0x45, 0x46, 0x47, 0x48, 0x49, 0x4a, 0x53, 0x54, 0x55, 0x56, 0x57, 0x58, 0x59, 0x5a, 0x63, 0x64,
+     0x65, 0x66, 0x67, 0x68, 0x69, 0x6a, 0x73, 0x74, 0x75, 0x76, 0x77, 0x78, 0x79, 0x7a, 0x82, 0x83, 0x84, 0x85, 0x86,
+     0x87, 0x88, 0x89, 0x8a, 0x92, 0x93, 0x94, 0x95, 0x96, 0x97, 0x98, 0x99, 0x9a, 0xa2, 0xa3, 0xa4, 0xa5, 0xa6, 0xa7,
+     0xa8, 0xa9, 0xaa, 0xb2, 0xb3, 0xb4, 0xb5, 0xb6, 0xb7, 0xb8, 0xb9, 0xba, 0xc2, 0xc3, 0xc4, 0xc5, 0xc6, 0xc7, 0xc8,
+     0xc9, 0xca, 0xd2, 0xd3, 0xd4, 0xd5, 0xd6, 0xd7, 0xd8, 0xd9, 0xda, 0xe2, 0xe3, 0xe4, 0xe5, 0xe6, 0xe7, 0xe8, 0xe9,
+     0xea, 0xf2, 0xf3, 0xf4, 0xf5, 0xf6, 0xf7, 0xf8, 0xf9, 0xfa}};
+
+// the standard table a Huffman table_at entry names, or nullptr when it is a file offset (or unset)
+inline const uint8_t* jpeg_std_huff(int32_t at) {
+    return at <= kJpegStdAt && at > kJpegStdAt - 4 ? kJpegStdHuff[kJpegStdAt - at] : nullptr;
+}
+
 // Parses the markers of a whole file (host only; done once per file when a dataset is built).  Returns JPARSE_*;
 // *why names the reason of a refusal.  h.offset = 0, h.len = len, pool[] = -1.
 inline int parse_jpeg(const uint8_t* b, size_t len, JpegHeader& h, const char** why) {
@@ -93,7 +130,7 @@ inline int parse_jpeg(const uint8_t* b, size_t len, JpegHeader& h, const char** 
     int32_t dqt_at[4] = {-1, -1, -1, -1}, dqt_prec[4] = {0, 0, 0, 0}, dht_at[2][4];
     for (int c = 0; c < 2; ++c) for (int k = 0; k < 4; ++k) dht_at[c][k] = -1;
     bool jfif = false, adobe = false, have_sof = false, have_scan = false;
-    int adobe_transform = -1, sof = 0;
+    int adobe_transform = -1;
     int comp_id[3] = {0, 0, 0}, comp_h[3] = {0, 0, 0}, comp_v[3] = {0, 0, 0}, comp_q[3] = {0, 0, 0};
     size_t i = 2;
     while (true) {
@@ -101,7 +138,7 @@ inline int parse_jpeg(const uint8_t* b, size_t len, JpegHeader& h, const char** 
             if (have_scan) break;                        // a file cut after its scan: decoded, status reports it
             FAA_BAD("file ends before its scan");
         }
-        if (b[i] != 0xFF) FAA_BAD("expected a marker");
+        while (i < len && b[i] != 0xFF) ++i;             // stray bytes before a marker: skipped, as libjpeg does
         while (i < len && b[i] == 0xFF) ++i;             // fill bytes
         if (i >= len) { if (have_scan) break; FAA_BAD("file ends before its scan"); }
         const int m = b[i++];
@@ -135,7 +172,7 @@ inline int parse_jpeg(const uint8_t* b, size_t len, JpegHeader& h, const char** 
                 if (comp_h[c] < 1 || comp_h[c] > 4 || comp_v[c] < 1 || comp_v[c] > 4) FAA_BAD("sampling factor out of range");
                 if (comp_q[c] > 3) FAA_BAD("quantisation table index out of range");
             }
-            h.ncomp = nf; sof = m; have_sof = true;
+            h.ncomp = nf; have_sof = true;
         } else if (m == 0xC2 || m == 0xC6 || m == 0xCA || m == 0xCE) {
             FAA_NO(m == 0xC2 ? "progressive coding" : m == 0xCA ? "progressive arithmetic coding" : "hierarchical coding");
         } else if (m == 0xC3 || m == 0xC7 || m == 0xCB || m == 0xCF) {
@@ -159,7 +196,8 @@ inline int parse_jpeg(const uint8_t* b, size_t len, JpegHeader& h, const char** 
                 for (int l = 0; l < 16; ++l) {
                     total += p[k + 1 + l];
                     code = (code + p[k + 1 + l]);
-                    if (code > (1u << (l + 1))) FAA_BAD("Huffman table with more codes than its lengths allow");
+                    // (>=: a table may not use the all-ones code of a length, T.81 C.2; libjpeg refuses it too)
+                    if (code >= (1u << (l + 1))) FAA_BAD("Huffman table with more codes than its lengths allow");
                     code <<= 1;
                 }
                 if (total > 256 || k + 17 + total > n) FAA_BAD("Huffman table symbol count out of range");
@@ -194,16 +232,18 @@ inline int parse_jpeg(const uint8_t* b, size_t len, JpegHeader& h, const char** 
             const int ns = p[0];
             if (n != 4 + 2 * ns) FAA_BAD("scan header length does not match its components");
             if (ns != h.ncomp) FAA_NO("a scan without every component (multi-scan sequential)");
-            const int max_tab = sof == 0xC0 ? 1 : 3;
             for (int c = 0; c < ns; ++c) {
                 if (p[1 + 2 * c] != comp_id[c]) FAA_NO("scan components out of frame order (multi-scan sequential)");
                 const int td = p[2 + 2 * c] >> 4, ta = p[2 + 2 * c] & 15;
-                if (td > max_tab || ta > max_tab) FAA_BAD("Huffman table index out of range for the frame type");
-                if (dht_at[0][td] < 0 || dht_at[1][ta] < 0) FAA_BAD("scan uses an undefined Huffman table");
+                // (tables 2 and 3 in a baseline frame too: libjpeg decodes them whatever the SOF says)
+                if (td > 3 || ta > 3) FAA_BAD("Huffman table index out of range");
+                const int32_t dc_at = dht_at[0][td] >= 0 ? dht_at[0][td] : td < 2 ? kJpegStdAt - td : -1;
+                const int32_t ac_at = dht_at[1][ta] >= 0 ? dht_at[1][ta] : ta < 2 ? kJpegStdAt - 2 - ta : -1;
+                if (dc_at == -1 || ac_at == -1) FAA_BAD("scan uses an undefined Huffman table");
                 if (dqt_at[comp_q[c]] < 0) FAA_BAD("component uses an undefined quantisation table");
                 h.table_at[c] = dqt_at[comp_q[c]];
-                h.table_at[3 + c] = dht_at[0][td];
-                h.table_at[6 + c] = dht_at[1][ta];
+                h.table_at[3 + c] = dc_at;
+                h.table_at[6 + c] = ac_at;
                 if (dqt_prec[comp_q[c]]) h.qprec |= 1 << c;
             }
             const uint8_t* q = p + 1 + 2 * ns;
@@ -252,7 +292,8 @@ inline void jpeg_tables(const uint8_t* b, const JpegHeader& h, JpegTable out[9])
         for (int k = 0; k < 64; ++k)
             out[c].q[kJpegZigzag[k]] = (h.qprec >> c & 1) ? (uint16_t)jpeg_u16(q + 2 * k) : q[k];
         for (int t = 1; t < 3; ++t) {
-            const uint8_t* d = b + h.table_at[3 * t + c];
+            const uint8_t* std_table = jpeg_std_huff(h.table_at[3 * t + c]);
+            const uint8_t* d = std_table ? std_table : b + h.table_at[3 * t + c];
             int total = 0;
             for (int l = 0; l < 16; ++l) { out[3 * t + c].bits[l] = d[l]; total += d[l]; }
             memcpy(out[3 * t + c].vals, d + 16, (size_t)total);
@@ -532,10 +573,11 @@ FAA_JHD void jpeg_idct_1d(const int32_t v[8], int32_t o[8], int shift) {
     o[3] = jpeg_descale(tmp13 + tmp0, shift); o[4] = jpeg_descale(tmp13 - tmp0, shift);
 }
 
-// libjpeg's post-IDCT range limit: +128, clamp to 0..255, the index taken modulo 1024
+// post-IDCT range limit: +128, saturated to 0..255 (libjpeg-turbo's x86-64 SIMD islow IDCT, which Pillow runs;
+// libjpeg's C table would wrap outputs outside [-512, 511] modulo 1024)
 FAA_JHD uint8_t jpeg_range_limit(int32_t x) {
-    const int32_t i = x & 1023;
-    return (uint8_t)(i < 128 ? i + 128 : i < 512 ? 255 : i < 896 ? 0 : i - 896);
+    const int32_t v = x + 128;
+    return (uint8_t)(v < 0 ? 0 : v > 255 ? 255 : v);
 }
 
 // column pass: column `col` of block `in` (natural order, stride 8) dequantised by q -> workspace column (stride 8)
@@ -594,6 +636,35 @@ FAA_JHD void jpeg_ycc_rgb(int y, int cb, int cr, uint8_t* o) {
 // downsampled chroma size
 FAA_JHD int jpeg_chroma_w(const JpegHeader& h) { return (h.w + h.hs - 1) / h.hs; }
 FAA_JHD int jpeg_chroma_h(const JpegHeader& h) { return (h.h + h.vs - 1) / h.vs; }
+
+// ------------------------------------------------------------------------------------------------ output tiles --
+constexpr int kJpegTileW = 64, kJpegTileH = 32;    // output pixels of one reconstruct CTA
+
+// component c's blocks [bx0, bx0 + nbx) x [by0, by0 + nby) cover what a tile reads of its plane; they are blocks
+// [first, first + nbx * nby) of the tile's blocks, row-major
+struct JpegTileWindow { int32_t bx0, by0, nbx, nby, first; };
+
+// Windows of the tile of output pixels [x0, x1) x [y0, y1): its luma blocks, and its chroma blocks with the one-sample
+// halo fancy upsampling reads (clamped to the plane).  Components past h.ncomp get empty windows.  Returns the number
+// of blocks of the tile.
+FAA_JHD int jpeg_tile_windows(const JpegHeader& h, int x0, int y0, int x1, int y1, JpegTileWindow pl[3]) {
+    const int cw = jpeg_chroma_w(h), ch = jpeg_chroma_h(h);
+    int n_blocks = 0;
+    for (int c = 0; c < 3; ++c) {
+        if (c >= h.ncomp) { pl[c] = {0, 0, 0, 0, n_blocks}; continue; }
+        int px0 = x0, px1 = x1 - 1, py0 = y0, py1 = y1 - 1;
+        if (c > 0) {
+            const int fx = h.hs == 2 ? 1 : 0, fy = h.vs == 2 ? 1 : 0;
+            px0 = x0 / h.hs - fx; px1 = (x1 - 1) / h.hs + fx;
+            py0 = y0 / h.vs - fy; py1 = (y1 - 1) / h.vs + fy;
+            px0 = px0 < 0 ? 0 : px0; px1 = px1 > cw - 1 ? cw - 1 : px1;
+            py0 = py0 < 0 ? 0 : py0; py1 = py1 > ch - 1 ? ch - 1 : py1;
+        }
+        pl[c] = {px0 >> 3, py0 >> 3, (px1 >> 3) - (px0 >> 3) + 1, (py1 >> 3) - (py0 >> 3) + 1, n_blocks};
+        n_blocks += pl[c].nbx * pl[c].nby;
+    }
+    return n_blocks;
+}
 
 // ------------------------------------------------------------------------------------------------ host decode --
 // The whole decode of one file on the host, serially, with the functions above: the CPU tests' model of the two

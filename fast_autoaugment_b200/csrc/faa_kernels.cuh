@@ -150,7 +150,6 @@ struct JpegDecodeParams {
     int32_t* status;            // [batch] JpegStatus bits
     int32_t batch;
 };
-constexpr int kJpegTileW = 64, kJpegTileH = 32;    // output pixels of one reconstruct CTA
 cudaError_t launch_jpeg_entropy(const JpegDecodeParams& p, cudaStream_t stream);
 cudaError_t launch_jpeg_reconstruct(const JpegDecodeParams& p, int n_tiles, cudaStream_t stream);
 

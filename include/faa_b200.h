@@ -333,7 +333,8 @@ typedef struct faa_jpeg_header {
     int32_t restart;          /* restart interval in MCUs, 0 = none                                                  */
     int32_t mcu_x, mcu_y;     /* MCUs per row / per column                                                           */
     int32_t table_at[9];      /* file offsets of the tables of components 0..2: quantisation [0..2], DC Huffman
-                                 [3..5], AC Huffman [6..8]; -1 for absent components                                 */
+                                 [3..5], AC Huffman [6..8]; -1 for absent components; -2 - k for a Huffman table
+                                 no DHT defines, which is standard table k of ITU T.81 K.3 (DC 0, DC 1, AC 0, AC 1)  */
     int32_t pool[9];          /* the same tables as indices into the caller's faa_jpeg_table_t pool (parse: -1)      */
     int32_t qprec;            /* bit c: component c's quantisation table has 16-bit entries                          */
     int32_t reserved;

@@ -106,17 +106,23 @@ def load_emu_jpeg():
         subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-o", so, src])
     lib = C.CDLL(so)
     lib.faa_emu_jpeg_decode.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    lib.faa_emu_jpeg_decode_mode.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int]
     return lib
 
 
-def emu_decode(lib, b):
-    """(parse result, status bits, uint8 [h, w, 3]) of the host build on file bytes b"""
+SERIAL, TILED, TILED_TRIMMED = 0, 1, 2      # decodes of the host build (faa_emu_jpeg_decode_mode)
+
+
+def emu_decode(lib, b, mode=SERIAL):
+    """(parse result, status bits, uint8 [h, w, 3]) of the host build on file bytes b: serially, or with the kernels'
+    split of the work (TILED; TILED_TRIMMED with chroma windows one block too narrow)"""
     src = np.frombuffer(b, np.uint8).copy()
     hw = np.zeros(2, np.int32)
     st = np.zeros(1, np.int32)
-    e = lib.faa_emu_jpeg_decode(src.ctypes.data, src.size, None, 0, st.ctypes.data, hw.ctypes.data)
+    e = lib.faa_emu_jpeg_decode_mode(src.ctypes.data, src.size, None, 0, st.ctypes.data, hw.ctypes.data, mode)
     if e:
         return e, 0, None
     out = np.zeros((int(hw[0]), int(hw[1]), 3), np.uint8)
-    e = lib.faa_emu_jpeg_decode(src.ctypes.data, src.size, out.ctypes.data, out.size, st.ctypes.data, hw.ctypes.data)
+    e = lib.faa_emu_jpeg_decode_mode(src.ctypes.data, src.size, out.ctypes.data, out.size, st.ctypes.data,
+                                     hw.ctypes.data, mode)
     return e, int(st[0]), out
