@@ -7,13 +7,16 @@
   ``train.py:47`` / ``search.py:101``: an iterable of ``(data, label)`` whose ``data`` is already
   the augmented, normalised CUDA tensor, so the caller's ``.cuda()`` (``train.py:49``) is a
   no-op.  The raw uint8 dataset lives on the device; no CUDA is touched in worker processes
-  because there are none.
+  because there are none.  The one exception is the ImageNet directory (``JpegFileDataset``): its files stay on disk
+  and are read, staged and decoded batch by batch, one batch ahead (``FileBatchStream``).
 """
 from __future__ import annotations
 
+import io
 import math
 import os
 import random
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import PIL.Image
@@ -24,7 +27,7 @@ from . import _lib, archive
 from .conf import Config as C
 from .engine import (CIFAR_MEAN, CIFAR_STD, IMAGENET_MEAN, IMAGENET_STD, CompiledPolicy, EncodedImages, RaggedImages,
                      TailSpec, augment_batch, center_crop_box, crop_cfg, crop_resize, decode_jpeg, make_rng,
-                     sample_philox_at)
+                     parse_jpeg_headers, sample_philox_at)
 
 
 class Augmentation(object):
@@ -549,6 +552,219 @@ class EncodedDeviceDataset:
         return d
 
 
+class FilePaths(list):
+    """Paths of image files that stay on disk (the ImageNet directory source of ``_load_arrays``)."""
+
+
+class JpegFileDataset:
+    """``EncodedDeviceDataset`` whose files stay on disk: it holds paths and targets only, so no byte of the split is on
+    the device.  ``GpuAugmentedLoader`` streams each batch's files through a ``FileBatchStream``."""
+
+    def __init__(self, paths, targets, device="cuda"):
+        self.paths = [os.fspath(p) for p in paths]
+        self.targets = [int(t) for t in targets]
+        if len(self.targets) != len(self.paths):
+            raise ValueError("need one target per image")
+        self.labels = torch.as_tensor(self.targets, dtype=torch.int64, device=device)
+        self.device = self.labels.device
+
+    def __len__(self):
+        return len(self.paths)
+
+    def select(self, idx):
+        """the paths of a batch"""
+        return [self.paths[int(i)] for i in idx]
+
+    def subset(self, idx):
+        idx = [int(i) for i in idx]
+        d = JpegFileDataset.__new__(JpegFileDataset)
+        d.paths = self.select(idx)
+        d.targets = [self.targets[i] for i in idx]
+        d.labels = self.labels.index_select(0, torch.as_tensor(idx, dtype=torch.int64, device=self.labels.device))
+        d.device = self.device
+        return d
+
+
+def _read_file(path):
+    with open(path, "rb") as f:
+        return f.read()
+
+
+def _pillow_rgb(path_and_bytes):
+    """``Image.open(f).convert('RGB')`` (reference imagenet.py:80, torchvision's ``pil_loader``) of a file the device
+    decoder refuses; Pillow's error names the path"""
+    path, b = path_and_bytes
+    try:
+        with PIL.Image.open(io.BytesIO(b)) as im:
+            return np.ascontiguousarray(np.asarray(im.convert("RGB")))
+    except OSError as e:
+        raise OSError("%s: %s" % (path, e)) from e
+
+
+class HostBatch:
+    """The host half of staging one batch of files (``read_jpeg_batch``): ``paths``; ``files``, ``headers`` and the
+    table ``pool`` of the files the device decoder takes (headers' ``offset`` places those files back to back, as
+    ``EncodedImages.from_bytes`` of them would); the batch positions of those files (``accepted``) and of the rest
+    (``refused``), and Pillow's pixels of the refused ones (``pixels``, uint8 [h, w, 3])."""
+
+    def __init__(self, paths, files, headers, pool, accepted, refused, pixels):
+        self.paths, self.files, self.headers, self.pool = paths, files, headers, pool
+        self.accepted, self.refused, self.pixels = accepted, refused, pixels
+
+    def sizes(self):
+        """(h, w) of every image of the batch, int32 [N, 2]"""
+        s = np.zeros((len(self.paths), 2), np.int32)
+        s[self.accepted, 0], s[self.accepted, 1] = self.headers["h"], self.headers["w"]
+        for i, px in zip(self.refused, self.pixels):
+            s[i] = px.shape[:2]
+        return s
+
+
+def read_jpeg_batch(paths, map=map):
+    """Read a batch of files and parse their headers (``parse_jpeg_headers``); decode the files the device decoder
+    refuses with Pillow.  No device is touched.  ``map``: an executor's ``map`` reads, parses and decodes in parallel."""
+    paths = list(paths)
+    files = list(map(_read_file, paths))
+    headers, pool, refused = parse_jpeg_headers(files, map)
+    bad = np.array([i for i, _ in refused], np.int64)
+    ok = np.setdiff1d(np.arange(len(files), dtype=np.int64), bad)
+    lengths = np.array([len(files[i]) for i in ok], np.int64)
+    headers = headers[ok]
+    headers["offset"] = np.cumsum(lengths) - lengths
+    pixels = list(map(_pillow_rgb, [(paths[i], files[i]) for i in bad]))
+    return HostBatch(paths, [files[i] for i in ok], headers, pool, ok, bad, pixels)
+
+
+def chunked_map(pool_map, n_chunks):
+    """``map`` over ``n_chunks`` contiguous chunks of the items, one ``pool_map`` task per chunk: a task per file
+    costs more than parsing a header"""
+    def run(fn, items):
+        items = list(items)
+        step = max(1, -(-len(items) // max(1, n_chunks)))
+        parts = pool_map(lambda xs: [fn(x) for x in xs], [items[i:i + step] for i in range(0, len(items), step)])
+        return [r for part in parts for r in part]
+    return run
+
+
+def _up16(n):
+    return (int(n) + 15) // 16 * 16
+
+
+class _Layout:
+    """Byte layout of one staged batch, the same in the pinned slot and in the batch's device buffer: headers, table
+    pool, the accepted files back to back, then the refused files' pixels, each part on a 16-byte boundary."""
+
+    def __init__(self, hb: HostBatch):
+        self.pool = _up16(hb.headers.nbytes)
+        self.files = self.pool + _up16(hb.pool.nbytes)
+        self.files_end = self.files + sum(len(f) for f in hb.files)
+        self.pixels, at = [], _up16(self.files_end)
+        for px in hb.pixels:
+            self.pixels.append(at)
+            at = _up16(at + px.nbytes)
+        self.total = max(at, 16)
+
+    def pack(self, hb: HostBatch, buf):
+        buf[:hb.headers.nbytes] = hb.headers.view(np.uint8).reshape(-1)
+        buf[self.pool:self.pool + hb.pool.nbytes] = hb.pool.view(np.uint8).reshape(-1)
+        at = self.files
+        for f in hb.files:
+            buf[at:at + len(f)] = np.frombuffer(f, np.uint8)
+            at += len(f)
+        for o, px in zip(self.pixels, hb.pixels):
+            buf[o:o + px.nbytes] = px.reshape(-1)
+
+
+_STATUS_BITS = ((_lib.JPEG_TRUNCATED, "scan truncated"), (_lib.JPEG_BAD_CODE, "bad Huffman code"),
+                (_lib.JPEG_BAD_COEF, "run past coefficient 63"), (_lib.JPEG_BAD_RESTART, "bad restart marker"))
+
+
+class FileBatchStream:
+    """Batches of JPEG files read from disk, decoded into ``RaggedImages`` on the device, staged one batch ahead.
+
+    While the device runs batch k, a host thread stages batch k + 1: a small thread pool reads its files and parses
+    their headers (``read_jpeg_batch``; ctypes releases the GIL in ``faa_jpeg_parse``), and the thread packs headers,
+    table pool, files and the Pillow pixels of refused files into one of ``SLOTS`` pinned staging buffers, once the
+    event recorded after that slot's previous copy shows the copy finished.  The caller's thread makes one
+    ``non_blocking`` copy of the slot into a device buffer of the batch, decodes the accepted files (``decode_jpeg``)
+    into their images of ``RaggedImages.empty(sizes)`` and copies the refused files' pixels into theirs.  Each batch's
+    decode status is copied to pinned host memory and checked once the next batch is staged, and at the end, so no
+    batch waits on its own decode: a non-zero status raises ``OSError`` naming the file."""
+
+    SLOTS = 2
+    WORKERS = 2
+
+    def __init__(self, workers=None):
+        self.workers = int(workers or self.WORKERS)
+        self.slots = [None] * self.SLOTS           # pinned uint8 staging buffers
+        self.copied = [None] * self.SLOTS          # event recorded after each slot's last host-to-device copy
+
+    def _stage(self, paths, slot, pool, dev):
+        hb = read_jpeg_batch(paths, chunked_map(pool.map, self.workers) if self.workers > 1 else map)
+        lay = _Layout(hb)
+        if self.copied[slot] is not None:
+            self.copied[slot].synchronize()
+        buf = self.slots[slot]
+        if buf is None or buf.numel() < lay.total:
+            with torch.cuda.device(dev):
+                buf = self.slots[slot] = torch.empty(lay.total + lay.total // 4, dtype=torch.uint8, pin_memory=True)
+        lay.pack(hb, buf.numpy())
+        return hb, lay, slot
+
+    def _decode(self, hb, lay, dbuf, dev, pending):
+        sizes = hb.sizes()
+        out = RaggedImages.empty(sizes, dev)
+        if len(hb.accepted):
+            enc = EncodedImages(dbuf[lay.files:lay.files_end], hb.headers, hb.pool, _d_pool=dbuf[lay.pool:lay.files],
+                                _d_headers=dbuf[:lay.pool])
+            _, status = decode_jpeg(enc, out.select(hb.accepted))
+            st = torch.empty(len(hb.accepted), dtype=torch.int32, pin_memory=True)
+            st.copy_(status, non_blocking=True)
+            ev = torch.cuda.Event()
+            ev.record(torch.cuda.current_stream(dev))
+            pending.append((ev, st, [hb.paths[i] for i in hb.accepted]))
+        for i, o in zip(hb.refused, lay.pixels):
+            h, w = (int(v) for v in sizes[i])
+            out.image(int(i)).copy_(dbuf[o:o + h * w * 3].view(h, w, 3))
+        return out
+
+    @staticmethod
+    def _check(pending, keep=0):
+        """check (and drop) every pending status but the last ``keep``"""
+        while len(pending) > keep:
+            ev, st, paths = pending.pop(0)
+            ev.synchronize()
+            bad = [(p, int(s)) for p, s in zip(paths, st.numpy().tolist()) if s]
+            if bad:
+                raise OSError("corrupt JPEG files (decode status): " + "; ".join(
+                    "%s: 0x%x (%s)" % (p, s, ", ".join(n for b, n in _STATUS_BITS if s & b)) for p, s in bad))
+
+    def __call__(self, batches, device):
+        """generator of one ``RaggedImages`` per batch of paths in ``batches``"""
+        dev = torch.device(device)
+        pool = ThreadPoolExecutor(self.workers, thread_name_prefix="faa-read")
+        ahead = ThreadPoolExecutor(1, thread_name_prefix="faa-stage")
+        pending = []                               # (event, pinned status, paths) of decodes not checked yet
+        try:
+            fut = ahead.submit(self._stage, batches[0], 0, pool, dev) if len(batches) else None
+            for k in range(len(batches)):
+                hb, lay, slot = fut.result()
+                dbuf = torch.empty(lay.total, dtype=torch.uint8, device=dev)
+                dbuf.copy_(self.slots[slot][:lay.total], non_blocking=True)
+                ev = torch.cuda.Event()
+                ev.record(torch.cuda.current_stream(dev))
+                self.copied[slot] = ev
+                if k + 1 < len(batches):
+                    fut = ahead.submit(self._stage, batches[k + 1], (k + 1) % self.SLOTS, pool, dev)
+                out = self._decode(hb, lay, dbuf, dev, pending)
+                self._check(pending, keep=1 if len(hb.accepted) else 0)      # the batches before this one
+                yield out
+            self._check(pending)
+        finally:
+            ahead.shutdown(wait=True, cancel_futures=True)
+            pool.shutdown(wait=True, cancel_futures=True)
+
+
 class GpuAugmentedLoader:
     """What ``get_dataloaders`` hands to ``train.py:47`` / ``search.py:101`` instead of a torch ``DataLoader``:
     an iterable of ``(data, label)`` whose ``data`` is the augmented, normalised CUDA batch (``.cuda()`` at
@@ -561,10 +777,13 @@ class GpuAugmentedLoader:
     torch generators (a ``num_workers=0`` DataLoader); the default draws on the device with Philox.
     """
 
-    def __init__(self, dataset: DeviceDataset | RaggedDeviceDataset | EncodedDeviceDataset, batch, policies, tail: TailSpec, sampler=None, shuffle=False,
-                 drop_last=False, seed=None, parity=False, chain=None, chain_mode="train"):
+    def __init__(self, dataset: DeviceDataset | RaggedDeviceDataset | EncodedDeviceDataset | JpegFileDataset, batch, policies,
+                 tail: TailSpec, sampler=None, shuffle=False, drop_last=False, seed=None, parity=False, chain=None,
+                 chain_mode="train"):
         """``chain``: an ``ImageNetChain`` that transforms the batches instead of the fused policy launch
-        (``chain_mode`` 'train' or 'test'); a ``RaggedDeviceDataset`` or ``EncodedDeviceDataset`` needs one."""
+        (``chain_mode`` 'train' or 'test'); a ``RaggedDeviceDataset``, ``EncodedDeviceDataset`` or ``JpegFileDataset``
+        needs one.  A ``JpegFileDataset``'s batches are read from disk one batch ahead (``FileBatchStream``; the stream
+        of the latest epoch is ``staging``)."""
         if not torch.cuda.is_available():
             raise _lib.FaaRuntimeError("fast_autoaugment_b200 needs a CUDA device (no CPU fallback)")
         self.dataset, self.batch_size, self.tail = dataset, int(batch), tail
@@ -572,9 +791,10 @@ class GpuAugmentedLoader:
         self.aug = Augmentation(policies) if policies is not None else Augmentation([[("Invert", 0.0, 0.0)]])
         self.seed = int(torch.initial_seed() if seed is None else seed) & 0x7FFFFFFFFFFFFFFF
         self.chain, self.chain_mode = chain, chain_mode
-        if isinstance(dataset, (RaggedDeviceDataset, EncodedDeviceDataset)) and chain is None:
+        if isinstance(dataset, (RaggedDeviceDataset, EncodedDeviceDataset, JpegFileDataset)) and chain is None:
             raise ValueError("images of different sizes need an ImageNetChain (conf['faa_crop_resize'])")
         self._drawn = 0                   # samples drawn so far: the Philox counter never repeats across epochs
+        self.staging = None
 
     def _n(self):
         return len(self.sampler) if self.sampler is not None else len(self.dataset)
@@ -591,22 +811,38 @@ class GpuAugmentedLoader:
 
     def __iter__(self):
         idx_all = self._indices()
-        dev = self.dataset.images.device
-        for k in range(len(self)):
-            idx = idx_all[k * self.batch_size:(k + 1) * self.batch_size]
-            t = torch.as_tensor(idx, dtype=torch.int64).to(dev, non_blocking=True)
-            if isinstance(self.dataset, (RaggedDeviceDataset, EncodedDeviceDataset)):
-                raw = self.dataset.images.select(idx)            # descriptors into the dataset's storage: no pixel copy
-            else:
-                raw = self.dataset.images.index_select(0, t)
-            if self.chain is None:
-                data = self.aug.augment_batch(raw, self.tail, seed=self.seed, first_index=self._drawn, parity=self.parity)
-            elif self.chain_mode == "test":
-                data = self.chain.test(raw)
-            else:
-                data = self.chain.train(raw, parity=self.parity, seed=self.seed, first_index=self._drawn)
-            self._drawn += len(idx)
-            yield data, self.dataset.labels.index_select(0, t)
+        files = None
+        if isinstance(self.dataset, JpegFileDataset):
+            dev = self.dataset.device
+            batches = [idx_all[k * self.batch_size:(k + 1) * self.batch_size] for k in range(len(self))]
+            self.staging = FileBatchStream()
+            files = self.staging([self.dataset.select(idx) for idx in batches], dev)
+        else:
+            dev = self.dataset.images.device
+        try:
+            for k in range(len(self)):
+                idx = idx_all[k * self.batch_size:(k + 1) * self.batch_size]
+                t = torch.as_tensor(idx, dtype=torch.int64).to(dev, non_blocking=True)
+                if files is not None:
+                    raw = next(files)                            # this batch's files, decoded on the device
+                elif isinstance(self.dataset, (RaggedDeviceDataset, EncodedDeviceDataset)):
+                    raw = self.dataset.images.select(idx)        # descriptors into the dataset's storage: no pixel copy
+                else:
+                    raw = self.dataset.images.index_select(0, t)
+                if self.chain is None:
+                    data = self.aug.augment_batch(raw, self.tail, seed=self.seed, first_index=self._drawn, parity=self.parity)
+                elif self.chain_mode == "test":
+                    data = self.chain.test(raw)
+                else:
+                    data = self.chain.train(raw, parity=self.parity, seed=self.seed, first_index=self._drawn)
+                self._drawn += len(idx)
+                yield data, self.dataset.labels.index_select(0, t)
+            if files is not None:
+                for _ in files:                                  # the last batches' decode status
+                    pass
+        finally:
+            if files is not None:
+                files.close()
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -622,7 +858,9 @@ def _load_arrays(dataset, dataroot):
     an .npz whose ``data`` is the images' bytes packed back to back with their ``sizes`` [N, 2] (h, w).  Those images
     come back as a list of arrays.  ImageNet sources may also be JPEG files: a mapping whose images are a list of
     ``bytes``, or an .npz with ``jpeg`` (the files packed back to back), ``lengths`` and ``targets``; they come back as a
-    list of ``bytes``, decoded on the device batch by batch."""
+    list of ``bytes``, decoded on the device batch by batch.  Without a mapping or .npz, ``imagenet`` reads the
+    reference's directory (``imagenet_index``: ``dataroot/imagenet-pytorch/{train,val}``): its images come back as
+    ``FilePaths``, read from disk batch by batch."""
     base = dataset.replace("reduced_", "")
     ragged_ok = "imagenet" in dataset
 
@@ -670,9 +908,61 @@ def _load_arrays(dataset, dataroot):
             ex = torchvision.datasets.SVHN(root=dataroot, split="extra", download=False)
             return (np.concatenate([hwc(tr), hwc(ex)]), list(tr.labels) + list(ex.labels), hwc(te), list(te.labels))
         return hwc(tr), list(tr.labels), hwc(te), list(te.labels)
-    raise ValueError("invalid dataset name=%s" % dataset) if "imagenet" not in dataset else NotImplementedError(
-        "ImageNet needs JPEG decoding (reference imagenet.py:80), which is outside this package's hot path: "
-        "pass fixed-size uint8 arrays through a mapping / .npz dataroot instead")
+    if dataset == "imagenet":                                   # data.py:146-150
+        tr, te = imagenet_index(dataroot, "train"), imagenet_index(dataroot, "val")
+        return FilePaths(p for p, _ in tr), [t for _, t in tr], FilePaths(p for p, _ in te), [t for _, t in te]
+    raise ValueError("invalid dataset name=%s" % dataset)
+
+
+def imagenet_index(dataroot, split):
+    """[(path, class index)] of the reference's ``ImageNet(os.path.join(dataroot, 'imagenet-pytorch'), split)``
+    (data.py:146-150, imagenet.py:52-90), in its order.  ``train`` with ``imagenet-pytorch/train_cls.txt``: the
+    file's non-empty lines in order, classes the sorted first path components, path ``train/<line>.JPEG``.  Otherwise
+    torchvision's own ``find_classes`` / ``make_dataset`` over the split folder, as ``ImageFolder`` walks it.  The
+    class names of ``meta.bin`` are not needed for the targets and are not read."""
+    root = os.path.expanduser(os.path.join(str(dataroot), "imagenet-pytorch"))
+    folder = os.path.join(root, split)
+    listfile = os.path.join(root, "train_cls.txt")
+    if split == "train" and os.path.exists(listfile):
+        with open(listfile, "r") as f:
+            lines = [line.strip().split(" ")[0] for line in f.readlines() if line.strip()]
+        classes = sorted(set(line.split("/")[0] for line in lines))
+        to_idx = {c: i for i, c in enumerate(classes)}
+        return [(os.path.join(folder, line + ".JPEG"), to_idx[line.split("/")[0]]) for line in lines]
+    if not os.path.isdir(folder):
+        raise FileNotFoundError("ImageNet %s folder not found: %s (the reference's layout is "
+                                "<dataroot>/imagenet-pytorch/{train,val}/<class>/...)" % (split, folder))
+    from torchvision.datasets.folder import IMG_EXTENSIONS, find_classes, make_dataset
+    return make_dataset(folder, find_classes(folder)[1], IMG_EXTENSIONS)
+
+
+def split_samplers(targets, split=0.15, split_idx=0, multinode=False, target_lb=-1):
+    """(train sampler or None, valid sampler) of ``get_dataloaders`` over a train set with these targets
+    (reference data.py:189-212)"""
+    from sklearn.model_selection import StratifiedShuffleSplit
+    import torch.distributed as dist
+
+    train_sampler = None
+    if split > 0.0:                                             # data.py:189-203
+        sss = StratifiedShuffleSplit(n_splits=5, test_size=split, random_state=0)
+        sss = sss.split(list(range(len(targets))), targets)
+        for _ in range(split_idx + 1):
+            train_idx, valid_idx = next(sss)
+        if target_lb >= 0:
+            train_idx = [i for i in train_idx if targets[i] == target_lb]
+            valid_idx = [i for i in valid_idx if targets[i] == target_lb]
+        train_sampler = SubsetRandomSampler(train_idx)
+        valid_sampler = SubsetSampler(valid_idx)
+        if multinode:
+            train_sampler = torch.utils.data.distributed.DistributedSampler(
+                torch.utils.data.Subset(range(len(targets)), train_idx),
+                num_replicas=dist.get_world_size(), rank=dist.get_rank())
+    else:
+        valid_sampler = SubsetSampler([])
+        if multinode:
+            train_sampler = torch.utils.data.distributed.DistributedSampler(
+                range(len(targets)), num_replicas=dist.get_world_size(), rank=dist.get_rank())
+    return train_sampler, valid_sampler
 
 
 def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode=False, target_lb=-1):
@@ -687,9 +977,11 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
     (ImageNet: the stored images are uncropped sources, of one size or of many, and the loaders run the reference's full chains,
     ``ImageNetChain``: train / valid = policy -> EfficientNetRandomCrop + bicubic Resize -> ColorJitter -> HFlip +
     Lighting + Normalize, test = EfficientNetCenterCrop + Resize + Normalize, at 224 or the EfficientNet size of
-    ``conf['model']['type']``; without it ImageNet images must already have the network's size)."""
+    ``conf['model']['type']``; without it ImageNet images must already have the network's size).
+
+    ``imagenet`` with the reference's ``dataroot`` (``imagenet-pytorch/{train,val}``, ``imagenet_index``) keeps the
+    files on disk (``JpegFileDataset``): the loaders read, stage and decode each batch's files one batch ahead."""
     from sklearn.model_selection import StratifiedShuffleSplit
-    import torch.distributed as dist
 
     conf = C.get()
     out_dtype = {"float32": torch.float32, "float16": torch.float16, "bfloat16": torch.bfloat16}[
@@ -712,6 +1004,8 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
                          "images are augmented at one fixed size")
 
     def device_dataset(x, y):
+        if isinstance(x, FilePaths):
+            return JpegFileDataset(x, y)
         if isinstance(x, list) and len(x) and isinstance(x[0], bytes):
             return EncodedDeviceDataset(x, y)
         return RaggedDeviceDataset(x, y) if isinstance(x, list) else DeviceDataset(x, y)
@@ -725,27 +1019,7 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
     else:
         raise ValueError("invalid dataset name=%s" % dataset)
 
-    train_sampler = None
-    if split > 0.0:                                             # data.py:189-203
-        sss = StratifiedShuffleSplit(n_splits=5, test_size=split, random_state=0)
-        sss = sss.split(list(range(len(total_trainset))), total_trainset.targets)
-        for _ in range(split_idx + 1):
-            train_idx, valid_idx = next(sss)
-        if target_lb >= 0:
-            train_idx = [i for i in train_idx if total_trainset.targets[i] == target_lb]
-            valid_idx = [i for i in valid_idx if total_trainset.targets[i] == target_lb]
-        train_sampler = SubsetRandomSampler(train_idx)
-        valid_sampler = SubsetSampler(valid_idx)
-        if multinode:
-            train_sampler = torch.utils.data.distributed.DistributedSampler(
-                torch.utils.data.Subset(range(len(total_trainset)), train_idx),
-                num_replicas=dist.get_world_size(), rank=dist.get_rank())
-    else:
-        valid_sampler = SubsetSampler([])
-        if multinode:
-            train_sampler = torch.utils.data.distributed.DistributedSampler(
-                range(len(total_trainset)), num_replicas=dist.get_world_size(), rank=dist.get_rank())
-
+    train_sampler, valid_sampler = split_samplers(total_trainset.targets, split, split_idx, multinode, target_lb)
     parity = bool(conf.get("faa_parity", False))
     if "imagenet" in dataset and conf.get("faa_crop_resize", False):      # data.py:49-80, 217-224
         model_type = (conf.get("model") or {}).get("type", "")

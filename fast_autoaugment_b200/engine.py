@@ -537,6 +537,40 @@ class RaggedImages:
         return self._desc
 
 
+def parse_jpeg(f):
+    """(header ``JPEG_HEADER_DTYPE`` [1], its tables ``JPEG_TABLE_DTYPE`` [9]) of one file (C ABI ``faa_jpeg_parse`` +
+    ``faa_jpeg_tables``; ctypes releases the GIL during both), or (None, reason) when the decoder does not take it"""
+    hdr = np.zeros(1, dtype=_lib.JPEG_HEADER_DTYPE)
+    if lib.faa_jpeg_parse(f, len(f), hdr.ctypes.data) != _lib.OK:
+        return None, (lib.faa_last_error() or b"").decode()
+    tabs = np.zeros(9, dtype=_lib.JPEG_TABLE_DTYPE)
+    check(lib.faa_jpeg_tables(f, len(f), hdr.ctypes.data, tabs.ctypes.data))
+    return hdr, tabs
+
+
+def parse_jpeg_headers(files, map=map):
+    """JPEG files (``bytes``) -> (headers [N], table pool, refused [(position, reason)]).  The tables the files use are
+    deduplicated into the pool in order of first use, which the headers' ``pool`` slots index; a refused file's header
+    row stays zero and adds nothing to the pool.  ``offset`` is left 0: the caller places the files.  ``map`` runs the
+    per-file parse (an executor's ``map`` parses files in parallel)."""
+    headers = np.zeros(len(files), dtype=_lib.JPEG_HEADER_DTYPE)
+    pool, index, refused = [], {}, []
+    for i, (hdr, tabs) in enumerate(map(parse_jpeg, files)):
+        if hdr is None:
+            refused.append((i, tabs))
+            continue
+        headers[i] = hdr[0]
+        for slot in range(9):
+            if slot % 3 >= int(hdr["ncomp"][0]):
+                continue
+            key = tabs[slot].tobytes()
+            if key not in index:
+                index[key] = len(pool)
+                pool.append(tabs[slot].copy())
+            headers["pool"][i, slot] = index[key]
+    return headers, np.array(pool, dtype=_lib.JPEG_TABLE_DTYPE).reshape(-1), refused
+
+
 class EncodedImages:
     """A batch or dataset of JPEG files: their bytes packed back to back in one device buffer, their headers parsed once
     on the host (C ABI ``faa_jpeg_parse``), and the quantisation and Huffman tables they use deduplicated into one table
@@ -544,7 +578,9 @@ class EncodedImages:
     copy and the pool's are made on first use.  ``select`` makes a batch of some of the files without copying a byte of
     them."""
 
-    def __init__(self, storage: torch.Tensor, headers, pool, _d_pool=None):
+    def __init__(self, storage: torch.Tensor, headers, pool, _d_pool=None, _d_headers=None):
+        """``_d_pool`` / ``_d_headers``: device copies of ``pool`` / ``headers`` the caller already made (uint8 tensors
+        of their bytes), used instead of uploading them on first use"""
         if not isinstance(storage, torch.Tensor) or storage.dtype != torch.uint8 or storage.dim() != 1 \
                 or not storage.is_contiguous():
             raise ValueError("storage must be a contiguous 1-D uint8 tensor")
@@ -555,39 +591,22 @@ class EncodedImages:
         if len(h) and (int(h["offset"].min()) < 0 or int((h["offset"] + h["len"]).max()) > storage.numel()):
             raise ValueError("every file must lie inside the storage")
         self._d_pool = _d_pool
-        self._d_headers = None
+        self._d_headers = _d_headers
 
     @staticmethod
     def from_bytes(files, device="cuda"):
         """JPEG files (``bytes``) -> EncodedImages on ``device``.  Raises ValueError naming every file the decoder
         does not take (progressive, arithmetic, 12-bit, CMYK, other sampling, malformed ...) and why."""
         files = [bytes(f) for f in files]
-        headers = np.zeros(len(files), dtype=_lib.JPEG_HEADER_DTYPE)
-        tabs = np.zeros(9, dtype=_lib.JPEG_TABLE_DTYPE)
-        pool, index, refused = [], {}, []
-        for i, f in enumerate(files):
-            hdr = headers[i:i + 1]
-            st = lib.faa_jpeg_parse(f, len(f), hdr.ctypes.data)
-            if st != _lib.OK:
-                refused.append("%d: %s" % (i, (lib.faa_last_error() or b"").decode()))
-                continue
-            check(lib.faa_jpeg_tables(f, len(f), hdr.ctypes.data, tabs.ctypes.data))
-            for slot in range(9):
-                if slot % 3 >= int(hdr["ncomp"][0]):
-                    continue
-                key = tabs[slot].tobytes()
-                if key not in index:
-                    index[key] = len(pool)
-                    pool.append(tabs[slot].copy())
-                headers["pool"][i, slot] = index[key]
+        headers, pool, refused = parse_jpeg_headers(files)
         if refused:
-            raise ValueError("JPEG files the decoder does not take: " + "; ".join(refused))
+            raise ValueError("JPEG files the decoder does not take: " + "; ".join("%d: %s" % r for r in refused))
         lengths = np.array([len(f) for f in files], dtype=np.int64)
         headers["offset"] = np.cumsum(lengths) - lengths
         packed = np.frombuffer(b"".join(files), dtype=np.uint8)
         storage = torch.from_numpy(packed.copy()).to(device) if packed.size else torch.zeros(1, dtype=torch.uint8,
                                                                                               device=device)
-        return EncodedImages(storage, headers, np.array(pool, dtype=_lib.JPEG_TABLE_DTYPE).reshape(-1))
+        return EncodedImages(storage, headers, pool)
 
     def __len__(self):
         return len(self.headers)
