@@ -794,7 +794,8 @@ static int launch_chained(faa_policy* p, const AugParams& P, ResolveParams& R, c
     // one resident wave each (launch bounds: light CTAs / SM; mid rows: ONE CTA per SM, so that the light CTAs that
     // follow share the SM with it from the start)
     const int lb = P.geo[1].bands > 0 ? P.geo[1].bands : 1;
-    Pc.grid_y = (p->sm_count * resident_ctas_per_sm(1)) / lb;
+    const int light = s.lean_light ? 3 : 1;
+    Pc.grid_y = (p->sm_count * resident_ctas_per_sm(light)) / lb;
     Pm.grid_y = p->sm_count / (Pm.bands > 0 ? Pm.bands : 1);
     if (Pc.grid_y < 1) Pc.grid_y = 1;
     if (Pm.grid_y < 1) Pm.grid_y = 1;
@@ -810,7 +811,7 @@ static int launch_chained(faa_policy* p, const AugParams& P, ResolveParams& R, c
     }
     if (s.use_split) {
         if (s.use_mid) { if (int e = launch(Pm, 2)) return e; }
-        if (int e = launch(Pc, 1)) return e;
+        if (int e = launch(Pc, light)) return e;
     }
     record_step(p, P, out_dtype, stream);
     return FAA_OK;
@@ -871,7 +872,7 @@ static int launch_event(faa_policy* p, AugParams& P, ResolveParams& R, const Sch
     AugParams Ph = P; Ph.pdl = 0;                           // not behind the resolve kernel in its stream
     CK(cudaStreamWaitEvent(p->light_stream, p->ev_res, 0));
     if (s.use_mid) CK(cudaStreamWaitEvent(p->mid_stream, p->ev_res, 0));
-    CK(launch_augment(P, out_dtype, s.use_tab, 1, stream));
+    CK(launch_augment(P, out_dtype, s.use_tab, s.lean_light ? 3 : 1, stream));
     g_launches++;
     if (!s.no_heavy) {
         CK(launch_augment(Ph, out_dtype, s.use_tab, 0, p->light_stream));
@@ -959,6 +960,7 @@ static int augment_common(faa_policy_t* p, const AugRequest& q) {
     P.lam = q.lam; P.one_minus_lam = q.one_minus_lam;
     P.bands = s.geo[0].bands; P.geo[0] = s.geo[0]; P.geo[1] = s.geo[1];
     P.stage = s.stage; P.band_cap = s.geo[0].band_cap; P.crop_pad = in.crop_pad; P.octets = s.octets; P.mat_cap = s.mat_cap;
+    P.allow = s.allow;
     // fastdiv reciprocals (host side: no divisions in the kernels)
     auto rcp = [](uint32_t d) { return d <= 1 ? 0u : (uint32_t)((0x100000000ull + d - 1) / d); };
     P.rcp_out_qpr = rcp((uint32_t)(tail->out_w + 3) / 4); P.rcp_w = rcp((uint32_t)w); P.rcp_wq = rcp((uint32_t)w / 4);

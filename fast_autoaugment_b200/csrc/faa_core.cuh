@@ -489,7 +489,8 @@ FAA_HD bool kind_is_lutlike(int k) { return k == K_NONE || kind_uses_lut(k); }
 // Sample + boxes -> Prog.  ops: compiled table [n_sub][n_op][2]; boxes: this sample's n_op boxes.
 // allow: bit 0 = the launch has a materialisation chunk of at least 3 rows, bit 1 = it has a global
 // scratch image (both only for single-source launches), bit 2 = split launch with the lean gather paths
-// (float planes of the image's own size, W % 8 == 0, no crop).
+// (float planes of the image's own size, W % 8 == 0, no crop), bit 3 = the light kernel is its lean variant
+// (octet paths only: prog_is_light; split launches, so only the resolve kernel's programs - see lean_order).
 FAA_HD void build_prog(const Sample& s_in, const Box* boxes, const OpRec* ops, int n_op, int op_base,
                        int apply_tail, int H, int W, int out_w, int allow, Prog& g) {
     const bool allow_mat = (allow & 1) != 0, allow_scratch = (allow & 2) != 0;
@@ -547,10 +548,33 @@ FAA_HD void build_prog(const Sample& s_in, const Box* boxes, const OpRec* ops, i
     else g.cls = C_GENERIC;
 }
 
+// Programs of lean light launches (allow bit 3), after build_prog: Color, then a gather == the gather, then Color (Color
+// is per pixel and maps the gather's zero fill to zero).  The lean light kernel has no path for Color in front of a
+// gather; the mid kernel runs gather -> Color (prog_two_stage).  Both slots are C_GEOM's, neither has a mask bit.
+FAA_HD void lean_order(Prog& g, int allow) {
+    if ((allow & 8) && g.op[0].kind == K_COLOR && (g.op[1].kind == K_AFFINE || g.op[1].kind == K_SHIFT)) {
+        const OpRec o = g.op[0]; g.op[0] = g.op[1]; g.op[1] = o;
+        const Box b = g.box[0]; g.box[0] = g.box[1]; g.box[1] = b;
+    }
+}
+
 // "Light" programs need no whole-image statistics and no neighbourhood: they run in the small
 // streaming kernel (no cluster, few registers); everything else runs in the cluster kernel.
-FAA_HD bool prog_is_light(const Prog& g) {
-    return g.stat_mask == 0 && (g.cls == C_PLAIN || g.cls == C_LUT || g.cls == C_POINT || g.cls == C_GEOM || g.cls == C_GEOM2);
+// allow bit 3: the light kernel is its lean variant, which has the octet paths only.  Its Color / Cutout programs are the
+// ones a float table can finish (alone, or followed by a static LUT) and Cutout followed by a gather; the other pairs with
+// Color or Cutout run in the mid kernel (prog_two_stage).
+FAA_HD bool prog_is_light(const Prog& g, int allow = 0) {
+    if (g.stat_mask != 0 || !(g.cls == C_PLAIN || g.cls == C_LUT || g.cls == C_POINT || g.cls == C_GEOM || g.cls == C_GEOM2))
+        return false;
+    if (!(allow & 8)) return true;
+    const int k0 = g.op[0].kind, k1 = g.op[1].kind;
+    if (g.cls == C_POINT) return k1 == K_NONE || kind_uses_lut(k1);
+    if (g.cls == C_GEOM) {
+        const bool g0 = k0 == K_AFFINE || k0 == K_SHIFT;
+        const int pk = g0 ? k1 : k0;                  // the pointwise partner
+        return pk == K_NONE || kind_uses_lut(pk) || (!g0 && pk == K_CUTOUT);
+    }
+    return true;
 }
 
 // "Mid" programs: whole-image statistics feeding per-channel LUTs, or Sharpness (+ a static LUT) - they need a
@@ -568,6 +592,8 @@ FAA_HD bool prog_two_stage(const Prog& g, int allow) {
                          ((k1 == K_AUTOCONTRAST || k1 == K_EQUALIZE || k1 == K_CONTRAST) && g.cls2 == C_LUT);
         return op0 && op1;
     }
+    // lean light launches: a static LUT, Color, Cutout or a gather, then Color / Cutout (stage A in place or a gather)
+    if ((allow & 8) && g.stat_mask == 0 && (g.cls == C_POINT || g.cls == C_GEOM)) return k1 == K_COLOR || k1 == K_CUTOUT;
     if (g.cls == C_SG) return true;                                                   // Sharpness, then a gather (scratch exists)
     if (g.cls == C_SHARP) return scratch && (k1 == K_COLOR || k1 == K_CUTOUT);        // Sharpness, then Color / Cutout
     if (g.cls == C_POINT) return g.stat_mask == 1 && (k1 == K_COLOR || k1 == K_CUTOUT);   // statistics LUT, then Color / Cutout
@@ -578,8 +604,9 @@ FAA_HD bool prog_is_mid(const Prog& g, int allow) {
     const int k0 = g.op[0].kind, k1 = g.op[1].kind;
     if (g.cls == C_LUT) return g.stat_mask != 0;
     // statistics LUT, then a gather: the table rides through the lean gather paths (fill colour = plain zero)
-    if (g.cls == C_GEOM) return (allow & 4) && g.stat_mask == 1 && (k0 == K_AUTOCONTRAST || k0 == K_EQUALIZE || k0 == K_CONTRAST) &&
-                                (k1 == K_AFFINE || k1 == K_SHIFT);
+    if (g.cls == C_GEOM && g.stat_mask != 0)
+        return (allow & 4) && g.stat_mask == 1 && (k0 == K_AUTOCONTRAST || k0 == K_EQUALIZE || k0 == K_CONTRAST) &&
+               (k1 == K_AFFINE || k1 == K_SHIFT);
     if (g.cls == C_SHARP && (k1 == K_NONE || k1 == K_LUT || k1 == K_BRIGHTNESS)) return true;
     return prog_two_stage(g, allow);
 }
@@ -844,7 +871,8 @@ struct LaunchPlan {
     bool use_split;             // the light streaming kernel (and the mid kernel) take the programs they cover
     bool use_mid;               // three-way split: statistics-LUT and Sharpness programs run in the mid kernel
     int32_t split;              // ResolveParams::split
-    int32_t allow;              // ResolveParams::allow: bit 0 chunk, bit 1 scratch image, bit 2 lean gathers
+    int32_t allow;              // ResolveParams::allow: bit 0 chunk, bit 1 scratch image, bit 2 lean gathers, bit 3 lean_light
+    bool lean_light;            // the light kernel runs its lean variant (octet paths only, 4 CTAs / SM)
     bool scratch;               // a scratch image per image (Sharpness -> gather)
     bool no_heavy;              // every program is light or mid: the cluster kernel is not launched
     bool self_resolving;        // one kernel that draws and builds its programs itself
@@ -903,6 +931,11 @@ inline LaunchPlan plan_launch(const PlanInput& in) {
     L.scratch = (in.has_sg || L.use_mid) && !in.two_src && (w & 3) == 0;
     // allow bit 0: the chunk, bit 1: a scratch image, bit 2: the lean gather paths exist in this launch
     L.allow = (L.mat_cap > 0 ? 1 : 0) | (L.scratch ? 2 : 0) | (L.use_split && L.octets && in.crop_pad == 0 ? 4 : 0);
+    // The lean light kernel has only the octet paths: every light entry must find its band staged and its output the
+    // (possibly mirrored) image itself.  Philox draws no crop offset without crop padding at the image's own size;
+    // resolved records carry whatever offsets their caller drew, so those launches keep the kernel with the generic paths.
+    L.lean_light = (L.allow & 4) && L.geo[1].band_cap > 0 && in.philox;
+    if (L.lean_light) L.allow |= 8;
     // With the lean gathers (allow bit 2) and a scratch image (bit 1) every program of a three-way split is light or mid
     // (prog_is_light / prog_is_mid cover all class combinations; tests/test_gpu_fastpaths.py runs every ordered op pair
     // through this schedule): the cluster kernel has nothing to do and is not launched.

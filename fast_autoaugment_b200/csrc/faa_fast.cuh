@@ -216,22 +216,25 @@ __device__ __forceinline__ bool map_xy(const MapRegs& m, int& x, int& y, int W, 
 
 // one source pixel (24 bits) of the gather, bit 24 set when it exists.  mA maps the output pixel into the image in
 // front of the last op; opB (shared memory, may be null: CTA-uniform) maps that position into the image in front of it.
+// cut (shared memory, may be null: CTA-uniform): the clipped box of a Cutout in front of the gather.
 template <bool COH = false>   // COH: the source image was written by this kernel (scratch, behind a cluster barrier): loads bypass L1
-__device__ __forceinline__ uint32_t gather_fetch(const uint8_t* raw, int W, int H, const MapRegs& mA, const OpRec* opB, int x, int y) {
+__device__ __forceinline__ uint32_t gather_fetch(const uint8_t* raw, int W, int H, const MapRegs& mA, const OpRec* opB, int x, int y,
+                                                 const Box* cut = nullptr) {
     bool ok = map_xy(mA, x, y, W, H);
     if (opB != nullptr) { const MapRegs mB = map_regs(*opB); const bool ok2 = map_xy(mB, x, y, W, H); ok = ok && ok2; }
     const uint32_t off = ok ? (uint32_t)(y * W + x) * 3u : 0u;
     const uint32_t* wp = reinterpret_cast<const uint32_t*>(raw + (off & ~3u));
     const uint32_t lo = COH ? __ldcg(wp) : __ldg(wp);
     const uint32_t hi = (off & 2u) ? (COH ? __ldcg(wp + 1) : __ldg(wp + 1)) : 0u;     // bytes 2,3 of the word: the pixel spills into the next one
-    const uint32_t px = __funnelshift_r(lo, hi, 8u * (off & 3u)) & 0xFFFFFFu;
+    uint32_t px = __funnelshift_r(lo, hi, 8u * (off & 3u)) & 0xFFFFFFu;
+    if (cut != nullptr && x >= cut->x0 && x <= cut->x1 && y >= cut->y0 && y <= cut->y1) px = kCutoutRGB;
     return ok ? (px | 0x01000000u) : 0u;
 }
 
 template <int OUT, bool USE_TAB, bool FULL, bool COH = false>
 __device__ __forceinline__ void final_rows_gather_t(const AugParams& P, const float* tab, const float pad[3], const Ctx& c,
                                                     const OpRec* opA, const OpRec* opB, int flip, void* out_img, int oy0, int oy1,
-                                                    uint32_t* tile) {
+                                                    uint32_t* tile, const Box* cut) {
     using T = typename OutElem<OUT>::T;
     const int W = P.W, H = P.H;
     const uint32_t npx = (uint32_t)(oy1 - oy0) * (uint32_t)W;
@@ -251,7 +254,7 @@ __device__ __forceinline__ void final_rows_gather_t(const AugParams& P, const fl
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 uint32_t v = 0u;
-                if (FULL || p + 32u * (uint32_t)i < npx) v = gather_fetch<COH>(raw, W, H, mA, opB, flip ? W - 1 - x : x, y);
+                if (FULL || p + 32u * (uint32_t)i < npx) v = gather_fetch<COH>(raw, W, H, mA, opB, flip ? W - 1 - x : x, y, cut);
                 my[lane + 32u * (uint32_t)i] = v;
                 x += 32;
                 if (x >= W) { x -= W; ++y; }
@@ -264,7 +267,7 @@ __device__ __forceinline__ void final_rows_gather_t(const AugParams& P, const fl
                 if (p < npx) {
                     const uint32_t r = dw.div(p);
                     const int x = (int)(p - r * (uint32_t)W);
-                    v = gather_fetch<COH>(raw, W, H, mA, opB, flip ? W - 1 - x : x, oy0 + (int)r);
+                    v = gather_fetch<COH>(raw, W, H, mA, opB, flip ? W - 1 - x : x, oy0 + (int)r, cut);
                 }
                 my[lane + 32u * (uint32_t)i] = v;
             }
@@ -347,17 +350,17 @@ __device__ __forceinline__ void gather_rows_to_band(const AugParams& P, const ui
 template <int OUT, bool USE_TAB>
 __device__ __forceinline__ void final_rows_gather(const AugParams& P, const float* tab, const float pad[3], const Ctx& c,
                                                   const OpRec* opA, const OpRec* opB, int flip, void* out_img, int oy0, int oy1,
-                                                  uint32_t* tile) {
+                                                  uint32_t* tile, const Box* cut = nullptr) {
     const uint32_t npx = (uint32_t)(oy1 - oy0) * (uint32_t)P.W;
-    if ((npx & 127u) == 0u) final_rows_gather_t<OUT, USE_TAB, true>(P, tab, pad, c, opA, opB, flip, out_img, oy0, oy1, tile);
-    else final_rows_gather_t<OUT, USE_TAB, false>(P, tab, pad, c, opA, opB, flip, out_img, oy0, oy1, tile);
+    if ((npx & 127u) == 0u) final_rows_gather_t<OUT, USE_TAB, true>(P, tab, pad, c, opA, opB, flip, out_img, oy0, oy1, tile, cut);
+    else final_rows_gather_t<OUT, USE_TAB, false>(P, tab, pad, c, opA, opB, flip, out_img, oy0, oy1, tile, cut);
 }
 
 // the gather reads an image this kernel wrote (c.raw = scratch): coherent loads
 template <int OUT, bool USE_TAB>
 __device__ __forceinline__ void final_rows_gather_coh(const AugParams& P, const float* tab, const float pad[3], const Ctx& c,
                                                       const OpRec* opA, int flip, void* out_img, int oy0, int oy1, uint32_t* tile) {
-    final_rows_gather_t<OUT, USE_TAB, false, true>(P, tab, pad, c, opA, nullptr, flip, out_img, oy0, oy1, tile);
+    final_rows_gather_t<OUT, USE_TAB, false, true>(P, tab, pad, c, opA, nullptr, flip, out_img, oy0, oy1, tile, nullptr);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -414,7 +417,7 @@ __device__ __forceinline__ void final_rows_color(const AugParams& P, const float
 #pragma unroll
             for (int k = 0; k < 8; ++k)
 #pragma unroll
-                for (int ch = 0; ch < 3; ++ch) ob[3 * k + ch] = f2b(v[ch][k]);
+                for (int ch = 0; ch < 3; ++ch) ob[3 * k + ch] = TAB ? f2b(s_norm[ch * 256 + (int)v[ch][k]]) : f2b(v[ch][k]);
             store_oct_u8(o, ob);
         } else {
 #pragma unroll

@@ -125,8 +125,9 @@ __global__ void __launch_bounds__(1024) faa_resolve_kernel(const __grid_constant
         if (P.progs != nullptr) {
             Prog g;
             build_prog(s, bx, P.ops, P.n_op, P.op_base, P.apply_tail, P.H, P.W, P.out_w, P.allow, g);
+            lean_order(g, P.allow);
             // weight class: 0 heavy (cluster kernel), 1 mid (statistics / Sharpness kernel, three-way split only), 2 light
-            const int wc = !P.split ? 0 : prog_is_light(g) ? 2 : (P.split == 2 && prog_is_mid(g, P.allow)) ? 1 : 0;
+            const int wc = !P.split ? 0 : prog_is_light(g, P.allow) ? 2 : (P.split == 2 && prog_is_mid(g, P.allow)) ? 1 : 0;
             g.bucket = (uint8_t)(cost_bucket(prog_cost(g)) + wc * kCostBuckets);
             P.progs[i] = g;
             atomicAdd(&s_count[g.bucket], 1);
@@ -970,12 +971,15 @@ __device__ __forceinline__ void stream_oct(const AugParams& P, const uint32_t w[
 template <int OUT, bool TAB>
 __device__ __forceinline__ void emit_oct(const AugParams& P, const float* s_norm, typename OutElem<OUT>::T* o, uint32_t plane,
                                          const uint32_t px[8]) {
-    if constexpr (OUT == OUT_U8_HWC) {                               // (s_norm is the plain normalisation here: bytes as they are)
+    if constexpr (OUT == OUT_U8_HWC) {                               // (TAB: a LUT's table of byte values)
         uint32_t ob[24];
 #pragma unroll
         for (int k = 0; k < 8; ++k)
 #pragma unroll
-            for (int ch = 0; ch < 3; ++ch) ob[3 * k + ch] = (px[k] >> (8 * ch)) & 255u;
+            for (int ch = 0; ch < 3; ++ch) {
+                const uint32_t u = (px[k] >> (8 * ch)) & 255u;
+                ob[3 * k + ch] = TAB ? f2b(s_norm[ch * 256 + u]) : u;
+            }
         store_oct_u8(o, ob);
     } else {
 #pragma unroll
@@ -1026,6 +1030,19 @@ __device__ __forceinline__ void final_rows_stream8(const AugParams& P, const flo
     }
 }
 
+// PLAIN / LUT octet streaming (octet geometry, band staged)
+template <int OUT, bool TAB, bool LUT>
+__device__ __forceinline__ void final_rows_plain_lut8(const AugParams& P, const float* s_norm, const float* ftab, const Ctx& c,
+                                                      int flip, void* out_img, int oy0, int oy1) {
+    if (flip) {
+        if (LUT) final_rows_stream8<OUT, true, true>(P, ftab, c, out_img, oy0, oy1);
+        else final_rows_stream8<OUT, TAB, true>(P, s_norm, c, out_img, oy0, oy1);
+    } else {
+        if (LUT) final_rows_stream8<OUT, true, false>(P, ftab, c, out_img, oy0, oy1);
+        else final_rows_stream8<OUT, TAB, false>(P, s_norm, c, out_img, oy0, oy1);
+    }
+}
+
 // PLAIN / LUT final pass: the streaming loop when possible, else the generic aligned loop.
 // `ftab` (768 floats) is only read for LUT programs and must hold normalise(ch, lutc[ch][b]).
 template <int OUT, bool TAB, bool LUT, bool OCT = false>
@@ -1034,13 +1051,7 @@ __device__ __forceinline__ void final_rows_plain_lut(const AugParams& P, const f
     if constexpr (OUT != OUT_U8_HWC || OCT) {                       // (uint8 HWC: only the octet paths of the light kernel)
         if ((!LUT || ftab != nullptr) && band_fully_staged(c, t, oy0, oy1) && (OUT != OUT_U8_HWC || (OCT && octet_geometry(P, t)))) {
             if (OCT && octet_geometry(P, t)) {                 // (the light kernel: 8 pixels per thread and iteration)
-                if (t.flip) {
-                    if (LUT) final_rows_stream8<OUT, true, true>(P, ftab, c, out_img, oy0, oy1);
-                    else final_rows_stream8<OUT, TAB, true>(P, s_norm, c, out_img, oy0, oy1);
-                } else {
-                    if (LUT) final_rows_stream8<OUT, true, false>(P, ftab, c, out_img, oy0, oy1);
-                    else final_rows_stream8<OUT, TAB, false>(P, s_norm, c, out_img, oy0, oy1);
-                }
+                final_rows_plain_lut8<OUT, TAB, LUT>(P, s_norm, ftab, c, t.flip, out_img, oy0, oy1);
                 return;
             }
             const float pad[3] = {normalise<TAB>(P, s_norm, 0, 0u), normalise<TAB>(P, s_norm, 1, 0u), normalise<TAB>(P, s_norm, 2, 0u)};
@@ -1628,7 +1639,7 @@ __global__ void __launch_bounds__(kMidThreadsMax, 2) faa_augment_mid_kernel(cons
     const Ctx c = make_ctx(P, P.in + (size_t)src_image(P, idx) * img_bytes, s_dyn, s_lo, s_len, P.H, P.W, st, true);
     const TailInfo t = make_tail(P, st.prog);
     float* ftab = reinterpret_cast<float*>(&st.hist[0][0]);      // 768 floats; the slot-0 histogram is idle by then
-    if (prog_two_stage(st.prog, P.scratch != nullptr ? 2 : 0)) {
+    if (prog_two_stage(st.prog, P.allow)) {
         // Stage A materialises op0 in the band buffer: a per-channel LUT (static or from statistics), Color or Cutout in
         // place (the raw bytes are not needed again; halo rows included); a gather straight from global memory; Sharpness
         // through the global scratch image (its neighbours' rows come back from there).  Stage B runs op1 on the band as a
@@ -1763,11 +1774,14 @@ __global__ void __launch_bounds__(kMidThreadsMax, 2) faa_augment_mid_kernel(cons
 // launch 3: the streaming kernel for "light" images (no statistics, no neighbourhood ops):
 // PLAIN / LUT / POINT / GEOM classes only - no cluster, 3 KB of static shared memory, a fraction of
 // the cluster kernel's registers and code.  It owns schedule entries [n_heavy, B).
+// LEAN: the variant for launches whose every light entry takes an octet path (LaunchPlan::lean_light, allow bit 3 of
+// prog_is_light).  Without the generic evaluators it fits 64 registers: four CTAs per SM, and two beside a mid CTA.
 #ifndef FAA_LIGHT_CTAS
 #define FAA_LIGHT_CTAS 3                  // (see FAA_MIN_CTAS)
 #endif
-template <int OUT, bool TAB>
-__global__ void __launch_bounds__(kThreads, FAA_LIGHT_CTAS) faa_augment_light_kernel(const __grid_constant__ AugParams P) {
+constexpr int kLeanLightCtas = 4;
+template <int OUT, bool TAB, bool LEAN>
+__global__ void __launch_bounds__(kThreads, LEAN ? kLeanLightCtas : FAA_LIGHT_CTAS) faa_augment_light_kernel(const __grid_constant__ AugParams P) {
     extern __shared__ __align__(128) uint8_t s_dyn[];           // staged row band
     __shared__ Prog s_prog;
     __shared__ __align__(16) uint8_t s_lut[2][768];
@@ -1808,7 +1822,8 @@ __global__ void __launch_bounds__(kThreads, FAA_LIGHT_CTAS) faa_augment_light_ke
                 for (int i = threadIdx.x; i < 768; i += blockDim.x)
                     s_lut[j][i] = (uint8_t)lut_entry_static(s_prog.op[j], (uint32_t)(i & 255), 0u);
         __syncthreads();
-        if (s_prog.cls == C_LUT || s_prog.cls == C_GEOM) {       // (GEOM: the one LUT slot rides in the float table)
+        // (GEOM: the one LUT slot rides in the float table; lean POINT: the static LUT behind Color / Cutout)
+        if (s_prog.cls == C_LUT || s_prog.cls == C_GEOM || (LEAN && s_prog.cls == C_POINT)) {
             for (int i = threadIdx.x; i < 768; i += blockDim.x) {
                 uint32_t v = (uint32_t)(i & 255), base = (uint32_t)(i & ~255);
                 if (lut_mask & 1u) v = s_lut[0][base + v];
@@ -1837,7 +1852,7 @@ __global__ void __launch_bounds__(kThreads, FAA_LIGHT_CTAS) faa_augment_light_ke
     {
         // lean octet paths (faa_fast.cuh) for the common geometry; everything else takes the generic evaluators
         // (C_GEOM2 only exists in launches whose geometry the lean gather handles: build_prog, allow bit 2)
-        if (cls == C_GEOM2 || ((cls == C_GEOM || cls == C_POINT) && octet_geometry(P, t) && band_fully_staged(c, t, oy0, oy1))) {
+        if (cls == C_GEOM2 || ((cls == C_GEOM || cls == C_POINT) && (LEAN || (octet_geometry(P, t) && band_fully_staged(c, t, oy0, oy1))))) {
             const int k0 = s_prog.op[0].kind, k1 = s_prog.op[1].kind;
             if (cls == C_GEOM2) {
                 // two gathers: out(x) = raw(map0(map1(x))), zero wherever either map leaves the image
@@ -1869,7 +1884,20 @@ __global__ void __launch_bounds__(kThreads, FAA_LIGHT_CTAS) faa_augment_light_ke
                         else final_rows_gather<OUT, TAB>(P, s_norm, pad, c, gp, nullptr, t.flip, out_img, oy0, oy1, s_tile);
                     }
                     done = true;
+                } else if (LEAN) {                                       // Cutout, then the gather (prog_is_light)
+                    const float pad[3] = {normalise<TAB>(P, s_norm, 0, 0u), normalise<TAB>(P, s_norm, 1, 0u), normalise<TAB>(P, s_norm, 2, 0u)};
+                    final_rows_gather<OUT, TAB>(P, s_norm, pad, c, &s_prog.op[1], nullptr, t.flip, out_img, oy0, oy1, s_tile, &s_prog.box[0]);
+                    done = true;
                 }
+            } else if (LEAN && k1 != K_NONE) {                           // Color / Cutout, then a static LUT: the float table
+                if (k0 == K_COLOR) {
+                    const float alpha = bits_to_float(s_prog.op[0].a[0]);
+                    if (s_prog.op[0].a[1]) final_rows_color<OUT, true, true>(P, s_ftab, c, alpha, t.flip, out_img, oy0, oy1);
+                    else final_rows_color<OUT, true, false>(P, s_ftab, c, alpha, t.flip, out_img, oy0, oy1);
+                } else {
+                    final_rows_cutout<OUT, true>(P, s_ftab, c, s_prog.box[0], t.flip, out_img, oy0, oy1);
+                }
+                done = true;
             } else if (k1 == K_NONE && k0 == K_COLOR) {
                 const float alpha = bits_to_float(s_prog.op[0].a[0]);
                 if (s_prog.op[0].a[1]) final_rows_color<OUT, TAB, true>(P, s_norm, c, alpha, t.flip, out_img, oy0, oy1);
@@ -1881,7 +1909,10 @@ __global__ void __launch_bounds__(kThreads, FAA_LIGHT_CTAS) faa_augment_light_ke
             }
         }
     }
-    if (!done) {
+    if (LEAN && !done) {                                         // C_PLAIN / C_LUT
+        if (cls == C_LUT) final_rows_plain_lut8<OUT, TAB, true>(P, s_norm, s_ftab, c, t.flip, out_img, oy0, oy1);
+        else final_rows_plain_lut8<OUT, TAB, false>(P, s_norm, s_ftab, c, t.flip, out_img, oy0, oy1);
+    } else if (!done) {
         switch (cls) {
         case C_PLAIN: final_rows_plain_lut<OUT, TAB, false, true>(P, s_norm, s_ftab, c, s_lutc, t, out_img, oy0, oy1); break;
         case C_LUT:   final_rows_plain_lut<OUT, TAB, true, true>(P, s_norm, s_ftab, c, s_lutc, t, out_img, oy0, oy1); break;
@@ -2390,10 +2421,10 @@ cudaError_t launch_augment_ragged(const RaggedParams& r, int bands, int count, s
 
 static inline int rows_of(const AugParams& p) { return (p.grid_y > 0 && p.grid_y < p.B) ? p.grid_y : p.B; }
 
-template <int OUT, bool TAB>
+template <int OUT, bool TAB, bool LEAN>
 static cudaError_t launch_light(const AugParams& p, cudaStream_t stream) {
     const size_t dyn = (size_t)p.geo[1].band_cap;
-    if (cudaError_t e = reserve_dyn_smem<faa_augment_light_kernel<OUT, TAB>>(dyn)) return e;
+    if (cudaError_t e = reserve_dyn_smem<faa_augment_light_kernel<OUT, TAB, LEAN>>(dyn)) return e;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)p.geo[1].bands, (unsigned)rows_of(p), 1);
     cfg.blockDim = dim3(kThreads, 1, 1);
@@ -2404,7 +2435,7 @@ static cudaError_t launch_light(const AugParams& p, cudaStream_t stream) {
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = p.chain ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, faa_augment_light_kernel<OUT, TAB>, p);
+    return cudaLaunchKernelEx(&cfg, faa_augment_light_kernel<OUT, TAB, LEAN>, p);
 }
 
 template <int OUT, bool TAB>
@@ -2430,9 +2461,9 @@ static cudaError_t launch_mid(const AugParams& p, cudaStream_t stream) {
 
 template <int OUT>
 cudaError_t launch_out(const AugParams& p, bool mix, bool tab, int which, cudaStream_t stream) {
-    const bool light = which == 1;
     if (which == 2) return tab ? launch_mid<OUT, true>(p, stream) : launch_mid<OUT, false>(p, stream);
-    if (light) return tab ? launch_light<OUT, true>(p, stream) : launch_light<OUT, false>(p, stream);
+    if (which == 1) return tab ? launch_light<OUT, true, false>(p, stream) : launch_light<OUT, false, false>(p, stream);
+    if (which == 3) return tab ? launch_light<OUT, true, true>(p, stream) : launch_light<OUT, false, true>(p, stream);
     if constexpr (OUT != OUT_U8_HWC) {                   // fused Mixup needs a float output
         if (mix) return tab ? launch_one<OUT, 2, true>(p, stream) : launch_one<OUT, 2, false>(p, stream);
     }
@@ -2449,7 +2480,8 @@ extern template cudaError_t launch_out<OUT_U8_HWC>(const AugParams&, bool, bool,
 
 // which == 0: the cluster kernel (all images, or the heavy part of a split launch);
 // which == 1: the streaming kernel for the light part of a split launch (p.n_heavy != nullptr);
-// which == 2: the statistics / Sharpness kernel for the mid part of a three-way split
+// which == 2: the statistics / Sharpness kernel for the mid part of a three-way split;
+// which == 3: the lean variant of the streaming kernel (LaunchPlan::lean_light)
 cudaError_t launch_augment(const AugParams& p, int out_type, bool use_tab, int which, cudaStream_t stream) {
     if (p.B <= 0) return cudaSuccess;
     const bool mix = p.partner != nullptr;
@@ -2462,11 +2494,11 @@ cudaError_t launch_augment(const AugParams& p, int out_type, bool use_tab, int w
     }
 }
 
-int resident_ctas_per_sm(int which) { return which == 1 ? FAA_LIGHT_CTAS : which == 2 ? 2 : FAA_MIN_CTAS; }
+int resident_ctas_per_sm(int which) { return which == 1 ? FAA_LIGHT_CTAS : which == 3 ? kLeanLightCtas : which == 2 ? 2 : FAA_MIN_CTAS; }
 
 unsigned augment_cta_count(const AugParams& p, int which) {
     if (p.B <= 0) return 0u;
-    if (which == 1) return (unsigned)p.geo[1].bands * (unsigned)rows_of(p);
+    if (which == 1 || which == 3) return (unsigned)p.geo[1].bands * (unsigned)rows_of(p);
     if (which == 2) return (unsigned)p.bands * (unsigned)rows_of(p);
     return (unsigned)p.bands * (unsigned)p.B;
 }

@@ -69,6 +69,7 @@ struct AugParams {
     int32_t band_cap;           // bytes of dynamic shared memory per staged band
     int32_t crop_pad;           // max |crop_dy| (RandomCrop padding)
     int32_t mat_cap;            // bytes of the materialisation chunk (0: none), a whole number of rows >= 3
+    int32_t allow;              // ResolveParams::allow of this launch (the mid kernel's two-stage programs depend on it)
     int32_t pdl;                // launched with programmatic stream serialization
     const int32_t* ready;       // chained steps: spin until *ready == ticket before reading programs / order / n_heavy
     int32_t ticket;
@@ -87,8 +88,9 @@ struct AugParams {
 };
 // number of CTAs launch_augment starts for (p, which): what `done` advances by
 unsigned augment_cta_count(const AugParams& p, int which);
-int resident_ctas_per_sm(int which);     // the launch bounds of the light (1) / mid (2) / cluster (0) kernel
-cudaError_t launch_augment(const AugParams& p, int out_type, bool use_tab, int which, cudaStream_t stream);   // which: 0 cluster, 1 light, 2 mid
+int resident_ctas_per_sm(int which);     // the launch bounds of the light (1, lean variant 3) / mid (2) / cluster (0) kernel
+// which: 0 cluster, 1 light, 2 mid, 3 the light kernel's lean variant (LaunchPlan::lean_light)
+cudaError_t launch_augment(const AugParams& p, int out_type, bool use_tab, int which, cudaStream_t stream);
 
 struct CropImage { const uint8_t* data; int32_t h, w; };               // == faa_image_t: one image of a ragged batch
 
