@@ -34,8 +34,9 @@ JPEG_HEADER_DTYPE = np.dtype([("offset", "<i8"), ("len", "<i8"), ("scan_off", "<
                               ("pool", "<i4", (9,)), ("qprec", "<i4"), ("reserved", "<i4")])   # faa_jpeg_header_t
 JPEG_TABLE_DTYPE = np.dtype([("q", "<u2", (64,)), ("bits", "u1", (16,)), ("vals", "u1", (256,))])   # faa_jpeg_table_t
 JPEG_TRUNCATED, JPEG_BAD_CODE, JPEG_BAD_COEF, JPEG_BAD_RESTART = 1, 2, 4, 8                       # faa_jpeg_status
+JPEG_SYNC_DTYPE = np.dtype([("mcu", "<i4"), ("byte", "<i4"), ("bit", "<i2"), ("pred", "<i2", (3,))])  # faa_jpeg_sync_t
 assert SAMPLE_DTYPE.itemsize == 16 and BOX_DTYPE.itemsize == 8 and IMAGE_DTYPE.itemsize == 16
-assert JPEG_HEADER_DTYPE.itemsize == 144 and JPEG_TABLE_DTYPE.itemsize == 400
+assert JPEG_HEADER_DTYPE.itemsize == 144 and JPEG_TABLE_DTYPE.itemsize == 400 and JPEG_SYNC_DTYPE.itemsize == 16
 
 
 class Tail(C.Structure):          # faa_tail_t
@@ -107,6 +108,9 @@ def _load():
         "faa_jpeg_decoder_create": (C.c_int, [P(vp)]),
         "faa_jpeg_decoder_destroy": (C.c_int, [vp]),
         "faa_jpeg_decode": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp]),
+        "faa_jpeg_index_capacity": (C.c_int, [vp]),
+        "faa_jpeg_index_build": (C.c_int, [vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp]),
+        "faa_jpeg_decode_indexed": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp]),
         "faa_launch_count": (u64, []),
     }
     for name, (res, args) in sig.items():

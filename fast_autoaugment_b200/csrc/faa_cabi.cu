@@ -1576,6 +1576,8 @@ int faa_augment_host(faa_policy_t* p, const uint8_t* h_in, void* h_out, void* d_
 static_assert(sizeof(faa_jpeg_header_t) == sizeof(JpegHeader) && sizeof(JpegHeader) == 144 &&
               offsetof(faa_jpeg_header_t, pool) == offsetof(JpegHeader, pool), "JPEG header layout");
 static_assert(sizeof(faa_jpeg_table_t) == sizeof(JpegTable), "JPEG table layout");
+static_assert(sizeof(faa_jpeg_sync_t) == sizeof(JpegSync) && sizeof(JpegSync) == 16 &&
+              offsetof(faa_jpeg_sync_t, pred) == offsetof(JpegSync, pred), "JPEG sync point layout");
 
 struct faa_jpeg_decoder {
     std::mutex mu;
@@ -1662,13 +1664,77 @@ int faa_jpeg_decoder_destroy(faa_jpeg_decoder_t* d) {
     return FAA_OK;
 }
 
+int faa_jpeg_index_capacity(const faa_jpeg_header_t* hdr) {
+    if (!hdr) return 0;
+    JpegHeader h; memcpy(&h, hdr, sizeof h);
+    return jpeg_index_capacity(h);
+}
+
 int faa_jpeg_decode(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
                     const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
                     const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status, void* stream_v) {
+    return faa_jpeg_decode_indexed(d, h_headers, d_headers, d_tables, n_tables, d_src, batch, h_out, d_out, d_status,
+                                   nullptr, nullptr, nullptr, stream_v);
+}
+
+}  // extern "C"
+
+// the point offsets of a call: [batch + 1], non-decreasing, from 0 up
+static int check_jpeg_first(const int64_t* h_first, int batch) {
+    if (h_first[0] < 0) return fail(FAA_ERR_VALUE, "point offsets: first[0] is negative");
+    for (int i = 0; i < batch; ++i)
+        if (h_first[i + 1] < h_first[i])
+            return fail(FAA_ERR_VALUE, "point offsets: first[" + std::to_string(i + 1) + "] < first[" + std::to_string(i) + "]");
+    if (h_first[batch] > (int64_t)INT32_MAX * 16) return fail(FAA_ERR_VALUE, "point offsets out of range");
+    return FAA_OK;
+}
+
+extern "C" {
+
+int faa_jpeg_index_build(const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
+                         const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
+                         const int64_t* h_first, const int64_t* d_first, faa_jpeg_sync_t* d_points, int32_t* d_count,
+                         int32_t* d_status, void* stream_v) {
+    if ((!h_headers || !d_headers || !d_tables || !d_src || !h_first || !d_first || !d_count || !d_status) && batch > 0)
+        return fail(FAA_ERR_VALUE, "null argument");
+    if (batch < 0) return fail(FAA_ERR_VALUE, "negative batch");
+    if (batch > 65535) return fail(FAA_ERR_UNSUPPORTED, "at most 65535 images per call: split the batch");
+    if (batch == 0) return FAA_OK;
+    if (int e = check_jpeg_first(h_first, batch)) return e;
+    if (!d_points && h_first[batch] > h_first[0]) return fail(FAA_ERR_VALUE, "null argument");
+    for (int i = 0; i < batch; ++i) {
+        JpegHeader h; memcpy(&h, &h_headers[i], sizeof h);
+        if (int e = check_jpeg_header(h, n_tables, "image " + std::to_string(i))) return e;
+    }
+    if (int e = ensure_device()) return e;
+    JpegDecodeParams P = {};
+    P.hdrs = reinterpret_cast<const JpegHeader*>(d_headers);
+    P.pool = reinterpret_cast<const JpegTable*>(d_tables);
+    P.src = d_src;
+    P.status = d_status;
+    P.batch = batch;
+    P.first = d_first;
+    P.points = reinterpret_cast<JpegSync*>(d_points);
+    P.count = d_count;
+    CK(launch_jpeg_index(P, (cudaStream_t)stream_v));
+    g_launches++;
+    return FAA_OK;
+}
+
+int faa_jpeg_decode_indexed(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
+                            const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
+                            const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status,
+                            const faa_jpeg_sync_t* d_points, const int64_t* h_first, const int64_t* d_first, void* stream_v) {
     if (!d || ((!h_headers || !d_headers || !d_tables || !d_src || !h_out || !d_out || !d_status) && batch > 0))
         return fail(FAA_ERR_VALUE, "null argument");
     if (batch < 0) return fail(FAA_ERR_VALUE, "negative batch");
     if (batch > 65535) return fail(FAA_ERR_UNSUPPORTED, "at most 65535 images per call: split the batch");
+    const bool indexed = h_first || d_first || d_points;
+    if (indexed && batch > 0) {
+        if (!h_first || !d_first) return fail(FAA_ERR_VALUE, "null argument: point offsets need h_first and d_first");
+        if (int e = check_jpeg_first(h_first, batch)) return e;
+        if (!d_points && h_first[batch] > h_first[0]) return fail(FAA_ERR_VALUE, "null argument: d_points");
+    }
     std::vector<JpegJob> jobs((size_t)batch + 1);
     int64_t blocks = 0, segs = 0, tiles = 0;
     for (int i = 0; i < batch; ++i) {
@@ -1704,7 +1770,7 @@ int faa_jpeg_decode(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, c
     if (int e = grow_async(&d->d_segs, &d->segs_bytes, (size_t)segs * sizeof(int32_t), stream)) return e;
     if (int e = grow_async(&d->d_jobs, &d->jobs_bytes, jobs.size() * sizeof(JpegJob), stream)) return e;
     CK(cudaMemcpyAsync(d->d_jobs, jobs.data(), jobs.size() * sizeof(JpegJob), cudaMemcpyHostToDevice, stream));  // (pageable: staged at once)
-    JpegDecodeParams P;
+    JpegDecodeParams P = {};
     P.hdrs = reinterpret_cast<const JpegHeader*>(d_headers);
     P.pool = reinterpret_cast<const JpegTable*>(d_tables);
     P.src = d_src;
@@ -1714,6 +1780,10 @@ int faa_jpeg_decode(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, c
     P.segs = reinterpret_cast<int32_t*>(d->d_segs);
     P.status = d_status;
     P.batch = batch;
+    if (indexed) {
+        P.first = d_first;
+        P.points = const_cast<JpegSync*>(reinterpret_cast<const JpegSync*>(d_points));
+    }
     CK(launch_jpeg_entropy(P, stream));
     g_launches++;
     CK(launch_jpeg_reconstruct(P, (int)tiles, stream));

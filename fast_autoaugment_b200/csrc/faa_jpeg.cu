@@ -5,7 +5,10 @@
 //                                memory; when the image has restart markers its threads find them in parallel (a
 //                                count, a prefix sum, then the positions); then one thread per restart segment turns
 //                                the scan into int16 coefficients.  An image without restart markers is one segment,
-//                                decoded serially by one thread: the known limit of this design.
+//                                decoded serially by one thread, unless the call gives it a scan index: then thread k
+//                                decodes from point k to point k + 1 and checks that it ended in that point's state;
+//                                if any segment disagrees, thread 0 decodes the scan serially over it.
+//   faa_jpeg_index_kernel        (faa_jpeg_index_build) one CTA per image; one thread records the scan index.
 //   faa_jpeg_reconstruct_kernel  one CTA per 64 x 32 output tile of one image.  It runs the islow IDCT of the tile's
 //                                blocks, with the one-block chroma halo fancy upsampling reads, into shared memory,
 //                                upsamples and converts to RGB, and writes uint8 HWC rows with 32-bit stores where the
@@ -21,6 +24,21 @@ constexpr int kEntropyThreads = 128;
 constexpr int kReconThreads = 256;
 constexpr int kReconMaxBlocks = 96;        // 4:4:4: 8 x 4 blocks of each of the three components
 
+// the image's Huffman tables in shared memory, built by the whole CTA (the lookup entries are complete after the
+// caller's next barrier); hp[t]: the table of slot t, slots of absent components pointing at component 0's
+__device__ __forceinline__ void jpeg_cta_tables(const JpegHeader& h, const JpegTable* pool, JpegHuff* s_huff, int tid,
+                                                const JpegHuff* hp[6]) {
+    if (tid < 6 && tid % 3 < h.ncomp) jpeg_huff_codes(pool[h.pool[3 + tid]], s_huff[tid]);
+    __syncthreads();
+    for (int e = tid; e < 6 << kJpegLookBits; e += kEntropyThreads) {
+        const int t = e >> kJpegLookBits;
+        if (t % 3 < h.ncomp) s_huff[t].look[e & ((1 << kJpegLookBits) - 1)] = jpeg_huff_look(s_huff[t], e & ((1 << kJpegLookBits) - 1));
+    }
+    for (int t = 0; t < 6; ++t) hp[t] = &s_huff[t % 3 < h.ncomp ? t : (t / 3) * 3];
+}
+
+// kIndexed: the call gives scan indexes (P.first, P.points); the other instantiation is the path without them.
+template <bool kIndexed>
 __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_entropy_kernel(const __grid_constant__ JpegDecodeParams P) {
     __shared__ JpegHuff s_huff[6];
     __shared__ __align__(16) int16_t s_scratch[kEntropyThreads][64];
@@ -34,13 +52,9 @@ __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_entropy_kernel(const
     int32_t* segs = P.segs + job.seg;
     const int64_t n_seg = jpeg_segments(h), mcus = jpeg_mcus(h);
     if (tid == 0) s_status = 0;
-    if (tid < 6 && tid % 3 < h.ncomp) jpeg_huff_codes(P.pool[h.pool[3 + tid]], s_huff[tid]);
     for (int64_t k = tid; k < n_seg; k += kEntropyThreads) segs[k] = k == 0 ? 0 : -1;
-    __syncthreads();
-    for (int e = tid; e < 6 << kJpegLookBits; e += kEntropyThreads) {
-        const int t = e >> kJpegLookBits;
-        if (t % 3 < h.ncomp) s_huff[t].look[e & ((1 << kJpegLookBits) - 1)] = jpeg_huff_look(s_huff[t], e & ((1 << kJpegLookBits) - 1));
-    }
+    const JpegHuff* hp[6];
+    jpeg_cta_tables(h, P.pool, s_huff, tid, hp);
     if (n_seg > 1) {                                       // restart markers: count, prefix, record
         const int64_t chunk = (h.scan_len + kEntropyThreads - 1) / kEntropyThreads;
         const int64_t a = min((int64_t)tid * chunk, h.scan_len), b = min(a + chunk, h.scan_len);
@@ -57,10 +71,24 @@ __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_entropy_kernel(const
         jpeg_markers(r, scan, a, b, h.scan_len, segs, 1 + s_count[tid], n_seg);
     }
     __syncthreads();
-    const JpegHuff* hp[6];
-    for (int t = 0; t < 6; ++t) hp[t] = &s_huff[t % 3 < h.ncomp ? t : (t / 3) * 3];
     int status = 0;
-    for (int64_t k = tid; k < n_seg; k += kEntropyThreads) {
+    bool serial = true;
+    const int64_t n_pts = kIndexed ? P.first[img + 1] - P.first[img] : 0;
+    if (kIndexed && n_pts > 0) {                                       // a scan index: one segment per thread from its points
+        const JpegSync* pts = P.points + P.first[img];
+        bool ok = jpeg_index_count_ok(h, n_pts);
+        if (ok && tid < n_pts) ok = jpeg_index_point_ok(h, pts[tid], tid ? pts[tid - 1].mcu : 0);
+        if (__syncthreads_and(ok)) {
+            bool linked = true;
+            if (tid <= n_pts)
+                status = jpeg_index_segment(h, hp, scan, pts, (int)n_pts, tid, P.coef + 64 * job.coef, s_scratch[tid], &linked);
+            // every segment ended where the next one starts: by induction each started in the serial decode's state.
+            // Otherwise thread 0 decodes the scan serially below, overwriting every block.
+            serial = !__syncthreads_and(linked);
+            if (serial) status = 0;
+        }
+    }
+    for (int64_t k = tid; serial && k < n_seg; k += kEntropyThreads) {
         const int64_t m0 = n_seg == 1 ? 0 : k * h.restart;
         const int64_t m1 = n_seg == 1 ? mcus : min(m0 + h.restart, mcus);
         const int32_t at = segs[k];
@@ -159,9 +187,35 @@ __global__ void __launch_bounds__(kReconThreads) faa_jpeg_reconstruct_kernel(con
     }
 }
 
+// One CTA per image: the CTA builds the Huffman tables, then one thread decodes the scan serially without storing a
+// coefficient and records the points of the placement rule (jpeg_index_parts), at most the capacity planned for it.
+__global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_index_kernel(const __grid_constant__ JpegDecodeParams P) {
+    __shared__ JpegHuff s_huff[6];
+    __shared__ __align__(16) int16_t s_scratch[64];
+    const int img = blockIdx.x, tid = threadIdx.x;
+    const JpegHeader h = P.hdrs[img];
+    const JpegHuff* hp[6];
+    jpeg_cta_tables(h, P.pool, s_huff, tid, hp);
+    __syncthreads();
+    if (tid != 0) return;
+    const int64_t cap = P.first[img + 1] - P.first[img];
+    int status = 0;
+    const int n = jpeg_index_record(h, hp, P.src + h.offset + h.scan_off, P.points + P.first[img],
+                                    cap < kJpegIndexMaxParts ? (int)cap : kJpegIndexMaxParts, s_scratch, &status);
+    P.count[img] = n;
+    P.status[img] = status;
+}
+
+cudaError_t launch_jpeg_index(const JpegDecodeParams& p, cudaStream_t stream) {
+    if (p.batch <= 0) return cudaSuccess;
+    faa_jpeg_index_kernel<<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_jpeg_entropy(const JpegDecodeParams& p, cudaStream_t stream) {
     if (p.batch <= 0) return cudaSuccess;
-    faa_jpeg_entropy_kernel<<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p);
+    if (p.first) faa_jpeg_entropy_kernel<true><<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p);
+    else faa_jpeg_entropy_kernel<false><<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p);
     return cudaGetLastError();
 }
 

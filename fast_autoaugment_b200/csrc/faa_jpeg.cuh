@@ -420,6 +420,77 @@ FAA_JHD int jpeg_decode(JpegBits& r, const JpegHuff& d) {
     return -1;
 }
 
+// ------------------------------------------------------------------------------------------------ sync points --
+// The decoder's state at an MCU boundary (layout of faa_jpeg_sync_t): MCU `mcu` is the next to decode, its first bit is
+// bit `bit` (0 = most significant) of the data byte at scan offset `byte` (a stuffed 0xFF 0x00 is one data byte, at the
+// 0xFF's offset), and pred[] are the DC predictors.  A scan index is a list of such points; a segment started at one
+// decodes as the serial decoder does from that MCU on.
+struct JpegSync {
+    int32_t mcu;
+    int32_t byte;
+    int16_t bit;
+    int16_t pred[3];
+};
+
+constexpr int kJpegIndexMaxParts = 128;        // segments of an indexed scan: the entropy kernel's threads
+constexpr int kJpegIndexBytesPerPart = 1024;
+
+// The placement rule of a scan index, the one place it is stated.  A scan of scan_len bytes without restart markers is
+// cut into P = min(128, scan_len / 1024) segments of about equal bytes (bytes are the work, not MCUs); point k (1 <= k
+// < P) is the first MCU boundary whose start byte is >= k * scan_len / P, and points that coincide are dropped.  Below
+// two segments, and for files with a restart interval, there is no index: jpeg_index_parts returns 0.
+FAA_JHD int jpeg_index_parts(const JpegHeader& h) {
+    if (h.restart > 0) return 0;
+    const int64_t p = h.scan_len / kJpegIndexBytesPerPart;
+    return p < 2 ? 0 : p > kJpegIndexMaxParts ? kJpegIndexMaxParts : (int)p;
+}
+// most points an index of this file holds
+FAA_JHD int jpeg_index_capacity(const JpegHeader& h) { const int p = jpeg_index_parts(h); return p ? p - 1 : 0; }
+FAA_JHD int64_t jpeg_index_threshold(const JpegHeader& h, int parts, int k) { return (int64_t)k * h.scan_len / parts; }
+
+// Whether an index can be used as it stands: a file the rule gives points to, at most 127 points, MCUs strictly
+// increasing inside (0, mcus), bytes inside the scan, bits 0..7.  Anything else decodes serially.
+FAA_JHD bool jpeg_index_point_ok(const JpegHeader& h, const JpegSync& s, int32_t prev_mcu) {
+    return s.mcu > prev_mcu && s.mcu > 0 && (int64_t)s.mcu < (int64_t)h.mcu_x * h.mcu_y && s.byte >= 0 &&
+           (int64_t)s.byte < h.scan_len && s.bit >= 0 && s.bit <= 7;
+}
+FAA_JHD bool jpeg_index_count_ok(const JpegHeader& h, int64_t n) {
+    return n > 0 && n < kJpegIndexMaxParts && jpeg_index_parts(h) > 0;
+}
+
+// the end state of one segment equals the point the next one starts at (its MCU is implied)
+FAA_JHD bool jpeg_sync_same(const JpegSync& a, const JpegSync& b) {
+    return a.byte == b.byte && a.bit == b.bit && a.pred[0] == b.pred[0] && a.pred[1] == b.pred[1] && a.pred[2] == b.pred[2];
+}
+
+// The bit reader's consumed position in canonical form, at an MCU boundary: walk back from the next unread byte over
+// the data bytes whose bits are still buffered (a 0x00 after a 0xFF is the stuffing of that 0xFF: one data byte).
+// Bits made up past the data (`fake`) were never in a byte.
+FAA_JHD void jpeg_bits_pos(JpegBits& r, int32_t* byte, int16_t* bit) {
+    const int u = r.n > r.fake ? r.n - r.fake : 0;        // real bits buffered, not consumed
+    const uint8_t* q = r.p;
+    for (int k = (u + 7) >> 3; k > 0; --k) {
+        --q;
+        if (q > r.lo && jpeg_byte_at(r, q) == 0 && jpeg_byte_at(r, q - 1) == 0xFF) --q;
+    }
+    *byte = (int32_t)(q - r.lo);
+    *bit = (int16_t)((8 - (u & 7)) & 7);
+}
+
+// Starts the bit reader of the scan [lo, end) at a sync point: at its data byte (`data`, lo + s.byte), with the first
+// s.bit bits of it dropped.
+FAA_JHD void jpeg_bits_start(JpegBits& r, const uint8_t* lo, const uint8_t* data, const uint8_t* end, const JpegSync& s) {
+    jpeg_bits_init(r, lo, data, end);
+    if (s.bit > 0) { jpeg_fill(r); jpeg_get(r, s.bit); }
+}
+
+// Where a recording decode puts the points of the placement rule: at most `cap`, `n` written so far.
+struct JpegIndexSink {
+    JpegSync* at;
+    int32_t cap, n;
+    int32_t parts, next;     // segments of the rule; the next point k to place
+};
+
 // ------------------------------------------------------------------------------------------------ coefficients --
 // Coefficient planes of one image: component c's blocks form a grid of (mcu_x * hc) x (mcu_y * vc) blocks of 64 int16
 // (natural order, not dequantised), plane after plane starting at `coef`.
@@ -471,19 +542,38 @@ FAA_JHD void jpeg_zero_block(int16_t* s) {
 #endif
 }
 
-// Decodes MCUs [m0, m1) from `data` (the segment's first byte) into coef.  huff[c] / huff[3 + c]: DC / AC tables of
-// component c.  On an error the blocks from the failing one to the end of the segment are zeroed.  Returns JpegStatus.
-FAA_JHD int jpeg_decode_segment(const JpegHeader& h, const JpegHuff* const* huff, const uint8_t* lo, const uint8_t* data,
-                                const uint8_t* end, int64_t m0, int64_t m1, int16_t* coef, int16_t* scratch) {
+// Decodes MCUs [from.mcu, m1) of the scan [lo, end), starting in the state `from` (a restart segment: its first byte,
+// bit 0, zero predictors), into coef.  huff[c] / huff[3 + c]: DC / AC tables of component c.  On an error the blocks
+// from the failing one to the end of the segment are zeroed.  With `to`, a segment that decodes cleanly reports the
+// state it ends in (MCU m1).  With `rec` (a recording decode of a whole restart-free scan) it stores no coefficient and
+// places the points of the rule (jpeg_index_parts) at the MCU boundaries it passes.  `data`: the start byte as a
+// pointer, instead of lo + from.byte (a restart segment whose marker is missing starts at `end`).  Returns JpegStatus.
+FAA_JHD int jpeg_decode_segment(const JpegHeader& h, const JpegHuff* const* huff, const uint8_t* lo, const uint8_t* end,
+                                const JpegSync& from, int64_t m1, int16_t* coef, int16_t* scratch, JpegSync* to = nullptr,
+                                JpegIndexSink* rec = nullptr, const uint8_t* data = nullptr) {
     JpegBits r;
-    jpeg_bits_init(r, lo, data, end);
-    int pred[3] = {0, 0, 0};
+    jpeg_bits_start(r, lo, data ? data : lo + from.byte, end, from);
+    int pred[3] = {from.pred[0], from.pred[1], from.pred[2]};
     const int nb = jpeg_blocks_per_mcu(h);
     const int ny = h.ncomp == 1 ? 1 : h.hs * h.vs;
     int status = JPEG_OK;
-    int64_t m = m0;
+    int64_t m = from.mcu;
     int b = 0;
     for (; m < m1; ++m) {
+        if (rec && m > from.mcu) {                       // an MCU boundary: the points whose threshold it reaches
+            JpegSync s;
+            jpeg_bits_pos(r, &s.byte, &s.bit);
+            bool placed = false;
+            while (rec->next < rec->parts && (int64_t)s.byte >= jpeg_index_threshold(h, rec->parts, rec->next)) {
+                if (!placed && rec->n < rec->cap) {
+                    s.mcu = (int32_t)m;
+                    for (int c = 0; c < 3; ++c) s.pred[c] = (int16_t)pred[c];
+                    rec->at[rec->n++] = s;
+                    placed = true;                       // (the later thresholds it reaches coincide: dropped)
+                }
+                ++rec->next;
+            }
+        }
         for (b = 0; b < nb; ++b) {
             const int c = b < ny ? 0 : b - ny + 1;
             const JpegHuff& dc = *huff[c];
@@ -512,17 +602,56 @@ FAA_JHD int jpeg_decode_segment(const JpegHeader& h, const JpegHuff* const* huff
                 }
             }
             if (status) break;
-            jpeg_store_block(coef + 64 * jpeg_block_of(h, m, b), scratch);
+            if (!rec) jpeg_store_block(coef + 64 * jpeg_block_of(h, m, b), scratch);
         }
         if (status) break;
         if (r.n < r.fake) { status = JPEG_TRUNCATED; ++m; b = 0; break; }     // this MCU used bits past the data
     }
-    if (status) {
+    if (status && !rec) {
         jpeg_zero_block(scratch);
         for (; m < m1; ++m, b = 0)
             for (; b < nb; ++b) jpeg_store_block(coef + 64 * jpeg_block_of(h, m, b), scratch);
     }
+    if (to && !status) {
+        to->mcu = (int32_t)m1;
+        jpeg_bits_pos(r, &to->byte, &to->bit);
+        for (int c = 0; c < 3; ++c) to->pred[c] = (int16_t)pred[c];
+    }
     return status;
+}
+
+// a restart segment: MCUs [m0, m1) from `data` (its first byte), zero predictors
+FAA_JHD int jpeg_decode_segment(const JpegHeader& h, const JpegHuff* const* huff, const uint8_t* lo, const uint8_t* data,
+                                const uint8_t* end, int64_t m0, int64_t m1, int16_t* coef, int16_t* scratch) {
+    const JpegSync from = {(int32_t)m0, 0, 0, {0, 0, 0}};
+    return jpeg_decode_segment(h, huff, lo, end, from, m1, coef, scratch, nullptr, nullptr, data);
+}
+
+// The recording decode of a scan index: the whole scan, serially, placing the points of the rule into at[0, cap).
+// Returns the number of points, 0 when the scan does not decode cleanly (or the file gets no index); *status gets the
+// decode's status.
+FAA_JHD int jpeg_index_record(const JpegHeader& h, const JpegHuff* const* huff, const uint8_t* scan, JpegSync* at,
+                              int cap, int16_t* scratch, int* status) {
+    *status = 0;
+    const int parts = jpeg_index_parts(h);
+    if (!parts || cap <= 0) return 0;
+    JpegIndexSink rec = {at, cap < parts - 1 ? cap : parts - 1, 0, parts, 1};
+    const JpegSync zero = {0, 0, 0, {0, 0, 0}};
+    *status = jpeg_decode_segment(h, huff, scan, scan + h.scan_len, zero, jpeg_mcus(h), nullptr, scratch, nullptr, &rec);
+    return *status ? 0 : rec.n;
+}
+
+// Segment k of an indexed scan with n points: MCUs [pts[k - 1].mcu, pts[k].mcu), the first from the scan's start and
+// the last to its end.  Its status, and whether it ended where the next segment starts (the last one always does).
+FAA_JHD int jpeg_index_segment(const JpegHeader& h, const JpegHuff* const* huff, const uint8_t* scan, const JpegSync* pts,
+                               int n, int k, int16_t* coef, int16_t* scratch, bool* linked) {
+    const JpegSync zero = {0, 0, 0, {0, 0, 0}};
+    const JpegSync& from = k == 0 ? zero : pts[k - 1];
+    const int64_t m1 = k < n ? (int64_t)pts[k].mcu : jpeg_mcus(h);
+    JpegSync to;
+    const int st = jpeg_decode_segment(h, huff, scan, scan + h.scan_len, from, m1, coef, scratch, &to);
+    *linked = k == n || (st == 0 && jpeg_sync_same(to, pts[k]));
+    return st;
 }
 
 // Restart markers of the scan bytes [from, to) (a marker is 0xFF 0xD0..0xD7; its 0xFF may be the last of the range):
@@ -668,8 +797,11 @@ FAA_JHD int jpeg_tile_windows(const JpegHeader& h, int x0, int y0, int x1, int y
 
 // ------------------------------------------------------------------------------------------------ host decode --
 // The whole decode of one file on the host, serially, with the functions above: the CPU tests' model of the two
-// kernels.  out: h.h * h.w * 3 bytes.  Returns the JpegStatus bits.
-inline int jpeg_decode_host(const uint8_t* file, const JpegHeader& h, const JpegTable* tabs, uint8_t* out) {
+// kernels.  out: h.h * h.w * 3 bytes.  With a scan index (npts points) the entropy decode runs as the entropy kernel's
+// indexed path does: validate, one segment per point, end states checked, a serial decode when anything disagrees.
+// Returns the JpegStatus bits.
+inline int jpeg_decode_host(const uint8_t* file, const JpegHeader& h, const JpegTable* tabs, uint8_t* out,
+                            const JpegSync* pts = nullptr, int64_t npts = 0) {
     static_assert(sizeof(JpegTable) == 400, "table layout");
     JpegHuff huffs[6];
     const JpegHuff* hp[6];
@@ -681,7 +813,8 @@ inline int jpeg_decode_host(const uint8_t* file, const JpegHeader& h, const Jpeg
     alignas(16) int16_t scratch[64];
     const uint8_t* scan = file + h.scan_off;
     const uint8_t* end = scan + h.scan_len;
-    const int64_t n_seg = jpeg_segments(h), mcus = jpeg_mcus(h);
+    int64_t n_seg = jpeg_segments(h);
+    const int64_t mcus = jpeg_mcus(h);
     int32_t* at = new int32_t[(size_t)n_seg];
     for (int64_t k = 0; k < n_seg; ++k) at[k] = -1;
     at[0] = 0;
@@ -689,6 +822,19 @@ inline int jpeg_decode_host(const uint8_t* file, const JpegHeader& h, const Jpeg
     if (n_seg > 1) {
         JpegBits r; jpeg_bits_init(r, scan, scan, end);
         if (jpeg_markers(r, scan, 0, h.scan_len, h.scan_len, at, 1, n_seg) != n_seg - 1) status |= JPEG_BAD_RESTART;
+    }
+    bool indexed = pts && jpeg_index_count_ok(h, npts);
+    for (int64_t k = 0; indexed && k < npts; ++k) indexed = jpeg_index_point_ok(h, pts[k], k ? pts[k - 1].mcu : 0);
+    if (indexed) {
+        bool linked = true;
+        for (int k = 0; k <= (int)npts; ++k) {
+            bool ok = true;
+            const int st = jpeg_index_segment(h, hp, scan, pts, (int)npts, k, coef, scratch, &ok);
+            linked = linked && ok;
+            if (k == (int)npts) status = st;
+        }
+        if (linked) n_seg = 0;                           // done; otherwise the serial decode below overwrites it all
+        else status = 0;
     }
     for (int64_t k = 0; k < n_seg; ++k) {
         const int64_t m0 = k * (h.restart > 0 ? h.restart : mcus), m1 = n_seg == 1 ? mcus : (m0 + h.restart < mcus ? m0 + h.restart : mcus);

@@ -151,8 +151,14 @@ struct JpegDecodeParams {
     int32_t* segs;              // restart-segment starts, relative to each scan (-1: marker not found)
     int32_t* status;            // [batch] JpegStatus bits
     int32_t batch;
+    // scan index: image i's points are points[first[i], first[i + 1]) (decode: null = none; index build: the
+    // capacities, with the points written in count[i])
+    const int64_t* first;
+    JpegSync* points;
+    int32_t* count;             // [batch] (index build only)
 };
 cudaError_t launch_jpeg_entropy(const JpegDecodeParams& p, cudaStream_t stream);
 cudaError_t launch_jpeg_reconstruct(const JpegDecodeParams& p, int n_tiles, cudaStream_t stream);
+cudaError_t launch_jpeg_index(const JpegDecodeParams& p, cudaStream_t stream);
 
 }  // namespace faa

@@ -553,15 +553,68 @@ class EncodedDeviceDataset:
 
 
 class FilePaths(list):
-    """Paths of image files that stay on disk (the ImageNet directory source of ``_load_arrays``)."""
+    """Paths of image files that stay on disk (the ImageNet directory source of ``_load_arrays``); ``split`` and
+    ``folder`` name the split folder they were listed from."""
+    split = folder = None
+
+
+JPEG_INDEX_VERSION = 1
+
+
+class JpegIndex:
+    """The scan indexes of one split folder's files (``python -m fast_autoaugment_b200.jpeg_index``, file
+    ``<split>.npz``: ``paths`` relative to the folder, ``sizes`` the file lengths, ``first`` / ``points`` as
+    ``build_jpeg_index`` gives them, ``version``).  A file is looked up by its path relative to ``folder``; a file the
+    index does not list, or whose length differs from the one indexed, gets no points.  Any other staleness (a file
+    rewritten at the same length) is caught by the decoder, which then decodes that file serially."""
+
+    def __init__(self, folder, paths, sizes, first, points):
+        self.folder = os.fspath(folder)
+        self.sizes = np.asarray(sizes, np.int64).reshape(-1)
+        self.first = np.asarray(first, np.int64).reshape(-1)
+        self.points = np.ascontiguousarray(points, dtype=_lib.JPEG_SYNC_DTYPE).reshape(-1)
+        self._at = {os.fsdecode(bytes(p)) if isinstance(p, (bytes, np.bytes_)) else os.fspath(p): i
+                    for i, p in enumerate(paths)}
+        if len(self.first) != len(self._at) + 1 or len(self.sizes) != len(self._at) or \
+                (np.diff(self.first) < 0).any() or self.first[0] != 0 or self.first[-1] != len(self.points):
+            raise ValueError("inconsistent JPEG index")
+
+    @staticmethod
+    def load(path, folder):
+        with np.load(path, allow_pickle=False) as z:
+            if int(z["version"]) != JPEG_INDEX_VERSION:
+                raise ValueError("%s: JPEG index version %d, this package reads version %d" % (
+                    path, int(z["version"]), JPEG_INDEX_VERSION))
+            return JpegIndex(folder, list(z["paths"]), z["sizes"], z["first"], z["points"])
+
+    def save(self, path):
+        rel = sorted(self._at, key=self._at.get)
+        np.savez(path, paths=np.array([os.fsencode(p) for p in rel], dtype=bytes), sizes=self.sizes,
+                 first=self.first, points=self.points, version=np.int64(JPEG_INDEX_VERSION))
+
+    def lookup(self, path, length):
+        """the points of the file at ``path`` (of ``length`` bytes), empty when it has none here"""
+        i = self._at.get(os.path.relpath(os.fspath(path), self.folder))
+        if i is None or int(self.sizes[i]) != int(length):
+            return self.points[:0]
+        return self.points[self.first[i]:self.first[i + 1]]
+
+    def gather(self, paths, lengths):
+        """(first, points) of a batch of files, as ``EncodedImages`` carries them"""
+        parts = [self.lookup(p, n) for p, n in zip(paths, lengths)]
+        first = np.zeros(len(parts) + 1, np.int64)
+        first[1:] = np.cumsum([len(q) for q in parts])
+        return first, (np.concatenate(parts) if parts else self.points[:0])
 
 
 class JpegFileDataset:
     """``EncodedDeviceDataset`` whose files stay on disk: it holds paths and targets only, so no byte of the split is on
-    the device.  ``GpuAugmentedLoader`` streams each batch's files through a ``FileBatchStream``."""
+    the device.  ``GpuAugmentedLoader`` streams each batch's files through a ``FileBatchStream``.  ``index``: a
+    ``JpegIndex`` of the files, whose scan indexes let the device decode each listed file on many threads."""
 
-    def __init__(self, paths, targets, device="cuda"):
+    def __init__(self, paths, targets, device="cuda", index=None):
         self.paths = [os.fspath(p) for p in paths]
+        self.index = index
         self.targets = [int(t) for t in targets]
         if len(self.targets) != len(self.paths):
             raise ValueError("need one target per image")
@@ -579,6 +632,7 @@ class JpegFileDataset:
         idx = [int(i) for i in idx]
         d = JpegFileDataset.__new__(JpegFileDataset)
         d.paths = self.select(idx)
+        d.index = self.index
         d.targets = [self.targets[i] for i in idx]
         d.labels = self.labels.index_select(0, torch.as_tensor(idx, dtype=torch.int64, device=self.labels.device))
         d.device = self.device
@@ -605,11 +659,13 @@ class HostBatch:
     """The host half of staging one batch of files (``read_jpeg_batch``): ``paths``; ``files``, ``headers`` and the
     table ``pool`` of the files the device decoder takes (headers' ``offset`` places those files back to back, as
     ``EncodedImages.from_bytes`` of them would); the batch positions of those files (``accepted``) and of the rest
-    (``refused``), and Pillow's pixels of the refused ones (``pixels``, uint8 [h, w, 3])."""
+    (``refused``), and Pillow's pixels of the refused ones (``pixels``, uint8 [h, w, 3]); with an index, the accepted
+    files' scan indexes (``first``, ``points``, as ``EncodedImages`` carries them; otherwise None)."""
 
-    def __init__(self, paths, files, headers, pool, accepted, refused, pixels):
+    def __init__(self, paths, files, headers, pool, accepted, refused, pixels, first=None, points=None):
         self.paths, self.files, self.headers, self.pool = paths, files, headers, pool
         self.accepted, self.refused, self.pixels = accepted, refused, pixels
+        self.first, self.points = first, points
 
     def sizes(self):
         """(h, w) of every image of the batch, int32 [N, 2]"""
@@ -620,9 +676,10 @@ class HostBatch:
         return s
 
 
-def read_jpeg_batch(paths, map=map):
+def read_jpeg_batch(paths, map=map, index=None):
     """Read a batch of files and parse their headers (``parse_jpeg_headers``); decode the files the device decoder
-    refuses with Pillow.  No device is touched.  ``map``: an executor's ``map`` reads, parses and decodes in parallel."""
+    refuses with Pillow; with a ``JpegIndex``, gather the accepted files' scan indexes.  No device is touched.  ``map``:
+    an executor's ``map`` reads, parses and decodes in parallel."""
     paths = list(paths)
     files = list(map(_read_file, paths))
     headers, pool, refused = parse_jpeg_headers(files, map)
@@ -632,7 +689,10 @@ def read_jpeg_batch(paths, map=map):
     headers = headers[ok]
     headers["offset"] = np.cumsum(lengths) - lengths
     pixels = list(map(_pillow_rgb, [(paths[i], files[i]) for i in bad]))
-    return HostBatch(paths, [files[i] for i in ok], headers, pool, ok, bad, pixels)
+    first = points = None
+    if index is not None:
+        first, points = index.gather([paths[i] for i in ok], lengths)
+    return HostBatch(paths, [files[i] for i in ok], headers, pool, ok, bad, pixels, first, points)
 
 
 def chunked_map(pool_map, n_chunks):
@@ -652,7 +712,8 @@ def _up16(n):
 
 class _Layout:
     """Byte layout of one staged batch, the same in the pinned slot and in the batch's device buffer: headers, table
-    pool, the accepted files back to back, then the refused files' pixels, each part on a 16-byte boundary."""
+    pool, the accepted files back to back, the refused files' pixels, then (with an index) the accepted files' point
+    offsets and points, each part on a 16-byte boundary."""
 
     def __init__(self, hb: HostBatch):
         self.pool = _up16(hb.headers.nbytes)
@@ -662,6 +723,12 @@ class _Layout:
         for px in hb.pixels:
             self.pixels.append(at)
             at = _up16(at + px.nbytes)
+        self.first = self.points = self.points_end = None
+        if hb.first is not None:
+            self.first = at
+            self.points = _up16(at + hb.first.nbytes)
+            self.points_end = self.points + hb.points.nbytes
+            at = _up16(self.points_end)
         self.total = max(at, 16)
 
     def pack(self, hb: HostBatch, buf):
@@ -673,6 +740,9 @@ class _Layout:
             at += len(f)
         for o, px in zip(self.pixels, hb.pixels):
             buf[o:o + px.nbytes] = px.reshape(-1)
+        if self.first is not None:
+            buf[self.first:self.first + hb.first.nbytes] = hb.first.view(np.uint8)
+            buf[self.points:self.points_end] = hb.points.view(np.uint8).reshape(-1)
 
 
 _STATUS_BITS = ((_lib.JPEG_TRUNCATED, "scan truncated"), (_lib.JPEG_BAD_CODE, "bad Huffman code"),
@@ -689,18 +759,20 @@ class FileBatchStream:
     ``non_blocking`` copy of the slot into a device buffer of the batch, decodes the accepted files (``decode_jpeg``)
     into their images of ``RaggedImages.empty(sizes)`` and copies the refused files' pixels into theirs.  Each batch's
     decode status is copied to pinned host memory and checked once the next batch is staged, and at the end, so no
-    batch waits on its own decode: a non-zero status raises ``OSError`` naming the file."""
+    batch waits on its own decode: a non-zero status raises ``OSError`` naming the file.  With a ``JpegIndex`` each
+    batch's scan indexes travel in the same slot and the decode uses them."""
 
     SLOTS = 2
     WORKERS = 2
 
-    def __init__(self, workers=None):
+    def __init__(self, workers=None, index=None):
         self.workers = int(workers or self.WORKERS)
+        self.index = index
         self.slots = [None] * self.SLOTS           # pinned uint8 staging buffers
         self.copied = [None] * self.SLOTS          # event recorded after each slot's last host-to-device copy
 
     def _stage(self, paths, slot, pool, dev):
-        hb = read_jpeg_batch(paths, chunked_map(pool.map, self.workers) if self.workers > 1 else map)
+        hb = read_jpeg_batch(paths, chunked_map(pool.map, self.workers) if self.workers > 1 else map, self.index)
         lay = _Layout(hb)
         if self.copied[slot] is not None:
             self.copied[slot].synchronize()
@@ -715,8 +787,13 @@ class FileBatchStream:
         sizes = hb.sizes()
         out = RaggedImages.empty(sizes, dev)
         if len(hb.accepted):
+            index = {}
+            if hb.first is not None:
+                index = dict(first=hb.first, points=hb.points,
+                             _d_first=dbuf[lay.first:lay.first + hb.first.nbytes].view(torch.int64),
+                             _d_points=dbuf[lay.points:lay.points_end])
             enc = EncodedImages(dbuf[lay.files:lay.files_end], hb.headers, hb.pool, _d_pool=dbuf[lay.pool:lay.files],
-                                _d_headers=dbuf[:lay.pool])
+                                _d_headers=dbuf[:lay.pool], **index)
             _, status = decode_jpeg(enc, out.select(hb.accepted))
             st = torch.empty(len(hb.accepted), dtype=torch.int32, pin_memory=True)
             st.copy_(status, non_blocking=True)
@@ -815,7 +892,7 @@ class GpuAugmentedLoader:
         if isinstance(self.dataset, JpegFileDataset):
             dev = self.dataset.device
             batches = [idx_all[k * self.batch_size:(k + 1) * self.batch_size] for k in range(len(self))]
-            self.staging = FileBatchStream()
+            self.staging = FileBatchStream(index=self.dataset.index)
             files = self.staging([self.dataset.select(idx) for idx in batches], dev)
         else:
             dev = self.dataset.images.device
@@ -909,9 +986,19 @@ def _load_arrays(dataset, dataroot):
             return (np.concatenate([hwc(tr), hwc(ex)]), list(tr.labels) + list(ex.labels), hwc(te), list(te.labels))
         return hwc(tr), list(tr.labels), hwc(te), list(te.labels)
     if dataset == "imagenet":                                   # data.py:146-150
-        tr, te = imagenet_index(dataroot, "train"), imagenet_index(dataroot, "val")
-        return FilePaths(p for p, _ in tr), [t for _, t in tr], FilePaths(p for p, _ in te), [t for _, t in te]
+        out = []
+        for split in ("train", "val"):
+            samples = imagenet_index(dataroot, split)
+            paths = FilePaths(p for p, _ in samples)
+            paths.split, paths.folder = split, imagenet_split_folder(dataroot, split)
+            out += [paths, [t for _, t in samples]]
+        return tuple(out)
     raise ValueError("invalid dataset name=%s" % dataset)
+
+
+def imagenet_split_folder(dataroot, split):
+    """``dataroot/imagenet-pytorch/<split>``: the folder ``imagenet_index``'s paths lie in"""
+    return os.path.join(os.path.expanduser(os.path.join(str(dataroot), "imagenet-pytorch")), split)
 
 
 def imagenet_index(dataroot, split):
@@ -980,7 +1067,10 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
     ``conf['model']['type']``; without it ImageNet images must already have the network's size).
 
     ``imagenet`` with the reference's ``dataroot`` (``imagenet-pytorch/{train,val}``, ``imagenet_index``) keeps the
-    files on disk (``JpegFileDataset``): the loaders read, stage and decode each batch's files one batch ahead."""
+    files on disk (``JpegFileDataset``): the loaders read, stage and decode each batch's files one batch ahead.
+    ``faa_jpeg_index``: a directory holding ``train.npz`` / ``val.npz`` written by ``python -m
+    fast_autoaugment_b200.jpeg_index DATAROOT DIR``; the files they index are decoded on many threads each, with the
+    same pixels."""
     from sklearn.model_selection import StratifiedShuffleSplit
 
     conf = C.get()
@@ -1003,9 +1093,18 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
         raise ValueError("ImageNet images of different sizes (or JPEG files) need conf['faa_crop_resize']: without it the "
                          "images are augmented at one fixed size")
 
+    index_dir = conf.get("faa_jpeg_index")
+
     def device_dataset(x, y):
         if isinstance(x, FilePaths):
-            return JpegFileDataset(x, y)
+            index = None
+            if index_dir:
+                path = os.path.join(os.fspath(index_dir), "%s.npz" % x.split)
+                if not os.path.exists(path):
+                    raise FileNotFoundError("conf['faa_jpeg_index']: no index of the %s split at %s (write it with "
+                                            "python -m fast_autoaugment_b200.jpeg_index)" % (x.split, path))
+                index = JpegIndex.load(path, x.folder)
+            return JpegFileDataset(x, y, index=index)
         if isinstance(x, list) and len(x) and isinstance(x[0], bytes):
             return EncodedDeviceDataset(x, y)
         return RaggedDeviceDataset(x, y) if isinstance(x, list) else DeviceDataset(x, y)

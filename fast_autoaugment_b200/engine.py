@@ -576,11 +576,17 @@ class EncodedImages:
     on the host (C ABI ``faa_jpeg_parse``), and the quantisation and Huffman tables they use deduplicated into one table
     pool.  ``headers`` (host ``JPEG_HEADER_DTYPE`` [N]) is what ``decode_jpeg`` validates and plans from; their device
     copy and the pool's are made on first use.  ``select`` makes a batch of some of the files without copying a byte of
-    them."""
+    them.
 
-    def __init__(self, storage: torch.Tensor, headers, pool, _d_pool=None, _d_headers=None):
-        """``_d_pool`` / ``_d_headers``: device copies of ``pool`` / ``headers`` the caller already made (uint8 tensors
-        of their bytes), used instead of uploading them on first use"""
+    Optionally the files carry a scan index (``build_jpeg_index``): ``first`` (int64 [N + 1]) and ``points``
+    (``JPEG_SYNC_DTYPE``), file i's points being ``points[first[i]:first[i + 1]]``.  ``decode_jpeg`` then decodes each
+    indexed file on many threads; the pixels and status are those of the decode without the index, whatever it holds."""
+
+    def __init__(self, storage: torch.Tensor, headers, pool, _d_pool=None, _d_headers=None, first=None, points=None,
+                 _d_first=None, _d_points=None):
+        """``_d_pool`` / ``_d_headers`` / ``_d_first`` / ``_d_points``: device copies of ``pool`` / ``headers`` /
+        ``first`` / ``points`` the caller already made (uint8 tensors of their bytes, ``first`` int64), used instead of
+        uploading them on first use"""
         if not isinstance(storage, torch.Tensor) or storage.dtype != torch.uint8 or storage.dim() != 1 \
                 or not storage.is_contiguous():
             raise ValueError("storage must be a contiguous 1-D uint8 tensor")
@@ -590,8 +596,19 @@ class EncodedImages:
         h = self.headers
         if len(h) and (int(h["offset"].min()) < 0 or int((h["offset"] + h["len"]).max()) > storage.numel()):
             raise ValueError("every file must lie inside the storage")
+        if (first is None) != (points is None):
+            raise ValueError("a scan index needs both first and points")
+        self.first = self.points = None
+        if first is not None:
+            self.first = np.ascontiguousarray(first, dtype=np.int64).reshape(-1)
+            self.points = np.ascontiguousarray(points, dtype=_lib.JPEG_SYNC_DTYPE).reshape(-1)
+            f = self.first
+            if len(f) != len(h) + 1 or f[0] != 0 or (np.diff(f) < 0).any() or f[-1] > len(self.points):
+                raise ValueError("first must be [N + 1] non-decreasing offsets from 0 into points")
         self._d_pool = _d_pool
         self._d_headers = _d_headers
+        self._d_first = _d_first
+        self._d_points = _d_points
 
     @staticmethod
     def from_bytes(files, device="cuda"):
@@ -620,9 +637,19 @@ class EncodedImages:
         """(h, w) of every image, int32 [N, 2]"""
         return np.stack([self.headers["h"], self.headers["w"]], axis=1).astype(np.int32).reshape(-1, 2)
 
+    def with_index(self, first, points):
+        """the same files carrying the scan index (first, points), e.g. ``build_jpeg_index``'s"""
+        return EncodedImages(self.storage, self.headers, self.pool, self.device_pool(), self._d_headers, first, points)
+
     def select(self, idx):
         idx = np.asarray(idx, dtype=np.int64).reshape(-1)
-        return EncodedImages(self.storage, self.headers[idx], self.pool, self.device_pool())
+        first = points = None
+        if self.first is not None:
+            counts = np.diff(self.first)[idx]
+            first = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)
+            at = np.repeat(self.first[:-1][idx] - first[:-1], counts) + np.arange(int(first[-1]), dtype=np.int64)
+            points = self.points[at]
+        return EncodedImages(self.storage, self.headers[idx], self.pool, self.device_pool(), first=first, points=points)
 
     def device_pool(self):
         """the table pool on the device (shared by every ``select`` of this set)"""
@@ -636,6 +663,45 @@ class EncodedImages:
             flat = self.headers.view(np.uint8).reshape(-1)
             self._d_headers = torch.from_numpy(flat.copy() if flat.size else np.zeros(1, np.uint8)).to(self.device)
         return self._d_headers
+
+    def device_index(self):
+        """(first, points) on the device: int64 [N + 1] and the points' bytes"""
+        if self._d_first is None:
+            self._d_first = torch.from_numpy(self.first.copy()).to(self.device)
+        if self._d_points is None:
+            flat = self.points.view(np.uint8).reshape(-1)
+            self._d_points = torch.from_numpy(flat.copy() if flat.size else np.zeros(16, np.uint8)).to(self.device)
+        return self._d_first, self._d_points
+
+
+def build_jpeg_index(encoded: EncodedImages):
+    """The scan index of every file of ``encoded`` (C ABI ``faa_jpeg_index_build``: one serial decode per file on the
+    device, one thread per file): ``(first, points)``, int64 [N + 1] offsets into ``JPEG_SYNC_DTYPE`` points, file i's
+    being ``points[first[i]:first[i + 1]]``.  Files with restart markers, scans under 2 KiB and files whose scan does
+    not decode cleanly get none.  Waits for the device."""
+    _require_cuda(encoded.storage, "encoded")
+    dev = encoded.device
+    B = len(encoded)
+    if B == 0:
+        return np.zeros(1, np.int64), np.zeros(0, _lib.JPEG_SYNC_DTYPE)
+    hdr0 = encoded.headers.ctypes.data
+    caps = np.array([lib.faa_jpeg_index_capacity(hdr0 + i * encoded.headers.itemsize) for i in range(B)], np.int64)
+    cap_first = np.concatenate([[0], np.cumsum(caps)]).astype(np.int64)
+    total = int(cap_first[-1])
+    with torch.cuda.device(dev):
+        d_first = torch.from_numpy(cap_first).to(dev)
+        d_points = torch.empty(max(total, 1) * 16, dtype=torch.uint8, device=dev)
+        d_count = torch.empty(B, dtype=torch.int32, device=dev)
+        d_status = torch.empty(B, dtype=torch.int32, device=dev)
+        check(lib.faa_jpeg_index_build(hdr0, encoded.device_headers().data_ptr(), encoded.device_pool().data_ptr(),
+                                       len(encoded.pool), encoded.storage.data_ptr(), B, cap_first.ctypes.data,
+                                       d_first.data_ptr(), d_points.data_ptr(), d_count.data_ptr(),
+                                       d_status.data_ptr(), _stream_ptr(dev)))
+        count = d_count.cpu().numpy().astype(np.int64)
+        pts = d_points.cpu().numpy()[:total * 16].view(_lib.JPEG_SYNC_DTYPE)
+    first = np.concatenate([[0], np.cumsum(count)]).astype(np.int64)
+    at = np.repeat(cap_first[:-1] - first[:-1], count) + np.arange(int(first[-1]), dtype=np.int64)
+    return first, pts[at].copy()
 
 
 class _JpegDecoder:
@@ -659,7 +725,8 @@ _DECODERS = {}
 
 
 def decode_jpeg(encoded: EncodedImages, out: RaggedImages | None = None):
-    """Decode every file of ``encoded`` on its device (C ABI ``faa_jpeg_decode``: two launches, no host wait), bit-exact
+    """Decode every file of ``encoded`` on its device (C ABI ``faa_jpeg_decode``, or ``faa_jpeg_decode_indexed`` when
+    the files carry a scan index: two launches, no host wait), bit-exact
     with ``Image.open(f).convert('RGB')`` (reference imagenet.py:80).  Returns ``(images, status)``: a ``RaggedImages``
     (``out``, by default ``RaggedImages.empty(encoded.sizes)``) and an int32 CUDA tensor of ``faa_jpeg_status`` bits per
     image, 0 where the scan decoded completely; a corrupt image still gets defined pixels."""
@@ -678,9 +745,17 @@ def decode_jpeg(encoded: EncodedImages, out: RaggedImages | None = None):
         dec = _DECODERS.get(dev.index)
         if dec is None:
             dec = _DECODERS[dev.index] = _JpegDecoder()
-        check(lib.faa_jpeg_decode(dec.handle, encoded.headers.ctypes.data, encoded.device_headers().data_ptr(),
-                                  encoded.device_pool().data_ptr(), len(encoded.pool), encoded.storage.data_ptr(), B,
-                                  h_out.ctypes.data, d_out.data_ptr(), status.data_ptr(), _stream_ptr(dev)))
+        if encoded.first is None:
+            check(lib.faa_jpeg_decode(dec.handle, encoded.headers.ctypes.data, encoded.device_headers().data_ptr(),
+                                      encoded.device_pool().data_ptr(), len(encoded.pool), encoded.storage.data_ptr(), B,
+                                      h_out.ctypes.data, d_out.data_ptr(), status.data_ptr(), _stream_ptr(dev)))
+        else:
+            d_first, d_points = encoded.device_index()
+            check(lib.faa_jpeg_decode_indexed(dec.handle, encoded.headers.ctypes.data, encoded.device_headers().data_ptr(),
+                                              encoded.device_pool().data_ptr(), len(encoded.pool),
+                                              encoded.storage.data_ptr(), B, h_out.ctypes.data, d_out.data_ptr(),
+                                              status.data_ptr(), d_points.data_ptr(), encoded.first.ctypes.data,
+                                              d_first.data_ptr(), _stream_ptr(dev)))
     return out, status
 
 

@@ -376,6 +376,43 @@ int faa_jpeg_decode(faa_jpeg_decoder_t* dec, const faa_jpeg_header_t* h_headers,
                     const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
                     const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status, void* stream);
 
+/* ---- scan index: lets a file without restart markers be decoded by many threads.  One serial pass (faa_jpeg_index_build)
+ * records the decoder's state at up to 127 MCU boundaries; every later decode of the file starts one thread at each of
+ * them.  Placement: a scan of scan_len bytes with no restart interval is cut into P = min(128, scan_len / 1024) parts
+ * of about equal bytes; point k (1 <= k < P) is the first MCU boundary whose start byte is >= k * scan_len / P, and
+ * points that coincide are dropped.  Below 2 parts (scans under 2 KiB), or with a restart interval, a file has no
+ * points.  The file itself is not changed. */
+typedef struct faa_jpeg_sync {
+    int32_t mcu;              /* the next MCU to decode                                                              */
+    int32_t byte;             /* scan offset of the data byte that holds its first bit (a stuffed 0xFF 0x00 is one data
+                                 byte, at the 0xFF's offset)                                                         */
+    int16_t bit;              /* bits of that byte already consumed, 0..7                                            */
+    int16_t pred[3];          /* DC predictors of the components (0 for absent ones)                                 */
+} faa_jpeg_sync_t;            /* 16 bytes */
+
+/* host only: the most points faa_jpeg_index_build records for a file with this header (P - 1, or 0) */
+int faa_jpeg_index_capacity(const faa_jpeg_header_t* hdr);
+
+/* Records the scan index of `batch` files (inputs as faa_jpeg_decode).  h_first / d_first: host and device copies of
+ * int64 [batch + 1] offsets into d_points, planned by the caller (image i may get first[i + 1] - first[i] points, at most
+ * faa_jpeg_index_capacity of its header); d_count: [batch] int32, the points written at d_points + first[i]; d_status:
+ * [batch] int32, the status of that serial decode (a file whose decode has a status gets no points; 0 for files that
+ * get none by the placement rule).  FAA_ERR_VALUE for offsets that decrease or are negative.  One launch, no host wait. */
+int faa_jpeg_index_build(const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
+                         const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
+                         const int64_t* h_first, const int64_t* d_first, faa_jpeg_sync_t* d_points, int32_t* d_count,
+                         int32_t* d_status, void* stream);
+
+/* faa_jpeg_decode with a scan index: image i's points are d_points[first[i], first[i + 1]) (h_first / d_first: host and
+ * device copies of int64 [batch + 1], validated on the host as in faa_jpeg_index_build).  The points are checked on the
+ * device before use, and every segment's end state against the next point; a file whose index is invalid, stale or
+ * from another file is decoded serially, so pixels and status always equal faa_jpeg_decode's.  Points of files with a
+ * restart interval are ignored.  All three null: faa_jpeg_decode. */
+int faa_jpeg_decode_indexed(faa_jpeg_decoder_t* dec, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
+                            const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
+                            const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status,
+                            const faa_jpeg_sync_t* d_points, const int64_t* h_first, const int64_t* d_first, void* stream);
+
 /* number of kernels this library has launched since load (bench bookkeeping) */
 uint64_t faa_launch_count(void);
 
