@@ -289,7 +289,7 @@ int faa_emu_philox(const void* ops_v, const double* probs, int n_sub, int n_op, 
 // their count.  split_min < 0: the library's default.
 const char* faa_emu_plan_fields() {
     return "bands band_cap stage light_bands light_staged octets mat_cap use_order use_split use_mid split mid_bands "
-           "mid_threads allow scratch no_heavy self_resolving use_chain speculate";
+           "mid_threads allow scratch no_heavy self_resolving use_chain speculate light_cap";
 }
 
 int faa_emu_plan(int H, int W, int out_h, int out_w, int batch, int crop_pad, int out_u8, int in_mod16, int out_mod16,
@@ -299,7 +299,7 @@ int faa_emu_plan(int H, int W, int out_h, int out_w, int batch, int crop_pad, in
                                       split_min < 0 ? kSplitMin : (uint64_t)split_min, philox != 0, allow_ahead != 0});
     const int32_t v[] = {L.geo[0].bands, L.geo[0].band_cap, L.stage, L.geo[1].bands, L.geo[1].band_cap > 0, L.octets,
                          L.mat_cap, L.use_order, L.use_split, L.use_mid, L.split, L.mid.bands, L.mid_threads, L.allow,
-                         L.scratch, L.no_heavy, L.self_resolving, L.use_chain, L.speculate};
+                         L.scratch, L.no_heavy, L.self_resolving, L.use_chain, L.speculate, L.geo[1].band_cap};
     memcpy(out, v, sizeof v);
     return (int)(sizeof v / sizeof v[0]);
 }

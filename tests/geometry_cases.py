@@ -13,6 +13,10 @@ CROP_CASES (RandomCrop: crop_pad and outputs smaller than the image) and MIX_CAS
 same for the other two inputs of the planner that change what the kernels run; tests/test_gpu_crop_mix_geometries.py
 runs them on the device.
 
+LEAN_CASES does it for the lean light kernel (`faa_augment_light_kernel<OUT, TAB, LEAN = true>`, allow bit 8), which runs
+every production Philox call at a fixed size: one case per `lean_regime()`, checked on the host by
+tests/test_lean_geometry_host.py and run on the device by tests/test_gpu_lean_geometries.py.
+
 RAGGED_CASES does it for the ragged policy launch (`faa_augment_ragged`, planned by `plan_ragged`): one image per
 per-image geometry, named by `ragged_regime()`, and RAGGED_MIXES, the calls tests/test_gpu_ragged_geometries.py makes
 of them with the pixel launches each one claims.
@@ -46,13 +50,20 @@ class Plan:
     mid_bands: int
     mid_threads: int
     no_heavy: bool            # the cluster kernel is not launched
-    allow: int                # resolve-kernel allow bits: 1 chunk, 2 scratch, 4 lean gathers
+    allow: int                # resolve-kernel allow bits: 1 chunk, 2 scratch, 4 lean gathers, 8 the lean light kernel
     band_cap: int = 0         # bytes of one source's staged cluster-kernel band (0: unstaged)
     crop: bool = False        # RandomCrop: crop_pad > 0 or an output smaller than the image
     smaller: bool = False     # the output is smaller than the image
     two_src: bool = False     # fused Mixup
     self_resolving: bool = False
     use_chain: bool = False   # chained schedule (Philox records, resolve-ahead allowed)
+    light_cap: int = 0        # bytes of the light kernel's largest staged band (0: unstaged)
+    H: int = 0                # image rows
+
+    @property
+    def lean(self):
+        """the light kernel runs its lean variant (LaunchPlan::lean_light): octet paths only, Philox records"""
+        return bool(self.allow & 8)
 
     def launches(self):
         """kernels of one call on resolved records (event schedule, faa_cabi.cu launch_event): the resolve kernel, then
@@ -66,15 +77,16 @@ class Plan:
 
 
 def plan(emu, H, W, batch, u8=False, in_off=0, out_off=0, split_min=-1, has_sg=True, out_h=None, out_w=None, crop_pad=0,
-         two_src=False, philox=False, allow_ahead=False):
+         two_src=False, philox=False, allow_ahead=False, apply_tail=True):
     """the planner's decisions for a launch of the final window (apply_tail), input and output at `in_off` / `out_off`
     bytes from a 256-byte aligned allocation (split_min -1: the library's default).  By default a single-source launch
     on resolved records, of the image's own size, no crop; out_h / out_w / crop_pad: RandomCrop; two_src: fused Mixup;
-    philox / allow_ahead: records drawn on the device, the next batch may be resolved ahead"""
+    philox / allow_ahead: records drawn on the device, the next batch may be resolved ahead; apply_tail False: a window of
+    a longer policy in front of the last one (uint8 HWC out)"""
     out_h, out_w = H if out_h is None else out_h, W if out_w is None else out_w
     names = emu.faa_emu_plan_fields().decode().split()
     out = (C.c_int32 * len(names))()
-    assert emu.faa_emu_plan(H, W, out_h, out_w, batch, crop_pad, int(u8), in_off % 16, out_off % 16, int(two_src), 1,
+    assert emu.faa_emu_plan(H, W, out_h, out_w, batch, crop_pad, int(u8), in_off % 16, out_off % 16, int(two_src), int(apply_tail),
                             int(has_sg), split_min, int(philox), int(allow_ahead), out) == len(names)
     d = dict(zip(names, out))
     stage_off = "" if d["stage"] else "size" if (H * W * 3) % 16 else "base" if in_off % 16 else "band"
@@ -84,7 +96,7 @@ def plan(emu, H, W, batch, u8=False, in_off=0, out_off=0, split_min=-1, has_sg=T
     return Plan(W, d["bands"], bool(d["stage"]), stage_off, d["light_bands"], bool(d["light_staged"]), bool(d["octets"]),
                 d["mat_cap"] > 0, bool(d["use_split"]), bool(d["use_mid"]), d["mid_bands"], d["mid_threads"],
                 bool(d["no_heavy"]), d["allow"], d["band_cap"], crop_pad > 0 or (out_h, out_w) != (H, W),
-                (out_h, out_w) != (H, W), two_src, bool(d["self_resolving"]), bool(d["use_chain"]))
+                (out_h, out_w) != (H, W), two_src, bool(d["self_resolving"]), bool(d["use_chain"]), d["light_cap"], H)
 
 
 def regime(p: Plan):
@@ -298,6 +310,111 @@ MIX_REGIMES = [
     "mix, unstaged (band)",
     "mix with a crop, staged",
     "mix with a crop, unstaged (doubled band)",
+]
+
+
+# ------------------------------------------------------------------------------------------ lean light launches --
+# `plan_launch` runs the lean variant of the light kernel (octet paths only, no generic fallbacks, no per-CTA
+# `octet_geometry` / `band_fully_staged` check) when the launch has octets, a staged light band, no crop and Philox
+# records.  What the kernel then assumes about its band depends on the light band count the planner picked, whether
+# those bands are equal, whether the row's octet count W / 8 is odd (the mirrored octets pair up across the middle),
+# how close the staged band is to its 100 KB limit, one-row bands, and whether the cluster kernel runs beside it (no
+# chunk: allow bit 0 off, so some programs stay heavy).
+LIGHT_STAGE_LIMIT = 100 * 1024   # bytes of a staged light band
+
+
+def lean_regime(p: Plan):
+    """the regime of a lean light launch (None when the lean kernel does not run): light bands, even / uneven, W / 8
+    parity, and "near the limit" (staged band within 4 KB of 100 KB), "one-row bands", "one octet per row",
+    "cluster kernel" (launched beside the lean kernel) when they hold"""
+    if not p.lean:
+        return None
+    r = "%d bands, %s, W/8 %s" % (p.light_bands, "uneven" if p.H % p.light_bands else "even", "odd" if p.W // 8 % 2 else "even")
+    extra = [what for what, on in (("near the limit", p.light_cap + 4096 > LIGHT_STAGE_LIMIT),
+                                   ("one-row bands", p.H == p.light_bands), ("one octet per row", p.W == 8),
+                                   ("cluster kernel", not p.no_heavy)) if on]
+    return ", ".join([r] + extra)
+
+
+@dataclass
+class LeanCase:
+    """a lean light launch: the image size, the batch the GPU test runs (at the default split threshold, and large enough
+    that the seed search finds every sub-policy in it) and the regime it claims"""
+    shape: tuple
+    batch: int
+    regime: str
+    why: str
+    full: bool = False        # production size: every output type and entry point (else fp16 + uint8, augment_batch)
+
+    @property
+    def id(self):
+        return "%dx%d" % self.shape
+
+    @property
+    def big(self):            # the record oracle checks a sample of the images
+        return max(self.shape) > 640
+
+    def plan(self, emu, u8=False, batch=None, allow_ahead=True):
+        return plan(emu, *self.shape, self.batch if batch is None else batch, u8=u8, philox=True, allow_ahead=allow_ahead)
+
+
+# Light bands: the cluster kernel's band count, or for 8 the count in 5..8 that fills whole 256-thread iterations best.
+# Band sizes are the largest staged light band (+ halo), rounded up to 128 bytes.
+LEAN_CASES = [
+    LeanCase((224, 224), 96, "7 bands, even, W/8 even", "the flagship step: 7 bands of 32 rows, 22912 B", full=True),
+    LeanCase((240, 240), 96, "6 bands, even, W/8 even", "EfficientNet-B1: 6 bands of 40 rows, 30336 B", full=True),
+    LeanCase((456, 456), 48, "8 bands, even, W/8 odd", "EfficientNet-B5: 8 bands of 57 rows, 80768 B; 57 octets per row",
+             full=True),
+    LeanCase((232, 232), 80, "6 bands, uneven, W/8 odd", "bands of 38 / 39 rows; 29 octets per row"),
+    LeanCase((300, 400), 48, "8 bands, uneven, W/8 even", "bands of 37 / 38 rows, not square"),
+    LeanCase((200, 456), 48, "7 bands, uneven, W/8 odd", "bands of 28 / 29 rows, wider than tall, 57 octets per row"),
+    LeanCase((512, 512), 48, "8 bands, even, W/8 even, near the limit", "a staged light band of 101376 B, 1024 B under 100 KB"),
+    LeanCase((240, 320), 64, "5 bands, even, W/8 even", "8 cluster bands, the light kernel picks 5 of 48 rows"),
+    LeanCase((120, 200), 176, "4 bands, even, W/8 odd", "4 cluster bands of 30 rows; 25 octets per row"),
+    LeanCase((96, 88), 512, "2 bands, even, W/8 odd", "2 bands of 48 rows, 11 octets per row"),
+    LeanCase((8, 8192), 64, "8 bands, even, W/8 even, one-row bands, cluster kernel",
+             "header limit: 8 one-row bands of 73728 B; pitch 24576 B: no chunk (allow = 14), so the cluster kernel runs "
+             "beside the lean kernel and the mid kernel"),
+    LeanCase((2, 8192), 256, "2 bands, even, W/8 even, one-row bands, cluster kernel",
+             "header limit: 2 one-row bands of 49152 B, no chunk"),
+    LeanCase((8192, 8), 64, "8 bands, even, W/8 odd, one octet per row", "header limit: 8 bands of 1024 rows, one octet per row"),
+    LeanCase((2048, 16), 128, "8 bands, even, W/8 even", "8 bands of 256 rows, two octets per row: the mirrored octets swap"),
+]
+
+# every regime LEAN_CASES must cover (a new lean geometry adds its regime here, and a case to LEAN_CASES)
+LEAN_REGIMES = [
+    "2 bands, even, W/8 odd",
+    "4 bands, even, W/8 odd",
+    "5 bands, even, W/8 even",
+    "6 bands, even, W/8 even",
+    "6 bands, uneven, W/8 odd",
+    "7 bands, even, W/8 even",
+    "7 bands, uneven, W/8 odd",
+    "8 bands, even, W/8 even",
+    "8 bands, even, W/8 even, near the limit",
+    "8 bands, even, W/8 odd",
+    "8 bands, even, W/8 odd, one octet per row",
+    "8 bands, uneven, W/8 even",
+    "8 bands, even, W/8 even, one-row bands, cluster kernel",
+    "2 bands, even, W/8 even, one-row bands, cluster kernel",
+]
+
+# lean shapes of the other tables (CASES, the EfficientNet sizes, PHOTO_SHAPES) that LEAN_CASES covers by a case of the
+# same regime instead of their own
+LEAN_COVERED_BY = {
+    (256, 256): "2048x16",          # 8 bands of 32 rows, W/8 = 32
+}
+
+# launches where the lean kernel must not run: (shape, input offset, fp16 output offset, why); float output, Philox
+LEAN_NEGATIVE = [
+    ((528, 528), 0, 0, "light band 105 KB > 100 KB: unstaged"),
+    ((600, 600), 0, 0, "light band 135 KB: unstaged"),
+    ((480, 640), 0, 0, "light band 116 KB: unstaged"),
+    ((480, 480), 0, 0, "5 light bands of 96 rows, 138 KB: unstaged"),
+    ((360, 480), 0, 0, "5 light bands of 72 rows, 104 KB: unstaged"),
+    ((375, 500), 0, 0, "375 * 500 * 3 % 16 == 4: no staging, no octets"),
+    ((224, 224), 4, 0, "input 4 bytes past a 16-byte boundary: no staging"),
+    ((224, 224), 0, 8, "fp16 output 8 bytes past 16: no octets"),
 ]
 
 
