@@ -111,6 +111,8 @@ def _load():
         "faa_jpeg_index_capacity": (C.c_int, [vp]),
         "faa_jpeg_index_build": (C.c_int, [vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp]),
         "faa_jpeg_decode_indexed": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp]),
+        "faa_jpeg_decode_recording": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp,
+                                                vp, vp, vp, vp]),
         "faa_launch_count": (u64, []),
     }
     for name, (res, args) in sig.items():

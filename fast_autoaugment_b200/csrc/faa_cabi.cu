@@ -1721,10 +1721,20 @@ int faa_jpeg_index_build(const faa_jpeg_header_t* h_headers, const faa_jpeg_head
     return FAA_OK;
 }
 
-int faa_jpeg_decode_indexed(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
+}  // extern "C"
+
+// faa_jpeg_decode_indexed, and with `rec` (the recording outputs, checked by the caller) faa_jpeg_decode_recording
+struct JpegRecordOut {
+    const int64_t* d_cap_first;
+    faa_jpeg_sync_t* d_points_out;
+    int32_t* d_count;
+};
+
+static int jpeg_decode_call(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
                             const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
                             const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status,
-                            const faa_jpeg_sync_t* d_points, const int64_t* h_first, const int64_t* d_first, void* stream_v) {
+                            const faa_jpeg_sync_t* d_points, const int64_t* h_first, const int64_t* d_first,
+                            const JpegRecordOut* rec, void* stream_v) {
     if (!d || ((!h_headers || !d_headers || !d_tables || !d_src || !h_out || !d_out || !d_status) && batch > 0))
         return fail(FAA_ERR_VALUE, "null argument");
     if (batch < 0) return fail(FAA_ERR_VALUE, "negative batch");
@@ -1784,11 +1794,42 @@ int faa_jpeg_decode_indexed(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_he
         P.first = d_first;
         P.points = const_cast<JpegSync*>(reinterpret_cast<const JpegSync*>(d_points));
     }
+    if (rec) {
+        P.rec_first = rec->d_cap_first;
+        P.rec_points = reinterpret_cast<JpegSync*>(rec->d_points_out);
+        P.count = rec->d_count;
+    }
     CK(launch_jpeg_entropy(P, stream));
     g_launches++;
     CK(launch_jpeg_reconstruct(P, (int)tiles, stream));
     g_launches++;
     return FAA_OK;
+}
+
+extern "C" {
+
+int faa_jpeg_decode_indexed(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
+                            const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
+                            const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status,
+                            const faa_jpeg_sync_t* d_points, const int64_t* h_first, const int64_t* d_first, void* stream_v) {
+    return jpeg_decode_call(d, h_headers, d_headers, d_tables, n_tables, d_src, batch, h_out, d_out, d_status, d_points,
+                            h_first, d_first, nullptr, stream_v);
+}
+
+int faa_jpeg_decode_recording(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
+                              const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
+                              const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status,
+                              const faa_jpeg_sync_t* d_points, const int64_t* h_first, const int64_t* d_first,
+                              const int64_t* h_cap_first, const int64_t* d_cap_first, faa_jpeg_sync_t* d_points_out,
+                              int32_t* d_count, void* stream_v) {
+    if (batch > 0) {
+        if (!h_cap_first || !d_cap_first || !d_count) return fail(FAA_ERR_VALUE, "null argument");
+        if (int e = check_jpeg_first(h_cap_first, batch)) return e;
+        if (!d_points_out && h_cap_first[batch] > h_cap_first[0]) return fail(FAA_ERR_VALUE, "null argument: d_points_out");
+    }
+    const JpegRecordOut rec = {d_cap_first, d_points_out, d_count};
+    return jpeg_decode_call(d, h_headers, d_headers, d_tables, n_tables, d_src, batch, h_out, d_out, d_status, d_points,
+                            h_first, d_first, &rec, stream_v);
 }
 
 }  // extern "C"

@@ -7,7 +7,9 @@
 //                                the scan into int16 coefficients.  An image without restart markers is one segment,
 //                                decoded serially by one thread, unless the call gives it a scan index: then thread k
 //                                decodes from point k to point k + 1 and checks that it ended in that point's state;
-//                                if any segment disagrees, thread 0 decodes the scan serially over it.
+//                                if any segment disagrees, thread 0 decodes the scan serially over it.  The recording
+//                                instantiation (faa_jpeg_decode_recording) also places the scan index of every scan
+//                                thread 0 decodes whole and serially, as faa_jpeg_index_kernel would.
 //   faa_jpeg_index_kernel        (faa_jpeg_index_build) one CTA per image; one thread records the scan index.
 //   faa_jpeg_reconstruct_kernel  one CTA per 64 x 32 output tile of one image.  It runs the islow IDCT of the tile's
 //                                blocks, with the one-block chroma halo fancy upsampling reads, into shared memory,
@@ -37,8 +39,11 @@ __device__ __forceinline__ void jpeg_cta_tables(const JpegHeader& h, const JpegT
     for (int t = 0; t < 6; ++t) hp[t] = &s_huff[t % 3 < h.ncomp ? t : (t / 3) * 3];
 }
 
-// kIndexed: the call gives scan indexes (P.first, P.points); the other instantiation is the path without them.
-template <bool kIndexed>
+// kIndexed: the call gives scan indexes (P.first, P.points); the plain instantiation is the path without them.
+// kRecord (with kIndexed, whose P.first may then be null): a restart-free scan that thread 0 decodes whole and serially
+// (no points, or points that failed) records its points into P.rec_points[P.rec_first[i], P.rec_first[i + 1]), and
+// P.count[i] gets their number; every other image gets count 0.
+template <bool kIndexed, bool kRecord>
 __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_entropy_kernel(const __grid_constant__ JpegDecodeParams P) {
     __shared__ JpegHuff s_huff[6];
     __shared__ __align__(16) int16_t s_scratch[kEntropyThreads][64];
@@ -73,7 +78,7 @@ __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_entropy_kernel(const
     __syncthreads();
     int status = 0;
     bool serial = true;
-    const int64_t n_pts = kIndexed ? P.first[img + 1] - P.first[img] : 0;
+    const int64_t n_pts = !kIndexed || (kRecord && !P.first) ? 0 : P.first[img + 1] - P.first[img];
     if (kIndexed && n_pts > 0) {                                       // a scan index: one segment per thread from its points
         const JpegSync* pts = P.points + P.first[img];
         bool ok = jpeg_index_count_ok(h, n_pts);
@@ -88,16 +93,28 @@ __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_entropy_kernel(const
             if (serial) status = 0;
         }
     }
+    JpegIndexSink sink;
+    JpegIndexSink* rec = nullptr;
+    if (kRecord && serial && n_seg == 1 && tid == 0 &&
+        jpeg_record_sink(h, P.rec_points + P.rec_first[img], P.rec_first[img + 1] - P.rec_first[img], sink))
+        rec = &sink;
     for (int64_t k = tid; serial && k < n_seg; k += kEntropyThreads) {
         const int64_t m0 = n_seg == 1 ? 0 : k * h.restart;
         const int64_t m1 = n_seg == 1 ? mcus : min(m0 + h.restart, mcus);
         const int32_t at = segs[k];
-        status |= jpeg_decode_segment(h, hp, scan, at < 0 ? end : scan + at, end, m0, m1, P.coef + 64 * job.coef,
-                                      s_scratch[tid]);
+        if constexpr (kRecord) {
+            const JpegSync from = {(int32_t)m0, 0, 0, {0, 0, 0}};
+            status |= jpeg_decode_segment(h, hp, scan, end, from, m1, P.coef + 64 * job.coef, s_scratch[tid], nullptr,
+                                          rec, at < 0 ? end : scan + at);
+        } else {
+            status |= jpeg_decode_segment(h, hp, scan, at < 0 ? end : scan + at, end, m0, m1, P.coef + 64 * job.coef,
+                                          s_scratch[tid]);
+        }
     }
     if (status) atomicOr(&s_status, status);
     __syncthreads();
     if (tid == 0) P.status[img] = s_status;
+    if (kRecord && tid == 0) P.count[img] = rec && !s_status ? rec->n : 0;
 }
 
 __global__ void __launch_bounds__(kReconThreads) faa_jpeg_reconstruct_kernel(const __grid_constant__ JpegDecodeParams P) {
@@ -214,8 +231,9 @@ cudaError_t launch_jpeg_index(const JpegDecodeParams& p, cudaStream_t stream) {
 
 cudaError_t launch_jpeg_entropy(const JpegDecodeParams& p, cudaStream_t stream) {
     if (p.batch <= 0) return cudaSuccess;
-    if (p.first) faa_jpeg_entropy_kernel<true><<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p);
-    else faa_jpeg_entropy_kernel<false><<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p);
+    if (p.rec_first) faa_jpeg_entropy_kernel<true, true><<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p);
+    else if (p.first) faa_jpeg_entropy_kernel<true, false><<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p);
+    else faa_jpeg_entropy_kernel<false, false><<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p);
     return cudaGetLastError();
 }
 

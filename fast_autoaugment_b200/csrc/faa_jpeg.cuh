@@ -545,9 +545,12 @@ FAA_JHD void jpeg_zero_block(int16_t* s) {
 // Decodes MCUs [from.mcu, m1) of the scan [lo, end), starting in the state `from` (a restart segment: its first byte,
 // bit 0, zero predictors), into coef.  huff[c] / huff[3 + c]: DC / AC tables of component c.  On an error the blocks
 // from the failing one to the end of the segment are zeroed.  With `to`, a segment that decodes cleanly reports the
-// state it ends in (MCU m1).  With `rec` (a recording decode of a whole restart-free scan) it stores no coefficient and
-// places the points of the rule (jpeg_index_parts) at the MCU boundaries it passes.  `data`: the start byte as a
-// pointer, instead of lo + from.byte (a restart segment whose marker is missing starts at `end`).  Returns JpegStatus.
+// state it ends in (MCU m1).  With `rec` (a recording decode of a whole restart-free scan) it places the points of the
+// rule (jpeg_index_parts) at the MCU boundaries it passes; a recording decode stores the coefficients (and zeroes the
+// blocks after an error) only when it has a `coef` (written `!rec || coef`: a decode without a sink always has one, and
+// compiles without the test).
+// `data`: the start byte as a pointer, instead of lo + from.byte (a restart segment whose marker is missing starts at
+// `end`).  Returns JpegStatus.
 FAA_JHD int jpeg_decode_segment(const JpegHeader& h, const JpegHuff* const* huff, const uint8_t* lo, const uint8_t* end,
                                 const JpegSync& from, int64_t m1, int16_t* coef, int16_t* scratch, JpegSync* to = nullptr,
                                 JpegIndexSink* rec = nullptr, const uint8_t* data = nullptr) {
@@ -602,12 +605,12 @@ FAA_JHD int jpeg_decode_segment(const JpegHeader& h, const JpegHuff* const* huff
                 }
             }
             if (status) break;
-            if (!rec) jpeg_store_block(coef + 64 * jpeg_block_of(h, m, b), scratch);
+            if (!rec || coef) jpeg_store_block(coef + 64 * jpeg_block_of(h, m, b), scratch);
         }
         if (status) break;
         if (r.n < r.fake) { status = JPEG_TRUNCATED; ++m; b = 0; break; }     // this MCU used bits past the data
     }
-    if (status && !rec) {
+    if (status && (!rec || coef)) {
         jpeg_zero_block(scratch);
         for (; m < m1; ++m, b = 0)
             for (; b < nb; ++b) jpeg_store_block(coef + 64 * jpeg_block_of(h, m, b), scratch);
@@ -639,6 +642,16 @@ FAA_JHD int jpeg_index_record(const JpegHeader& h, const JpegHuff* const* huff, 
     const JpegSync zero = {0, 0, 0, {0, 0, 0}};
     *status = jpeg_decode_segment(h, huff, scan, scan + h.scan_len, zero, jpeg_mcus(h), nullptr, scratch, nullptr, &rec);
     return *status ? 0 : rec.n;
+}
+
+// The sink of a recording entropy decode (faa_jpeg_decode_recording) of a restart-free scan decoded whole and serially:
+// the file's points go to at[0, cap), cap being the room the caller planned for it (faa_jpeg_index_capacity).  False,
+// and no sink, when the rule gives the file no points or it has no room.
+FAA_JHD bool jpeg_record_sink(const JpegHeader& h, JpegSync* at, int64_t cap, JpegIndexSink& s) {
+    const int parts = jpeg_index_parts(h);
+    if (!parts || cap <= 0) return false;
+    s = {at, cap < parts - 1 ? (int32_t)cap : parts - 1, 0, parts, 1};
+    return true;
 }
 
 // Segment k of an indexed scan with n points: MCUs [pts[k - 1].mcu, pts[k].mcu), the first from the scan's start and
@@ -799,9 +812,13 @@ FAA_JHD int jpeg_tile_windows(const JpegHeader& h, int x0, int y0, int x1, int y
 // The whole decode of one file on the host, serially, with the functions above: the CPU tests' model of the two
 // kernels.  out: h.h * h.w * 3 bytes.  With a scan index (npts points) the entropy decode runs as the entropy kernel's
 // indexed path does: validate, one segment per point, end states checked, a serial decode when anything disagrees.
-// Returns the JpegStatus bits.
+// With rec_count, as the recording kernel does: a restart-free scan decoded whole and serially places its points into
+// rec_at[0, rec_cap) (jpeg_record_sink), and *rec_count gets their number, or 0 when the scan was not decoded that way,
+// gets no points or did not decode cleanly.  coef_out: the coefficients (jpeg_image_blocks(h) blocks).  Returns the
+// JpegStatus bits.
 inline int jpeg_decode_host(const uint8_t* file, const JpegHeader& h, const JpegTable* tabs, uint8_t* out,
-                            const JpegSync* pts = nullptr, int64_t npts = 0) {
+                            const JpegSync* pts = nullptr, int64_t npts = 0, JpegSync* rec_at = nullptr,
+                            int64_t rec_cap = 0, int32_t* rec_count = nullptr, int16_t* coef_out = nullptr) {
     static_assert(sizeof(JpegTable) == 400, "table layout");
     JpegHuff huffs[6];
     const JpegHuff* hp[6];
@@ -836,11 +853,16 @@ inline int jpeg_decode_host(const uint8_t* file, const JpegHeader& h, const Jpeg
         if (linked) n_seg = 0;                           // done; otherwise the serial decode below overwrites it all
         else status = 0;
     }
+    JpegIndexSink sink;
+    JpegIndexSink* rec = rec_count && n_seg == 1 && jpeg_record_sink(h, rec_at, rec_cap, sink) ? &sink : nullptr;
     for (int64_t k = 0; k < n_seg; ++k) {
         const int64_t m0 = k * (h.restart > 0 ? h.restart : mcus), m1 = n_seg == 1 ? mcus : (m0 + h.restart < mcus ? m0 + h.restart : mcus);
         const uint8_t* p = at[k] < 0 ? end : scan + at[k];
-        status |= jpeg_decode_segment(h, hp, scan, p, end, m0, m1, coef, scratch);
+        const JpegSync from = {(int32_t)m0, 0, 0, {0, 0, 0}};
+        status |= jpeg_decode_segment(h, hp, scan, end, from, m1, coef, scratch, nullptr, rec, p);
     }
+    if (rec_count) *rec_count = rec && !status ? rec->n : 0;
+    if (coef_out) memcpy(coef_out, coef, (size_t)nblk * 128);
     // planes of samples
     uint8_t* planes[3] = {nullptr, nullptr, nullptr};
     int pw[3], ph[3];

@@ -155,7 +155,10 @@ struct JpegDecodeParams {
     // capacities, with the points written in count[i])
     const int64_t* first;
     JpegSync* points;
-    int32_t* count;             // [batch] (index build only)
+    int32_t* count;             // [batch] (index build, recording decode)
+    // recording decode only (null otherwise): image i's recorded points go to rec_points[rec_first[i], rec_first[i + 1])
+    const int64_t* rec_first;
+    JpegSync* rec_points;
 };
 cudaError_t launch_jpeg_entropy(const JpegDecodeParams& p, cudaStream_t stream);
 cudaError_t launch_jpeg_reconstruct(const JpegDecodeParams& p, int n_tiles, cudaStream_t stream);

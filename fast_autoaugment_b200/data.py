@@ -26,8 +26,8 @@ from torch.utils.data import Sampler, SubsetRandomSampler
 from . import _lib, archive
 from .conf import Config as C
 from .engine import (CIFAR_MEAN, CIFAR_STD, IMAGENET_MEAN, IMAGENET_STD, CompiledPolicy, EncodedImages, RaggedImages,
-                     TailSpec, augment_batch, center_crop_box, crop_cfg, crop_resize, decode_jpeg, make_rng,
-                     parse_jpeg_headers, sample_philox_at)
+                     TailSpec, augment_batch, center_crop_box, compact_jpeg_index, crop_cfg, crop_resize, decode_jpeg,
+                     make_rng, parse_jpeg_headers, sample_philox_at)
 
 
 class Augmentation(object):
@@ -566,10 +566,15 @@ class JpegIndex:
     ``<split>.npz``: ``paths`` relative to the folder, ``sizes`` the file lengths, ``first`` / ``points`` as
     ``build_jpeg_index`` gives them, ``version``).  A file is looked up by its path relative to ``folder``; a file the
     index does not list, or whose length differs from the one indexed, gets no points.  Any other staleness (a file
-    rewritten at the same length) is caught by the decoder, which then decodes that file serially."""
+    rewritten at the same length) is caught by the decoder, which then decodes that file serially.
+
+    ``add`` enters files' points found later (``conf['faa_jpeg_index_learn']``: a loader's recording decodes); they
+    replace the ones listed for the same path.  In memory an index takes about what its file takes on disk: 16 bytes a
+    point, up to 127 points a file (about 1.7 KB at ImageNet's mean file size of about 110 KB)."""
 
     def __init__(self, folder, paths, sizes, first, points):
         self.folder = os.fspath(folder)
+        self._added = {}                           # relative path -> (length, points) entered by add
         self.sizes = np.asarray(sizes, np.int64).reshape(-1)
         self.first = np.asarray(first, np.int64).reshape(-1)
         self.points = np.ascontiguousarray(points, dtype=_lib.JPEG_SYNC_DTYPE).reshape(-1)
@@ -587,14 +592,42 @@ class JpegIndex:
                     path, int(z["version"]), JPEG_INDEX_VERSION))
             return JpegIndex(folder, list(z["paths"]), z["sizes"], z["first"], z["points"])
 
+    @staticmethod
+    def empty(folder):
+        """an index of ``folder`` that lists no file"""
+        return JpegIndex(folder, [], np.zeros(0, np.int64), np.zeros(1, np.int64), np.zeros(0, _lib.JPEG_SYNC_DTYPE))
+
     def save(self, path):
+        """write the index, ``add``'s files included, as ``<split>.npz`` of ``python -m fast_autoaugment_b200.jpeg_index``"""
         rel = sorted(self._at, key=self._at.get)
-        np.savez(path, paths=np.array([os.fsencode(p) for p in rel], dtype=bytes), sizes=self.sizes,
-                 first=self.first, points=self.points, version=np.int64(JPEG_INDEX_VERSION))
+        sizes, first, points = self.sizes, self.first, self.points
+        if self._added:
+            added = dict(self._added)
+            rel = [p for p in rel if p not in added]
+            at = [self._at[p] for p in rel]
+            parts = [self.points[self.first[i]:self.first[i + 1]] for i in at] + [q for _, q in added.values()]
+            sizes = np.array([int(self.sizes[i]) for i in at] + [n for n, _ in added.values()], np.int64)
+            first = np.zeros(len(parts) + 1, np.int64)
+            first[1:] = np.cumsum([len(q) for q in parts])
+            points = np.concatenate(parts) if parts else self.points[:0]
+            rel += list(added)
+        np.savez(path, paths=np.array([os.fsencode(p) for p in rel], dtype=bytes), sizes=sizes,
+                 first=first, points=points, version=np.int64(JPEG_INDEX_VERSION))
+
+    def add(self, paths, lengths, first, points):
+        """enter the points of the files at ``paths`` (of ``lengths`` bytes): file k's are ``points[first[k]:first[k +
+        1]]`` (``build_jpeg_index``'s form); they replace what the index lists for those paths"""
+        for k, p in enumerate(paths):
+            q = np.array(points[int(first[k]):int(first[k + 1])], dtype=_lib.JPEG_SYNC_DTYPE)
+            self._added[os.path.relpath(os.fspath(p), self.folder)] = (int(lengths[k]), q)
 
     def lookup(self, path, length):
         """the points of the file at ``path`` (of ``length`` bytes), empty when it has none here"""
-        i = self._at.get(os.path.relpath(os.fspath(path), self.folder))
+        rel = os.path.relpath(os.fspath(path), self.folder)
+        e = self._added.get(rel)
+        if e is not None:
+            return e[1] if e[0] == int(length) else self.points[:0]
+        i = self._at.get(rel)
         if i is None or int(self.sizes[i]) != int(length):
             return self.points[:0]
         return self.points[self.first[i]:self.first[i + 1]]
@@ -610,11 +643,16 @@ class JpegIndex:
 class JpegFileDataset:
     """``EncodedDeviceDataset`` whose files stay on disk: it holds paths and targets only, so no byte of the split is on
     the device.  ``GpuAugmentedLoader`` streams each batch's files through a ``FileBatchStream``.  ``index``: a
-    ``JpegIndex`` of the files, whose scan indexes let the device decode each listed file on many threads."""
+    ``JpegIndex`` of the files, whose scan indexes let the device decode each listed file on many threads.  ``learn``:
+    the loaders enter into ``index`` (which it needs) the scan index of every file they decode serially, so the next
+    epoch decodes it on many threads; subsets share the index, and ``index.save`` writes it."""
 
-    def __init__(self, paths, targets, device="cuda", index=None):
+    def __init__(self, paths, targets, device="cuda", index=None, learn=False):
+        if learn and index is None:
+            raise ValueError("learn needs an index to enter the files' points into (JpegIndex.empty)")
         self.paths = [os.fspath(p) for p in paths]
         self.index = index
+        self.learn = bool(learn)
         self.targets = [int(t) for t in targets]
         if len(self.targets) != len(self.paths):
             raise ValueError("need one target per image")
@@ -632,7 +670,7 @@ class JpegFileDataset:
         idx = [int(i) for i in idx]
         d = JpegFileDataset.__new__(JpegFileDataset)
         d.paths = self.select(idx)
-        d.index = self.index
+        d.index, d.learn = self.index, self.learn
         d.targets = [self.targets[i] for i in idx]
         d.labels = self.labels.index_select(0, torch.as_tensor(idx, dtype=torch.int64, device=self.labels.device))
         d.device = self.device
@@ -760,14 +798,20 @@ class FileBatchStream:
     into their images of ``RaggedImages.empty(sizes)`` and copies the refused files' pixels into theirs.  Each batch's
     decode status is copied to pinned host memory and checked once the next batch is staged, and at the end, so no
     batch waits on its own decode: a non-zero status raises ``OSError`` naming the file.  With a ``JpegIndex`` each
-    batch's scan indexes travel in the same slot and the decode uses them."""
+    batch's scan indexes travel in the same slot and the decode uses them.  With ``learn`` as well, every batch is
+    decoded in recording mode (``decode_jpeg(record=True)``): its point counts and the points they cover are copied to
+    pinned memory behind the decode with its status, and at the same check the files that got points are entered into
+    the index (``JpegIndex.add``), so the batches read after that decode them on many threads."""
 
     SLOTS = 2
     WORKERS = 2
 
-    def __init__(self, workers=None, index=None):
+    def __init__(self, workers=None, index=None, learn=False):
+        if learn and index is None:
+            raise ValueError("learn needs an index")
         self.workers = int(workers or self.WORKERS)
         self.index = index
+        self.learn = bool(learn)
         self.slots = [None] * self.SLOTS           # pinned uint8 staging buffers
         self.copied = [None] * self.SLOTS          # event recorded after each slot's last host-to-device copy
 
@@ -794,23 +838,38 @@ class FileBatchStream:
                              _d_points=dbuf[lay.points:lay.points_end])
             enc = EncodedImages(dbuf[lay.files:lay.files_end], hb.headers, hb.pool, _d_pool=dbuf[lay.pool:lay.files],
                                 _d_headers=dbuf[:lay.pool], **index)
-            _, status = decode_jpeg(enc, out.select(hb.accepted))
+            learned = None
+            if self.learn:
+                _, status, count, points, cap_first = decode_jpeg(enc, out.select(hb.accepted), record=True)
+                h_count = torch.empty(len(hb.accepted), dtype=torch.int32, pin_memory=True)
+                h_count.copy_(count, non_blocking=True)
+                h_points = torch.empty(points.numel(), dtype=torch.uint8, pin_memory=True)
+                h_points.copy_(points, non_blocking=True)
+                learned = (h_count, h_points, cap_first, [len(f) for f in hb.files])
+            else:
+                _, status = decode_jpeg(enc, out.select(hb.accepted))
             st = torch.empty(len(hb.accepted), dtype=torch.int32, pin_memory=True)
             st.copy_(status, non_blocking=True)
             ev = torch.cuda.Event()
             ev.record(torch.cuda.current_stream(dev))
-            pending.append((ev, st, [hb.paths[i] for i in hb.accepted]))
+            pending.append((ev, st, [hb.paths[i] for i in hb.accepted], learned))
         for i, o in zip(hb.refused, lay.pixels):
             h, w = (int(v) for v in sizes[i])
             out.image(int(i)).copy_(dbuf[o:o + h * w * 3].view(h, w, 3))
         return out
 
-    @staticmethod
-    def _check(pending, keep=0):
-        """check (and drop) every pending status but the last ``keep``"""
+    def _check(self, pending, keep=0):
+        """check (and drop) every pending status but the last ``keep``; enter what recording decodes found"""
         while len(pending) > keep:
-            ev, st, paths = pending.pop(0)
+            ev, st, paths, learned = pending.pop(0)
             ev.synchronize()
+            if learned is not None:
+                h_count, h_points, cap_first, lengths = learned
+                count = h_count.numpy()
+                first, points = compact_jpeg_index(cap_first, count, h_points.numpy())
+                got = np.flatnonzero(count > 0)
+                self.index.add([paths[i] for i in got], [lengths[i] for i in got],
+                               np.concatenate([[0], np.cumsum(count[got])]), points)
             bad = [(p, int(s)) for p, s in zip(paths, st.numpy().tolist()) if s]
             if bad:
                 raise OSError("corrupt JPEG files (decode status): " + "; ".join(
@@ -821,7 +880,7 @@ class FileBatchStream:
         dev = torch.device(device)
         pool = ThreadPoolExecutor(self.workers, thread_name_prefix="faa-read")
         ahead = ThreadPoolExecutor(1, thread_name_prefix="faa-stage")
-        pending = []                               # (event, pinned status, paths) of decodes not checked yet
+        pending = []                               # (event, pinned status, paths, recorded points) of unchecked decodes
         try:
             fut = ahead.submit(self._stage, batches[0], 0, pool, dev) if len(batches) else None
             for k in range(len(batches)):
@@ -892,7 +951,7 @@ class GpuAugmentedLoader:
         if isinstance(self.dataset, JpegFileDataset):
             dev = self.dataset.device
             batches = [idx_all[k * self.batch_size:(k + 1) * self.batch_size] for k in range(len(self))]
-            self.staging = FileBatchStream(index=self.dataset.index)
+            self.staging = FileBatchStream(index=self.dataset.index, learn=self.dataset.learn)
             files = self.staging([self.dataset.select(idx) for idx in batches], dev)
         else:
             dev = self.dataset.images.device
@@ -1070,7 +1129,11 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
     files on disk (``JpegFileDataset``): the loaders read, stage and decode each batch's files one batch ahead.
     ``faa_jpeg_index``: a directory holding ``train.npz`` / ``val.npz`` written by ``python -m
     fast_autoaugment_b200.jpeg_index DATAROOT DIR``; the files they index are decoded on many threads each, with the
-    same pixels."""
+    same pixels.  ``faa_jpeg_index_learn``: the datasets start from that index, or from an empty one, and the loaders
+    enter the scan index of every file they decode serially, so from the second epoch on the files the loaders have
+    seen are decoded on many threads, with the same pixels; the train and valid loaders share what they learn
+    (``trainloader.dataset.index.save(path)`` writes it as ``faa_jpeg_index`` reads it).  It costs host memory: 16
+    bytes a point, about 1.7 KB a file at ImageNet's mean file size."""
     from sklearn.model_selection import StratifiedShuffleSplit
 
     conf = C.get()
@@ -1094,6 +1157,7 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
                          "images are augmented at one fixed size")
 
     index_dir = conf.get("faa_jpeg_index")
+    learn = bool(conf.get("faa_jpeg_index_learn", False))
 
     def device_dataset(x, y):
         if isinstance(x, FilePaths):
@@ -1104,7 +1168,9 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
                     raise FileNotFoundError("conf['faa_jpeg_index']: no index of the %s split at %s (write it with "
                                             "python -m fast_autoaugment_b200.jpeg_index)" % (x.split, path))
                 index = JpegIndex.load(path, x.folder)
-            return JpegFileDataset(x, y, index=index)
+            if learn and index is None:
+                index = JpegIndex.empty(x.folder)
+            return JpegFileDataset(x, y, index=index, learn=learn)
         if isinstance(x, list) and len(x) and isinstance(x[0], bytes):
             return EncodedDeviceDataset(x, y)
         return RaggedDeviceDataset(x, y) if isinstance(x, list) else DeviceDataset(x, y)

@@ -685,8 +685,7 @@ def build_jpeg_index(encoded: EncodedImages):
     if B == 0:
         return np.zeros(1, np.int64), np.zeros(0, _lib.JPEG_SYNC_DTYPE)
     hdr0 = encoded.headers.ctypes.data
-    caps = np.array([lib.faa_jpeg_index_capacity(hdr0 + i * encoded.headers.itemsize) for i in range(B)], np.int64)
-    cap_first = np.concatenate([[0], np.cumsum(caps)]).astype(np.int64)
+    cap_first = jpeg_index_capacities(encoded.headers)
     total = int(cap_first[-1])
     with torch.cuda.device(dev):
         d_first = torch.from_numpy(cap_first).to(dev)
@@ -697,11 +696,33 @@ def build_jpeg_index(encoded: EncodedImages):
                                        len(encoded.pool), encoded.storage.data_ptr(), B, cap_first.ctypes.data,
                                        d_first.data_ptr(), d_points.data_ptr(), d_count.data_ptr(),
                                        d_status.data_ptr(), _stream_ptr(dev)))
-        count = d_count.cpu().numpy().astype(np.int64)
+        count = d_count.cpu().numpy()
         pts = d_points.cpu().numpy()[:total * 16].view(_lib.JPEG_SYNC_DTYPE)
+    return compact_jpeg_index(cap_first, count, pts)
+
+
+def jpeg_index_capacities(headers):
+    """int64 [N + 1] offsets giving each file of ``headers`` (``JPEG_HEADER_DTYPE``) room for the most points it can
+    get (``faa_jpeg_index_capacity``): the layout ``faa_jpeg_index_build`` and ``faa_jpeg_decode_recording`` write into"""
+    hdr0, size = headers.ctypes.data, headers.itemsize
+    caps = np.array([lib.faa_jpeg_index_capacity(hdr0 + i * size) for i in range(len(headers))], np.int64)
+    return np.concatenate([[0], np.cumsum(caps)]).astype(np.int64)
+
+
+def compact_jpeg_index(cap_first, count, points):
+    """``(first, points)`` as ``build_jpeg_index`` returns them, from points written into the capacity layout
+    ``cap_first`` (``jpeg_index_capacities``) with ``count[i]`` of them for file i (host arrays; ``points`` a
+    ``JPEG_SYNC_DTYPE`` array or its bytes)"""
+    cap_first = np.asarray(cap_first, np.int64)
+    count = np.asarray(count).astype(np.int64)
+    points = np.asarray(points)
+    if points.dtype != _lib.JPEG_SYNC_DTYPE:
+        points = np.ascontiguousarray(points, np.uint8).reshape(-1)[:int(cap_first[-1]) * 16].view(_lib.JPEG_SYNC_DTYPE)
+    if len(count) != len(cap_first) - 1 or (count < 0).any() or (count > np.diff(cap_first)).any():
+        raise ValueError("count must be [N] and within each file's capacity")
     first = np.concatenate([[0], np.cumsum(count)]).astype(np.int64)
     at = np.repeat(cap_first[:-1] - first[:-1], count) + np.arange(int(first[-1]), dtype=np.int64)
-    return first, pts[at].copy()
+    return first, points[at].copy()
 
 
 class _JpegDecoder:
@@ -724,12 +745,19 @@ class _JpegDecoder:
 _DECODERS = {}
 
 
-def decode_jpeg(encoded: EncodedImages, out: RaggedImages | None = None):
+def decode_jpeg(encoded: EncodedImages, out: RaggedImages | None = None, record=False):
     """Decode every file of ``encoded`` on its device (C ABI ``faa_jpeg_decode``, or ``faa_jpeg_decode_indexed`` when
     the files carry a scan index: two launches, no host wait), bit-exact
     with ``Image.open(f).convert('RGB')`` (reference imagenet.py:80).  Returns ``(images, status)``: a ``RaggedImages``
     (``out``, by default ``RaggedImages.empty(encoded.sizes)``) and an int32 CUDA tensor of ``faa_jpeg_status`` bits per
-    image, 0 where the scan decoded completely; a corrupt image still gets defined pixels."""
+    image, 0 where the scan decoded completely; a corrupt image still gets defined pixels.
+
+    ``record=True`` (``faa_jpeg_decode_recording``, same pixels and status, still no host wait) also records the scan
+    index of every file the decode ran serially as a whole (no points, or points that failed their checks) and returns
+    ``(images, status, count, points, cap_first)``: ``count`` int32 [N] and ``points`` (uint8, the bytes of
+    ``JPEG_SYNC_DTYPE`` points) CUDA tensors, file i's ``count[i]`` new points at point ``cap_first[i]``
+    (``jpeg_index_capacities``, host int64 [N + 1]).  ``count[i] > 0`` means these are file i's points now;
+    ``compact_jpeg_index`` turns them into ``build_jpeg_index``'s form."""
     _require_cuda(encoded.storage, "encoded")
     dev = encoded.device
     if out is None:
@@ -738,13 +766,30 @@ def decode_jpeg(encoded: EncodedImages, out: RaggedImages | None = None):
         raise ValueError("out must be a RaggedImages of the files' sizes on their device")
     B = len(encoded)
     status = torch.empty(max(B, 1), dtype=torch.int32, device=dev)[:B]
+    if record:
+        cap_first = jpeg_index_capacities(encoded.headers)
+        count = torch.empty(max(B, 1), dtype=torch.int32, device=dev)[:B]
+        points = torch.empty(max(int(cap_first[-1]), 1) * 16, dtype=torch.uint8, device=dev)
     if B == 0:
-        return out, status
+        return (out, status, count, points, cap_first) if record else (out, status)
     h_out, d_out = out.descriptors()
     with torch.cuda.device(dev):
         dec = _DECODERS.get(dev.index)
         if dec is None:
             dec = _DECODERS[dev.index] = _JpegDecoder()
+        if record:
+            d_first = d_points = None
+            if encoded.first is not None:
+                d_first, d_points = encoded.device_index()
+            d_cap_first = torch.from_numpy(cap_first).to(dev)
+            check(lib.faa_jpeg_decode_recording(
+                dec.handle, encoded.headers.ctypes.data, encoded.device_headers().data_ptr(),
+                encoded.device_pool().data_ptr(), len(encoded.pool), encoded.storage.data_ptr(), B, h_out.ctypes.data,
+                d_out.data_ptr(), status.data_ptr(), None if d_points is None else d_points.data_ptr(),
+                None if encoded.first is None else encoded.first.ctypes.data,
+                None if d_first is None else d_first.data_ptr(), cap_first.ctypes.data, d_cap_first.data_ptr(),
+                points.data_ptr(), count.data_ptr(), _stream_ptr(dev)))
+            return out, status, count, points, cap_first
         if encoded.first is None:
             check(lib.faa_jpeg_decode(dec.handle, encoded.headers.ctypes.data, encoded.device_headers().data_ptr(),
                                       encoded.device_pool().data_ptr(), len(encoded.pool), encoded.storage.data_ptr(), B,

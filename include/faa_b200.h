@@ -413,6 +413,21 @@ int faa_jpeg_decode_indexed(faa_jpeg_decoder_t* dec, const faa_jpeg_header_t* h_
                             const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status,
                             const faa_jpeg_sync_t* d_points, const int64_t* h_first, const int64_t* d_first, void* stream);
 
+/* faa_jpeg_decode_indexed (the input points may all be null) that also records the scan index of every file it decodes
+ * serially as a whole: a file without points, or whose points failed their checks.  h_cap_first / d_cap_first: host
+ * and device copies of int64 [batch + 1] offsets into d_points_out, laid out and validated as faa_jpeg_index_build's
+ * h_first / d_first (image i may get cap_first[i + 1] - cap_first[i] points, at most faa_jpeg_index_capacity of its
+ * header).  d_count: [batch] int32, the points written at d_points_out + cap_first[i]; 0 for a file with a restart
+ * interval, a scan the placement rule gives no points, a non-zero status, or points that were used as they stood.  So
+ * count[i] > 0 means these are file i's points now.  Pixels and status equal faa_jpeg_decode's.  Two launches, no host
+ * wait. */
+int faa_jpeg_decode_recording(faa_jpeg_decoder_t* dec, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
+                              const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
+                              const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status,
+                              const faa_jpeg_sync_t* d_points, const int64_t* h_first, const int64_t* d_first,
+                              const int64_t* h_cap_first, const int64_t* d_cap_first, faa_jpeg_sync_t* d_points_out,
+                              int32_t* d_count, void* stream);
+
 /* number of kernels this library has launched since load (bench bookkeeping) */
 uint64_t faa_launch_count(void);
 
