@@ -1293,16 +1293,23 @@ int faa_augment_ragged(faa_policy_t* p, const faa_image_t* h_in, const faa_image
         for (int c = 0; c < 3; ++c) { a.scale[c] = 1.0f; a.bias[c] = 0.0f; }      // uint8 output: the byte value itself
     }
     // per image: scratch images (Sharpness -> gather) and re-aligned copies of inputs whose base breaks the 32-bit loads
-    // of W % 4 == 0 images, as byte offsets into the handle's buffers
+    // of W % 4 == 0 images, as byte offsets into the handle's buffers.  Descriptors that share a source (the replicas of
+    // a TTA batch) share its copy: each distinct (base, bytes) is copied once.
     std::vector<int64_t> scratch_at((size_t)batch, -1), copy_at((size_t)batch, -1);
+    std::vector<int> copy_src;                                  // the first image of each copied source
+    std::map<std::pair<const uint8_t*, size_t>, int64_t> copied;
     size_t scratch_bytes = 0, copy_bytes = 0;
-    int n_copy = 0;
     for (int i = 0; i < batch; ++i) {
         const RaggedGeom& g = plan.geoms[(size_t)plan.geom_of[(size_t)i]];
         const size_t bytes = (size_t)g.H * g.W * 3;
         if (g.plan.scratch) { scratch_at[(size_t)i] = (int64_t)scratch_bytes; scratch_bytes += align16(bytes); }
-        if ((g.W & 3) == 0 && ((uintptr_t)h_in[i].data & 3)) { copy_at[(size_t)i] = (int64_t)copy_bytes; copy_bytes += align16(bytes); ++n_copy; }
+        if ((g.W & 3) == 0 && ((uintptr_t)h_in[i].data & 3)) {
+            const auto at = copied.emplace(std::make_pair(h_in[i].data, bytes), (int64_t)copy_bytes);
+            if (at.second) { copy_bytes += align16(bytes); copy_src.push_back(i); }
+            copy_at[(size_t)i] = at.first->second;
+        }
     }
+    const int n_copy = (int)copy_src.size();
     const size_t off_img = align16(n_geo * sizeof(AugParams));
     const size_t off_list = off_img + align16((size_t)batch * sizeof(RaggedImg));
     const size_t off_copy = off_list + align16((size_t)batch * sizeof(int32_t));
@@ -1316,18 +1323,17 @@ int faa_augment_ragged(faa_policy_t* p, const faa_image_t* h_in, const faa_image
     memcpy(host.data(), geo.data(), n_geo * sizeof(AugParams));
     RaggedImg* imgs = reinterpret_cast<RaggedImg*>(host.data() + off_img);
     RaggedCopy* copies = reinterpret_cast<RaggedCopy*>(host.data() + off_copy);
-    for (int i = 0, c = 0; i < batch; ++i) {
+    for (int i = 0; i < batch; ++i) {
         const int k = plan.geom_of[(size_t)i];
         RaggedImg& m = imgs[i];
         m.ops = geo_ops[(size_t)k]; m.H = plan.geoms[(size_t)k].H; m.W = plan.geoms[(size_t)k].W;
         m.allow = plan.geoms[(size_t)k].plan.allow; m.geom = k;
         m.scratch = scratch_at[(size_t)i] < 0 ? nullptr : (uint8_t*)p->d_rg_scratch + scratch_at[(size_t)i];
-        m.realigned = nullptr;
-        if (copy_at[(size_t)i] >= 0) {
-            uint8_t* dst = (uint8_t*)p->d_rg_copy + copy_at[(size_t)i];
-            copies[c++] = {h_in[i].data, dst, (uint64_t)m.H * m.W * 3};
-            m.realigned = dst;
-        }
+        m.realigned = copy_at[(size_t)i] < 0 ? nullptr : (uint8_t*)p->d_rg_copy + copy_at[(size_t)i];
+    }
+    for (int c = 0; c < n_copy; ++c) {
+        const int i = copy_src[(size_t)c];
+        copies[c] = {h_in[i].data, (uint8_t*)p->d_rg_copy + copy_at[(size_t)i], (uint64_t)imgs[i].H * imgs[i].W * 3};
     }
     memcpy(host.data() + off_list, plan.order.data(), (size_t)batch * sizeof(int32_t));
     CK(cudaMemcpyAsync(d_tab, host.data(), tab_bytes, cudaMemcpyHostToDevice, stream));   // (pageable: staged at once)

@@ -12,6 +12,7 @@
 """
 from __future__ import annotations
 
+import contextlib
 import io
 import math
 import os
@@ -26,8 +27,8 @@ from torch.utils.data import Sampler, SubsetRandomSampler
 from . import _lib, archive
 from .conf import Config as C
 from .engine import (CIFAR_MEAN, CIFAR_STD, IMAGENET_MEAN, IMAGENET_STD, CompiledPolicy, EncodedImages, RaggedImages,
-                     TailSpec, augment_batch, center_crop_box, compact_jpeg_index, crop_cfg, crop_resize, decode_jpeg,
-                     make_rng, parse_jpeg_headers, sample_philox_at)
+                     TailSpec, augment_batch, augment_tta, center_crop_box, check_tta, compact_jpeg_index, crop_cfg,
+                     crop_resize, decode_jpeg, make_rng, parse_jpeg_headers, sample_philox_at, tta_positions, tta_select)
 
 
 class Augmentation(object):
@@ -446,6 +447,59 @@ class ImageNetChain(object):
             _lib.check(_lib.lib.faa_color_jitter(y.data_ptr(), y.data_ptr(), b, s, s, recs.data_ptr(),
                                                  C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
         return augment_batch(self.flip_policy, y, self.tail, rng=make_rng(seed, first_index, self.tail), lighting_rgb=rgb)
+
+    def _device_records_tta(self, n, dev, seed, first_index, replicas):
+        """the jitter records and Lighting offsets of ``replicas`` replicas of an n-image batch, replica-major: replica r's
+        are ``_device_records(n, dev, seed, first_index + r * n)``, those of ``train(first_index=first_index + r * n)``"""
+        parts = [self._device_records(n, dev, seed, int(first_index) + r * n) for r in range(int(replicas))]
+        return torch.cat([p[0] for p in parts]), torch.cat([p[1] for p in parts])
+
+    def check_tta(self, n, replicas, parity=False):
+        """ValueError for a ``train_tta`` call this chain refuses: parity draws (K reference loaders have no single draw
+        order), replicas < 1, more than 65535 images per launch, a policy longer than one fused window"""
+        if parity:
+            raise ValueError("train_tta draws with Philox only: K reference loaders have no single parity draw order")
+        check_tta(n, replicas)
+        if self.aug is not None and self.aug.compiled.n_op > _lib.MAX_FUSED_OPS:
+            raise ValueError("train_tta supports policies of at most %d ops per sub-policy (replicated launches)"
+                             % _lib.MAX_FUSED_OPS)
+
+    def train_tta(self, batch, replicas, seed=0, first_index=0, parity=False):
+        """The train chain's test-time-augmentation replicas of one batch: uint8 [B,H,W,3] CUDA, ``RaggedImages`` or
+        ``EncodedImages`` (decoded once; ``last_status`` set once) -> [replicas, B, 3, s, s] ``out_dtype`` with
+
+            out[r] == train(batch, seed=seed, first_index=first_index + r * B)      (bit for bit)
+
+        Each stage is one launch (group) over all replicas * B images, schedule entry v = r * B + i drawing the Philox
+        keys of global sample first_index + v: the policy (``augment_tta``: one replicated launch for a uniform batch,
+        one ``faa_augment_ragged`` group over replicated descriptors for a ragged one), crop + resize, ColorJitter and
+        HFlip + Lighting + Normalize.  Without a policy the crop reads the sources through replicated descriptors.
+        Raises ValueError before any device work for what ``check_tta`` refuses."""
+        B = len(batch) if isinstance(batch, (RaggedImages, EncodedImages)) else int(batch.shape[0])
+        self.check_tta(B, replicas, parity)
+        K = int(replicas)
+        x = self._decoded(batch)
+        dev = x.device
+        raw = TailSpec.raw_u8()
+        if self.aug is not None:
+            y = augment_tta(self.aug.compiled, x, raw, K, seed, first_index)
+            if not isinstance(y, RaggedImages):
+                y = y.view(K * B, *y.shape[2:])
+        elif isinstance(x, RaggedImages):
+            y = tta_select(x, K)
+        else:                                               # the sources themselves, K descriptors each
+            x = x.contiguous()
+            h, w = int(x.shape[1]), int(x.shape[2])
+            y = RaggedImages(x.view(-1), tta_positions(B, K) * (h * w * 3), [(h, w)] * (K * B))
+        s = self.input_size
+        z = crop_resize(y, s, rng=self.crop.cfg(seed, first_index))
+        recs, rgb = self._device_records_tta(B, dev, seed, first_index, K)
+        with torch.cuda.device(dev):
+            import ctypes as C
+            _lib.check(_lib.lib.faa_color_jitter(z.data_ptr(), z.data_ptr(), K * B, s, s, recs.data_ptr(),
+                                                 C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+        out = augment_batch(self.flip_policy, z, self.tail, rng=make_rng(seed, first_index, self.tail), lighting_rgb=rgb)
+        return out.view(K, B, *out.shape[1:])
 
     def test(self, batch_u8, out=None):
         """uint8 [B,H,W,3] CUDA (or ``RaggedImages``) -> [B, 3, s, s]: center crop + resize + ToTensor + Normalize, one
@@ -945,7 +999,10 @@ class GpuAugmentedLoader:
         n = len(self.dataset)
         return torch.randperm(n).tolist() if self.shuffle else list(range(n))
 
-    def __iter__(self):
+    def _batches(self):
+        """generator of (device int64 indices, source batch) over one epoch of the index stream: the gathered uint8
+        images, descriptors into a ragged or encoded dataset, or a ``JpegFileDataset`` batch's files decoded on the
+        device (whose decode status is checked as the epoch goes and at its end)"""
         idx_all = self._indices()
         files = None
         if isinstance(self.dataset, JpegFileDataset):
@@ -965,20 +1022,57 @@ class GpuAugmentedLoader:
                     raw = self.dataset.images.select(idx)        # descriptors into the dataset's storage: no pixel copy
                 else:
                     raw = self.dataset.images.index_select(0, t)
-                if self.chain is None:
-                    data = self.aug.augment_batch(raw, self.tail, seed=self.seed, first_index=self._drawn, parity=self.parity)
-                elif self.chain_mode == "test":
-                    data = self.chain.test(raw)
-                else:
-                    data = self.chain.train(raw, parity=self.parity, seed=self.seed, first_index=self._drawn)
-                self._drawn += len(idx)
-                yield data, self.dataset.labels.index_select(0, t)
+                yield t, raw
             if files is not None:
                 for _ in files:                                  # the last batches' decode status
                     pass
         finally:
             if files is not None:
                 files.close()
+
+    def __iter__(self):
+        with contextlib.closing(self._batches()) as batches:
+            for t, raw in batches:
+                if self.chain is None:
+                    data = self.aug.augment_batch(raw, self.tail, seed=self.seed, first_index=self._drawn, parity=self.parity)
+                elif self.chain_mode == "test":
+                    data = self.chain.test(raw)
+                else:
+                    data = self.chain.train(raw, parity=self.parity, seed=self.seed, first_index=self._drawn)
+                self._drawn += len(t)
+                yield data, self.dataset.labels.index_select(0, t)
+
+    def tta(self, replicas):
+        """The policy search's test-time augmentation (reference search.py:87-125, ``eval_tta``) from one loader: an
+        iterator over one epoch of this loader's index stream yielding ``(data[replicas, B, ...], labels[B])``, replica r
+        of batch k being what this loader's own ``__iter__`` would yield for it with the Philox keys of
+        ``first_index = drawn + r * B`` (``drawn``: samples drawn before the batch).  Each batch is gathered, read or
+        decoded once; the replicas come from ``augment_tta`` (no chain) or ``ImageNetChain.train_tta``.  The batch
+        draws replicas * B keys, so no key repeats within or across batches or epochs, unlike replicas separate loaders
+        built with one seed.  Raises ValueError for parity draws, a test-chain loader and what ``check_tta`` refuses."""
+        if self.parity:
+            raise ValueError("tta draws with Philox only: K reference loaders have no single parity draw order")
+        if self.chain is not None and self.chain_mode != "train":
+            raise ValueError("tta replicates the train chain: a %r chain loader draws nothing" % self.chain_mode)
+        n = min(self.batch_size, self._n())
+        if self.chain is not None:
+            self.chain.check_tta(n, replicas)
+        else:
+            check_tta(n, replicas)
+            if self.aug.compiled.n_op > _lib.MAX_FUSED_OPS:
+                raise ValueError("tta supports policies of at most %d ops per sub-policy (replicated launches)"
+                                 % _lib.MAX_FUSED_OPS)
+        return self._tta(int(replicas))
+
+    def _tta(self, K):
+        with contextlib.closing(self._batches()) as batches:
+            for t, raw in batches:
+                if self.chain is None:
+                    data = augment_tta(self.aug.compiled, raw, self.tail, K, self.seed, self._drawn)
+                else:
+                    data = self.chain.train_tta(raw, K, seed=self.seed, first_index=self._drawn)
+                self._drawn += K * len(t)
+                yield data, self.dataset.labels.index_select(0, t)
 
 
 # ---------------------------------------------------------------------------------------------------

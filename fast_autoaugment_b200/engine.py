@@ -409,7 +409,17 @@ def augment_tta(policy: CompiledPolicy, batch_u8: torch.Tensor, tail: TailSpec, 
 
         out[r] == augment_batch(policy, batch_u8, tail, rng=make_rng(seed, first_index + r * B, tail))
 
-    uint8 [B,H,W,3] CUDA batch -> [replicas, B, 3, out_h, out_w] (or [replicas, B, out_h, out_w, 3] uint8)."""
+    uint8 [B,H,W,3] CUDA batch -> [replicas, B, 3, out_h, out_w] (or [replicas, B, out_h, out_w, 3] uint8).
+
+    A ``RaggedImages`` batch (``tail`` must be ``TailSpec.raw_u8()``) gives a ``RaggedImages`` of replicas * B images
+    in replica-major order, each at its source size: one ``faa_augment_ragged`` launch group over replicas * B
+    descriptors (``tta_select``) into the batch's storage, so image r * B + i is
+    ``augment_batch(policy, batch, tail, rng=make_rng(seed, first_index + r * B, tail))``'s image i.  ``out`` may be a
+    ``RaggedImages`` of those sizes."""
+    if isinstance(batch_u8, RaggedImages):
+        check_tta(len(batch_u8), replicas)
+        return _augment_ragged(policy, tta_select(batch_u8, replicas), tail, None, None,
+                               make_rng(seed, first_index, tail), out)
     _require_cuda(batch_u8, "batch")
     if batch_u8.dtype != torch.uint8 or batch_u8.dim() != 4 or batch_u8.shape[-1] != 3:
         raise ValueError("batch must be uint8 [B, H, W, 3]")
@@ -426,6 +436,28 @@ def augment_tta(policy: CompiledPolicy, batch_u8: torch.Tensor, tail: TailSpec, 
         check(lib.faa_augment_tta(policy.handle, batch_u8.data_ptr(), out.data_ptr(), B, int(replicas), H, W, C.byref(t),
                                   C.byref(rng), _stream_ptr(batch_u8.device)))
     return out
+
+
+MAX_LAUNCH_IMAGES = 65535          # images per launch (one grid row each)
+
+
+def check_tta(batch, replicas):
+    """ValueError unless ``replicas`` >= 1 and the ``replicas * batch`` images of a TTA call fit in one launch"""
+    if int(replicas) != replicas or replicas < 1:
+        raise ValueError("replicas must be a positive integer, not %r" % (replicas,))
+    if int(replicas) * int(batch) > MAX_LAUNCH_IMAGES:
+        raise ValueError("replicas * batch = %d images: at most %d per launch" % (int(replicas) * int(batch),
+                                                                                MAX_LAUNCH_IMAGES))
+
+
+def tta_positions(batch, replicas):
+    """int64 [replicas * batch]: the batch position each TTA schedule entry v = r * batch + i reads (i)"""
+    return np.tile(np.arange(int(batch), dtype=np.int64), int(replicas))
+
+
+def tta_select(batch: RaggedImages, replicas):
+    """``replicas`` copies of the batch's descriptors, replica-major, into the same storage (no pixel is copied)"""
+    return batch.select(tta_positions(len(batch), replicas))
 
 
 def crop_cfg(img_size, center=False, min_covered=0.1, aspect_ratio_range=(3. / 4, 4. / 3), area_range=(0.08, 1.0),
