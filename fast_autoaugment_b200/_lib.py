@@ -35,8 +35,14 @@ JPEG_HEADER_DTYPE = np.dtype([("offset", "<i8"), ("len", "<i8"), ("scan_off", "<
 JPEG_TABLE_DTYPE = np.dtype([("q", "<u2", (64,)), ("bits", "u1", (16,)), ("vals", "u1", (256,))])   # faa_jpeg_table_t
 JPEG_TRUNCATED, JPEG_BAD_CODE, JPEG_BAD_COEF, JPEG_BAD_RESTART = 1, 2, 4, 8                       # faa_jpeg_status
 JPEG_SYNC_DTYPE = np.dtype([("mcu", "<i4"), ("byte", "<i4"), ("bit", "<i2"), ("pred", "<i2", (3,))])  # faa_jpeg_sync_t
+JPEG_SCAN_DTYPE = np.dtype([("off", "<i8"), ("len", "<i8"), ("restart", "<i4"), ("ns", "<i4"), ("comp", "<i4", (3,)),
+                            ("ss", "<i4"), ("se", "<i4"), ("ah", "<i4"), ("al", "<i4"), ("wave", "<i4"),
+                            ("dc_at", "<i4", (3,)), ("ac_at", "<i4", (3,)), ("pool", "<i4", (6,)),
+                            ("reserved", "<i4", (2,))])                                            # faa_jpeg_scan_t
+JPEG_PROGRESSIVE, JPEG_MAX_SCANS = 1, 64
 assert SAMPLE_DTYPE.itemsize == 16 and BOX_DTYPE.itemsize == 8 and IMAGE_DTYPE.itemsize == 16
 assert JPEG_HEADER_DTYPE.itemsize == 144 and JPEG_TABLE_DTYPE.itemsize == 400 and JPEG_SYNC_DTYPE.itemsize == 16
+assert JPEG_SCAN_DTYPE.itemsize == 112
 
 
 class Tail(C.Structure):          # faa_tail_t
@@ -113,6 +119,10 @@ def _load():
         "faa_jpeg_decode_indexed": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp]),
         "faa_jpeg_decode_recording": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp,
                                                 vp, vp, vp, vp]),
+        "faa_jpeg_parse_progressive": (C.c_int, [C.c_char_p, C.c_size_t, vp, vp, C.c_int, P(C.c_int)]),
+        "faa_jpeg_scan_tables": (C.c_int, [C.c_char_p, C.c_size_t, vp, vp, C.c_int, vp]),
+        "faa_jpeg_decode_progressive": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp,
+                                                  vp]),
         "faa_launch_count": (u64, []),
     }
     for name, (res, args) in sig.items():

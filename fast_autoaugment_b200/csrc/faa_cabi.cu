@@ -1606,7 +1606,12 @@ static int grow_async(void** ptr, size_t* have, size_t need, cudaStream_t stream
     return FAA_OK;
 }
 
-static int check_jpeg_header(const JpegHeader& h, int n_tables, const std::string& who) {
+// a header the decode calls take: baseline (the quantisation and both Huffman pool slots of every component), or with
+// `progressive` a progressive one (quantisation slots only: the Huffman tables are the scans')
+static int check_jpeg_header(const JpegHeader& h, int n_tables, const std::string& who, bool progressive = false) {
+    if (jpeg_is_progressive(h) != progressive)
+        return fail(FAA_ERR_VALUE, who + (progressive ? ": not a progressive header (faa_jpeg_decode takes it)"
+                                                      : ": a progressive header (faa_jpeg_decode_progressive takes it)"));
     if (h.ncomp != 1 && h.ncomp != 3) return fail(FAA_ERR_VALUE, who + ": component count must be 1 or 3");
     if (check_shape(h.h, h.w)) return fail(FAA_ERR_VALUE, who + ": size out of range");
     const bool samp = h.ncomp == 1 ? (h.hs == 1 && h.vs == 1)
@@ -1617,7 +1622,7 @@ static int check_jpeg_header(const JpegHeader& h, int n_tables, const std::strin
     if (h.restart < 0 || h.offset < 0 || h.len < 0 || h.scan_off < 0 || h.scan_len < 0 || h.scan_off + h.scan_len > h.len)
         return fail(FAA_ERR_VALUE, who + ": restart interval or byte ranges out of range");
     for (int c = 0; c < h.ncomp; ++c)
-        for (int k = 0; k < 3; ++k)
+        for (int k = 0; k < (progressive ? 1 : 3); ++k)
             if (h.pool[3 * k + c] < 0 || h.pool[3 * k + c] >= n_tables)
                 return fail(FAA_ERR_VALUE, who + ": table pool index out of range");
     return FAA_OK;
@@ -1673,7 +1678,7 @@ int faa_jpeg_decoder_destroy(faa_jpeg_decoder_t* d) {
 int faa_jpeg_index_capacity(const faa_jpeg_header_t* hdr) {
     if (!hdr) return 0;
     JpegHeader h; memcpy(&h, hdr, sizeof h);
-    return jpeg_index_capacity(h);
+    return jpeg_is_progressive(h) ? 0 : jpeg_index_capacity(h);
 }
 
 int faa_jpeg_decode(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
@@ -1729,6 +1734,31 @@ int faa_jpeg_index_build(const faa_jpeg_header_t* h_headers, const faa_jpeg_head
 
 }  // extern "C"
 
+// Binds the handle to the current device, orders this call's use of its scratch after the previous call's, grows the
+// coefficient, segment and job buffers to what the call needs and uploads the job table.  Every decode call goes
+// through here, under the handle's lock until its launches are queued, so calls of either kind may follow each other on
+// any streams.
+static int jpeg_call_scratch(faa_jpeg_decoder_t* d, cudaStream_t stream, const std::vector<JpegJob>& jobs, int64_t blocks,
+                             int64_t segs) {
+    int dev = -1;
+    if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); return fail(FAA_ERR_NO_DEVICE, "no current CUDA device"); }
+    if (d->device < 0) d->device = dev;
+    if (d->device != dev)
+        return fail(FAA_ERR_VALUE, "JPEG decoder is bound to device " + std::to_string(d->device) + " but the current device is " +
+                    std::to_string(dev) + ": create one decoder per device");
+    if (d->have_last_stream && d->last_stream != stream) {          // buffers are reused in the order of the calls
+        if (!d->ev_switch) CK(cudaEventCreateWithFlags(&d->ev_switch, cudaEventDisableTiming));
+        CK(cudaEventRecord(d->ev_switch, d->last_stream));
+        CK(cudaStreamWaitEvent(stream, d->ev_switch, 0));
+    }
+    d->last_stream = stream; d->have_last_stream = true;
+    if (int e = grow_async(&d->d_coef, &d->coef_bytes, (size_t)blocks * 128, stream)) return e;
+    if (int e = grow_async(&d->d_segs, &d->segs_bytes, (size_t)segs * sizeof(int32_t), stream)) return e;
+    if (int e = grow_async(&d->d_jobs, &d->jobs_bytes, jobs.size() * sizeof(JpegJob), stream)) return e;
+    CK(cudaMemcpyAsync(d->d_jobs, jobs.data(), jobs.size() * sizeof(JpegJob), cudaMemcpyHostToDevice, stream));  // (pageable: staged at once)
+    return FAA_OK;
+}
+
 // faa_jpeg_decode_indexed, and with `rec` (the recording outputs, checked by the caller) faa_jpeg_decode_recording
 struct JpegRecordOut {
     const int64_t* d_cap_first;
@@ -1768,24 +1798,9 @@ static int jpeg_decode_call(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_he
     jobs[(size_t)batch] = {blocks, (int32_t)segs, (int32_t)tiles};
     if (int e = ensure_device()) return e;
     if (batch == 0) return FAA_OK;
-    int dev = -1;
-    if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); return fail(FAA_ERR_NO_DEVICE, "no current CUDA device"); }
-    std::lock_guard<std::mutex> lk(d->mu);
-    if (d->device < 0) d->device = dev;
-    if (d->device != dev)
-        return fail(FAA_ERR_VALUE, "JPEG decoder is bound to device " + std::to_string(d->device) + " but the current device is " +
-                    std::to_string(dev) + ": create one decoder per device");
     cudaStream_t stream = (cudaStream_t)stream_v;
-    if (d->have_last_stream && d->last_stream != stream) {          // buffers are reused in the order of the calls
-        if (!d->ev_switch) CK(cudaEventCreateWithFlags(&d->ev_switch, cudaEventDisableTiming));
-        CK(cudaEventRecord(d->ev_switch, d->last_stream));
-        CK(cudaStreamWaitEvent(stream, d->ev_switch, 0));
-    }
-    d->last_stream = stream; d->have_last_stream = true;
-    if (int e = grow_async(&d->d_coef, &d->coef_bytes, (size_t)blocks * 128, stream)) return e;
-    if (int e = grow_async(&d->d_segs, &d->segs_bytes, (size_t)segs * sizeof(int32_t), stream)) return e;
-    if (int e = grow_async(&d->d_jobs, &d->jobs_bytes, jobs.size() * sizeof(JpegJob), stream)) return e;
-    CK(cudaMemcpyAsync(d->d_jobs, jobs.data(), jobs.size() * sizeof(JpegJob), cudaMemcpyHostToDevice, stream));  // (pageable: staged at once)
+    std::lock_guard<std::mutex> lk(d->mu);
+    if (int e = jpeg_call_scratch(d, stream, jobs, blocks, segs)) return e;
     JpegDecodeParams P = {};
     P.hdrs = reinterpret_cast<const JpegHeader*>(d_headers);
     P.pool = reinterpret_cast<const JpegTable*>(d_tables);
@@ -1836,6 +1851,144 @@ int faa_jpeg_decode_recording(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_
     const JpegRecordOut rec = {d_cap_first, d_points_out, d_count};
     return jpeg_decode_call(d, h_headers, d_headers, d_tables, n_tables, d_src, batch, h_out, d_out, d_status, d_points,
                             h_first, d_first, &rec, stream_v);
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------ progressive JPEG decode --
+static_assert(sizeof(faa_jpeg_scan_t) == sizeof(JpegScan) && sizeof(JpegScan) == 112 &&
+              offsetof(faa_jpeg_scan_t, pool) == offsetof(JpegScan, pool) && FAA_JPEG_MAX_SCANS == kJpegMaxScans &&
+              FAA_JPEG_PROGRESSIVE == kJpegProgressive, "JPEG scan layout");
+
+// image `who`'s scans [0, n): parameters a progression can have, byte ranges inside the file, pool slots in range, and
+// the waves the dependency rule gives (a wrong wave would let two work items race on a coefficient)
+static int check_jpeg_scans(const JpegHeader& h, const JpegScan* scans, int64_t n, int n_tables, const std::string& who) {
+    if (n < 1 || n > kJpegMaxScans) return fail(FAA_ERR_VALUE, who + ": 1 to 64 scans per image");
+    JpegScan w[kJpegMaxScans];
+    memcpy(w, scans, (size_t)n * sizeof(JpegScan));
+    for (int64_t i = 0; i < n; ++i) {
+        const JpegScan& s = scans[i];
+        const std::string at = who + " scan " + std::to_string(i);
+        if (s.ns < 1 || s.ns > h.ncomp) return fail(FAA_ERR_VALUE, at + ": component count out of range");
+        for (int k = 0; k < s.ns; ++k)
+            if (s.comp[k] < (k ? s.comp[k - 1] + 1 : 0) || s.comp[k] >= h.ncomp)
+                return fail(FAA_ERR_VALUE, at + ": components out of range or out of frame order");
+        if (s.ss < 0 || s.ss > s.se || s.se > 63 || (s.ss == 0) != (s.se == 0) || (s.ss > 0 && s.ns != 1) || s.al < 0 ||
+            s.al > 13 || (s.ah != 0 && s.ah != s.al + 1))
+            return fail(FAA_ERR_VALUE, at + ": spectral band or approximation out of range");
+        if (s.restart < 0 || s.off < 0 || s.len < 0 || s.off + s.len > h.len)
+            return fail(FAA_ERR_VALUE, at + ": restart interval or byte range out of range");
+        for (int k = 0; k < jpeg_scan_tables(s); ++k) {
+            const int32_t p = s.pool[s.ss == 0 ? k : 3];
+            if (p < 0 || p >= n_tables) return fail(FAA_ERR_VALUE, at + ": table pool index out of range");
+        }
+    }
+    jpeg_scan_waves(w, (int)n);
+    for (int64_t i = 0; i < n; ++i)
+        if (w[i].wave != scans[i].wave)
+            return fail(FAA_ERR_VALUE, who + " scan " + std::to_string(i) + ": wave does not follow the scans' dependencies");
+    return FAA_OK;
+}
+
+extern "C" {
+
+int faa_jpeg_parse_progressive(const uint8_t* bytes, size_t len, faa_jpeg_header_t* out, faa_jpeg_scan_t* scans,
+                               int max_scans, int* n_scans) {
+    if (!bytes || !out || !scans || !n_scans || max_scans < 1) return fail(FAA_ERR_VALUE, "null argument");
+    JpegHeader h;
+    const char* why = "";
+    const int e = parse_jpeg_progressive(bytes, len, h, reinterpret_cast<JpegScan*>(scans),
+                                         std::min(max_scans, kJpegMaxScans), n_scans, &why);
+    memcpy(out, &h, sizeof h);
+    if (e == JPARSE_UNSUPPORTED) return fail(FAA_ERR_UNSUPPORTED, std::string("unsupported JPEG: ") + why);
+    if (e == JPARSE_MALFORMED) return fail(FAA_ERR_VALUE, std::string("malformed JPEG: ") + why);
+    return FAA_OK;
+}
+
+int faa_jpeg_scan_tables(const uint8_t* bytes, size_t len, const faa_jpeg_header_t* hdr, const faa_jpeg_scan_t* scans,
+                         int n_scans, faa_jpeg_table_t* out) {
+    if (!bytes || !hdr || !scans || !out) return fail(FAA_ERR_VALUE, "null argument");
+    JpegHeader h; memcpy(&h, hdr, sizeof h);
+    if (!jpeg_is_progressive(h) || (h.ncomp != 1 && h.ncomp != 3)) return fail(FAA_ERR_VALUE, "not a progressive header");
+    if (n_scans < 1 || n_scans > kJpegMaxScans) return fail(FAA_ERR_VALUE, "1 to 64 scans");
+    for (int c = 0; c < h.ncomp; ++c) {
+        const size_t qbytes = (h.qprec >> c & 1) ? 128 : 64;
+        if (h.table_at[c] < 0 || (size_t)h.table_at[c] + qbytes > len) return fail(FAA_ERR_VALUE, "quantisation table outside the file");
+    }
+    const JpegScan* s = reinterpret_cast<const JpegScan*>(scans);
+    for (int i = 0; i < n_scans; ++i)
+        for (int k = 0; k < 6; ++k) {
+            const int32_t at = k < 3 ? s[i].dc_at[k] : s[i].ac_at[k - 3];
+            if (at == -1 || jpeg_std_huff(at)) continue;
+            if (at < 0 || (size_t)at + 16 > len) return fail(FAA_ERR_VALUE, "Huffman table outside the file");
+            size_t total = 0;
+            for (int l = 0; l < 16; ++l) total += bytes[at + l];
+            if (total > 256 || (size_t)at + 16 + total > len) return fail(FAA_ERR_VALUE, "Huffman table outside the file");
+        }
+    jpeg_progressive_tables(bytes, h, s, n_scans, reinterpret_cast<JpegTable*>(out));
+    return FAA_OK;
+}
+
+int faa_jpeg_decode_progressive(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers,
+                                const faa_jpeg_header_t* d_headers, const faa_jpeg_table_t* d_tables, int n_tables,
+                                const uint8_t* d_src, int batch, const faa_image_t* h_out, const faa_image_t* d_out,
+                                int32_t* d_status, const faa_jpeg_scan_t* h_scans, const faa_jpeg_scan_t* d_scans,
+                                const int64_t* h_scan_first, const int64_t* d_scan_first, void* stream_v) {
+    if (!d || ((!h_headers || !d_headers || !d_tables || !d_src || !h_out || !d_out || !d_status || !h_scans || !d_scans ||
+                !h_scan_first || !d_scan_first) && batch > 0))
+        return fail(FAA_ERR_VALUE, "null argument");
+    if (batch < 0) return fail(FAA_ERR_VALUE, "negative batch");
+    if (batch > 65535) return fail(FAA_ERR_UNSUPPORTED, "at most 65535 images per call: split the batch");
+    if (batch > 0)
+        if (int e = check_jpeg_first(h_scan_first, batch)) return e;
+    std::vector<JpegJob> jobs((size_t)batch + 1);
+    int64_t blocks = 0, segs = 0, tiles = 0;
+    const JpegScan* scans = reinterpret_cast<const JpegScan*>(h_scans);
+    for (int i = 0; i < batch; ++i) {
+        JpegHeader h; memcpy(&h, &h_headers[i], sizeof h);
+        const std::string who = "image " + std::to_string(i);
+        if (int e = check_jpeg_header(h, n_tables, who, true)) return e;
+        if (!h_out[i].data) return fail(FAA_ERR_VALUE, "output " + who + " has no data");
+        if (h_out[i].h != h.h || h_out[i].w != h.w) return fail(FAA_ERR_VALUE, "output " + who + " is not the size of its JPEG");
+        const int64_t n = h_scan_first[i + 1] - h_scan_first[i];
+        if (int e = check_jpeg_scans(h, scans + h_scan_first[i], n, n_tables, who)) return e;
+        jobs[(size_t)i] = {blocks, (int32_t)segs, (int32_t)tiles};
+        blocks += jpeg_image_blocks(h);
+        for (int64_t k = 0; k < n; ++k) segs += jpeg_scan_segments(h, scans[h_scan_first[i] + k]);
+        tiles += (int64_t)((h.w + kJpegTileW - 1) / kJpegTileW) * ((h.h + kJpegTileH - 1) / kJpegTileH);
+        if (segs > INT32_MAX || tiles > INT32_MAX) return fail(FAA_ERR_UNSUPPORTED, "batch too large: split it");
+    }
+    jobs[(size_t)batch] = {blocks, (int32_t)segs, (int32_t)tiles};
+    if (int e = ensure_device()) return e;
+    if (batch == 0) return FAA_OK;
+    cudaStream_t stream = (cudaStream_t)stream_v;
+    std::lock_guard<std::mutex> lk(d->mu);
+    if (int e = jpeg_call_scratch(d, stream, jobs, blocks, segs)) return e;
+    JpegProgressiveParams Q = {};
+    Q.hdrs = reinterpret_cast<const JpegHeader*>(d_headers);
+    Q.pool = reinterpret_cast<const JpegTable*>(d_tables);
+    Q.src = d_src;
+    Q.jobs = reinterpret_cast<const JpegJob*>(d->d_jobs);
+    Q.scans = reinterpret_cast<const JpegScan*>(d_scans);
+    Q.scan_first = d_scan_first;
+    Q.coef = reinterpret_cast<int16_t*>(d->d_coef);
+    Q.segs = reinterpret_cast<int32_t*>(d->d_segs);
+    Q.status = d_status;
+    Q.batch = batch;
+    CK(launch_jpeg_progressive(Q, stream));
+    g_launches++;
+    JpegDecodeParams P = {};
+    P.hdrs = Q.hdrs;
+    P.pool = Q.pool;
+    P.src = d_src;
+    P.jobs = Q.jobs;
+    P.out = reinterpret_cast<const CropImage*>(d_out);
+    P.coef = Q.coef;
+    P.status = d_status;
+    P.batch = batch;
+    CK(launch_jpeg_reconstruct(P, (int)tiles, stream));
+    g_launches++;
+    return FAA_OK;
 }
 
 }  // extern "C"

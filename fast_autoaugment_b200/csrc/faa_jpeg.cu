@@ -11,6 +11,8 @@
 //                                instantiation (faa_jpeg_decode_recording) also places the scan index of every scan
 //                                thread 0 decodes whole and serially, as faa_jpeg_index_kernel would.
 //   faa_jpeg_index_kernel        (faa_jpeg_index_build) one CTA per image; one thread records the scan index.
+//   faa_jpeg_progressive_kernel  (faa_jpeg_decode_progressive) one CTA per progressive image: the entropy stage of
+//                                progressive files, scans run wave by wave; the reconstruct kernel follows it.
 //   faa_jpeg_reconstruct_kernel  one CTA per 64 x 32 output tile of one image.  It runs the islow IDCT of the tile's
 //                                blocks, with the one-block chroma halo fancy upsampling reads, into shared memory,
 //                                upsamples and converts to RGB, and writes uint8 HWC rows with 32-bit stores where the
@@ -221,6 +223,120 @@ __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_index_kernel(const _
                                     cap < kJpegIndexMaxParts ? (int)cap : kJpegIndexMaxParts, s_scratch, &status);
     P.count[img] = n;
     P.status[img] = status;
+}
+
+// Progressive entropy decode, one CTA per image.  The CTA zeroes the image's coefficient planes (progressive scans
+// accumulate into them), finds every scan's restart markers as the baseline kernel does, then runs the scans wave by
+// wave.  A wave's scans share no (component, coefficient), so its work items, one per (scan, restart segment), run on
+// all threads at once; a barrier separates waves.  A wave whose scans need more Huffman tables than kProgSlots (or has
+// more than kProgGroup scans) runs as several groups, one after the other.
+constexpr int kProgSlots = 8, kProgGroup = 16;
+
+__global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_progressive_kernel(const __grid_constant__ JpegProgressiveParams P) {
+    __shared__ JpegHuff s_huff[kProgSlots];
+    __shared__ JpegScan s_scan[kJpegMaxScans];
+    __shared__ int32_t s_seg[kJpegMaxScans];              // first segment-start entry of each scan
+    __shared__ uint8_t s_order[kJpegMaxScans];            // scans by wave, file order within a wave
+    __shared__ int32_t s_count[kEntropyThreads];
+    __shared__ int32_t s_gscan[kProgGroup], s_gslot[kProgGroup], s_gitem[kProgGroup + 1], s_gtab[kProgSlots];
+    __shared__ int32_t s_ng, s_nslot, s_pos, s_status;
+    const int img = blockIdx.x, tid = threadIdx.x;
+    const JpegHeader h = P.hdrs[img];
+    const JpegJob job = P.jobs[img];
+    const uint8_t* file = P.src + h.offset;
+    const int n = (int)(P.scan_first[img + 1] - P.scan_first[img]);
+    int16_t* coef = P.coef + 64 * job.coef;
+    int32_t* segs = P.segs + job.seg;
+    for (int k = tid; k < n; k += kEntropyThreads) s_scan[k] = P.scans[P.scan_first[img] + k];
+    {
+        uint4* z = reinterpret_cast<uint4*>(coef);
+        const int64_t n16 = jpeg_image_blocks(h) * 8;
+        for (int64_t k = tid; k < n16; k += kEntropyThreads) z[k] = make_uint4(0, 0, 0, 0);
+    }
+    __syncthreads();
+    if (tid == 0) {
+        s_status = 0;
+        int32_t at = 0, o = 0;
+        for (int k = 0; k < n; ++k) { s_seg[k] = at; at += (int32_t)jpeg_scan_segments(h, s_scan[k]); }
+        for (int w = 0; o < n; ++w)
+            for (int k = 0; k < n; ++k) if (s_scan[k].wave == w) s_order[o++] = (uint8_t)k;
+    }
+    __syncthreads();
+    // restart-segment starts of every scan: count, prefix, record (as faa_jpeg_entropy_kernel)
+    for (int k = 0; k < n; ++k) {
+        const JpegScan& s = s_scan[k];
+        const int64_t n_seg = jpeg_scan_segments(h, s);
+        int32_t* ss = segs + s_seg[k];
+        for (int64_t j = tid; j < n_seg; j += kEntropyThreads) ss[j] = j == 0 ? 0 : -1;
+        if (n_seg == 1) continue;
+        const uint8_t* scan = file + s.off;
+        const int64_t chunk = (s.len + kEntropyThreads - 1) / kEntropyThreads;
+        const int64_t a = min((int64_t)tid * chunk, s.len), b = min(a + chunk, s.len);
+        JpegBits r;
+        jpeg_bits_init(r, scan, scan, scan + s.len);
+        s_count[tid] = jpeg_markers(r, scan, a, b, s.len, nullptr, 0, 0);
+        __syncthreads();
+        if (tid == 0) {
+            int32_t run = 0;
+            for (int t = 0; t < kEntropyThreads; ++t) { const int32_t c = s_count[t]; s_count[t] = run; run += c; }
+            if (run != n_seg - 1) s_status = JPEG_BAD_RESTART;
+        }
+        __syncthreads();
+        jpeg_markers(r, scan, a, b, s.len, ss, 1 + s_count[tid], n_seg);
+        __syncthreads();
+    }
+    int status = 0;
+    for (int pos = 0; pos < n;) {
+        if (tid == 0) {                                  // the next group: scans of one wave, tables in kProgSlots
+            int ng = 0, slots = 0, items = 0, q = pos;
+            const int w = s_scan[s_order[pos]].wave;
+            while (q < n && ng < kProgGroup) {
+                const int k = s_order[q];
+                const JpegScan& s = s_scan[k];
+                const int need = jpeg_scan_tables(s);
+                if (s.wave != w || slots + need > kProgSlots) break;
+                s_gscan[ng] = k; s_gslot[ng] = slots; s_gitem[ng] = items;
+                for (int t = 0; t < need; ++t) s_gtab[slots + t] = s.pool[s.ss == 0 ? t : 3];
+                slots += need;
+                items += (int)jpeg_scan_segments(h, s);
+                ++ng; ++q;
+            }
+            s_gitem[ng] = items; s_ng = ng; s_nslot = slots; s_pos = q;
+        }
+        __syncthreads();
+        const int ng = s_ng, nslot = s_nslot, items = s_gitem[ng];
+        pos = s_pos;
+        if (tid < nslot) jpeg_huff_codes(P.pool[s_gtab[tid]], s_huff[tid]);
+        __syncthreads();
+        for (int e = tid; e < nslot << kJpegLookBits; e += kEntropyThreads) {
+            const int t = e >> kJpegLookBits;
+            s_huff[t].look[e & ((1 << kJpegLookBits) - 1)] = jpeg_huff_look(s_huff[t], e & ((1 << kJpegLookBits) - 1));
+        }
+        __syncthreads();
+        for (int it = tid; it < items; it += kEntropyThreads) {
+            int g = 0;
+            while (it >= s_gitem[g + 1]) ++g;
+            const int k = s_gscan[g];
+            const JpegScan& s = s_scan[k];
+            const int64_t j = it - s_gitem[g], units = jpeg_scan_units(h, s);
+            const int64_t u0 = s.restart > 0 ? j * s.restart : 0, u1 = s.restart > 0 ? min(u0 + s.restart, units) : units;
+            const JpegHuff* hp[3] = {&s_huff[s_gslot[g]], &s_huff[min(s_gslot[g] + 1, kProgSlots - 1)],
+                                     &s_huff[min(s_gslot[g] + 2, kProgSlots - 1)]};
+            const uint8_t* scan = file + s.off;
+            const int32_t at = segs[s_seg[k] + j];
+            status |= jpeg_prog_segment(h, s, hp, scan, at < 0 ? scan + s.len : scan + at, scan + s.len, u0, u1, coef);
+        }
+        __syncthreads();                                 // the wave's coefficients are complete; s_huff is free
+    }
+    if (status) atomicOr(&s_status, status);
+    __syncthreads();
+    if (tid == 0) P.status[img] = s_status;
+}
+
+cudaError_t launch_jpeg_progressive(const JpegProgressiveParams& p, cudaStream_t stream) {
+    if (p.batch <= 0) return cudaSuccess;
+    faa_jpeg_progressive_kernel<<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p);
+    return cudaGetLastError();
 }
 
 cudaError_t launch_jpeg_index(const JpegDecodeParams& p, cudaStream_t stream) {

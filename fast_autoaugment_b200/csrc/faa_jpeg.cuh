@@ -816,6 +816,7 @@ FAA_JHD int jpeg_tile_windows(const JpegHeader& h, int x0, int y0, int x1, int y
 // rec_at[0, rec_cap) (jpeg_record_sink), and *rec_count gets their number, or 0 when the scan was not decoded that way,
 // gets no points or did not decode cleanly.  coef_out: the coefficients (jpeg_image_blocks(h) blocks).  Returns the
 // JpegStatus bits.
+inline void jpeg_reconstruct_host(const JpegHeader& h, const JpegTable* tabs, const int16_t* coef, uint8_t* out);
 inline int jpeg_decode_host(const uint8_t* file, const JpegHeader& h, const JpegTable* tabs, uint8_t* out,
                             const JpegSync* pts = nullptr, int64_t npts = 0, JpegSync* rec_at = nullptr,
                             int64_t rec_cap = 0, int32_t* rec_count = nullptr, int16_t* coef_out = nullptr) {
@@ -863,7 +864,14 @@ inline int jpeg_decode_host(const uint8_t* file, const JpegHeader& h, const Jpeg
     }
     if (rec_count) *rec_count = rec && !status ? rec->n : 0;
     if (coef_out) memcpy(coef_out, coef, (size_t)nblk * 128);
-    // planes of samples
+    jpeg_reconstruct_host(h, tabs, coef, out);
+    delete[] at;
+    delete[] coef;
+    return status;
+}
+
+// The reconstruct kernel's work on the host: coefficient planes -> islow IDCT -> fancy upsampling -> RGB (h.h * h.w * 3)
+inline void jpeg_reconstruct_host(const JpegHeader& h, const JpegTable* tabs, const int16_t* coef, uint8_t* out) {
     uint8_t* planes[3] = {nullptr, nullptr, nullptr};
     int pw[3], ph[3];
     int64_t base = 0;
@@ -891,7 +899,434 @@ inline int jpeg_decode_host(const uint8_t* file, const JpegHeader& h, const Jpeg
             jpeg_ycc_rgb(Y, cb, cr, o);
         }
     for (int c = 0; c < 3; ++c) delete[] planes[c];
-    delete[] at;
+}
+
+// ------------------------------------------------------------------------------------------------ progressive --
+// Progressive Huffman files (SOF2), ITU T.81 G.1.2, decoded as libjpeg does, into the same coefficient planes the
+// reconstruct stage reads.  parse_jpeg_progressive takes what parse_jpeg takes (8-bit, 1 or 3 components, 4:4:4 / 4:2:2 /
+// 4:2:0) when it is coded progressively and every coefficient of every component ends at bit 0; libjpeg smooths the
+// blocks of an incomplete progression, which is not modelled, so those files are refused.  Its header has
+// reserved = kJpegProgressive, restart = 0 and no scan_off / scan_len; the scans are a separate list.
+constexpr int32_t kJpegProgressive = 1;      // JpegHeader::reserved of a progressive file (0 for every other)
+constexpr int kJpegMaxScans = 64;
+
+// layout of faa_jpeg_scan_t
+struct JpegScan {
+    int64_t off, len;            // entropy-coded data, relative to the file
+    int32_t restart;             // restart interval in force at its SOS (0: none)
+    int32_t ns;                  // components in the scan, comp[0, ns) their frame indices in frame order
+    int32_t comp[3];
+    int32_t ss, se, ah, al;      // spectral band [ss, se], successive approximation bits
+    int32_t wave;                // 1 + the largest wave of an earlier scan sharing a (component, coefficient)
+    int32_t dc_at[3], ac_at[3];  // file offsets of the DC tables of comp[k] (DC first scans) / the AC table (k = 0; AC
+                                 // scans) as defined at its SOS, kJpegStdAt - k for standard table k, -1 when unused
+    int32_t pool[6];             // the same tables as pool indices: DC of comp[k] at k, AC at 3 (-1 when unused)
+    int32_t reserved[2];
+};
+
+FAA_JHD bool jpeg_is_progressive(const JpegHeader& h) { return h.reserved == kJpegProgressive; }
+
+// Huffman tables a scan uses: DC first: one per component; DC refinement: none; AC: one
+FAA_JHD int jpeg_scan_tables(const JpegScan& s) { return s.ss == 0 ? (s.ah == 0 ? s.ns : 0) : 1; }
+
+// Wave numbers of scans [0, n) (the dependency rule of JpegScan::wave).  Scans of one wave share no (component,
+// coefficient), so they can be decoded in any order.
+inline void jpeg_scan_waves(JpegScan* s, int n) {
+    int8_t last[3][64];
+    memset(last, -1, sizeof last);
+    for (int i = 0; i < n; ++i) {
+        int w = 0;
+        for (int k = 0; k < s[i].ns; ++k)
+            for (int q = s[i].ss; q <= s[i].se; ++q) w = last[s[i].comp[k]][q] + 1 > w ? last[s[i].comp[k]][q] + 1 : w;
+        s[i].wave = w;
+        for (int k = 0; k < s[i].ns; ++k)
+            for (int q = s[i].ss; q <= s[i].se; ++q) last[s[i].comp[k]][q] = (int8_t)w;
+    }
+}
+
+// Parses a progressive file (host only): its header and at most max_scans scans (*n_scans of them).  Returns JPARSE_*
+// with the reason of a refusal in *why, as parse_jpeg does; a file that is not progressive is refused too.
+inline int parse_jpeg_progressive(const uint8_t* b, size_t len, JpegHeader& h, JpegScan* scans, int max_scans,
+                                  int* n_scans, const char** why) {
+    memset(&h, 0, sizeof h);
+    for (int k = 0; k < 9; ++k) { h.table_at[k] = -1; h.pool[k] = -1; }
+    h.len = (int64_t)len;
+    h.reserved = kJpegProgressive;
+    *n_scans = 0;
+    *why = "";
+#define FAA_BAD(msg) do { *why = msg; return JPARSE_MALFORMED; } while (0)
+#define FAA_NO(msg) do { *why = msg; return JPARSE_UNSUPPORTED; } while (0)
+    if (len < 4 || b[0] != 0xFF || b[1] != 0xD8) FAA_BAD("no SOI marker: not a JPEG file");
+    if (len > 0x7FFFFFFF) FAA_NO("file larger than 2 GiB");
+    int32_t dqt_at[4] = {-1, -1, -1, -1}, dqt_prec[4] = {0, 0, 0, 0}, dht_at[2][4];
+    for (int c = 0; c < 2; ++c) for (int k = 0; k < 4; ++k) dht_at[c][k] = -1;
+    bool jfif = false, adobe = false, have_sof = false;
+    int adobe_transform = -1, restart = 0;
+    int comp_id[3] = {0, 0, 0}, comp_h[3] = {0, 0, 0}, comp_v[3] = {0, 0, 0}, comp_q[3] = {0, 0, 0};
+    int bitpos[3][64];                                   // current bit position of each coefficient, -1: not yet sent
+    for (int c = 0; c < 3; ++c) for (int k = 0; k < 64; ++k) bitpos[c][k] = -1;
+    size_t i = 2;
+    while (true) {
+        while (i < len && b[i] != 0xFF) ++i;
+        while (i < len && b[i] == 0xFF) ++i;
+        if (i >= len) break;                             // a file cut short: the progression check below judges it
+        const int m = b[i++];
+        if (m == 0xD9) break;                            // EOI
+        if (m == 0x01 || (m >= 0xD0 && m <= 0xD7)) continue;
+        if (m == 0xD8) FAA_BAD("second SOI marker");
+        if (i + 2 > len) FAA_BAD("marker segment cut off");
+        const int L = jpeg_u16(b + i);
+        if (L < 2 || i + (size_t)L > len) FAA_BAD("marker segment length out of range");
+        const uint8_t* p = b + i + 2;
+        const int n = L - 2;
+        const size_t seg_end = i + (size_t)L;
+        if (m == 0xC2) {
+            if (have_sof) FAA_BAD("second frame header");
+            if (n < 6) FAA_BAD("frame header too short");
+            if (p[0] != 8) FAA_NO("12-bit (or other non-8-bit) samples");
+            h.h = jpeg_u16(p + 1); h.w = jpeg_u16(p + 3);
+            const int nf = p[5];
+            if (h.h == 0) FAA_NO("height defined by a DNL marker");
+            if (h.w == 0) FAA_BAD("zero width");
+            if (h.h > 8192 || h.w > 8192) FAA_NO("image larger than 8192 pixels on a side");
+            if (nf == 4) FAA_NO("4 components (CMYK or YCCK)");
+            if (nf != 1 && nf != 3) FAA_NO("component count other than 1 or 3");
+            if (n != 6 + 3 * nf) FAA_BAD("frame header length does not match its components");
+            for (int c = 0; c < nf; ++c) {
+                comp_id[c] = p[6 + 3 * c]; comp_h[c] = p[7 + 3 * c] >> 4; comp_v[c] = p[7 + 3 * c] & 15;
+                comp_q[c] = p[8 + 3 * c];
+                if (comp_h[c] < 1 || comp_h[c] > 4 || comp_v[c] < 1 || comp_v[c] > 4) FAA_BAD("sampling factor out of range");
+                if (comp_q[c] > 3) FAA_BAD("quantisation table index out of range");
+            }
+            h.ncomp = nf; have_sof = true;
+        } else if (m == 0xC0 || m == 0xC1) {
+            FAA_NO("not a progressive frame (parse_jpeg takes it)");
+        } else if (m == 0xCA) {
+            FAA_NO("progressive arithmetic coding");
+        } else if (m == 0xC6 || m == 0xCE || m == 0xC5 || m == 0xCD) {
+            FAA_NO("hierarchical coding");
+        } else if (m == 0xC3 || m == 0xC7 || m == 0xCB || m == 0xCF) {
+            FAA_NO("lossless coding");
+        } else if (m == 0xC9 || m == 0xCC) {
+            FAA_NO("arithmetic coding");
+        } else if (m == 0xC8) {
+            FAA_NO("JPG extension frame");
+        } else if (m == 0xDC) {
+            FAA_NO("DNL marker");
+        } else if (m == 0xC4) {                          // DHT (the checks of parse_jpeg)
+            int k = 0;
+            while (k < n) {
+                if (k + 17 > n) FAA_BAD("Huffman table cut off");
+                const int tc = p[k] >> 4, th = p[k] & 15;
+                if (tc > 1 || th > 3) FAA_BAD("Huffman table class or index out of range");
+                int total = 0;
+                unsigned code = 0;
+                for (int l = 0; l < 16; ++l) {
+                    total += p[k + 1 + l];
+                    code = (code + p[k + 1 + l]);
+                    if (code >= (1u << (l + 1))) FAA_BAD("Huffman table with more codes than its lengths allow");
+                    code <<= 1;
+                }
+                if (total > 256 || k + 17 + total > n) FAA_BAD("Huffman table symbol count out of range");
+                if (tc == 0)
+                    for (int s = 0; s < total; ++s)
+                        if (p[k + 17 + s] > 15) FAA_BAD("DC Huffman symbol above 15");
+                dht_at[tc][th] = (int32_t)(p + k + 1 - b);
+                k += 17 + total;
+            }
+        } else if (m == 0xDB) {                          // DQT
+            int k = 0;
+            while (k < n) {
+                const int pq = p[k] >> 4, tq = p[k] & 15;
+                if (pq > 1 || tq > 3) FAA_BAD("quantisation table precision or index out of range");
+                if (k + 1 + 64 * (pq + 1) > n) FAA_BAD("quantisation table cut off");
+                dqt_at[tq] = (int32_t)(p + k + 1 - b); dqt_prec[tq] = pq;
+                k += 1 + 64 * (pq + 1);
+            }
+        } else if (m == 0xDD) {                          // DRI: in force from the next SOS on
+            if (n < 2) FAA_BAD("restart interval segment too short");
+            restart = jpeg_u16(p);
+        } else if (m == 0xE0) {
+            if (n >= 14 && p[0] == 'J' && p[1] == 'F' && p[2] == 'I' && p[3] == 'F' && p[4] == 0) jfif = true;
+        } else if (m == 0xEE) {
+            if (n >= 12 && p[0] == 'A' && p[1] == 'd' && p[2] == 'o' && p[3] == 'b' && p[4] == 'e') {
+                adobe = true; adobe_transform = p[11];
+            }
+        } else if (m == 0xDA) {                          // SOS
+            if (!have_sof) FAA_BAD("scan before the frame header");
+            if (n < 1) FAA_BAD("scan header too short");
+            const int ns = p[0];
+            if (ns < 1 || ns > h.ncomp || n != 4 + 2 * ns) FAA_BAD("scan header length does not match its components");
+            if (*n_scans >= max_scans) FAA_NO("more scans than the decoder takes (64)");
+            JpegScan& sc = scans[*n_scans];
+            memset(&sc, 0, sizeof sc);
+            for (int k = 0; k < 3; ++k) { sc.comp[k] = -1; sc.dc_at[k] = sc.ac_at[k] = -1; }
+            for (int k = 0; k < 6; ++k) sc.pool[k] = -1;
+            sc.ns = ns;
+            const uint8_t* q = p + 1 + 2 * ns;
+            sc.ss = q[0]; sc.se = q[1]; sc.ah = q[2] >> 4; sc.al = q[2] & 15;
+            // the parameter checks of libjpeg's progressive decoder (it refuses these files too)
+            if (sc.ss == 0 ? sc.se != 0 : ns != 1) FAA_BAD("bad progression: a DC scan with AC coefficients or an AC scan of several components");
+            if (sc.se > 63 || sc.ss > sc.se) FAA_BAD("bad progression: spectral band out of range");
+            if (sc.al > 13) FAA_BAD("bad progression: Al above 13");
+            if (sc.ah != 0 && sc.ah != sc.al + 1) FAA_BAD("bad progression: Ah is neither 0 nor Al + 1");
+            int prev = -1;
+            for (int k = 0; k < ns; ++k) {
+                int c = 0;
+                while (c < h.ncomp && comp_id[c] != p[1 + 2 * k]) ++c;
+                if (c == h.ncomp) FAA_BAD("scan names a component the frame does not have");
+                if (c <= prev) FAA_NO("scan components out of frame order");
+                prev = c;
+                sc.comp[k] = c;
+                const int td = p[2 + 2 * k] >> 4, ta = p[2 + 2 * k] & 15;
+                if (td > 3 || ta > 3) FAA_BAD("Huffman table index out of range");
+                if (sc.ss == 0 && sc.ah == 0) {
+                    sc.dc_at[k] = dht_at[0][td] >= 0 ? dht_at[0][td] : td < 2 ? kJpegStdAt - td : -1;
+                    if (sc.dc_at[k] == -1) FAA_BAD("scan uses an undefined Huffman table");
+                } else if (sc.ss > 0) {
+                    sc.ac_at[k] = dht_at[1][ta] >= 0 ? dht_at[1][ta] : ta < 2 ? kJpegStdAt - 2 - ta : -1;
+                    if (sc.ac_at[k] == -1) FAA_BAD("scan uses an undefined Huffman table");
+                }
+                if (h.table_at[c] < 0) {                 // the quantisation table is latched at the first scan
+                    if (dqt_at[comp_q[c]] < 0) FAA_BAD("component uses an undefined quantisation table");
+                    h.table_at[c] = dqt_at[comp_q[c]];
+                    if (dqt_prec[comp_q[c]]) h.qprec |= 1 << c;
+                }
+                // the progression: libjpeg decodes these with a warning; refused here
+                if (sc.ss > 0 && bitpos[c][0] < 0) FAA_NO("bad progression: AC before the component's first DC scan");
+                for (int z = sc.ss; z <= sc.se; ++z) {
+                    if (sc.ah == 0 && bitpos[c][z] >= 0) FAA_NO("bad progression: a second first pass over a coefficient");
+                    if (sc.ah != 0 && bitpos[c][z] != sc.ah) FAA_NO("bad progression: a refinement whose Ah is not the coefficient's bit position");
+                    bitpos[c][z] = sc.al;
+                }
+            }
+            sc.restart = restart;
+            size_t s = seg_end, e = s;
+            while (e < len) {
+                if (b[e] != 0xFF) { ++e; continue; }
+                size_t f = e + 1;
+                while (f < len && b[f] == 0xFF) ++f;
+                if (f >= len) break;
+                if (b[f] == 0x00 || (b[f] >= 0xD0 && b[f] <= 0xD7)) { e = f + 1; continue; }
+                break;
+            }
+            if (e > len) e = len;
+            sc.off = (int64_t)s; sc.len = (int64_t)(e - s);
+            ++*n_scans;
+            i = e;
+            continue;
+        }
+        i = seg_end;
+    }
+    if (!have_sof) FAA_BAD("no progressive frame header");
+    if (*n_scans == 0) FAA_BAD("no scan");
+    for (int c = 0; c < h.ncomp; ++c)
+        for (int z = 0; z < 64; ++z)
+            if (bitpos[c][z] != 0) FAA_NO("incomplete progression (a coefficient does not end at bit 0)");
+    if (h.ncomp == 3) {
+        if (!jfif && adobe && adobe_transform == 0) FAA_NO("Adobe-transformed RGB (APP14 transform 0)");
+        if (!jfif && !adobe && comp_id[0] == 'R' && comp_id[1] == 'G' && comp_id[2] == 'B') FAA_NO("RGB components");
+        const bool ok = comp_h[1] == 1 && comp_v[1] == 1 && comp_h[2] == 1 && comp_v[2] == 1 &&
+                        ((comp_h[0] == 1 && comp_v[0] == 1) || (comp_h[0] == 2 && comp_v[0] == 1) ||
+                         (comp_h[0] == 2 && comp_v[0] == 2));
+        if (!ok) FAA_NO("sampling factors other than 4:4:4, 4:2:2 (2x1) or 4:2:0 (2x2)");
+        h.hs = comp_h[0]; h.vs = comp_v[0];
+    } else {
+        h.hs = h.vs = 1;
+    }
+    h.mcu_x = (h.w + 8 * h.hs - 1) / (8 * h.hs);
+    h.mcu_y = (h.h + 8 * h.vs - 1) / (8 * h.vs);
+    jpeg_scan_waves(scans, *n_scans);
+    return JPARSE_OK;
+#undef FAA_BAD
+#undef FAA_NO
+}
+
+// the quantisation tables of a progressive header (out[0, 3)) and the Huffman tables of its scans (out[3 + 6 s + k]:
+// DC of comp[k] at k, AC at 3), in pool form, unused slots zeroed
+inline void jpeg_progressive_tables(const uint8_t* b, const JpegHeader& h, const JpegScan* scans, int n, JpegTable* out) {
+    memset(out, 0, (size_t)(3 + 6 * n) * sizeof(JpegTable));
+    for (int c = 0; c < h.ncomp; ++c) {
+        const uint8_t* q = b + h.table_at[c];
+        for (int k = 0; k < 64; ++k) out[c].q[kJpegZigzag[k]] = (h.qprec >> c & 1) ? (uint16_t)jpeg_u16(q + 2 * k) : q[k];
+    }
+    for (int s = 0; s < n; ++s)
+        for (int k = 0; k < 6; ++k) {
+            const int32_t at = k < 3 ? scans[s].dc_at[k] : scans[s].ac_at[k - 3];
+            if (at == -1) continue;
+            const uint8_t* std_table = jpeg_std_huff(at);
+            const uint8_t* d = std_table ? std_table : b + at;
+            JpegTable& t = out[3 + 6 * s + k];
+            int total = 0;
+            for (int l = 0; l < 16; ++l) { t.bits[l] = d[l]; total += d[l]; }
+            memcpy(t.vals, d + 16, (size_t)total);
+        }
+}
+
+// Block extent of component c in a scan of that component alone (T.81 A.2): ceil(comp_w / 8) x ceil(comp_h / 8)
+FAA_JHD int jpeg_comp_bw(const JpegHeader& h, int c) { return ((c == 0 ? h.w : jpeg_chroma_w(h)) + 7) / 8; }
+FAA_JHD int jpeg_comp_bh(const JpegHeader& h, int c) { return ((c == 0 ? h.h : jpeg_chroma_h(h)) + 7) / 8; }
+// units of a scan: the frame's MCUs (interleaved) or the component's blocks (one component)
+FAA_JHD int64_t jpeg_scan_units(const JpegHeader& h, const JpegScan& s) {
+    return s.ns > 1 ? jpeg_mcus(h) : (int64_t)jpeg_comp_bw(h, s.comp[0]) * jpeg_comp_bh(h, s.comp[0]);
+}
+FAA_JHD int64_t jpeg_scan_segments(const JpegHeader& h, const JpegScan& s) {
+    return s.restart > 0 ? (jpeg_scan_units(h, s) + s.restart - 1) / s.restart : 1;
+}
+// block index (within the image's coefficient buffer) of block (bx, by) of component c's padded grid
+FAA_JHD int64_t jpeg_comp_block(const JpegHeader& h, int c, int64_t bx, int64_t by) {
+    if (c == 0) return by * ((int64_t)h.mcu_x * h.hs) + bx;
+    return jpeg_plane_blocks(h, 0) + (int64_t)(c - 1) * jpeg_mcus(h) + by * h.mcu_x + bx;
+}
+
+FAA_JHD uint32_t jpeg_bit(JpegBits& r) {
+    if (r.n < 1) jpeg_fill(r);
+    return jpeg_get(r, 1);
+}
+
+// Decodes units [u0, u1) of scan s (a restart segment: its data from `data`, EOBRUN and predictors zero) of the scan
+// bytes [lo, end) into coef, accumulating into what earlier waves wrote.  huff[k]: the table of slot k
+// (jpeg_scan_tables).  Stops at the first error; returns JpegStatus.
+FAA_JHD int jpeg_prog_segment(const JpegHeader& h, const JpegScan& s, const JpegHuff* const* huff, const uint8_t* lo,
+                              const uint8_t* data, const uint8_t* end, int64_t u0, int64_t u1, int16_t* coef) {
+    JpegBits r;
+    jpeg_bits_init(r, lo, data, end);
+    int pred[3] = {0, 0, 0};
+    int eobrun = 0;
+    const int p1 = 1 << s.al, m1 = -p1;
+    const int bw = s.ns == 1 ? jpeg_comp_bw(h, s.comp[0]) : 1;
+    for (int64_t u = u0; u < u1; ++u) {
+        if (s.ss == 0) {                                 // DC: every block of the MCU (one block without interleaving)
+            for (int k = 0; k < s.ns; ++k) {
+                const int c = s.comp[k];
+                const int hc = s.ns == 1 || c > 0 ? 1 : h.hs, vc = s.ns == 1 || c > 0 ? 1 : h.vs;
+                const int64_t ux = s.ns == 1 ? u % bw : (u % h.mcu_x) * hc, uy = s.ns == 1 ? u / bw : (u / h.mcu_x) * vc;
+                for (int b = 0; b < hc * vc; ++b) {
+                    int16_t* blk = coef + 64 * jpeg_comp_block(h, c, ux + b % hc, uy + b / hc);
+                    jpeg_fill(r);
+                    if (s.ah == 0) {
+                        int t = jpeg_decode(r, *huff[k]);
+                        if (t < 0) return JPEG_BAD_CODE;
+                        if (t) t = jpeg_extend(jpeg_get(r, t), t);
+                        pred[k] += t;
+                        blk[0] = (int16_t)(int32_t)((uint32_t)pred[k] << s.al);
+                    } else if (jpeg_get(r, 1)) {
+                        blk[0] = (int16_t)(blk[0] | p1);
+                    }
+                }
+            }
+        } else {
+            int16_t* blk = coef + 64 * jpeg_comp_block(h, s.comp[0], u % bw, u / bw);
+            int k = s.ss;
+            if (s.ah == 0) {                             // AC first pass
+                if (eobrun > 0) {
+                    --eobrun;
+                } else {
+                    for (; k <= s.se; ++k) {
+                        jpeg_fill(r);
+                        const int rs = jpeg_decode(r, *huff[0]);
+                        if (rs < 0) return JPEG_BAD_CODE;
+                        const int run = rs >> 4, sz = rs & 15;
+                        if (sz) {
+                            k += run;
+                            if (k > s.se) return JPEG_BAD_COEF;
+                            blk[jpeg_zigzag(k)] = (int16_t)(int32_t)((uint32_t)jpeg_extend(jpeg_get(r, sz), sz) << s.al);
+                        } else if (run == 15) {
+                            // (libjpeg lets a ZRL run past Se end the band; no encoder writes one, so it is reported
+                            // as BAD_COEF here, as the baseline decoder reports one past coefficient 63)
+                            k += 15;
+                            if (k > s.se) return JPEG_BAD_COEF;
+                        } else {
+                            eobrun = 1 << run;
+                            if (run) eobrun += (int)jpeg_get(r, run);
+                            --eobrun;
+                            break;
+                        }
+                    }
+                }
+            } else {                                     // AC refinement (libjpeg's decode_mcu_AC_refine)
+                if (eobrun == 0) {
+                    for (; k <= s.se; ++k) {
+                        jpeg_fill(r);
+                        const int rs = jpeg_decode(r, *huff[0]);
+                        if (rs < 0) return JPEG_BAD_CODE;
+                        int run = rs >> 4, val = 0;
+                        if (rs & 15) {                   // (a size other than 1 is decoded as 1, as libjpeg does)
+                            val = jpeg_get(r, 1) ? p1 : m1;
+                        } else if (run != 15) {
+                            eobrun = 1 << run;
+                            if (run) eobrun += (int)jpeg_get(r, run);
+                            break;
+                        }
+                        // correction bits of the nonzero coefficients passed; stop at the run's last zero
+                        for (; k <= s.se; ++k) {
+                            int16_t& v = blk[jpeg_zigzag(k)];
+                            if (v != 0) {
+                                if (jpeg_bit(r) && (v & p1) == 0) v = (int16_t)(v >= 0 ? v + p1 : v + m1);
+                            } else if (--run < 0) {
+                                break;
+                            }
+                        }
+                        // (a run past Se: libjpeg ends the band, or writes the new coefficient at natural index 63;
+                        // no encoder writes either, so it is reported as BAD_COEF)
+                        if (k > s.se) return JPEG_BAD_COEF;
+                        if (val) blk[jpeg_zigzag(k)] = (int16_t)val;
+                    }
+                }
+                if (eobrun > 0) {                        // in an EOB run: correction bits of the band's rest
+                    for (; k <= s.se; ++k) {
+                        int16_t& v = blk[jpeg_zigzag(k)];
+                        if (v != 0 && jpeg_bit(r) && (v & p1) == 0) v = (int16_t)(v >= 0 ? v + p1 : v + m1);
+                    }
+                    --eobrun;
+                }
+            }
+        }
+        if (r.n < r.fake) return JPEG_TRUNCATED;        // this unit used bits past the data
+    }
+    return JPEG_OK;
+}
+
+// The progressive kernel's entropy work on the host, one scan after another in file order (waves are an order the
+// kernel may use instead: they give the same coefficients).  coef: jpeg_image_blocks(h) blocks, zeroed here.  tabs: the
+// scans' tables in jpeg_progressive_tables' layout.  Returns JpegStatus bits.
+inline int jpeg_progressive_entropy_host(const uint8_t* file, const JpegHeader& h, const JpegScan* scans, int n,
+                                         const JpegTable* tabs, int16_t* coef) {
+    memset(coef, 0, (size_t)jpeg_image_blocks(h) * 128);
+    int status = 0;
+    JpegHuff* huffs = new JpegHuff[3];
+    for (int i = 0; i < n; ++i) {
+        const JpegScan& s = scans[i];
+        const JpegHuff* hp[3] = {&huffs[0], &huffs[1], &huffs[2]};
+        for (int k = 0; k < jpeg_scan_tables(s); ++k) jpeg_huff_build(tabs[3 + 6 * i + (s.ss == 0 ? k : 3)], huffs[k]);
+        const uint8_t* scan = file + s.off;
+        const uint8_t* end = scan + s.len;
+        const int64_t n_seg = jpeg_scan_segments(h, s), units = jpeg_scan_units(h, s);
+        int32_t* at = new int32_t[(size_t)n_seg];
+        for (int64_t k = 0; k < n_seg; ++k) at[k] = k ? -1 : 0;
+        if (n_seg > 1) {
+            JpegBits r; jpeg_bits_init(r, scan, scan, end);
+            if (jpeg_markers(r, scan, 0, s.len, s.len, at, 1, n_seg) != n_seg - 1) status |= JPEG_BAD_RESTART;
+        }
+        for (int64_t k = 0; k < n_seg; ++k) {
+            const int64_t u0 = k * (n_seg > 1 ? s.restart : 0), u1 = n_seg == 1 ? units : (u0 + s.restart < units ? u0 + s.restart : units);
+            status |= jpeg_prog_segment(h, s, hp, scan, at[k] < 0 ? end : scan + at[k], end, u0, u1, coef);
+        }
+        delete[] at;
+    }
+    delete[] huffs;
+    return status;
+}
+
+// The whole decode of one progressive file on the host (the progressive entropy kernel, then the reconstruct kernel).
+// out: h.h * h.w * 3 bytes; coef_out: the coefficients, when given.  Returns JpegStatus bits.
+inline int jpeg_decode_progressive_host(const uint8_t* file, const JpegHeader& h, const JpegScan* scans, int n,
+                                        const JpegTable* tabs, uint8_t* out, int16_t* coef_out = nullptr) {
+    const int64_t nblk = jpeg_image_blocks(h);
+    int16_t* coef = new int16_t[(size_t)nblk * 64];
+    const int status = jpeg_progressive_entropy_host(file, h, scans, n, tabs, coef);
+    if (coef_out) memcpy(coef_out, coef, (size_t)nblk * 128);
+    jpeg_reconstruct_host(h, tabs, coef, out);
     delete[] coef;
     return status;
 }

@@ -163,5 +163,19 @@ struct JpegDecodeParams {
 cudaError_t launch_jpeg_entropy(const JpegDecodeParams& p, cudaStream_t stream);
 cudaError_t launch_jpeg_reconstruct(const JpegDecodeParams& p, int n_tiles, cudaStream_t stream);
 cudaError_t launch_jpeg_index(const JpegDecodeParams& p, cudaStream_t stream);
+// progressive entropy decode (faa_jpeg_decode_progressive): one CTA per image; the reconstruct kernel follows it
+struct JpegProgressiveParams {
+    const JpegHeader* hdrs;     // [batch] (device copy)
+    const JpegTable* pool;
+    const uint8_t* src;
+    const JpegJob* jobs;        // [batch + 1]; seg: first entry of the image's segment starts (all its scans)
+    const JpegScan* scans;      // image i's scans are scans[scan_first[i], scan_first[i + 1])
+    const int64_t* scan_first;
+    int16_t* coef;
+    int32_t* segs;
+    int32_t* status;
+    int32_t batch;
+};
+cudaError_t launch_jpeg_progressive(const JpegProgressiveParams& p, cudaStream_t stream);
 
 }  // namespace faa

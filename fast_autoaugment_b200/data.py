@@ -585,10 +585,11 @@ class RaggedDeviceDataset:
 
 class EncodedDeviceDataset:
     """``RaggedDeviceDataset`` of JPEG files: the files' bytes stay on the device (``EncodedImages``, headers parsed
-    once here) and every batch is decoded on the device before its chain runs."""
+    once here) and every batch is decoded on the device before its chain runs.  ``progressive``: progressive files
+    are taken too (``EncodedImages.from_bytes(..., progressive=True)``)."""
 
-    def __init__(self, files, targets, device="cuda"):
-        self.images = files if isinstance(files, EncodedImages) else EncodedImages.from_bytes(files, device)
+    def __init__(self, files, targets, device="cuda", progressive=False):
+        self.images = files if isinstance(files, EncodedImages) else EncodedImages.from_bytes(files, device, progressive)
         self.targets = [int(t) for t in targets]
         if len(self.targets) != len(self.images):
             raise ValueError("need one target per image")
@@ -699,14 +700,16 @@ class JpegFileDataset:
     the device.  ``GpuAugmentedLoader`` streams each batch's files through a ``FileBatchStream``.  ``index``: a
     ``JpegIndex`` of the files, whose scan indexes let the device decode each listed file on many threads.  ``learn``:
     the loaders enter into ``index`` (which it needs) the scan index of every file they decode serially, so the next
-    epoch decodes it on many threads; subsets share the index, and ``index.save`` writes it."""
+    epoch decodes it on many threads; subsets share the index, and ``index.save`` writes it.  ``progressive``: the
+    loaders decode progressive files on the device instead of with Pillow (``read_jpeg_batch``)."""
 
-    def __init__(self, paths, targets, device="cuda", index=None, learn=False):
+    def __init__(self, paths, targets, device="cuda", index=None, learn=False, progressive=False):
         if learn and index is None:
             raise ValueError("learn needs an index to enter the files' points into (JpegIndex.empty)")
         self.paths = [os.fspath(p) for p in paths]
         self.index = index
         self.learn = bool(learn)
+        self.progressive = bool(progressive)
         self.targets = [int(t) for t in targets]
         if len(self.targets) != len(self.paths):
             raise ValueError("need one target per image")
@@ -724,7 +727,7 @@ class JpegFileDataset:
         idx = [int(i) for i in idx]
         d = JpegFileDataset.__new__(JpegFileDataset)
         d.paths = self.select(idx)
-        d.index, d.learn = self.index, self.learn
+        d.index, d.learn, d.progressive = self.index, self.learn, self.progressive
         d.targets = [self.targets[i] for i in idx]
         d.labels = self.labels.index_select(0, torch.as_tensor(idx, dtype=torch.int64, device=self.labels.device))
         d.device = self.device
@@ -752,12 +755,16 @@ class HostBatch:
     table ``pool`` of the files the device decoder takes (headers' ``offset`` places those files back to back, as
     ``EncodedImages.from_bytes`` of them would); the batch positions of those files (``accepted``) and of the rest
     (``refused``), and Pillow's pixels of the refused ones (``pixels``, uint8 [h, w, 3]); with an index, the accepted
-    files' scan indexes (``first``, ``points``, as ``EncodedImages`` carries them; otherwise None)."""
+    files' scan indexes (``first``, ``points``, as ``EncodedImages`` carries them; otherwise None); when progressive
+    files were accepted, the accepted files' scans (``scans``, ``scan_first``, as ``EncodedImages`` carries them;
+    otherwise None)."""
 
-    def __init__(self, paths, files, headers, pool, accepted, refused, pixels, first=None, points=None):
+    def __init__(self, paths, files, headers, pool, accepted, refused, pixels, first=None, points=None, scans=None,
+                 scan_first=None):
         self.paths, self.files, self.headers, self.pool = paths, files, headers, pool
         self.accepted, self.refused, self.pixels = accepted, refused, pixels
         self.first, self.points = first, points
+        self.scans, self.scan_first = scans, scan_first
 
     def sizes(self):
         """(h, w) of every image of the batch, int32 [N, 2]"""
@@ -768,13 +775,18 @@ class HostBatch:
         return s
 
 
-def read_jpeg_batch(paths, map=map, index=None):
+def read_jpeg_batch(paths, map=map, index=None, progressive=False):
     """Read a batch of files and parse their headers (``parse_jpeg_headers``); decode the files the device decoder
     refuses with Pillow; with a ``JpegIndex``, gather the accepted files' scan indexes.  No device is touched.  ``map``:
-    an executor's ``map`` reads, parses and decodes in parallel."""
+    an executor's ``map`` reads, parses and decodes in parallel.  ``progressive=True``: progressive files are accepted
+    with their scans instead of decoded by Pillow."""
     paths = list(paths)
     files = list(map(_read_file, paths))
-    headers, pool, refused = parse_jpeg_headers(files, map)
+    scans = scan_first = None
+    if progressive:
+        headers, pool, refused, scans, scan_first = parse_jpeg_headers(files, map, progressive=True)
+    else:
+        headers, pool, refused = parse_jpeg_headers(files, map)
     bad = np.array([i for i, _ in refused], np.int64)
     ok = np.setdiff1d(np.arange(len(files), dtype=np.int64), bad)
     lengths = np.array([len(files[i]) for i in ok], np.int64)
@@ -784,7 +796,11 @@ def read_jpeg_batch(paths, map=map, index=None):
     first = points = None
     if index is not None:
         first, points = index.gather([paths[i] for i in ok], lengths)
-    return HostBatch(paths, [files[i] for i in ok], headers, pool, ok, bad, pixels, first, points)
+    if scans is not None and len(scans):
+        scan_first = np.concatenate([scan_first[ok], scan_first[-1:]]).astype(np.int64)
+    else:
+        scans = scan_first = None
+    return HostBatch(paths, [files[i] for i in ok], headers, pool, ok, bad, pixels, first, points, scans, scan_first)
 
 
 def chunked_map(pool_map, n_chunks):
@@ -805,7 +821,8 @@ def _up16(n):
 class _Layout:
     """Byte layout of one staged batch, the same in the pinned slot and in the batch's device buffer: headers, table
     pool, the accepted files back to back, the refused files' pixels, then (with an index) the accepted files' point
-    offsets and points, each part on a 16-byte boundary."""
+    offsets and points, then (with progressive files) their scan offsets and scans, each part on a 16-byte boundary.
+    A batch without progressive files has the layout it would have without the option."""
 
     def __init__(self, hb: HostBatch):
         self.pool = _up16(hb.headers.nbytes)
@@ -821,6 +838,12 @@ class _Layout:
             self.points = _up16(at + hb.first.nbytes)
             self.points_end = self.points + hb.points.nbytes
             at = _up16(self.points_end)
+        self.scan_first = self.scans = self.scans_end = None
+        if hb.scans is not None:
+            self.scan_first = at
+            self.scans = _up16(at + hb.scan_first.nbytes)
+            self.scans_end = self.scans + hb.scans.nbytes
+            at = _up16(self.scans_end)
         self.total = max(at, 16)
 
     def pack(self, hb: HostBatch, buf):
@@ -835,6 +858,9 @@ class _Layout:
         if self.first is not None:
             buf[self.first:self.first + hb.first.nbytes] = hb.first.view(np.uint8)
             buf[self.points:self.points_end] = hb.points.view(np.uint8).reshape(-1)
+        if self.scans is not None:
+            buf[self.scan_first:self.scan_first + hb.scan_first.nbytes] = hb.scan_first.view(np.uint8)
+            buf[self.scans:self.scans_end] = hb.scans.view(np.uint8).reshape(-1)
 
 
 _STATUS_BITS = ((_lib.JPEG_TRUNCATED, "scan truncated"), (_lib.JPEG_BAD_CODE, "bad Huffman code"),
@@ -855,22 +881,25 @@ class FileBatchStream:
     batch's scan indexes travel in the same slot and the decode uses them.  With ``learn`` as well, every batch is
     decoded in recording mode (``decode_jpeg(record=True)``): its point counts and the points they cover are copied to
     pinned memory behind the decode with its status, and at the same check the files that got points are entered into
-    the index (``JpegIndex.add``), so the batches read after that decode them on many threads."""
+    the index (``JpegIndex.add``), so the batches read after that decode them on many threads.  With ``progressive``,
+    progressive files are decoded on the device too: their scans travel in the same slot."""
 
     SLOTS = 2
     WORKERS = 2
 
-    def __init__(self, workers=None, index=None, learn=False):
+    def __init__(self, workers=None, index=None, learn=False, progressive=False):
         if learn and index is None:
             raise ValueError("learn needs an index")
         self.workers = int(workers or self.WORKERS)
         self.index = index
         self.learn = bool(learn)
+        self.progressive = bool(progressive)
         self.slots = [None] * self.SLOTS           # pinned uint8 staging buffers
         self.copied = [None] * self.SLOTS          # event recorded after each slot's last host-to-device copy
 
     def _stage(self, paths, slot, pool, dev):
-        hb = read_jpeg_batch(paths, chunked_map(pool.map, self.workers) if self.workers > 1 else map, self.index)
+        hb = read_jpeg_batch(paths, chunked_map(pool.map, self.workers) if self.workers > 1 else map, self.index,
+                             self.progressive)
         lay = _Layout(hb)
         if self.copied[slot] is not None:
             self.copied[slot].synchronize()
@@ -890,6 +919,9 @@ class FileBatchStream:
                 index = dict(first=hb.first, points=hb.points,
                              _d_first=dbuf[lay.first:lay.first + hb.first.nbytes].view(torch.int64),
                              _d_points=dbuf[lay.points:lay.points_end])
+            if hb.scans is not None:
+                index.update(scans=hb.scans, scan_first=hb.scan_first, _d_scans=dbuf[lay.scans:lay.scans_end],
+                             _d_scan_first=dbuf[lay.scan_first:lay.scan_first + hb.scan_first.nbytes].view(torch.int64))
             enc = EncodedImages(dbuf[lay.files:lay.files_end], hb.headers, hb.pool, _d_pool=dbuf[lay.pool:lay.files],
                                 _d_headers=dbuf[:lay.pool], **index)
             learned = None
@@ -1008,7 +1040,8 @@ class GpuAugmentedLoader:
         if isinstance(self.dataset, JpegFileDataset):
             dev = self.dataset.device
             batches = [idx_all[k * self.batch_size:(k + 1) * self.batch_size] for k in range(len(self))]
-            self.staging = FileBatchStream(index=self.dataset.index, learn=self.dataset.learn)
+            self.staging = FileBatchStream(index=self.dataset.index, learn=self.dataset.learn,
+                                           progressive=self.dataset.progressive)
             files = self.staging([self.dataset.select(idx) for idx in batches], dev)
         else:
             dev = self.dataset.images.device
@@ -1227,7 +1260,9 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
     enter the scan index of every file they decode serially, so from the second epoch on the files the loaders have
     seen are decoded on many threads, with the same pixels; the train and valid loaders share what they learn
     (``trainloader.dataset.index.save(path)`` writes it as ``faa_jpeg_index`` reads it).  It costs host memory: 16
-    bytes a point, about 1.7 KB a file at ImageNet's mean file size."""
+    bytes a point, about 1.7 KB a file at ImageNet's mean file size.  ``faa_jpeg_progressive`` (default False): the
+    train, valid, test and ``tta`` loaders decode progressive JPEG files on the device, bit-exact with Pillow, instead of
+    with Pillow on the host; files whose progression is incomplete still go to Pillow.  They get no scan index."""
     from sklearn.model_selection import StratifiedShuffleSplit
 
     conf = C.get()
@@ -1252,6 +1287,7 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
 
     index_dir = conf.get("faa_jpeg_index")
     learn = bool(conf.get("faa_jpeg_index_learn", False))
+    progressive = bool(conf.get("faa_jpeg_progressive", False))
 
     def device_dataset(x, y):
         if isinstance(x, FilePaths):
@@ -1264,9 +1300,9 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
                 index = JpegIndex.load(path, x.folder)
             if learn and index is None:
                 index = JpegIndex.empty(x.folder)
-            return JpegFileDataset(x, y, index=index, learn=learn)
+            return JpegFileDataset(x, y, index=index, learn=learn, progressive=progressive)
         if isinstance(x, list) and len(x) and isinstance(x[0], bytes):
-            return EncodedDeviceDataset(x, y)
+            return EncodedDeviceDataset(x, y, progressive=progressive)
         return RaggedDeviceDataset(x, y) if isinstance(x, list) else DeviceDataset(x, y)
     if dataset in ("cifar10", "cifar100", "svhn", "imagenet"):
         total_trainset, testset = device_dataset(tr_x, tr_y), device_dataset(te_x, te_y)

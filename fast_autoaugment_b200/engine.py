@@ -580,27 +580,79 @@ def parse_jpeg(f):
     return hdr, tabs
 
 
-def parse_jpeg_headers(files, map=map):
+def parse_jpeg_progressive(f):
+    """(header [1], its tables ``JPEG_TABLE_DTYPE`` [3 + 6 S], its scans ``JPEG_SCAN_DTYPE`` [S]) of one progressive
+    file (C ABI ``faa_jpeg_parse_progressive`` + ``faa_jpeg_scan_tables``): tables [0, 3) are the components'
+    quantisation tables, 3 + 6 s + k slot k of scan s.  (None, reason, None) when the decoder does not take it."""
+    hdr = np.zeros(1, dtype=_lib.JPEG_HEADER_DTYPE)
+    scans = np.zeros(_lib.JPEG_MAX_SCANS, dtype=_lib.JPEG_SCAN_DTYPE)
+    n = C.c_int(0)
+    if lib.faa_jpeg_parse_progressive(f, len(f), hdr.ctypes.data, scans.ctypes.data, len(scans), C.byref(n)) != _lib.OK:
+        return None, (lib.faa_last_error() or b"").decode(), None
+    scans = scans[:n.value].copy()
+    tabs = np.zeros(3 + 6 * len(scans), dtype=_lib.JPEG_TABLE_DTYPE)
+    check(lib.faa_jpeg_scan_tables(f, len(f), hdr.ctypes.data, scans.ctypes.data, len(scans), tabs.ctypes.data))
+    return hdr, tabs, scans
+
+
+def _parse_any(f):
+    """``parse_jpeg``, and for a file it refuses as progressive ``parse_jpeg_progressive``: (header, tables, scans or
+    None), or (None, reason, None)"""
+    hdr, tabs = parse_jpeg(f)
+    if hdr is None and tabs.endswith(": progressive coding"):
+        return parse_jpeg_progressive(f)
+    return hdr, tabs, None
+
+
+def parse_jpeg_headers(files, map=map, progressive=False):
     """JPEG files (``bytes``) -> (headers [N], table pool, refused [(position, reason)]).  The tables the files use are
     deduplicated into the pool in order of first use, which the headers' ``pool`` slots index; a refused file's header
     row stays zero and adds nothing to the pool.  ``offset`` is left 0: the caller places the files.  ``map`` runs the
-    per-file parse (an executor's ``map`` parses files in parallel)."""
+    per-file parse (an executor's ``map`` parses files in parallel).
+
+    ``progressive=True`` also takes progressive files (``parse_jpeg_progressive``; their headers' ``reserved`` is
+    ``JPEG_PROGRESSIVE``), their scans' Huffman tables going into the same pool, and returns ``(headers, pool, refused,
+    scans, scan_first)``: ``JPEG_SCAN_DTYPE`` scans with pool slots set, file i's being
+    ``scans[scan_first[i]:scan_first[i + 1]]`` (none for the other files)."""
     headers = np.zeros(len(files), dtype=_lib.JPEG_HEADER_DTYPE)
     pool, index, refused = [], {}, []
-    for i, (hdr, tabs) in enumerate(map(parse_jpeg, files)):
+    scans, counts = [], np.zeros(len(files), np.int64)
+
+    def slot_of(t):
+        key = t.tobytes()
+        if key not in index:
+            index[key] = len(pool)
+            pool.append(t.copy())
+        return index[key]
+
+    for i, parsed in enumerate(map(_parse_any if progressive else parse_jpeg, files)):
+        hdr, tabs = parsed[0], parsed[1]
         if hdr is None:
             refused.append((i, tabs))
             continue
         headers[i] = hdr[0]
+        nc = int(hdr["ncomp"][0])
+        if progressive and parsed[2] is not None:
+            sc = parsed[2]
+            for c in range(nc):
+                headers["pool"][i, c] = slot_of(tabs[c])
+            for k in range(len(sc)):
+                for t in range(6):
+                    if (sc["dc_at"][k] if t < 3 else sc["ac_at"][k])[t % 3] != -1:
+                        sc["pool"][k, t] = slot_of(tabs[3 + 6 * k + t])
+            scans.append(sc)
+            counts[i] = len(sc)
+            continue
         for slot in range(9):
-            if slot % 3 >= int(hdr["ncomp"][0]):
+            if slot % 3 >= nc:
                 continue
-            key = tabs[slot].tobytes()
-            if key not in index:
-                index[key] = len(pool)
-                pool.append(tabs[slot].copy())
-            headers["pool"][i, slot] = index[key]
-    return headers, np.array(pool, dtype=_lib.JPEG_TABLE_DTYPE).reshape(-1), refused
+            headers["pool"][i, slot] = slot_of(tabs[slot])
+    pool = np.array(pool, dtype=_lib.JPEG_TABLE_DTYPE).reshape(-1)
+    if not progressive:
+        return headers, pool, refused
+    scan_first = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)
+    scans = np.concatenate(scans) if scans else np.zeros(0, _lib.JPEG_SCAN_DTYPE)
+    return headers, pool, refused, scans, scan_first
 
 
 class EncodedImages:
@@ -612,13 +664,17 @@ class EncodedImages:
 
     Optionally the files carry a scan index (``build_jpeg_index``): ``first`` (int64 [N + 1]) and ``points``
     (``JPEG_SYNC_DTYPE``), file i's points being ``points[first[i]:first[i + 1]]``.  ``decode_jpeg`` then decodes each
-    indexed file on many threads; the pixels and status are those of the decode without the index, whatever it holds."""
+    indexed file on many threads; the pixels and status are those of the decode without the index, whatever it holds.
+
+    Progressive files (``from_bytes(..., progressive=True)``) carry their scans the same way: ``scan_first`` (int64
+    [N + 1]) and ``scans`` (``JPEG_SCAN_DTYPE``), file i's being ``scans[scan_first[i]:scan_first[i + 1]]``; the other
+    files have none.  Without them every header must be a baseline one."""
 
     def __init__(self, storage: torch.Tensor, headers, pool, _d_pool=None, _d_headers=None, first=None, points=None,
-                 _d_first=None, _d_points=None):
-        """``_d_pool`` / ``_d_headers`` / ``_d_first`` / ``_d_points``: device copies of ``pool`` / ``headers`` /
-        ``first`` / ``points`` the caller already made (uint8 tensors of their bytes, ``first`` int64), used instead of
-        uploading them on first use"""
+                 _d_first=None, _d_points=None, scans=None, scan_first=None, _d_scans=None, _d_scan_first=None):
+        """``_d_pool`` / ``_d_headers`` / ``_d_first`` / ``_d_points`` / ``_d_scans`` / ``_d_scan_first``: device copies
+        of ``pool`` / ``headers`` / ``first`` / ``points`` / ``scans`` / ``scan_first`` the caller already made (uint8
+        tensors of their bytes, ``first`` and ``scan_first`` int64), used instead of uploading them on first use"""
         if not isinstance(storage, torch.Tensor) or storage.dtype != torch.uint8 or storage.dim() != 1 \
                 or not storage.is_contiguous():
             raise ValueError("storage must be a contiguous 1-D uint8 tensor")
@@ -637,17 +693,35 @@ class EncodedImages:
             f = self.first
             if len(f) != len(h) + 1 or f[0] != 0 or (np.diff(f) < 0).any() or f[-1] > len(self.points):
                 raise ValueError("first must be [N + 1] non-decreasing offsets from 0 into points")
+        if (scans is None) != (scan_first is None):
+            raise ValueError("scans need both scans and scan_first")
+        self.scans = self.scan_first = None
+        if scans is not None:
+            self.scans = np.ascontiguousarray(scans, dtype=_lib.JPEG_SCAN_DTYPE).reshape(-1)
+            self.scan_first = np.ascontiguousarray(scan_first, dtype=np.int64).reshape(-1)
+            f = self.scan_first
+            if len(f) != len(h) + 1 or f[0] != 0 or (np.diff(f) < 0).any() or f[-1] > len(self.scans):
+                raise ValueError("scan_first must be [N + 1] non-decreasing offsets from 0 into scans")
+        if self.scans is None and self.progressive().any():
+            raise ValueError("progressive files need their scans")
         self._d_pool = _d_pool
         self._d_headers = _d_headers
         self._d_first = _d_first
         self._d_points = _d_points
+        self._d_scans = _d_scans
+        self._d_scan_first = _d_scan_first
 
     @staticmethod
-    def from_bytes(files, device="cuda"):
+    def from_bytes(files, device="cuda", progressive=False):
         """JPEG files (``bytes``) -> EncodedImages on ``device``.  Raises ValueError naming every file the decoder
-        does not take (progressive, arithmetic, 12-bit, CMYK, other sampling, malformed ...) and why."""
+        does not take (progressive, arithmetic, 12-bit, CMYK, other sampling, malformed ...) and why.
+        ``progressive=True`` takes progressive files too (``parse_jpeg_headers``)."""
         files = [bytes(f) for f in files]
-        headers, pool, refused = parse_jpeg_headers(files)
+        scans = scan_first = None
+        if progressive:
+            headers, pool, refused, scans, scan_first = parse_jpeg_headers(files, progressive=True)
+        else:
+            headers, pool, refused = parse_jpeg_headers(files)
         if refused:
             raise ValueError("JPEG files the decoder does not take: " + "; ".join("%d: %s" % r for r in refused))
         lengths = np.array([len(f) for f in files], dtype=np.int64)
@@ -655,7 +729,7 @@ class EncodedImages:
         packed = np.frombuffer(b"".join(files), dtype=np.uint8)
         storage = torch.from_numpy(packed.copy()).to(device) if packed.size else torch.zeros(1, dtype=torch.uint8,
                                                                                               device=device)
-        return EncodedImages(storage, headers, pool)
+        return EncodedImages(storage, headers, pool, scans=scans, scan_first=scan_first)
 
     def __len__(self):
         return len(self.headers)
@@ -669,19 +743,22 @@ class EncodedImages:
         """(h, w) of every image, int32 [N, 2]"""
         return np.stack([self.headers["h"], self.headers["w"]], axis=1).astype(np.int32).reshape(-1, 2)
 
+    def progressive(self):
+        """bool [N]: which files are progressive"""
+        return self.headers["reserved"] == _lib.JPEG_PROGRESSIVE
+
     def with_index(self, first, points):
         """the same files carrying the scan index (first, points), e.g. ``build_jpeg_index``'s"""
-        return EncodedImages(self.storage, self.headers, self.pool, self.device_pool(), self._d_headers, first, points)
+        return EncodedImages(self.storage, self.headers, self.pool, self.device_pool(), self._d_headers, first, points,
+                             scans=self.scans, scan_first=self.scan_first, _d_scans=self._d_scans,
+                             _d_scan_first=self._d_scan_first)
 
     def select(self, idx):
         idx = np.asarray(idx, dtype=np.int64).reshape(-1)
-        first = points = None
-        if self.first is not None:
-            counts = np.diff(self.first)[idx]
-            first = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)
-            at = np.repeat(self.first[:-1][idx] - first[:-1], counts) + np.arange(int(first[-1]), dtype=np.int64)
-            points = self.points[at]
-        return EncodedImages(self.storage, self.headers[idx], self.pool, self.device_pool(), first=first, points=points)
+        first, points = _gather_ranges(self.first, self.points, idx)
+        scan_first, scans = _gather_ranges(self.scan_first, self.scans, idx)
+        return EncodedImages(self.storage, self.headers[idx], self.pool, self.device_pool(), first=first, points=points,
+                             scans=scans, scan_first=scan_first)
 
     def device_pool(self):
         """the table pool on the device (shared by every ``select`` of this set)"""
@@ -696,6 +773,15 @@ class EncodedImages:
             self._d_headers = torch.from_numpy(flat.copy() if flat.size else np.zeros(1, np.uint8)).to(self.device)
         return self._d_headers
 
+    def device_scans(self):
+        """(scans, scan_first) on the device: the scans' bytes and int64 [N + 1]"""
+        if self._d_scans is None:
+            flat = self.scans.view(np.uint8).reshape(-1)
+            self._d_scans = torch.from_numpy(flat.copy() if flat.size else np.zeros(112, np.uint8)).to(self.device)
+        if self._d_scan_first is None:
+            self._d_scan_first = torch.from_numpy(self.scan_first.copy()).to(self.device)
+        return self._d_scans, self._d_scan_first
+
     def device_index(self):
         """(first, points) on the device: int64 [N + 1] and the points' bytes"""
         if self._d_first is None:
@@ -706,12 +792,29 @@ class EncodedImages:
         return self._d_first, self._d_points
 
 
+def _gather_ranges(first, items, idx):
+    """(first, items) of the files ``idx`` of per-file ranges ``items[first[i]:first[i + 1]]`` (None, None: none)"""
+    if first is None:
+        return None, None
+    counts = np.diff(first)[idx]
+    out = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)
+    at = np.repeat(first[:-1][idx] - out[:-1], counts) + np.arange(int(out[-1]), dtype=np.int64)
+    return out, items[at]
+
+
 def build_jpeg_index(encoded: EncodedImages):
     """The scan index of every file of ``encoded`` (C ABI ``faa_jpeg_index_build``: one serial decode per file on the
     device, one thread per file): ``(first, points)``, int64 [N + 1] offsets into ``JPEG_SYNC_DTYPE`` points, file i's
     being ``points[first[i]:first[i + 1]]``.  Files with restart markers, scans under 2 KiB and files whose scan does
-    not decode cleanly get none.  Waits for the device."""
+    not decode cleanly get none, and so do progressive files.  Waits for the device."""
     _require_cuda(encoded.storage, "encoded")
+    prog = encoded.progressive()
+    if prog.any():
+        at = np.flatnonzero(~prog)
+        first, points = build_jpeg_index(encoded.select(at))
+        counts = np.zeros(len(encoded), np.int64)
+        counts[at] = np.diff(first)
+        return np.concatenate([[0], np.cumsum(counts)]).astype(np.int64), points
     dev = encoded.device
     B = len(encoded)
     if B == 0:
@@ -789,13 +892,65 @@ def decode_jpeg(encoded: EncodedImages, out: RaggedImages | None = None, record=
     ``(images, status, count, points, cap_first)``: ``count`` int32 [N] and ``points`` (uint8, the bytes of
     ``JPEG_SYNC_DTYPE`` points) CUDA tensors, file i's ``count[i]`` new points at point ``cap_first[i]``
     (``jpeg_index_capacities``, host int64 [N + 1]).  ``count[i] > 0`` means these are file i's points now;
-    ``compact_jpeg_index`` turns them into ``build_jpeg_index``'s form."""
+    ``compact_jpeg_index`` turns them into ``build_jpeg_index``'s form.
+
+    Progressive files (``EncodedImages.from_bytes(..., progressive=True)``) are decoded by
+    ``faa_jpeg_decode_progressive`` into the same images, the other files of the batch by the calls above (``select``
+    copies no byte of them); status comes back in batch order.  They get no scan index: count 0 with ``record=True``,
+    and points given to them are not used."""
     _require_cuda(encoded.storage, "encoded")
     dev = encoded.device
     if out is None:
         out = RaggedImages.empty(encoded.sizes, dev)
     elif not isinstance(out, RaggedImages) or not np.array_equal(out.sizes, encoded.sizes) or out.device != dev:
         raise ValueError("out must be a RaggedImages of the files' sizes on their device")
+    prog = encoded.progressive()
+    if not prog.any():
+        return _decode_baseline(encoded, out, record)
+    B = len(encoded)
+    at = np.flatnonzero(~prog)
+    pat = np.flatnonzero(prog)
+    # The progressive files' scans are contiguous in encoded.scans (the others have none), so their call reuses the
+    # device copy of every scan with offsets scan_first[pat] + [end].  One upload carries those offsets and the
+    # permutation that puts the two calls' status (and counts) back in batch order.
+    p_first = np.concatenate([encoded.scan_first[pat], encoded.scan_first[-1:]]).astype(np.int64)
+    inv = np.argsort(np.concatenate([at, pat]), kind="stable").astype(np.int64)
+    d_small = torch.from_numpy(np.concatenate([inv, p_first])).to(dev)
+    d_scans, _ = encoded.device_scans()
+    p_enc = EncodedImages(encoded.storage, encoded.headers[pat], encoded.pool, encoded.device_pool(),
+                          scans=encoded.scans, scan_first=p_first, _d_scans=d_scans, _d_scan_first=d_small[B:])
+    p_out = out.select(pat)
+    res = _decode_baseline(encoded.select(at), out.select(at), record) if len(at) else None
+    p_status = torch.empty(len(pat), dtype=torch.int32, device=dev)
+    h_out, d_out = p_out.descriptors()
+    with torch.cuda.device(dev):
+        check(lib.faa_jpeg_decode_progressive(
+            _decoder(dev).handle, p_enc.headers.ctypes.data, p_enc.device_headers().data_ptr(),
+            p_enc.device_pool().data_ptr(), len(p_enc.pool), p_enc.storage.data_ptr(), len(pat), h_out.ctypes.data,
+            d_out.data_ptr(), p_status.data_ptr(), p_enc.scans.ctypes.data, d_scans.data_ptr(), p_first.ctypes.data,
+            p_enc.device_scans()[1].data_ptr(), _stream_ptr(dev)))
+        status = p_status if res is None else torch.cat([res[1], p_status])[d_small[:B]]
+        if not record:
+            return out, status
+        # a progressive file's capacity is 0, so the baseline files' capacity layout is the batch's
+        cap_first = jpeg_index_capacities(encoded.headers)
+        if res is None:
+            return out, status, torch.zeros(B, dtype=torch.int32, device=dev), \
+                torch.empty(16, dtype=torch.uint8, device=dev), cap_first
+        count = torch.cat([res[2], torch.zeros(len(pat), dtype=torch.int32, device=dev)])[d_small[:B]]
+    return out, status, count, res[3], cap_first
+
+
+def _decoder(dev):
+    dec = _DECODERS.get(dev.index)
+    if dec is None:
+        dec = _DECODERS[dev.index] = _JpegDecoder()
+    return dec
+
+
+def _decode_baseline(encoded: EncodedImages, out: RaggedImages, record):
+    """``decode_jpeg`` of a batch without progressive files"""
+    dev = encoded.device
     B = len(encoded)
     status = torch.empty(max(B, 1), dtype=torch.int32, device=dev)[:B]
     if record:
@@ -806,9 +961,7 @@ def decode_jpeg(encoded: EncodedImages, out: RaggedImages | None = None, record=
         return (out, status, count, points, cap_first) if record else (out, status)
     h_out, d_out = out.descriptors()
     with torch.cuda.device(dev):
-        dec = _DECODERS.get(dev.index)
-        if dec is None:
-            dec = _DECODERS[dev.index] = _JpegDecoder()
+        dec = _decoder(dev)
         if record:
             d_first = d_points = None
             if encoded.first is not None:

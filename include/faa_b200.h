@@ -428,6 +428,54 @@ int faa_jpeg_decode_recording(faa_jpeg_decoder_t* dec, const faa_jpeg_header_t* 
                               const int64_t* h_cap_first, const int64_t* d_cap_first, faa_jpeg_sync_t* d_points_out,
                               int32_t* d_count, void* stream);
 
+/* ---- progressive JPEG decode (SOF2 Huffman), for callers that opt in: the files faa_jpeg_parse takes, coded
+ * progressively, bit-exact with Pillow as above.  The parse accepts a file only when every coefficient of every component
+ * ends at bit 0 (libjpeg smooths the blocks of an incomplete progression, which is not modelled), with at most
+ * FAA_JPEG_MAX_SCANS scans; multi-scan sequential, arithmetic coding and the rest stay refused.  Its header has
+ * reserved = FAA_JPEG_PROGRESSIVE, restart = 0 and no scan_off / scan_len, and its quantisation tables are those in force at
+ * each component's first scan.  faa_jpeg_decode, _indexed, _recording and faa_jpeg_index_build refuse such a header with
+ * FAA_ERR_VALUE, and faa_jpeg_index_capacity gives it 0: progressive files have no scan index. */
+#define FAA_JPEG_PROGRESSIVE 1
+#define FAA_JPEG_MAX_SCANS 64
+typedef struct faa_jpeg_scan {
+    int64_t off;              /* entropy-coded data: bytes [off, off + len) of the file                              */
+    int64_t len;
+    int32_t restart;          /* restart interval in force at its SOS, in units (MCUs, or blocks of a one-component scan) */
+    int32_t ns;               /* components in the scan: comp[0, ns), frame indices in frame order (-1 past ns)      */
+    int32_t comp[3];
+    int32_t ss, se, ah, al;   /* spectral band [ss, se] and successive approximation bits (ITU T.81 G.1.1.1)          */
+    int32_t wave;             /* 1 + the largest wave of an earlier scan that shares a component and a coefficient
+                                 (DC counts as coefficient 0): the scans of one wave are decoded concurrently         */
+    int32_t dc_at[3];         /* file offsets of the DC tables of comp[k] (DC first scans) and of the AC table (ac_at[0],
+                                 AC scans) as defined at its SOS; -2 - k for standard table k; -1 when unused          */
+    int32_t ac_at[3];
+    int32_t pool[6];          /* the same tables as pool indices: DC of comp[k] at k, AC at 3; -1 when unused        */
+    int32_t reserved[2];
+} faa_jpeg_scan_t;            /* 112 bytes */
+
+/* host only: parse a progressive file into its header and scans[0, *n_scans) (room for max_scans).  FAA_OK,
+ * FAA_ERR_UNSUPPORTED (not progressive, an incomplete progression, more scans than max_scans or FAA_JPEG_MAX_SCANS, or
+ * what faa_jpeg_parse refuses; reason in faa_last_error()) or FAA_ERR_VALUE (malformed header or progression). */
+int faa_jpeg_parse_progressive(const uint8_t* bytes, size_t len, faa_jpeg_header_t* out, faa_jpeg_scan_t* scans,
+                               int max_scans, int* n_scans);
+/* host only: the tables of a progressive file in pool form: out[c] (c < 3) the quantisation table of component c, and
+ * out[3 + 6 s + k] the Huffman tables of scan s (slot k as in faa_jpeg_scan_t::pool); unused slots zeroed.  out has
+ * 3 + 6 n_scans entries. */
+int faa_jpeg_scan_tables(const uint8_t* bytes, size_t len, const faa_jpeg_header_t* hdr, const faa_jpeg_scan_t* scans,
+                         int n_scans, faa_jpeg_table_t* out);
+/* decodes `batch` progressive files (inputs as faa_jpeg_decode; the headers' pool[0, ncomp) index the quantisation
+ * tables).  h_scans / d_scans: host and device copies of the scans, whose pool slots index d_tables; h_scan_first /
+ * d_scan_first: int64 [batch + 1] offsets, image i's scans being scans[first[i], first[i + 1]) (1 to FAA_JPEG_MAX_SCANS
+ * of them).  Everything, the waves included, is validated on the host before any device work.  d_status as
+ * faa_jpeg_decode's (a segment that fails stops there; the image still gets defined pixels).  Two launches (progressive
+ * entropy decode, the reconstruct kernel of faa_jpeg_decode), no host wait; the handle's scratch is shared with the
+ * other decode calls. */
+int faa_jpeg_decode_progressive(faa_jpeg_decoder_t* dec, const faa_jpeg_header_t* h_headers,
+                                const faa_jpeg_header_t* d_headers, const faa_jpeg_table_t* d_tables, int n_tables,
+                                const uint8_t* d_src, int batch, const faa_image_t* h_out, const faa_image_t* d_out,
+                                int32_t* d_status, const faa_jpeg_scan_t* h_scans, const faa_jpeg_scan_t* d_scans,
+                                const int64_t* h_scan_first, const int64_t* d_scan_first, void* stream);
+
 /* number of kernels this library has launched since load (bench bookkeeping) */
 uint64_t faa_launch_count(void);
 
