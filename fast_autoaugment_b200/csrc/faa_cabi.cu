@@ -1732,6 +1732,35 @@ int faa_jpeg_index_build(const faa_jpeg_header_t* h_headers, const faa_jpeg_head
     return FAA_OK;
 }
 
+int faa_jpeg_index_find(const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
+                        const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
+                        const int64_t* h_first, const int64_t* d_first, faa_jpeg_sync_t* d_points, int32_t* d_count,
+                        void* stream_v) {
+    if ((!h_headers || !d_headers || !d_tables || !d_src || !h_first || !d_first || !d_count) && batch > 0)
+        return fail(FAA_ERR_VALUE, "null argument");
+    if (batch < 0) return fail(FAA_ERR_VALUE, "negative batch");
+    if (batch > 65535) return fail(FAA_ERR_UNSUPPORTED, "at most 65535 images per call: split the batch");
+    if (batch == 0) return FAA_OK;
+    if (int e = check_jpeg_first(h_first, batch)) return e;
+    if (!d_points && h_first[batch] > h_first[0]) return fail(FAA_ERR_VALUE, "null argument");
+    for (int i = 0; i < batch; ++i) {
+        JpegHeader h; memcpy(&h, &h_headers[i], sizeof h);
+        if (int e = check_jpeg_header(h, n_tables, "image " + std::to_string(i))) return e;
+    }
+    if (int e = ensure_device()) return e;
+    JpegDecodeParams P = {};
+    P.hdrs = reinterpret_cast<const JpegHeader*>(d_headers);
+    P.pool = reinterpret_cast<const JpegTable*>(d_tables);
+    P.src = d_src;
+    P.batch = batch;
+    P.rec_first = d_first;
+    P.rec_points = reinterpret_cast<JpegSync*>(d_points);
+    P.count = d_count;
+    CK(launch_jpeg_find(P, false, (cudaStream_t)stream_v));
+    g_launches++;
+    return FAA_OK;
+}
+
 }  // extern "C"
 
 // Binds the handle to the current device, orders this call's use of its scratch after the previous call's, grows the
@@ -1759,11 +1788,13 @@ static int jpeg_call_scratch(faa_jpeg_decoder_t* d, cudaStream_t stream, const s
     return FAA_OK;
 }
 
-// faa_jpeg_decode_indexed, and with `rec` (the recording outputs, checked by the caller) faa_jpeg_decode_recording
+// faa_jpeg_decode_indexed, and with `rec` (the recording outputs, checked by the caller) faa_jpeg_decode_recording, or
+// with rec->find faa_jpeg_decode_found
 struct JpegRecordOut {
     const int64_t* d_cap_first;
     faa_jpeg_sync_t* d_points_out;
     int32_t* d_count;
+    bool find;
 };
 
 static int jpeg_decode_call(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
@@ -1820,7 +1851,11 @@ static int jpeg_decode_call(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_he
         P.rec_points = reinterpret_cast<JpegSync*>(rec->d_points_out);
         P.count = rec->d_count;
     }
-    CK(launch_jpeg_entropy(P, stream));
+    if (rec && rec->find) {
+        CK(launch_jpeg_find(P, true, stream));
+        g_launches++;
+    }
+    CK(launch_jpeg_entropy(P, stream, rec && rec->find));
     g_launches++;
     CK(launch_jpeg_reconstruct(P, (int)tiles, stream));
     g_launches++;
@@ -1848,7 +1883,23 @@ int faa_jpeg_decode_recording(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_
         if (int e = check_jpeg_first(h_cap_first, batch)) return e;
         if (!d_points_out && h_cap_first[batch] > h_cap_first[0]) return fail(FAA_ERR_VALUE, "null argument: d_points_out");
     }
-    const JpegRecordOut rec = {d_cap_first, d_points_out, d_count};
+    const JpegRecordOut rec = {d_cap_first, d_points_out, d_count, false};
+    return jpeg_decode_call(d, h_headers, d_headers, d_tables, n_tables, d_src, batch, h_out, d_out, d_status, d_points,
+                            h_first, d_first, &rec, stream_v);
+}
+
+int faa_jpeg_decode_found(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
+                          const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
+                          const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status,
+                          const faa_jpeg_sync_t* d_points, const int64_t* h_first, const int64_t* d_first,
+                          const int64_t* h_cap_first, const int64_t* d_cap_first, faa_jpeg_sync_t* d_points_out,
+                          int32_t* d_count, void* stream_v) {
+    if (batch > 0) {
+        if (!h_cap_first || !d_cap_first || !d_count) return fail(FAA_ERR_VALUE, "null argument");
+        if (int e = check_jpeg_first(h_cap_first, batch)) return e;
+        if (!d_points_out && h_cap_first[batch] > h_cap_first[0]) return fail(FAA_ERR_VALUE, "null argument: d_points_out");
+    }
+    const JpegRecordOut rec = {d_cap_first, d_points_out, d_count, true};
     return jpeg_decode_call(d, h_headers, d_headers, d_tables, n_tables, d_src, batch, h_out, d_out, d_status, d_points,
                             h_first, d_first, &rec, stream_v);
 }

@@ -11,6 +11,9 @@
 //                                instantiation (faa_jpeg_decode_recording) also places the scan index of every scan
 //                                thread 0 decodes whole and serially, as faa_jpeg_index_kernel would.
 //   faa_jpeg_index_kernel        (faa_jpeg_index_build) one CTA per image; one thread records the scan index.
+//   faa_jpeg_find_kernel         (faa_jpeg_index_find, faa_jpeg_decode_found) one CTA per image; thread k finds point k
+//                                of the scan index in parallel, and links checked against the next point verify a
+//                                prefix of it.  The found decode's entropy instantiation reads the counts it leaves.
 //   faa_jpeg_progressive_kernel  (faa_jpeg_decode_progressive) one CTA per progressive image: the entropy stage of
 //                                progressive files, scans run wave by wave; the reconstruct kernel follows it.
 //   faa_jpeg_reconstruct_kernel  one CTA per 64 x 32 output tile of one image.  It runs the islow IDCT of the tile's
@@ -45,7 +48,10 @@ __device__ __forceinline__ void jpeg_cta_tables(const JpegHeader& h, const JpegT
 // kRecord (with kIndexed, whose P.first may then be null): a restart-free scan that thread 0 decodes whole and serially
 // (no points, or points that failed) records its points into P.rec_points[P.rec_first[i], P.rec_first[i + 1]), and
 // P.count[i] gets their number; every other image gets count 0.
-template <bool kIndexed, bool kRecord>
+// kFound (with both, faa_jpeg_decode_found): an image without input points uses the points faa_jpeg_find_kernel left
+// in its recording range, P.count[i] of them (~n: a prefix of n that did not converge); count[i] stays n when they were
+// the whole index and were used.
+template <bool kIndexed, bool kRecord, bool kFound = false>
 __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_entropy_kernel(const __grid_constant__ JpegDecodeParams P) {
     __shared__ JpegHuff s_huff[6];
     __shared__ __align__(16) int16_t s_scratch[kEntropyThreads][64];
@@ -80,9 +86,18 @@ __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_entropy_kernel(const
     __syncthreads();
     int status = 0;
     bool serial = true;
-    const int64_t n_pts = !kIndexed || (kRecord && !P.first) ? 0 : P.first[img + 1] - P.first[img];
+    int64_t n_pts = !kIndexed || (kRecord && !P.first) ? 0 : P.first[img + 1] - P.first[img];
+    const JpegSync* pts = kIndexed && n_pts > 0 ? P.points + P.first[img] : nullptr;
+    bool found_all = false;
+    if constexpr (kFound) {
+        if (n_pts == 0) {
+            const int32_t c = P.count[img];
+            found_all = c >= 0;
+            n_pts = found_all ? c : ~c;
+            pts = P.rec_points + P.rec_first[img];
+        }
+    }
     if (kIndexed && n_pts > 0) {                                       // a scan index: one segment per thread from its points
-        const JpegSync* pts = P.points + P.first[img];
         bool ok = jpeg_index_count_ok(h, n_pts);
         if (ok && tid < n_pts) ok = jpeg_index_point_ok(h, pts[tid], tid ? pts[tid - 1].mcu : 0);
         if (__syncthreads_and(ok)) {
@@ -116,7 +131,11 @@ __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_entropy_kernel(const
     if (status) atomicOr(&s_status, status);
     __syncthreads();
     if (tid == 0) P.status[img] = s_status;
-    if (kRecord && tid == 0) P.count[img] = rec && !s_status ? rec->n : 0;
+    if constexpr (kFound) {
+        if (tid == 0) P.count[img] = s_status ? 0 : rec ? rec->n : found_all && !serial ? (int32_t)n_pts : 0;
+    } else {
+        if (kRecord && tid == 0) P.count[img] = rec && !s_status ? rec->n : 0;
+    }
 }
 
 __global__ void __launch_bounds__(kReconThreads) faa_jpeg_reconstruct_kernel(const __grid_constant__ JpegDecodeParams P) {
@@ -223,6 +242,57 @@ __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_index_kernel(const _
                                     cap < kJpegIndexMaxParts ? (int)cap : kJpegIndexMaxParts, s_scratch, &status);
     P.count[img] = n;
     P.status[img] = status;
+}
+
+// Finds scan indexes in parallel (jpeg_index_find's steps, faa_jpeg.cuh), one CTA per image, thread k on part k.  The
+// CTA builds the Huffman tables; threads 1 .. P - 1 find their candidates (pass 1); then up to kJpegFindRounds rounds of
+// links (pass 2) and repairs, a barrier between each, stop early when every link holds; thread 0 walks the verified
+// prefix in shared memory and writes it to P.rec_points[P.rec_first[i], P.rec_first[i + 1]), the count to P.count[i].
+// Images with input points (P.first, may be null) and images the rule gives no points get count 0.  `mark`: a prefix
+// that did not converge gets count ~n instead of n (the found decode's entropy kernel reads it so).
+__global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_find_kernel(const __grid_constant__ JpegDecodeParams P, int mark) {
+    __shared__ JpegHuff s_huff[6];
+    __shared__ __align__(16) int16_t s_scratch[kEntropyThreads][64];
+    __shared__ JpegSync s_cand[kJpegIndexMaxParts], s_link[kJpegIndexMaxParts];
+    __shared__ uint8_t s_stale[kJpegIndexMaxParts];
+    static_assert(kJpegIndexMaxParts == kEntropyThreads, "one thread per part");
+    const int img = blockIdx.x, tid = threadIdx.x;
+    const JpegHeader h = P.hdrs[img];
+    const bool given = P.first && P.first[img + 1] > P.first[img];
+    const int parts = given ? 0 : jpeg_index_parts(h);
+    if (parts == 0) {
+        if (tid == 0) P.count[img] = 0;
+        return;
+    }
+    const JpegHuff* hp[6];
+    jpeg_cta_tables(h, P.pool, s_huff, tid, hp);
+    __syncthreads();
+    const uint8_t* scan = P.src + h.offset + h.scan_off;
+    if (tid == 0) s_cand[0] = {0, 0, 0, {0, 0, 0}};
+    else if (tid < parts) jpeg_find_candidate(h, hp, scan, parts, tid, kJpegFindWindow, s_scratch[tid], &s_cand[tid]);
+    s_stale[tid] = tid + 1 < parts;
+    __syncthreads();
+    for (int r = 0; r < kJpegFindRounds; ++r) {
+        if (s_stale[tid]) jpeg_find_link(h, hp, scan, parts, tid, s_cand[tid], s_scratch[tid], &s_link[tid]);
+        __syncthreads();
+        // thread k alone writes c_{k + 1} and stale[k + 1]; nobody reads them until the barrier
+        const bool again = tid + 1 < parts && jpeg_find_repair(s_link, s_cand, parts, tid);
+        if (tid + 1 < parts) s_stale[tid + 1] = again;
+        if (tid == 0) s_stale[0] = 0;
+        if (!__syncthreads_or(again)) break;
+    }
+    if (tid != 0) return;
+    const int64_t cap = P.rec_first[img + 1] - P.rec_first[img];
+    bool full = false;
+    const int n = jpeg_find_prefix(h, parts, s_cand, s_link, s_stale, P.rec_points + P.rec_first[img],
+                                   cap < kJpegIndexMaxParts ? (int)cap : kJpegIndexMaxParts, &full);
+    P.count[img] = mark && !full ? ~n : n;
+}
+
+cudaError_t launch_jpeg_find(const JpegDecodeParams& p, bool mark, cudaStream_t stream) {
+    if (p.batch <= 0) return cudaSuccess;
+    faa_jpeg_find_kernel<<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p, mark ? 1 : 0);
+    return cudaGetLastError();
 }
 
 // Progressive entropy decode, one CTA per image.  The CTA zeroes the image's coefficient planes (progressive scans
@@ -345,9 +415,10 @@ cudaError_t launch_jpeg_index(const JpegDecodeParams& p, cudaStream_t stream) {
     return cudaGetLastError();
 }
 
-cudaError_t launch_jpeg_entropy(const JpegDecodeParams& p, cudaStream_t stream) {
+cudaError_t launch_jpeg_entropy(const JpegDecodeParams& p, cudaStream_t stream, bool found) {
     if (p.batch <= 0) return cudaSuccess;
-    if (p.rec_first) faa_jpeg_entropy_kernel<true, true><<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p);
+    if (found) faa_jpeg_entropy_kernel<true, true, true><<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p);
+    else if (p.rec_first) faa_jpeg_entropy_kernel<true, true><<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p);
     else if (p.first) faa_jpeg_entropy_kernel<true, false><<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p);
     else faa_jpeg_entropy_kernel<false, false><<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p);
     return cudaGetLastError();

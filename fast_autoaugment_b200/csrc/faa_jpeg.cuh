@@ -491,6 +491,13 @@ struct JpegIndexSink {
     int32_t parts, next;     // segments of the rule; the next point k to place
 };
 
+// Where a decode that finds a scan index stops (jpeg_find_candidate, jpeg_find_link): at the first MCU boundary, its
+// start state included, whose canonical start byte (jpeg_bits_pos) is >= `at`.  `hit`: it got there before its last MCU.
+struct JpegStop {
+    int64_t at;
+    bool hit;
+};
+
 // ------------------------------------------------------------------------------------------------ coefficients --
 // Coefficient planes of one image: component c's blocks form a grid of (mcu_x * hc) x (mcu_y * vc) blocks of 64 int16
 // (natural order, not dequantised), plane after plane starting at `coef`.
@@ -550,10 +557,11 @@ FAA_JHD void jpeg_zero_block(int16_t* s) {
 // blocks after an error) only when it has a `coef` (written `!rec || coef`: a decode without a sink always has one, and
 // compiles without the test).
 // `data`: the start byte as a pointer, instead of lo + from.byte (a restart segment whose marker is missing starts at
-// `end`).  Returns JpegStatus.
+// `end`).  With `stop` it stores nothing and ends at the stop's boundary (unless it has a `coef`); `to` then reports that
+// boundary, with to->mcu the MCUs decoded.  Returns JpegStatus.
 FAA_JHD int jpeg_decode_segment(const JpegHeader& h, const JpegHuff* const* huff, const uint8_t* lo, const uint8_t* end,
                                 const JpegSync& from, int64_t m1, int16_t* coef, int16_t* scratch, JpegSync* to = nullptr,
-                                JpegIndexSink* rec = nullptr, const uint8_t* data = nullptr) {
+                                JpegIndexSink* rec = nullptr, const uint8_t* data = nullptr, JpegStop* stop = nullptr) {
     JpegBits r;
     jpeg_bits_start(r, lo, data ? data : lo + from.byte, end, from);
     int pred[3] = {from.pred[0], from.pred[1], from.pred[2]};
@@ -563,6 +571,12 @@ FAA_JHD int jpeg_decode_segment(const JpegHeader& h, const JpegHuff* const* huff
     int64_t m = from.mcu;
     int b = 0;
     for (; m < m1; ++m) {
+        if (stop) {                                      // an MCU boundary (the start included): far enough?
+            int32_t byte;
+            int16_t bit;
+            jpeg_bits_pos(r, &byte, &bit);
+            if ((int64_t)byte >= stop->at) { stop->hit = true; break; }
+        }
         if (rec && m > from.mcu) {                       // an MCU boundary: the points whose threshold it reaches
             JpegSync s;
             jpeg_bits_pos(r, &s.byte, &s.bit);
@@ -605,18 +619,18 @@ FAA_JHD int jpeg_decode_segment(const JpegHeader& h, const JpegHuff* const* huff
                 }
             }
             if (status) break;
-            if (!rec || coef) jpeg_store_block(coef + 64 * jpeg_block_of(h, m, b), scratch);
+            if ((!rec && !stop) || coef) jpeg_store_block(coef + 64 * jpeg_block_of(h, m, b), scratch);
         }
         if (status) break;
         if (r.n < r.fake) { status = JPEG_TRUNCATED; ++m; b = 0; break; }     // this MCU used bits past the data
     }
-    if (status && (!rec || coef)) {
+    if (status && ((!rec && !stop) || coef)) {
         jpeg_zero_block(scratch);
         for (; m < m1; ++m, b = 0)
             for (; b < nb; ++b) jpeg_store_block(coef + 64 * jpeg_block_of(h, m, b), scratch);
     }
     if (to && !status) {
-        to->mcu = (int32_t)m1;
+        to->mcu = (int32_t)(stop && stop->hit ? m - from.mcu : m1);
         jpeg_bits_pos(r, &to->byte, &to->bit);
         for (int c = 0; c < 3; ++c) to->pred[c] = (int16_t)pred[c];
     }
@@ -665,6 +679,127 @@ FAA_JHD int jpeg_index_segment(const JpegHeader& h, const JpegHuff* const* huff,
     const int st = jpeg_decode_segment(h, huff, scan, scan + h.scan_len, from, m1, coef, scratch, &to);
     *linked = k == n || (st == 0 && jpeg_sync_same(to, pts[k]));
     return st;
+}
+
+// ------------------------------------------------------------------------------------------------ finding an index --
+// The points of the placement rule found in parallel, without a serial decode, for a restart-free scan of P =
+// jpeg_index_parts parts with thresholds T_k = jpeg_index_threshold(k).  Huffman streams self-synchronise: a parse
+// started at an arbitrary bit soon falls onto the true code boundaries, and onto the true block of its MCU.
+//   pass 1  part k (1 <= k < P) starts W bytes before T_k (bit 0, past the 0x00 of a stuffed pair), assumes block 0 of
+//           an MCU, and decodes to the first MCU boundary of its own parse at or past T_k: candidate c_k.  c_0 is the
+//           scan's start.
+//   pass 2  link k (0 <= k < P - 1) decodes from c_k, with MCU count and DC predictors 0, to the first MCU boundary at
+//           or past T_{k + 1} (c_k itself when it is there already: the points coincide).  It holds when it ends at
+//           c_{k + 1}; when it does not, its end becomes c_{k + 1} and link k + 1 runs again in the next round.
+//   prefix  from the scan's start, each link that holds gives the next point its MCU and predictors (the start's plus
+//           the link's); the walk stops at the first link that does not hold or is stale.
+// By induction every point of the prefix is the rule's, with the serial decoder's MCU and predictors: found points are
+// always a prefix of jpeg_index_record's, and all of them once every link holds.  Each round extends the verified
+// prefix by at least one link.  The window W and the round cap R are measured (DESIGN §4.8).
+constexpr int kJpegFindWindow = 512;           // W, bytes
+constexpr int kJpegFindRounds = 8;             // R, rounds of pass 2
+
+// pass 1 for part k: candidate c_k (byte -1 when the parse fails before T_k)
+FAA_JHD void jpeg_find_candidate(const JpegHeader& h, const JpegHuff* const* huff, const uint8_t* scan, int parts, int k,
+                                 int window, int16_t* scratch, JpegSync* c) {
+    const int64_t t = jpeg_index_threshold(h, parts, k);
+    int64_t s = t > window ? t - window : 0;
+    if (s > 0 && scan[s] == 0 && scan[s - 1] == 0xFF) ++s;        // the stuffing of a 0xFF is no data byte
+    const JpegSync from = {0, (int32_t)s, 0, {0, 0, 0}};
+    JpegStop stop = {t, false};
+    JpegSync to;
+    const int st = jpeg_decode_segment(h, huff, scan, scan + h.scan_len, from, jpeg_mcus(h), nullptr, scratch, &to,
+                                       nullptr, nullptr, &stop);
+    *c = to;
+    if (st || !stop.hit) c->byte = -1;
+}
+
+// pass 2, link k from c: the end it reaches, with mcu = the MCUs it decoded and pred = the DC differences (mcu -1 when
+// it fails: a bad start, a decode error, or no boundary at or past T_{k + 1})
+FAA_JHD void jpeg_find_link(const JpegHeader& h, const JpegHuff* const* huff, const uint8_t* scan, int parts, int k,
+                            const JpegSync& c, int16_t* scratch, JpegSync* e) {
+    e->mcu = -1;
+    if (c.byte < 0) return;
+    const JpegSync from = {0, c.byte, c.bit, {0, 0, 0}};
+    JpegStop stop = {jpeg_index_threshold(h, parts, k + 1), false};
+    JpegSync to;
+    const int st = jpeg_decode_segment(h, huff, scan, scan + h.scan_len, from, jpeg_mcus(h), nullptr, scratch, &to,
+                                       nullptr, nullptr, &stop);
+    if (!st && stop.hit) *e = to;
+}
+
+FAA_JHD bool jpeg_find_holds(const JpegSync& e, const JpegSync& c) { return e.mcu >= 0 && e.byte == c.byte && e.bit == c.bit; }
+
+// the repair after a round, for link k: a link that ended cleanly elsewhere than c_{k + 1} moves it there.  Returns
+// whether link k + 1 is now stale (and runs again next round).
+FAA_JHD bool jpeg_find_repair(const JpegSync* link, JpegSync* cand, int parts, int k) {
+    const JpegSync& e = link[k];
+    if (e.mcu < 0 || jpeg_find_holds(e, cand[k + 1])) return false;
+    cand[k + 1] = e;
+    return k + 2 < parts;
+}
+
+// The verified prefix into at[0, cap): walk the links from the scan's start while each is fresh (stale[k] == 0) and
+// holds.  Returns the number of points; *full: every point of the rule was found (the walk passed the last link, or a
+// link went past the scan's last MCU, after which the rule places nothing).
+FAA_JHD int jpeg_find_prefix(const JpegHeader& h, int parts, const JpegSync* cand, const JpegSync* link,
+                             const uint8_t* stale, JpegSync* at, int cap, bool* full) {
+    JpegSync p = {0, 0, 0, {0, 0, 0}};
+    int n = 0;
+    *full = false;
+    for (int k = 0; k + 1 < parts; ++k) {
+        const JpegSync& e = link[k];
+        if (stale[k] || !jpeg_find_holds(e, cand[k + 1])) return n;
+        if (e.mcu == 0) continue;                                  // point k + 1 coincides with point k: dropped
+        if ((int64_t)p.mcu + e.mcu >= jpeg_mcus(h)) { *full = true; return n; }
+        if (n == cap) return n;
+        p.mcu += e.mcu;
+        p.byte = e.byte;
+        p.bit = e.bit;
+        for (int c = 0; c < 3; ++c) p.pred[c] = (int16_t)(p.pred[c] + e.pred[c]);
+        at[n++] = p;
+    }
+    *full = true;
+    return n;
+}
+
+// what one find did, for the measurement of W and R
+struct JpegFindStats {
+    int32_t links, held_first, rounds;       // links of the chain, links that held in round 1, rounds run
+    int32_t full;                            // every point of the rule was found
+};
+
+// The whole find on one thread, as the find kernel runs it on one thread per part (host build and measurement): at
+// most `rounds` rounds of pass 2, window W = `window` bytes.  Returns the number of points written to at[0, cap).
+inline int jpeg_index_find(const JpegHeader& h, const JpegHuff* const* huff, const uint8_t* scan, int window, int rounds,
+                           JpegSync* at, int cap, int16_t* scratch, JpegFindStats* stats) {
+    JpegFindStats st = {0, 0, 0, 0};
+    const int parts = jpeg_index_parts(h);
+    int n = 0;
+    if (parts) {
+        JpegSync cand[kJpegIndexMaxParts], link[kJpegIndexMaxParts];
+        uint8_t stale[kJpegIndexMaxParts];
+        cand[0] = {0, 0, 0, {0, 0, 0}};
+        for (int k = 1; k < parts; ++k) jpeg_find_candidate(h, huff, scan, parts, k, window, scratch, &cand[k]);
+        for (int k = 0; k < parts; ++k) stale[k] = k + 1 < parts;
+        st.links = parts - 1;
+        for (int r = 0; r < rounds; ++r) {
+            for (int k = 0; k + 1 < parts; ++k)
+                if (stale[k]) jpeg_find_link(h, huff, scan, parts, k, cand[k], scratch, &link[k]);
+            if (r == 0)
+                for (int k = 0; k + 1 < parts; ++k) st.held_first += jpeg_find_holds(link[k], cand[k + 1]);
+            bool any = false;
+            stale[0] = 0;
+            for (int k = 0; k + 1 < parts; ++k) any |= stale[k + 1] = jpeg_find_repair(link, cand, parts, k);
+            st.rounds = r + 1;
+            if (!any) break;
+        }
+        bool full = false;
+        n = jpeg_find_prefix(h, parts, cand, link, stale, at, cap, &full);
+        st.full = full;
+    }
+    if (stats) *stats = st;
+    return n;
 }
 
 // Restart markers of the scan bytes [from, to) (a marker is 0xFF 0xD0..0xD7; its 0xFF may be the last of the range):

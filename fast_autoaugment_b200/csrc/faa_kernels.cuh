@@ -160,9 +160,13 @@ struct JpegDecodeParams {
     const int64_t* rec_first;
     JpegSync* rec_points;
 };
-cudaError_t launch_jpeg_entropy(const JpegDecodeParams& p, cudaStream_t stream);
+// found: the found decode's instantiation (counts from faa_jpeg_find_kernel, faa_jpeg_decode_found)
+cudaError_t launch_jpeg_entropy(const JpegDecodeParams& p, cudaStream_t stream, bool found = false);
 cudaError_t launch_jpeg_reconstruct(const JpegDecodeParams& p, int n_tiles, cudaStream_t stream);
 cudaError_t launch_jpeg_index(const JpegDecodeParams& p, cudaStream_t stream);
+// finds scan indexes into rec_points / rec_first, counts into count, skipping images with input points (first, may be
+// null); mark: a prefix that did not converge gets count ~n
+cudaError_t launch_jpeg_find(const JpegDecodeParams& p, bool mark, cudaStream_t stream);
 // progressive entropy decode (faa_jpeg_decode_progressive): one CTA per image; the reconstruct kernel follows it
 struct JpegProgressiveParams {
     const JpegHeader* hdrs;     // [batch] (device copy)

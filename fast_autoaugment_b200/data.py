@@ -586,10 +586,13 @@ class RaggedDeviceDataset:
 class EncodedDeviceDataset:
     """``RaggedDeviceDataset`` of JPEG files: the files' bytes stay on the device (``EncodedImages``, headers parsed
     once here) and every batch is decoded on the device before its chain runs.  ``progressive``: progressive files
-    are taken too (``EncodedImages.from_bytes(..., progressive=True)``)."""
+    are taken too (``EncodedImages.from_bytes(..., progressive=True)``).  ``find``: each batch's restart-free files
+    without a scan index get one found on the device first (``decode_jpeg(find=True)``), so they decode on many
+    threads; the pixels are the same."""
 
-    def __init__(self, files, targets, device="cuda", progressive=False):
+    def __init__(self, files, targets, device="cuda", progressive=False, find=False):
         self.images = files if isinstance(files, EncodedImages) else EncodedImages.from_bytes(files, device, progressive)
+        self.find = bool(find)
         self.targets = [int(t) for t in targets]
         if len(self.targets) != len(self.images):
             raise ValueError("need one target per image")
@@ -602,6 +605,7 @@ class EncodedDeviceDataset:
         idx = [int(i) for i in idx]
         d = EncodedDeviceDataset.__new__(EncodedDeviceDataset)
         d.images = self.images.select(idx)
+        d.find = self.find
         d.targets = [self.targets[i] for i in idx]
         d.labels = self.labels.index_select(0, torch.as_tensor(idx, dtype=torch.int64, device=self.labels.device))
         return d
@@ -701,15 +705,18 @@ class JpegFileDataset:
     ``JpegIndex`` of the files, whose scan indexes let the device decode each listed file on many threads.  ``learn``:
     the loaders enter into ``index`` (which it needs) the scan index of every file they decode serially, so the next
     epoch decodes it on many threads; subsets share the index, and ``index.save`` writes it.  ``progressive``: the
-    loaders decode progressive files on the device instead of with Pillow (``read_jpeg_batch``)."""
+    loaders decode progressive files on the device instead of with Pillow (``read_jpeg_batch``).  ``find``: the loaders
+    find the scan index of every restart-free file the index does not list on the device, in parallel, before decoding
+    it on many threads (``decode_jpeg(find=True)``); with ``learn`` the found points are what the index learns."""
 
-    def __init__(self, paths, targets, device="cuda", index=None, learn=False, progressive=False):
+    def __init__(self, paths, targets, device="cuda", index=None, learn=False, progressive=False, find=False):
         if learn and index is None:
             raise ValueError("learn needs an index to enter the files' points into (JpegIndex.empty)")
         self.paths = [os.fspath(p) for p in paths]
         self.index = index
         self.learn = bool(learn)
         self.progressive = bool(progressive)
+        self.find = bool(find)
         self.targets = [int(t) for t in targets]
         if len(self.targets) != len(self.paths):
             raise ValueError("need one target per image")
@@ -727,7 +734,7 @@ class JpegFileDataset:
         idx = [int(i) for i in idx]
         d = JpegFileDataset.__new__(JpegFileDataset)
         d.paths = self.select(idx)
-        d.index, d.learn, d.progressive = self.index, self.learn, self.progressive
+        d.index, d.learn, d.progressive, d.find = self.index, self.learn, self.progressive, self.find
         d.targets = [self.targets[i] for i in idx]
         d.labels = self.labels.index_select(0, torch.as_tensor(idx, dtype=torch.int64, device=self.labels.device))
         d.device = self.device
@@ -882,18 +889,21 @@ class FileBatchStream:
     decoded in recording mode (``decode_jpeg(record=True)``): its point counts and the points they cover are copied to
     pinned memory behind the decode with its status, and at the same check the files that got points are entered into
     the index (``JpegIndex.add``), so the batches read after that decode them on many threads.  With ``progressive``,
-    progressive files are decoded on the device too: their scans travel in the same slot."""
+    progressive files are decoded on the device too: their scans travel in the same slot.  With ``find``, every batch
+    is decoded by ``decode_jpeg(find=True)``: files without points get a scan index found on the device first and
+    decode on many threads; with ``learn``, the files whose found index converged are entered with those points."""
 
     SLOTS = 2
     WORKERS = 2
 
-    def __init__(self, workers=None, index=None, learn=False, progressive=False):
+    def __init__(self, workers=None, index=None, learn=False, progressive=False, find=False):
         if learn and index is None:
             raise ValueError("learn needs an index")
         self.workers = int(workers or self.WORKERS)
         self.index = index
         self.learn = bool(learn)
         self.progressive = bool(progressive)
+        self.find = bool(find)
         self.slots = [None] * self.SLOTS           # pinned uint8 staging buffers
         self.copied = [None] * self.SLOTS          # event recorded after each slot's last host-to-device copy
 
@@ -925,15 +935,16 @@ class FileBatchStream:
             enc = EncodedImages(dbuf[lay.files:lay.files_end], hb.headers, hb.pool, _d_pool=dbuf[lay.pool:lay.files],
                                 _d_headers=dbuf[:lay.pool], **index)
             learned = None
+            find = {"find": True} if self.find else {}
             if self.learn:
-                _, status, count, points, cap_first = decode_jpeg(enc, out.select(hb.accepted), record=True)
+                _, status, count, points, cap_first = decode_jpeg(enc, out.select(hb.accepted), record=True, **find)
                 h_count = torch.empty(len(hb.accepted), dtype=torch.int32, pin_memory=True)
                 h_count.copy_(count, non_blocking=True)
                 h_points = torch.empty(points.numel(), dtype=torch.uint8, pin_memory=True)
                 h_points.copy_(points, non_blocking=True)
                 learned = (h_count, h_points, cap_first, [len(f) for f in hb.files])
             else:
-                _, status = decode_jpeg(enc, out.select(hb.accepted))
+                _, status = decode_jpeg(enc, out.select(hb.accepted), **find)
             st = torch.empty(len(hb.accepted), dtype=torch.int32, pin_memory=True)
             st.copy_(status, non_blocking=True)
             ev = torch.cuda.Event()
@@ -1041,7 +1052,7 @@ class GpuAugmentedLoader:
             dev = self.dataset.device
             batches = [idx_all[k * self.batch_size:(k + 1) * self.batch_size] for k in range(len(self))]
             self.staging = FileBatchStream(index=self.dataset.index, learn=self.dataset.learn,
-                                           progressive=self.dataset.progressive)
+                                           progressive=self.dataset.progressive, find=self.dataset.find)
             files = self.staging([self.dataset.select(idx) for idx in batches], dev)
         else:
             dev = self.dataset.images.device
@@ -1053,6 +1064,8 @@ class GpuAugmentedLoader:
                     raw = next(files)                            # this batch's files, decoded on the device
                 elif isinstance(self.dataset, (RaggedDeviceDataset, EncodedDeviceDataset)):
                     raw = self.dataset.images.select(idx)        # descriptors into the dataset's storage: no pixel copy
+                    if getattr(self.dataset, "find", False):     # decoded here, as the chain would, with found indexes
+                        raw, self.chain.last_status = decode_jpeg(raw, find=True)
                 else:
                     raw = self.dataset.images.index_select(0, t)
                 yield t, raw
@@ -1262,7 +1275,12 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
     (``trainloader.dataset.index.save(path)`` writes it as ``faa_jpeg_index`` reads it).  It costs host memory: 16
     bytes a point, about 1.7 KB a file at ImageNet's mean file size.  ``faa_jpeg_progressive`` (default False): the
     train, valid, test and ``tta`` loaders decode progressive JPEG files on the device, bit-exact with Pillow, instead of
-    with Pillow on the host; files whose progression is incomplete still go to Pillow.  They get no scan index."""
+    with Pillow on the host; files whose progression is incomplete still go to Pillow.  They get no scan index.
+    ``faa_jpeg_index_find`` (default False): the loaders find, on the device and in parallel, the scan index of every
+    restart-free file that has none (``decode_jpeg(find=True)``), so even the first epoch and files no index lists
+    decode on many threads, with the same pixels; with ``faa_jpeg_index_learn`` the index learns the found points, and
+    the first epoch pays no serial decode.  A find that does not converge within its rounds still splits the file at
+    the points it verified (DESIGN §4.8)."""
     from sklearn.model_selection import StratifiedShuffleSplit
 
     conf = C.get()
@@ -1288,6 +1306,7 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
     index_dir = conf.get("faa_jpeg_index")
     learn = bool(conf.get("faa_jpeg_index_learn", False))
     progressive = bool(conf.get("faa_jpeg_progressive", False))
+    find = bool(conf.get("faa_jpeg_index_find", False))
 
     def device_dataset(x, y):
         if isinstance(x, FilePaths):
@@ -1300,9 +1319,9 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
                 index = JpegIndex.load(path, x.folder)
             if learn and index is None:
                 index = JpegIndex.empty(x.folder)
-            return JpegFileDataset(x, y, index=index, learn=learn, progressive=progressive)
+            return JpegFileDataset(x, y, index=index, learn=learn, progressive=progressive, find=find)
         if isinstance(x, list) and len(x) and isinstance(x[0], bytes):
-            return EncodedDeviceDataset(x, y, progressive=progressive)
+            return EncodedDeviceDataset(x, y, progressive=progressive, find=find)
         return RaggedDeviceDataset(x, y) if isinstance(x, list) else DeviceDataset(x, y)
     if dataset in ("cifar10", "cifar100", "svhn", "imagenet"):
         total_trainset, testset = device_dataset(tr_x, tr_y), device_dataset(te_x, te_y)

@@ -802,16 +802,20 @@ def _gather_ranges(first, items, idx):
     return out, items[at]
 
 
-def build_jpeg_index(encoded: EncodedImages):
+def build_jpeg_index(encoded: EncodedImages, find=False):
     """The scan index of every file of ``encoded`` (C ABI ``faa_jpeg_index_build``: one serial decode per file on the
     device, one thread per file): ``(first, points)``, int64 [N + 1] offsets into ``JPEG_SYNC_DTYPE`` points, file i's
     being ``points[first[i]:first[i + 1]]``.  Files with restart markers, scans under 2 KiB and files whose scan does
-    not decode cleanly get none, and so do progressive files.  Waits for the device."""
+    not decode cleanly get none, and so do progressive files.  Waits for the device.
+
+    ``find=True`` finds the index in parallel instead (``faa_jpeg_index_find``: one CTA per file, no serial decode).
+    Each file's points are then the verified prefix of the chain: always the first points of the serial build's for a
+    file that decodes cleanly, and all of them when the chain converged (DESIGN §4.8)."""
     _require_cuda(encoded.storage, "encoded")
     prog = encoded.progressive()
     if prog.any():
         at = np.flatnonzero(~prog)
-        first, points = build_jpeg_index(encoded.select(at))
+        first, points = build_jpeg_index(encoded.select(at), find)
         counts = np.zeros(len(encoded), np.int64)
         counts[at] = np.diff(first)
         return np.concatenate([[0], np.cumsum(counts)]).astype(np.int64), points
@@ -826,6 +830,13 @@ def build_jpeg_index(encoded: EncodedImages):
         d_first = torch.from_numpy(cap_first).to(dev)
         d_points = torch.empty(max(total, 1) * 16, dtype=torch.uint8, device=dev)
         d_count = torch.empty(B, dtype=torch.int32, device=dev)
+        if find:
+            check(lib.faa_jpeg_index_find(hdr0, encoded.device_headers().data_ptr(), encoded.device_pool().data_ptr(),
+                                          len(encoded.pool), encoded.storage.data_ptr(), B, cap_first.ctypes.data,
+                                          d_first.data_ptr(), d_points.data_ptr(), d_count.data_ptr(), _stream_ptr(dev)))
+            count = d_count.cpu().numpy()
+            pts = d_points.cpu().numpy()[:total * 16].view(_lib.JPEG_SYNC_DTYPE)
+            return compact_jpeg_index(cap_first, count, pts)
         d_status = torch.empty(B, dtype=torch.int32, device=dev)
         check(lib.faa_jpeg_index_build(hdr0, encoded.device_headers().data_ptr(), encoded.device_pool().data_ptr(),
                                        len(encoded.pool), encoded.storage.data_ptr(), B, cap_first.ctypes.data,
@@ -880,7 +891,7 @@ class _JpegDecoder:
 _DECODERS = {}
 
 
-def decode_jpeg(encoded: EncodedImages, out: RaggedImages | None = None, record=False):
+def decode_jpeg(encoded: EncodedImages, out: RaggedImages | None = None, record=False, find=False):
     """Decode every file of ``encoded`` on its device (C ABI ``faa_jpeg_decode``, or ``faa_jpeg_decode_indexed`` when
     the files carry a scan index: two launches, no host wait), bit-exact
     with ``Image.open(f).convert('RGB')`` (reference imagenet.py:80).  Returns ``(images, status)``: a ``RaggedImages``
@@ -894,6 +905,12 @@ def decode_jpeg(encoded: EncodedImages, out: RaggedImages | None = None, record=
     (``jpeg_index_capacities``, host int64 [N + 1]).  ``count[i] > 0`` means these are file i's points now;
     ``compact_jpeg_index`` turns them into ``build_jpeg_index``'s form.
 
+    ``find=True`` (``faa_jpeg_decode_found``: three launches, still no host wait) first finds, in parallel, the scan
+    index of every restart-free file that carries none, then decodes every file with its points, so such files decode on
+    many threads without a saved index.  Same pixels and status; the return values keep their shapes, with and without
+    ``record``.  With ``record``, ``count[i] > 0`` still means "these are file i's points now": the found index when its
+    chain converged, or the serial decode's recording when the file's points could not be used.
+
     Progressive files (``EncodedImages.from_bytes(..., progressive=True)``) are decoded by
     ``faa_jpeg_decode_progressive`` into the same images, the other files of the batch by the calls above (``select``
     copies no byte of them); status comes back in batch order.  They get no scan index: count 0 with ``record=True``,
@@ -906,7 +923,7 @@ def decode_jpeg(encoded: EncodedImages, out: RaggedImages | None = None, record=
         raise ValueError("out must be a RaggedImages of the files' sizes on their device")
     prog = encoded.progressive()
     if not prog.any():
-        return _decode_baseline(encoded, out, record)
+        return _decode_baseline(encoded, out, record, find)
     B = len(encoded)
     at = np.flatnonzero(~prog)
     pat = np.flatnonzero(prog)
@@ -920,7 +937,7 @@ def decode_jpeg(encoded: EncodedImages, out: RaggedImages | None = None, record=
     p_enc = EncodedImages(encoded.storage, encoded.headers[pat], encoded.pool, encoded.device_pool(),
                           scans=encoded.scans, scan_first=p_first, _d_scans=d_scans, _d_scan_first=d_small[B:])
     p_out = out.select(pat)
-    res = _decode_baseline(encoded.select(at), out.select(at), record) if len(at) else None
+    res = _decode_baseline(encoded.select(at), out.select(at), record, find) if len(at) else None
     p_status = torch.empty(len(pat), dtype=torch.int32, device=dev)
     h_out, d_out = p_out.descriptors()
     with torch.cuda.device(dev):
@@ -948,12 +965,12 @@ def _decoder(dev):
     return dec
 
 
-def _decode_baseline(encoded: EncodedImages, out: RaggedImages, record):
+def _decode_baseline(encoded: EncodedImages, out: RaggedImages, record, find=False):
     """``decode_jpeg`` of a batch without progressive files"""
     dev = encoded.device
     B = len(encoded)
     status = torch.empty(max(B, 1), dtype=torch.int32, device=dev)[:B]
-    if record:
+    if record or find:
         cap_first = jpeg_index_capacities(encoded.headers)
         count = torch.empty(max(B, 1), dtype=torch.int32, device=dev)[:B]
         points = torch.empty(max(int(cap_first[-1]), 1) * 16, dtype=torch.uint8, device=dev)
@@ -962,19 +979,20 @@ def _decode_baseline(encoded: EncodedImages, out: RaggedImages, record):
     h_out, d_out = out.descriptors()
     with torch.cuda.device(dev):
         dec = _decoder(dev)
-        if record:
+        if record or find:
             d_first = d_points = None
             if encoded.first is not None:
                 d_first, d_points = encoded.device_index()
             d_cap_first = torch.from_numpy(cap_first).to(dev)
-            check(lib.faa_jpeg_decode_recording(
+            call = lib.faa_jpeg_decode_found if find else lib.faa_jpeg_decode_recording
+            check(call(
                 dec.handle, encoded.headers.ctypes.data, encoded.device_headers().data_ptr(),
                 encoded.device_pool().data_ptr(), len(encoded.pool), encoded.storage.data_ptr(), B, h_out.ctypes.data,
                 d_out.data_ptr(), status.data_ptr(), None if d_points is None else d_points.data_ptr(),
                 None if encoded.first is None else encoded.first.ctypes.data,
                 None if d_first is None else d_first.data_ptr(), cap_first.ctypes.data, d_cap_first.data_ptr(),
                 points.data_ptr(), count.data_ptr(), _stream_ptr(dev)))
-            return out, status, count, points, cap_first
+            return (out, status, count, points, cap_first) if record else (out, status)
         if encoded.first is None:
             check(lib.faa_jpeg_decode(dec.handle, encoded.headers.ctypes.data, encoded.device_headers().data_ptr(),
                                       encoded.device_pool().data_ptr(), len(encoded.pool), encoded.storage.data_ptr(), B,

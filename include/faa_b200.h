@@ -428,6 +428,33 @@ int faa_jpeg_decode_recording(faa_jpeg_decoder_t* dec, const faa_jpeg_header_t* 
                               const int64_t* h_cap_first, const int64_t* d_cap_first, faa_jpeg_sync_t* d_points_out,
                               int32_t* d_count, void* stream);
 
+/* Finds the scan index of `batch` files in parallel, without a serial decode (inputs, offsets and points as
+ * faa_jpeg_index_build, no status).  One CTA per file: thread k parses from a little before part k's threshold until its
+ * parse meets an MCU boundary (Huffman streams self-synchronise), then decodes from there to the next part's threshold,
+ * and each such link is checked against the next part's start; a few rounds repair the links that disagree.  d_count[i]
+ * is the number of verified points: always the first d_count[i] of faa_jpeg_index_build's points for a file whose serial
+ * decode is clean, and all of them when the chain converged (DESIGN §4.8 measures how often).  A file the placement rule
+ * gives no points gets 0.  FAA_ERR_VALUE for offsets that decrease or are negative and for progressive headers.  One
+ * launch, no host wait. */
+int faa_jpeg_index_find(const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
+                        const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
+                        const int64_t* h_first, const int64_t* d_first, faa_jpeg_sync_t* d_points, int32_t* d_count,
+                        void* stream);
+
+/* faa_jpeg_decode_recording whose files without input points get their scan index found first (faa_jpeg_index_find,
+ * into d_points_out), so that a restart-free file decodes on many threads without a saved index.  Same parameters, same
+ * meaning: files with input points keep them; pixels and status equal faa_jpeg_decode's whatever the find produced;
+ * count[i] > 0 means these are file i's points now: the found index when its chain converged and was used, or the
+ * serial decode's recording when the file's points (given or found) could not be used.  A found prefix that did not
+ * converge is used for the decode and gets count 0.  Three launches (find, entropy decode, reconstruct), no host
+ * wait. */
+int faa_jpeg_decode_found(faa_jpeg_decoder_t* dec, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
+                          const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
+                          const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status,
+                          const faa_jpeg_sync_t* d_points, const int64_t* h_first, const int64_t* d_first,
+                          const int64_t* h_cap_first, const int64_t* d_cap_first, faa_jpeg_sync_t* d_points_out,
+                          int32_t* d_count, void* stream);
+
 /* ---- progressive JPEG decode (SOF2 Huffman), for callers that opt in: the files faa_jpeg_parse takes, coded
  * progressively, bit-exact with Pillow as above.  The parse accepts a file only when every coefficient of every component
  * ends at bit 0 (libjpeg smooths the blocks of an incomplete progression, which is not modelled), with at most
