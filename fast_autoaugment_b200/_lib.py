@@ -113,15 +113,11 @@ def _load():
         "faa_jpeg_tables": (C.c_int, [C.c_char_p, C.c_size_t, vp, vp]),
         "faa_jpeg_decoder_create": (C.c_int, [P(vp)]),
         "faa_jpeg_decoder_destroy": (C.c_int, [vp]),
-        "faa_jpeg_decode": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp]),
         "faa_jpeg_index_capacity": (C.c_int, [vp]),
         "faa_jpeg_index_build": (C.c_int, [vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp]),
-        "faa_jpeg_decode_indexed": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp]),
-        "faa_jpeg_decode_recording": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp,
-                                                vp, vp, vp, vp]),
         "faa_jpeg_index_find": (C.c_int, [vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp]),
-        "faa_jpeg_decode_found": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp,
-                                            vp, vp, vp, vp]),
+        "faa_jpeg_decode": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp,
+                                      C.c_int, vp]),
         "faa_jpeg_parse_progressive": (C.c_int, [C.c_char_p, C.c_size_t, vp, vp, C.c_int, P(C.c_int)]),
         "faa_jpeg_scan_tables": (C.c_int, [C.c_char_p, C.c_size_t, vp, vp, C.c_int, vp]),
         "faa_jpeg_decode_progressive": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp,

@@ -1681,13 +1681,6 @@ int faa_jpeg_index_capacity(const faa_jpeg_header_t* hdr) {
     return jpeg_is_progressive(h) ? 0 : jpeg_index_capacity(h);
 }
 
-int faa_jpeg_decode(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
-                    const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
-                    const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status, void* stream_v) {
-    return faa_jpeg_decode_indexed(d, h_headers, d_headers, d_tables, n_tables, d_src, batch, h_out, d_out, d_status,
-                                   nullptr, nullptr, nullptr, stream_v);
-}
-
 }  // extern "C"
 
 // the point offsets of a call: [batch + 1], non-decreasing, from 0 up
@@ -1700,6 +1693,22 @@ static int check_jpeg_first(const int64_t* h_first, int batch) {
     return FAA_OK;
 }
 
+// the batch sizes the JPEG device calls take: their grids have one CTA per image
+static int check_jpeg_batch(int batch) {
+    if (batch < 0) return fail(FAA_ERR_VALUE, "negative batch");
+    if (batch > 65535) return fail(FAA_ERR_UNSUPPORTED, "at most 65535 images per call: split the batch");
+    return FAA_OK;
+}
+
+// check_jpeg_header of every image of a call
+static int check_jpeg_headers(const faa_jpeg_header_t* h_headers, int batch, int n_tables, bool progressive = false) {
+    for (int i = 0; i < batch; ++i) {
+        JpegHeader h; memcpy(&h, &h_headers[i], sizeof h);
+        if (int e = check_jpeg_header(h, n_tables, "image " + std::to_string(i), progressive)) return e;
+    }
+    return FAA_OK;
+}
+
 extern "C" {
 
 int faa_jpeg_index_build(const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
@@ -1708,15 +1717,11 @@ int faa_jpeg_index_build(const faa_jpeg_header_t* h_headers, const faa_jpeg_head
                          int32_t* d_status, void* stream_v) {
     if ((!h_headers || !d_headers || !d_tables || !d_src || !h_first || !d_first || !d_count || !d_status) && batch > 0)
         return fail(FAA_ERR_VALUE, "null argument");
-    if (batch < 0) return fail(FAA_ERR_VALUE, "negative batch");
-    if (batch > 65535) return fail(FAA_ERR_UNSUPPORTED, "at most 65535 images per call: split the batch");
+    if (int e = check_jpeg_batch(batch)) return e;
     if (batch == 0) return FAA_OK;
     if (int e = check_jpeg_first(h_first, batch)) return e;
     if (!d_points && h_first[batch] > h_first[0]) return fail(FAA_ERR_VALUE, "null argument");
-    for (int i = 0; i < batch; ++i) {
-        JpegHeader h; memcpy(&h, &h_headers[i], sizeof h);
-        if (int e = check_jpeg_header(h, n_tables, "image " + std::to_string(i))) return e;
-    }
+    if (int e = check_jpeg_headers(h_headers, batch, n_tables)) return e;
     if (int e = ensure_device()) return e;
     JpegDecodeParams P = {};
     P.hdrs = reinterpret_cast<const JpegHeader*>(d_headers);
@@ -1738,15 +1743,11 @@ int faa_jpeg_index_find(const faa_jpeg_header_t* h_headers, const faa_jpeg_heade
                         void* stream_v) {
     if ((!h_headers || !d_headers || !d_tables || !d_src || !h_first || !d_first || !d_count) && batch > 0)
         return fail(FAA_ERR_VALUE, "null argument");
-    if (batch < 0) return fail(FAA_ERR_VALUE, "negative batch");
-    if (batch > 65535) return fail(FAA_ERR_UNSUPPORTED, "at most 65535 images per call: split the batch");
+    if (int e = check_jpeg_batch(batch)) return e;
     if (batch == 0) return FAA_OK;
     if (int e = check_jpeg_first(h_first, batch)) return e;
     if (!d_points && h_first[batch] > h_first[0]) return fail(FAA_ERR_VALUE, "null argument");
-    for (int i = 0; i < batch; ++i) {
-        JpegHeader h; memcpy(&h, &h_headers[i], sizeof h);
-        if (int e = check_jpeg_header(h, n_tables, "image " + std::to_string(i))) return e;
-    }
+    if (int e = check_jpeg_headers(h_headers, batch, n_tables)) return e;
     if (int e = ensure_device()) return e;
     JpegDecodeParams P = {};
     P.hdrs = reinterpret_cast<const JpegHeader*>(d_headers);
@@ -1762,154 +1763,6 @@ int faa_jpeg_index_find(const faa_jpeg_header_t* h_headers, const faa_jpeg_heade
 }
 
 }  // extern "C"
-
-// Binds the handle to the current device, orders this call's use of its scratch after the previous call's, grows the
-// coefficient, segment and job buffers to what the call needs and uploads the job table.  Every decode call goes
-// through here, under the handle's lock until its launches are queued, so calls of either kind may follow each other on
-// any streams.
-static int jpeg_call_scratch(faa_jpeg_decoder_t* d, cudaStream_t stream, const std::vector<JpegJob>& jobs, int64_t blocks,
-                             int64_t segs) {
-    int dev = -1;
-    if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); return fail(FAA_ERR_NO_DEVICE, "no current CUDA device"); }
-    if (d->device < 0) d->device = dev;
-    if (d->device != dev)
-        return fail(FAA_ERR_VALUE, "JPEG decoder is bound to device " + std::to_string(d->device) + " but the current device is " +
-                    std::to_string(dev) + ": create one decoder per device");
-    if (d->have_last_stream && d->last_stream != stream) {          // buffers are reused in the order of the calls
-        if (!d->ev_switch) CK(cudaEventCreateWithFlags(&d->ev_switch, cudaEventDisableTiming));
-        CK(cudaEventRecord(d->ev_switch, d->last_stream));
-        CK(cudaStreamWaitEvent(stream, d->ev_switch, 0));
-    }
-    d->last_stream = stream; d->have_last_stream = true;
-    if (int e = grow_async(&d->d_coef, &d->coef_bytes, (size_t)blocks * 128, stream)) return e;
-    if (int e = grow_async(&d->d_segs, &d->segs_bytes, (size_t)segs * sizeof(int32_t), stream)) return e;
-    if (int e = grow_async(&d->d_jobs, &d->jobs_bytes, jobs.size() * sizeof(JpegJob), stream)) return e;
-    CK(cudaMemcpyAsync(d->d_jobs, jobs.data(), jobs.size() * sizeof(JpegJob), cudaMemcpyHostToDevice, stream));  // (pageable: staged at once)
-    return FAA_OK;
-}
-
-// faa_jpeg_decode_indexed, and with `rec` (the recording outputs, checked by the caller) faa_jpeg_decode_recording, or
-// with rec->find faa_jpeg_decode_found
-struct JpegRecordOut {
-    const int64_t* d_cap_first;
-    faa_jpeg_sync_t* d_points_out;
-    int32_t* d_count;
-    bool find;
-};
-
-static int jpeg_decode_call(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
-                            const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
-                            const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status,
-                            const faa_jpeg_sync_t* d_points, const int64_t* h_first, const int64_t* d_first,
-                            const JpegRecordOut* rec, void* stream_v) {
-    if (!d || ((!h_headers || !d_headers || !d_tables || !d_src || !h_out || !d_out || !d_status) && batch > 0))
-        return fail(FAA_ERR_VALUE, "null argument");
-    if (batch < 0) return fail(FAA_ERR_VALUE, "negative batch");
-    if (batch > 65535) return fail(FAA_ERR_UNSUPPORTED, "at most 65535 images per call: split the batch");
-    const bool indexed = h_first || d_first || d_points;
-    if (indexed && batch > 0) {
-        if (!h_first || !d_first) return fail(FAA_ERR_VALUE, "null argument: point offsets need h_first and d_first");
-        if (int e = check_jpeg_first(h_first, batch)) return e;
-        if (!d_points && h_first[batch] > h_first[0]) return fail(FAA_ERR_VALUE, "null argument: d_points");
-    }
-    std::vector<JpegJob> jobs((size_t)batch + 1);
-    int64_t blocks = 0, segs = 0, tiles = 0;
-    for (int i = 0; i < batch; ++i) {
-        JpegHeader h; memcpy(&h, &h_headers[i], sizeof h);
-        const std::string who = "image " + std::to_string(i);
-        if (int e = check_jpeg_header(h, n_tables, who)) return e;
-        if (!h_out[i].data) return fail(FAA_ERR_VALUE, "output " + who + " has no data");
-        if (h_out[i].h != h.h || h_out[i].w != h.w) return fail(FAA_ERR_VALUE, "output " + who + " is not the size of its JPEG");
-        jobs[(size_t)i] = {blocks, (int32_t)segs, (int32_t)tiles};
-        blocks += jpeg_image_blocks(h);
-        segs += jpeg_segments(h);
-        tiles += (int64_t)((h.w + kJpegTileW - 1) / kJpegTileW) * ((h.h + kJpegTileH - 1) / kJpegTileH);
-        if (segs > INT32_MAX || tiles > INT32_MAX) return fail(FAA_ERR_UNSUPPORTED, "batch too large: split it");
-    }
-    jobs[(size_t)batch] = {blocks, (int32_t)segs, (int32_t)tiles};
-    if (int e = ensure_device()) return e;
-    if (batch == 0) return FAA_OK;
-    cudaStream_t stream = (cudaStream_t)stream_v;
-    std::lock_guard<std::mutex> lk(d->mu);
-    if (int e = jpeg_call_scratch(d, stream, jobs, blocks, segs)) return e;
-    JpegDecodeParams P = {};
-    P.hdrs = reinterpret_cast<const JpegHeader*>(d_headers);
-    P.pool = reinterpret_cast<const JpegTable*>(d_tables);
-    P.src = d_src;
-    P.jobs = reinterpret_cast<const JpegJob*>(d->d_jobs);
-    P.out = reinterpret_cast<const CropImage*>(d_out);
-    P.coef = reinterpret_cast<int16_t*>(d->d_coef);
-    P.segs = reinterpret_cast<int32_t*>(d->d_segs);
-    P.status = d_status;
-    P.batch = batch;
-    if (indexed) {
-        P.first = d_first;
-        P.points = const_cast<JpegSync*>(reinterpret_cast<const JpegSync*>(d_points));
-    }
-    if (rec) {
-        P.rec_first = rec->d_cap_first;
-        P.rec_points = reinterpret_cast<JpegSync*>(rec->d_points_out);
-        P.count = rec->d_count;
-    }
-    if (rec && rec->find) {
-        CK(launch_jpeg_find(P, true, stream));
-        g_launches++;
-    }
-    CK(launch_jpeg_entropy(P, stream, rec && rec->find));
-    g_launches++;
-    CK(launch_jpeg_reconstruct(P, (int)tiles, stream));
-    g_launches++;
-    return FAA_OK;
-}
-
-extern "C" {
-
-int faa_jpeg_decode_indexed(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
-                            const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
-                            const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status,
-                            const faa_jpeg_sync_t* d_points, const int64_t* h_first, const int64_t* d_first, void* stream_v) {
-    return jpeg_decode_call(d, h_headers, d_headers, d_tables, n_tables, d_src, batch, h_out, d_out, d_status, d_points,
-                            h_first, d_first, nullptr, stream_v);
-}
-
-int faa_jpeg_decode_recording(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
-                              const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
-                              const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status,
-                              const faa_jpeg_sync_t* d_points, const int64_t* h_first, const int64_t* d_first,
-                              const int64_t* h_cap_first, const int64_t* d_cap_first, faa_jpeg_sync_t* d_points_out,
-                              int32_t* d_count, void* stream_v) {
-    if (batch > 0) {
-        if (!h_cap_first || !d_cap_first || !d_count) return fail(FAA_ERR_VALUE, "null argument");
-        if (int e = check_jpeg_first(h_cap_first, batch)) return e;
-        if (!d_points_out && h_cap_first[batch] > h_cap_first[0]) return fail(FAA_ERR_VALUE, "null argument: d_points_out");
-    }
-    const JpegRecordOut rec = {d_cap_first, d_points_out, d_count, false};
-    return jpeg_decode_call(d, h_headers, d_headers, d_tables, n_tables, d_src, batch, h_out, d_out, d_status, d_points,
-                            h_first, d_first, &rec, stream_v);
-}
-
-int faa_jpeg_decode_found(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
-                          const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
-                          const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status,
-                          const faa_jpeg_sync_t* d_points, const int64_t* h_first, const int64_t* d_first,
-                          const int64_t* h_cap_first, const int64_t* d_cap_first, faa_jpeg_sync_t* d_points_out,
-                          int32_t* d_count, void* stream_v) {
-    if (batch > 0) {
-        if (!h_cap_first || !d_cap_first || !d_count) return fail(FAA_ERR_VALUE, "null argument");
-        if (int e = check_jpeg_first(h_cap_first, batch)) return e;
-        if (!d_points_out && h_cap_first[batch] > h_cap_first[0]) return fail(FAA_ERR_VALUE, "null argument: d_points_out");
-    }
-    const JpegRecordOut rec = {d_cap_first, d_points_out, d_count, true};
-    return jpeg_decode_call(d, h_headers, d_headers, d_tables, n_tables, d_src, batch, h_out, d_out, d_status, d_points,
-                            h_first, d_first, &rec, stream_v);
-}
-
-}  // extern "C"
-
-// ------------------------------------------------------------------ progressive JPEG decode --
-static_assert(sizeof(faa_jpeg_scan_t) == sizeof(JpegScan) && sizeof(JpegScan) == 112 &&
-              offsetof(faa_jpeg_scan_t, pool) == offsetof(JpegScan, pool) && FAA_JPEG_MAX_SCANS == kJpegMaxScans &&
-              FAA_JPEG_PROGRESSIVE == kJpegProgressive, "JPEG scan layout");
 
 // image `who`'s scans [0, n): parameters a progression can have, byte ranges inside the file, pool slots in range, and
 // the waves the dependency rule gives (a wrong wave would let two work items race on a coefficient)
@@ -1940,6 +1793,126 @@ static int check_jpeg_scans(const JpegHeader& h, const JpegScan* scans, int64_t 
             return fail(FAA_ERR_VALUE, who + " scan " + std::to_string(i) + ": wave does not follow the scans' dependencies");
     return FAA_OK;
 }
+
+// The JpegJob table of a decode call whose headers are checked: jobs[i] holds where image i's coefficient blocks,
+// restart-segment starts and reconstruct tiles begin, jobs[batch] the totals.  Also checks each image's output
+// descriptor, and with `scans` (a progressive call: image i's scans are scans[scan_first[i], scan_first[i + 1])) its
+// scans, whose segments it counts where a baseline image has jpeg_segments.
+static int plan_jpeg_jobs(const faa_jpeg_header_t* h_headers, const faa_image_t* h_out, int batch, int n_tables,
+                          const JpegScan* scans, const int64_t* scan_first, std::vector<JpegJob>& jobs) {
+    jobs.resize((size_t)batch + 1);
+    int64_t blocks = 0, segs = 0, tiles = 0;
+    for (int i = 0; i < batch; ++i) {
+        JpegHeader h; memcpy(&h, &h_headers[i], sizeof h);
+        const std::string who = "image " + std::to_string(i);
+        if (!h_out[i].data) return fail(FAA_ERR_VALUE, "output " + who + " has no data");
+        if (h_out[i].h != h.h || h_out[i].w != h.w) return fail(FAA_ERR_VALUE, "output " + who + " is not the size of its JPEG");
+        jobs[(size_t)i] = {blocks, (int32_t)segs, (int32_t)tiles};
+        blocks += jpeg_image_blocks(h);
+        if (!scans) {
+            segs += jpeg_segments(h);
+        } else {
+            const int64_t n = scan_first[i + 1] - scan_first[i];
+            if (int e = check_jpeg_scans(h, scans + scan_first[i], n, n_tables, who)) return e;
+            for (int64_t k = 0; k < n; ++k) segs += jpeg_scan_segments(h, scans[scan_first[i] + k]);
+        }
+        tiles += (int64_t)((h.w + kJpegTileW - 1) / kJpegTileW) * ((h.h + kJpegTileH - 1) / kJpegTileH);
+        if (segs > INT32_MAX || tiles > INT32_MAX) return fail(FAA_ERR_UNSUPPORTED, "batch too large: split it");
+    }
+    jobs[(size_t)batch] = {blocks, (int32_t)segs, (int32_t)tiles};
+    return FAA_OK;
+}
+
+// Binds the handle to the current device, orders this call's use of its scratch after the previous call's, grows the
+// coefficient, segment and job buffers to what the call's job table needs and uploads the table.  Every decode call
+// goes through here, under the handle's lock until its launches are queued, so calls of either kind may follow each
+// other on any streams.
+static int jpeg_call_scratch(faa_jpeg_decoder_t* d, cudaStream_t stream, const std::vector<JpegJob>& jobs) {
+    int dev = -1;
+    if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); return fail(FAA_ERR_NO_DEVICE, "no current CUDA device"); }
+    if (d->device < 0) d->device = dev;
+    if (d->device != dev)
+        return fail(FAA_ERR_VALUE, "JPEG decoder is bound to device " + std::to_string(d->device) + " but the current device is " +
+                    std::to_string(dev) + ": create one decoder per device");
+    if (d->have_last_stream && d->last_stream != stream) {          // buffers are reused in the order of the calls
+        if (!d->ev_switch) CK(cudaEventCreateWithFlags(&d->ev_switch, cudaEventDisableTiming));
+        CK(cudaEventRecord(d->ev_switch, d->last_stream));
+        CK(cudaStreamWaitEvent(stream, d->ev_switch, 0));
+    }
+    d->last_stream = stream; d->have_last_stream = true;
+    if (int e = grow_async(&d->d_coef, &d->coef_bytes, (size_t)jobs.back().coef * 128, stream)) return e;
+    if (int e = grow_async(&d->d_segs, &d->segs_bytes, (size_t)jobs.back().seg * sizeof(int32_t), stream)) return e;
+    if (int e = grow_async(&d->d_jobs, &d->jobs_bytes, jobs.size() * sizeof(JpegJob), stream)) return e;
+    CK(cudaMemcpyAsync(d->d_jobs, jobs.data(), jobs.size() * sizeof(JpegJob), cudaMemcpyHostToDevice, stream));  // (pageable: staged at once)
+    return FAA_OK;
+}
+
+extern "C" {
+
+int faa_jpeg_decode(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
+                    const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
+                    const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status,
+                    const faa_jpeg_sync_t* d_points, const int64_t* h_first, const int64_t* d_first,
+                    const int64_t* h_cap_first, const int64_t* d_cap_first, faa_jpeg_sync_t* d_points_out,
+                    int32_t* d_count, int find, void* stream_v) {
+    if (!d || ((!h_headers || !d_headers || !d_tables || !d_src || !h_out || !d_out || !d_status) && batch > 0))
+        return fail(FAA_ERR_VALUE, "null argument");
+    if (int e = check_jpeg_batch(batch)) return e;
+    const bool indexed = d_points || h_first || d_first;
+    const bool recording = h_cap_first || d_cap_first || d_points_out || d_count;
+    if (find && !recording)
+        return fail(FAA_ERR_VALUE, "find needs the recording outputs h_cap_first, d_cap_first, d_points_out and d_count");
+    if (recording && batch > 0) {
+        if (!h_cap_first || !d_cap_first || !d_count) return fail(FAA_ERR_VALUE, "null argument");
+        if (int e = check_jpeg_first(h_cap_first, batch)) return e;
+        if (!d_points_out && h_cap_first[batch] > h_cap_first[0]) return fail(FAA_ERR_VALUE, "null argument: d_points_out");
+    }
+    if (indexed && batch > 0) {
+        if (!h_first || !d_first) return fail(FAA_ERR_VALUE, "null argument: point offsets need h_first and d_first");
+        if (int e = check_jpeg_first(h_first, batch)) return e;
+        if (!d_points && h_first[batch] > h_first[0]) return fail(FAA_ERR_VALUE, "null argument: d_points");
+    }
+    if (int e = check_jpeg_headers(h_headers, batch, n_tables)) return e;
+    std::vector<JpegJob> jobs;
+    if (int e = plan_jpeg_jobs(h_headers, h_out, batch, n_tables, nullptr, nullptr, jobs)) return e;
+    if (int e = ensure_device()) return e;
+    if (batch == 0) return FAA_OK;
+    cudaStream_t stream = (cudaStream_t)stream_v;
+    std::lock_guard<std::mutex> lk(d->mu);
+    if (int e = jpeg_call_scratch(d, stream, jobs)) return e;
+    // launch_jpeg_entropy picks its instantiation from the groups: the pointers of one that is not given are null
+    JpegDecodeParams P = {};
+    P.hdrs = reinterpret_cast<const JpegHeader*>(d_headers);
+    P.pool = reinterpret_cast<const JpegTable*>(d_tables);
+    P.src = d_src;
+    P.jobs = reinterpret_cast<const JpegJob*>(d->d_jobs);
+    P.out = reinterpret_cast<const CropImage*>(d_out);
+    P.coef = reinterpret_cast<int16_t*>(d->d_coef);
+    P.segs = reinterpret_cast<int32_t*>(d->d_segs);
+    P.status = d_status;
+    P.batch = batch;
+    P.first = d_first;
+    P.points = const_cast<JpegSync*>(reinterpret_cast<const JpegSync*>(d_points));
+    P.rec_first = d_cap_first;
+    P.rec_points = reinterpret_cast<JpegSync*>(d_points_out);
+    P.count = d_count;
+    if (find) {
+        CK(launch_jpeg_find(P, true, stream));
+        g_launches++;
+    }
+    CK(launch_jpeg_entropy(P, stream, find != 0));
+    g_launches++;
+    CK(launch_jpeg_reconstruct(P, jobs.back().tile0, stream));
+    g_launches++;
+    return FAA_OK;
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------ progressive JPEG decode --
+static_assert(sizeof(faa_jpeg_scan_t) == sizeof(JpegScan) && sizeof(JpegScan) == 112 &&
+              offsetof(faa_jpeg_scan_t, pool) == offsetof(JpegScan, pool) && FAA_JPEG_MAX_SCANS == kJpegMaxScans &&
+              FAA_JPEG_PROGRESSIVE == kJpegProgressive, "JPEG scan layout");
 
 extern "C" {
 
@@ -1988,33 +1961,19 @@ int faa_jpeg_decode_progressive(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* 
     if (!d || ((!h_headers || !d_headers || !d_tables || !d_src || !h_out || !d_out || !d_status || !h_scans || !d_scans ||
                 !h_scan_first || !d_scan_first) && batch > 0))
         return fail(FAA_ERR_VALUE, "null argument");
-    if (batch < 0) return fail(FAA_ERR_VALUE, "negative batch");
-    if (batch > 65535) return fail(FAA_ERR_UNSUPPORTED, "at most 65535 images per call: split the batch");
+    if (int e = check_jpeg_batch(batch)) return e;
     if (batch > 0)
         if (int e = check_jpeg_first(h_scan_first, batch)) return e;
-    std::vector<JpegJob> jobs((size_t)batch + 1);
-    int64_t blocks = 0, segs = 0, tiles = 0;
-    const JpegScan* scans = reinterpret_cast<const JpegScan*>(h_scans);
-    for (int i = 0; i < batch; ++i) {
-        JpegHeader h; memcpy(&h, &h_headers[i], sizeof h);
-        const std::string who = "image " + std::to_string(i);
-        if (int e = check_jpeg_header(h, n_tables, who, true)) return e;
-        if (!h_out[i].data) return fail(FAA_ERR_VALUE, "output " + who + " has no data");
-        if (h_out[i].h != h.h || h_out[i].w != h.w) return fail(FAA_ERR_VALUE, "output " + who + " is not the size of its JPEG");
-        const int64_t n = h_scan_first[i + 1] - h_scan_first[i];
-        if (int e = check_jpeg_scans(h, scans + h_scan_first[i], n, n_tables, who)) return e;
-        jobs[(size_t)i] = {blocks, (int32_t)segs, (int32_t)tiles};
-        blocks += jpeg_image_blocks(h);
-        for (int64_t k = 0; k < n; ++k) segs += jpeg_scan_segments(h, scans[h_scan_first[i] + k]);
-        tiles += (int64_t)((h.w + kJpegTileW - 1) / kJpegTileW) * ((h.h + kJpegTileH - 1) / kJpegTileH);
-        if (segs > INT32_MAX || tiles > INT32_MAX) return fail(FAA_ERR_UNSUPPORTED, "batch too large: split it");
-    }
-    jobs[(size_t)batch] = {blocks, (int32_t)segs, (int32_t)tiles};
+    if (int e = check_jpeg_headers(h_headers, batch, n_tables, true)) return e;
+    std::vector<JpegJob> jobs;
+    if (int e = plan_jpeg_jobs(h_headers, h_out, batch, n_tables, reinterpret_cast<const JpegScan*>(h_scans), h_scan_first,
+                               jobs))
+        return e;
     if (int e = ensure_device()) return e;
     if (batch == 0) return FAA_OK;
     cudaStream_t stream = (cudaStream_t)stream_v;
     std::lock_guard<std::mutex> lk(d->mu);
-    if (int e = jpeg_call_scratch(d, stream, jobs, blocks, segs)) return e;
+    if (int e = jpeg_call_scratch(d, stream, jobs)) return e;
     JpegProgressiveParams Q = {};
     Q.hdrs = reinterpret_cast<const JpegHeader*>(d_headers);
     Q.pool = reinterpret_cast<const JpegTable*>(d_tables);
@@ -2037,7 +1996,7 @@ int faa_jpeg_decode_progressive(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* 
     P.coef = Q.coef;
     P.status = d_status;
     P.batch = batch;
-    CK(launch_jpeg_reconstruct(P, (int)tiles, stream));
+    CK(launch_jpeg_reconstruct(P, jobs.back().tile0, stream));
     g_launches++;
     return FAA_OK;
 }

@@ -8,10 +8,10 @@
 //                                decoded serially by one thread, unless the call gives it a scan index: then thread k
 //                                decodes from point k to point k + 1 and checks that it ended in that point's state;
 //                                if any segment disagrees, thread 0 decodes the scan serially over it.  The recording
-//                                instantiation (faa_jpeg_decode_recording) also places the scan index of every scan
+//                                instantiation (a recording faa_jpeg_decode) also places the scan index of every scan
 //                                thread 0 decodes whole and serially, as faa_jpeg_index_kernel would.
 //   faa_jpeg_index_kernel        (faa_jpeg_index_build) one CTA per image; one thread records the scan index.
-//   faa_jpeg_find_kernel         (faa_jpeg_index_find, faa_jpeg_decode_found) one CTA per image; thread k finds point k
+//   faa_jpeg_find_kernel         (faa_jpeg_index_find, faa_jpeg_decode's find) one CTA per image; thread k finds point k
 //                                of the scan index in parallel, and links checked against the next point verify a
 //                                prefix of it.  The found decode's entropy instantiation reads the counts it leaves.
 //   faa_jpeg_progressive_kernel  (faa_jpeg_decode_progressive) one CTA per progressive image: the entropy stage of
@@ -48,7 +48,7 @@ __device__ __forceinline__ void jpeg_cta_tables(const JpegHeader& h, const JpegT
 // kRecord (with kIndexed, whose P.first may then be null): a restart-free scan that thread 0 decodes whole and serially
 // (no points, or points that failed) records its points into P.rec_points[P.rec_first[i], P.rec_first[i + 1]), and
 // P.count[i] gets their number; every other image gets count 0.
-// kFound (with both, faa_jpeg_decode_found): an image without input points uses the points faa_jpeg_find_kernel left
+// kFound (with both, faa_jpeg_decode's find): an image without input points uses the points faa_jpeg_find_kernel left
 // in its recording range, P.count[i] of them (~n: a prefix of n that did not converge); count[i] stays n when they were
 // the whole index and were used.
 template <bool kIndexed, bool kRecord, bool kFound = false>

@@ -658,7 +658,7 @@ FAA_JHD int jpeg_index_record(const JpegHeader& h, const JpegHuff* const* huff, 
     return *status ? 0 : rec.n;
 }
 
-// The sink of a recording entropy decode (faa_jpeg_decode_recording) of a restart-free scan decoded whole and serially:
+// The sink of a recording entropy decode (a recording faa_jpeg_decode) of a restart-free scan decoded whole and serially:
 // the file's points go to at[0, cap), cap being the room the caller planned for it (faa_jpeg_index_capacity).  False,
 // and no sink, when the rule gives the file no points or it has no room.
 FAA_JHD bool jpeg_record_sink(const JpegHeader& h, JpegSync* at, int64_t cap, JpegIndexSink& s) {

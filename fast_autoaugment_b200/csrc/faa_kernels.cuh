@@ -160,7 +160,7 @@ struct JpegDecodeParams {
     const int64_t* rec_first;
     JpegSync* rec_points;
 };
-// found: the found decode's instantiation (counts from faa_jpeg_find_kernel, faa_jpeg_decode_found)
+// found: the found decode's instantiation (counts from faa_jpeg_find_kernel, faa_jpeg_decode's find)
 cudaError_t launch_jpeg_entropy(const JpegDecodeParams& p, cudaStream_t stream, bool found = false);
 cudaError_t launch_jpeg_reconstruct(const JpegDecodeParams& p, int n_tiles, cudaStream_t stream);
 cudaError_t launch_jpeg_index(const JpegDecodeParams& p, cudaStream_t stream);

@@ -830,18 +830,14 @@ def build_jpeg_index(encoded: EncodedImages, find=False):
         d_first = torch.from_numpy(cap_first).to(dev)
         d_points = torch.empty(max(total, 1) * 16, dtype=torch.uint8, device=dev)
         d_count = torch.empty(B, dtype=torch.int32, device=dev)
+        args = (hdr0, encoded.device_headers().data_ptr(), encoded.device_pool().data_ptr(), len(encoded.pool),
+                encoded.storage.data_ptr(), B, cap_first.ctypes.data, d_first.data_ptr(), d_points.data_ptr(),
+                d_count.data_ptr())
         if find:
-            check(lib.faa_jpeg_index_find(hdr0, encoded.device_headers().data_ptr(), encoded.device_pool().data_ptr(),
-                                          len(encoded.pool), encoded.storage.data_ptr(), B, cap_first.ctypes.data,
-                                          d_first.data_ptr(), d_points.data_ptr(), d_count.data_ptr(), _stream_ptr(dev)))
-            count = d_count.cpu().numpy()
-            pts = d_points.cpu().numpy()[:total * 16].view(_lib.JPEG_SYNC_DTYPE)
-            return compact_jpeg_index(cap_first, count, pts)
-        d_status = torch.empty(B, dtype=torch.int32, device=dev)
-        check(lib.faa_jpeg_index_build(hdr0, encoded.device_headers().data_ptr(), encoded.device_pool().data_ptr(),
-                                       len(encoded.pool), encoded.storage.data_ptr(), B, cap_first.ctypes.data,
-                                       d_first.data_ptr(), d_points.data_ptr(), d_count.data_ptr(),
-                                       d_status.data_ptr(), _stream_ptr(dev)))
+            check(lib.faa_jpeg_index_find(*args, _stream_ptr(dev)))
+        else:
+            d_status = torch.empty(B, dtype=torch.int32, device=dev)
+            check(lib.faa_jpeg_index_build(*args, d_status.data_ptr(), _stream_ptr(dev)))
         count = d_count.cpu().numpy()
         pts = d_points.cpu().numpy()[:total * 16].view(_lib.JPEG_SYNC_DTYPE)
     return compact_jpeg_index(cap_first, count, pts)
@@ -849,7 +845,7 @@ def build_jpeg_index(encoded: EncodedImages, find=False):
 
 def jpeg_index_capacities(headers):
     """int64 [N + 1] offsets giving each file of ``headers`` (``JPEG_HEADER_DTYPE``) room for the most points it can
-    get (``faa_jpeg_index_capacity``): the layout ``faa_jpeg_index_build`` and ``faa_jpeg_decode_recording`` write into"""
+    get (``faa_jpeg_index_capacity``): the layout ``faa_jpeg_index_build`` and a recording ``faa_jpeg_decode`` write into"""
     hdr0, size = headers.ctypes.data, headers.itemsize
     caps = np.array([lib.faa_jpeg_index_capacity(hdr0 + i * size) for i in range(len(headers))], np.int64)
     return np.concatenate([[0], np.cumsum(caps)]).astype(np.int64)
@@ -892,27 +888,27 @@ _DECODERS = {}
 
 
 def decode_jpeg(encoded: EncodedImages, out: RaggedImages | None = None, record=False, find=False):
-    """Decode every file of ``encoded`` on its device (C ABI ``faa_jpeg_decode``, or ``faa_jpeg_decode_indexed`` when
-    the files carry a scan index: two launches, no host wait), bit-exact
+    """Decode every file of ``encoded`` on its device (C ABI ``faa_jpeg_decode``, with the files' scan index when they
+    carry one: two launches, no host wait), bit-exact
     with ``Image.open(f).convert('RGB')`` (reference imagenet.py:80).  Returns ``(images, status)``: a ``RaggedImages``
     (``out``, by default ``RaggedImages.empty(encoded.sizes)``) and an int32 CUDA tensor of ``faa_jpeg_status`` bits per
     image, 0 where the scan decoded completely; a corrupt image still gets defined pixels.
 
-    ``record=True`` (``faa_jpeg_decode_recording``, same pixels and status, still no host wait) also records the scan
+    ``record=True`` (the call's recording outputs, same pixels and status, still no host wait) also records the scan
     index of every file the decode ran serially as a whole (no points, or points that failed their checks) and returns
     ``(images, status, count, points, cap_first)``: ``count`` int32 [N] and ``points`` (uint8, the bytes of
     ``JPEG_SYNC_DTYPE`` points) CUDA tensors, file i's ``count[i]`` new points at point ``cap_first[i]``
     (``jpeg_index_capacities``, host int64 [N + 1]).  ``count[i] > 0`` means these are file i's points now;
     ``compact_jpeg_index`` turns them into ``build_jpeg_index``'s form.
 
-    ``find=True`` (``faa_jpeg_decode_found``: three launches, still no host wait) first finds, in parallel, the scan
+    ``find=True`` (the call's ``find`` flag: three launches, still no host wait) first finds, in parallel, the scan
     index of every restart-free file that carries none, then decodes every file with its points, so such files decode on
     many threads without a saved index.  Same pixels and status; the return values keep their shapes, with and without
     ``record``.  With ``record``, ``count[i] > 0`` still means "these are file i's points now": the found index when its
     chain converged, or the serial decode's recording when the file's points could not be used.
 
     Progressive files (``EncodedImages.from_bytes(..., progressive=True)``) are decoded by
-    ``faa_jpeg_decode_progressive`` into the same images, the other files of the batch by the calls above (``select``
+    ``faa_jpeg_decode_progressive`` into the same images, the other files of the batch by the call above (``select``
     copies no byte of them); status comes back in batch order.  They get no scan index: count 0 with ``record=True``,
     and points given to them are not used."""
     _require_cuda(encoded.storage, "encoded")
@@ -978,33 +974,18 @@ def _decode_baseline(encoded: EncodedImages, out: RaggedImages, record, find=Fal
         return (out, status, count, points, cap_first) if record else (out, status)
     h_out, d_out = out.descriptors()
     with torch.cuda.device(dev):
-        dec = _decoder(dev)
-        if record or find:
-            d_first = d_points = None
-            if encoded.first is not None:
-                d_first, d_points = encoded.device_index()
-            d_cap_first = torch.from_numpy(cap_first).to(dev)
-            call = lib.faa_jpeg_decode_found if find else lib.faa_jpeg_decode_recording
-            check(call(
-                dec.handle, encoded.headers.ctypes.data, encoded.device_headers().data_ptr(),
-                encoded.device_pool().data_ptr(), len(encoded.pool), encoded.storage.data_ptr(), B, h_out.ctypes.data,
-                d_out.data_ptr(), status.data_ptr(), None if d_points is None else d_points.data_ptr(),
-                None if encoded.first is None else encoded.first.ctypes.data,
-                None if d_first is None else d_first.data_ptr(), cap_first.ctypes.data, d_cap_first.data_ptr(),
-                points.data_ptr(), count.data_ptr(), _stream_ptr(dev)))
-            return (out, status, count, points, cap_first) if record else (out, status)
-        if encoded.first is None:
-            check(lib.faa_jpeg_decode(dec.handle, encoded.headers.ctypes.data, encoded.device_headers().data_ptr(),
-                                      encoded.device_pool().data_ptr(), len(encoded.pool), encoded.storage.data_ptr(), B,
-                                      h_out.ctypes.data, d_out.data_ptr(), status.data_ptr(), _stream_ptr(dev)))
-        else:
+        index, rec = (None,) * 3, (None,) * 4            # the C call's optional groups: scan index in, recording out
+        if encoded.first is not None:
             d_first, d_points = encoded.device_index()
-            check(lib.faa_jpeg_decode_indexed(dec.handle, encoded.headers.ctypes.data, encoded.device_headers().data_ptr(),
-                                              encoded.device_pool().data_ptr(), len(encoded.pool),
-                                              encoded.storage.data_ptr(), B, h_out.ctypes.data, d_out.data_ptr(),
-                                              status.data_ptr(), d_points.data_ptr(), encoded.first.ctypes.data,
-                                              d_first.data_ptr(), _stream_ptr(dev)))
-    return out, status
+            index = (d_points.data_ptr(), encoded.first.ctypes.data, d_first.data_ptr())
+        if record or find:
+            d_cap_first = torch.from_numpy(cap_first).to(dev)
+            rec = (cap_first.ctypes.data, d_cap_first.data_ptr(), points.data_ptr(), count.data_ptr())
+        check(lib.faa_jpeg_decode(_decoder(dev).handle, encoded.headers.ctypes.data, encoded.device_headers().data_ptr(),
+                                  encoded.device_pool().data_ptr(), len(encoded.pool), encoded.storage.data_ptr(), B,
+                                  h_out.ctypes.data, d_out.data_ptr(), status.data_ptr(), *index, *rec, int(find),
+                                  _stream_ptr(dev)))
+    return (out, status, count, points, cap_first) if record else (out, status)
 
 
 def _augment_ragged(policy, batch: RaggedImages, tail, samples, boxes, rng, out):

@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define FAA_ABI_VERSION 1
+#define FAA_ABI_VERSION 2
 #define FAA_MAX_FUSED_OPS 2      /* ops of one sub-policy applied by one launch */
 #define FAA_MAX_POLICY_OPS 8     /* ops per sub-policy (search.py --num-op); >2 runs as chained launches */
 #define FAA_MAX_DIM 8192         /* max H or W */
@@ -366,16 +366,6 @@ typedef struct faa_jpeg_decoder faa_jpeg_decoder_t;
 int faa_jpeg_decoder_create(faa_jpeg_decoder_t** out);
 int faa_jpeg_decoder_destroy(faa_jpeg_decoder_t* dec);
 
-/* decodes `batch` files into uint8 HWC images.  h_headers / d_headers: host and device copies of the same headers (the
- * host copy validates and plans without waiting for the device); d_tables: the pool of n_tables entries; d_src: the
- * device bytes the headers' offsets point into; h_out / d_out: host and device copies of the destinations, each of its
- * header's size (rows packed, any byte offset); d_status: [batch] int32 (device), enum faa_jpeg_status bits.  A corrupt
- * scan never faults: its image gets a status and defined pixels.  Two launches (entropy decode, reconstruct), one
- * cudaMemcpyAsync of the per-call table, no host wait. */
-int faa_jpeg_decode(faa_jpeg_decoder_t* dec, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
-                    const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
-                    const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status, void* stream);
-
 /* ---- scan index: lets a file without restart markers be decoded by many threads.  One serial pass (faa_jpeg_index_build)
  * records the decoder's state at up to 127 MCU boundaries; every later decode of the file starts one thread at each of
  * them.  Placement: a scan of scan_len bytes with no restart interval is cut into P = min(128, scan_len / 1024) parts
@@ -403,31 +393,6 @@ int faa_jpeg_index_build(const faa_jpeg_header_t* h_headers, const faa_jpeg_head
                          const int64_t* h_first, const int64_t* d_first, faa_jpeg_sync_t* d_points, int32_t* d_count,
                          int32_t* d_status, void* stream);
 
-/* faa_jpeg_decode with a scan index: image i's points are d_points[first[i], first[i + 1]) (h_first / d_first: host and
- * device copies of int64 [batch + 1], validated on the host as in faa_jpeg_index_build).  The points are checked on the
- * device before use, and every segment's end state against the next point; a file whose index is invalid, stale or
- * from another file is decoded serially, so pixels and status always equal faa_jpeg_decode's.  Points of files with a
- * restart interval are ignored.  All three null: faa_jpeg_decode. */
-int faa_jpeg_decode_indexed(faa_jpeg_decoder_t* dec, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
-                            const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
-                            const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status,
-                            const faa_jpeg_sync_t* d_points, const int64_t* h_first, const int64_t* d_first, void* stream);
-
-/* faa_jpeg_decode_indexed (the input points may all be null) that also records the scan index of every file it decodes
- * serially as a whole: a file without points, or whose points failed their checks.  h_cap_first / d_cap_first: host
- * and device copies of int64 [batch + 1] offsets into d_points_out, laid out and validated as faa_jpeg_index_build's
- * h_first / d_first (image i may get cap_first[i + 1] - cap_first[i] points, at most faa_jpeg_index_capacity of its
- * header).  d_count: [batch] int32, the points written at d_points_out + cap_first[i]; 0 for a file with a restart
- * interval, a scan the placement rule gives no points, a non-zero status, or points that were used as they stood.  So
- * count[i] > 0 means these are file i's points now.  Pixels and status equal faa_jpeg_decode's.  Two launches, no host
- * wait. */
-int faa_jpeg_decode_recording(faa_jpeg_decoder_t* dec, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
-                              const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
-                              const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status,
-                              const faa_jpeg_sync_t* d_points, const int64_t* h_first, const int64_t* d_first,
-                              const int64_t* h_cap_first, const int64_t* d_cap_first, faa_jpeg_sync_t* d_points_out,
-                              int32_t* d_count, void* stream);
-
 /* Finds the scan index of `batch` files in parallel, without a serial decode (inputs, offsets and points as
  * faa_jpeg_index_build, no status).  One CTA per file: thread k parses from a little before part k's threshold until its
  * parse meets an MCU boundary (Huffman streams self-synchronise), then decodes from there to the next part's threshold,
@@ -441,27 +406,48 @@ int faa_jpeg_index_find(const faa_jpeg_header_t* h_headers, const faa_jpeg_heade
                         const int64_t* h_first, const int64_t* d_first, faa_jpeg_sync_t* d_points, int32_t* d_count,
                         void* stream);
 
-/* faa_jpeg_decode_recording whose files without input points get their scan index found first (faa_jpeg_index_find,
- * into d_points_out), so that a restart-free file decodes on many threads without a saved index.  Same parameters, same
- * meaning: files with input points keep them; pixels and status equal faa_jpeg_decode's whatever the find produced;
- * count[i] > 0 means these are file i's points now: the found index when its chain converged and was used, or the
- * serial decode's recording when the file's points (given or found) could not be used.  A found prefix that did not
- * converge is used for the decode and gets count 0.  Three launches (find, entropy decode, reconstruct), no host
- * wait. */
-int faa_jpeg_decode_found(faa_jpeg_decoder_t* dec, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
-                          const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
-                          const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status,
-                          const faa_jpeg_sync_t* d_points, const int64_t* h_first, const int64_t* d_first,
-                          const int64_t* h_cap_first, const int64_t* d_cap_first, faa_jpeg_sync_t* d_points_out,
-                          int32_t* d_count, void* stream);
+/* decodes `batch` baseline files into uint8 HWC images.  h_headers / d_headers: host and device copies of the same
+ * headers (the host copy validates and plans without waiting for the device); d_tables: the pool of n_tables entries;
+ * d_src: the device bytes the headers' offsets point into; h_out / d_out: host and device copies of the destinations,
+ * each of its header's size (rows packed, any byte offset); d_status: [batch] int32 (device), enum faa_jpeg_status bits.
+ * A corrupt scan never faults: its image gets a status and defined pixels.  Two launches (entropy decode, reconstruct),
+ * one cudaMemcpyAsync of the per-call table, no host wait.
+ *
+ * Two optional groups of arguments, each all null or given; a group that is given is validated on the host as
+ * faa_jpeg_index_build's offsets and points are (FAA_ERR_VALUE for a missing array or bad offsets):
+ *   - scan index in (d_points, h_first, d_first): image i's points are d_points[first[i], first[i + 1]), host and device
+ *     copies of int64 [batch + 1] offsets; d_points may be null when the offsets give no image a point.  The points are
+ *     checked on the device before use, and every segment's end state against the next point; a file whose index is
+ *     invalid, stale or from another file is decoded serially.  Points of files with a restart interval are ignored.
+ *   - recording out (h_cap_first, d_cap_first, d_points_out, d_count): the decode also records the scan index of every
+ *     file it decodes serially as a whole (a file without points, or whose points failed their checks) into d_points_out,
+ *     laid out as faa_jpeg_index_build's: image i may get cap_first[i + 1] - cap_first[i] points, at most
+ *     faa_jpeg_index_capacity of its header; d_points_out may be null when every capacity is 0.  d_count: [batch] int32,
+ *     the points written at d_points_out + cap_first[i]; 0 for a file with a restart interval, a scan the placement rule
+ *     gives no points, a non-zero status, or points that were used as they stood.  So count[i] > 0 means these are
+ *     file i's points now.
+ * find != 0 needs the recording group (FAA_ERR_VALUE without it): the files without input points first get their scan
+ * index found in parallel (faa_jpeg_index_find, into d_points_out), so that a restart-free file decodes on many threads
+ * without a saved index; files with input points keep them.  count[i] > 0 still means these are file i's points now:
+ * the found index when its chain converged and was used, or the serial decode's recording when the file's points (given
+ * or found) could not be used.  A found prefix that did not converge is used for the decode and gets count 0.  Three
+ * launches (find, entropy decode, reconstruct), no host wait.
+ *
+ * Whatever the index holds, given or found, pixels and status equal those of the decode without one. */
+int faa_jpeg_decode(faa_jpeg_decoder_t* dec, const faa_jpeg_header_t* h_headers, const faa_jpeg_header_t* d_headers,
+                    const faa_jpeg_table_t* d_tables, int n_tables, const uint8_t* d_src, int batch,
+                    const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status,
+                    const faa_jpeg_sync_t* d_points, const int64_t* h_first, const int64_t* d_first,
+                    const int64_t* h_cap_first, const int64_t* d_cap_first, faa_jpeg_sync_t* d_points_out,
+                    int32_t* d_count, int find, void* stream);
 
 /* ---- progressive JPEG decode (SOF2 Huffman), for callers that opt in: the files faa_jpeg_parse takes, coded
  * progressively, bit-exact with Pillow as above.  The parse accepts a file only when every coefficient of every component
  * ends at bit 0 (libjpeg smooths the blocks of an incomplete progression, which is not modelled), with at most
  * FAA_JPEG_MAX_SCANS scans; multi-scan sequential, arithmetic coding and the rest stay refused.  Its header has
  * reserved = FAA_JPEG_PROGRESSIVE, restart = 0 and no scan_off / scan_len, and its quantisation tables are those in force at
- * each component's first scan.  faa_jpeg_decode, _indexed, _recording and faa_jpeg_index_build refuse such a header with
- * FAA_ERR_VALUE, and faa_jpeg_index_capacity gives it 0: progressive files have no scan index. */
+ * each component's first scan.  faa_jpeg_decode, faa_jpeg_index_build and faa_jpeg_index_find refuse such a header
+ * with FAA_ERR_VALUE, and faa_jpeg_index_capacity gives it 0: progressive files have no scan index. */
 #define FAA_JPEG_PROGRESSIVE 1
 #define FAA_JPEG_MAX_SCANS 64
 typedef struct faa_jpeg_scan {

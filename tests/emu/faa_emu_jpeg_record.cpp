@@ -13,7 +13,7 @@ using namespace faa;
 extern "C" {
 
 // Decodes a file with npts points (none: pts null) into out (h * w * 3 bytes, out_cap at most) and, with coef, its
-// coefficients (coef_cap int16 at most).  With rec_count it records as faa_jpeg_decode_recording does: points into
+// coefficients (coef_cap int16 at most).  With rec_count it records as a recording faa_jpeg_decode does: points into
 // rec_at[0, rec_cap), their number in *rec_count.  hw gets the size.  Returns the parse result (JPARSE_*); the decode
 // runs only when the file parses and out and coef have room.
 int faa_emu_jpeg_decode_recording(const uint8_t* bytes, int64_t len, const JpegSync* pts, int64_t npts, uint8_t* out,

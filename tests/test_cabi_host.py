@@ -30,7 +30,7 @@ def test_every_header_symbol_is_exported():
     for n in sorted(names):
         assert hasattr(lib, n), n
     assert set(_lib.EXPORTS) == names
-    assert lib.faa_abi_version() == 1
+    assert lib.faa_abi_version() == 2
 
 
 def test_op_registry_matches_reference_augment_list():

@@ -1,5 +1,5 @@
 """The scan index found on the device in parallel (``build_jpeg_index(find=True)``, C ABI ``faa_jpeg_index_find``) and
-the decode that finds one first (``decode_jpeg(find=True)``, ``faa_jpeg_decode_found``).  The found points equal the
+the decode that finds one first (``decode_jpeg(find=True)``, ``faa_jpeg_decode`` with ``find``).  The found points equal the
 host build's (tests/emu/faa_emu_jpeg_find.cpp at the kernel's window and rounds) byte for byte, and
 ``build_jpeg_index``'s where the chain converged; the found decode's pixels and status equal the plain decode's on the
 grid, the geometry streams, the adversarial streams and corrupt files; a batch mixing given, stale, foreign and absent
@@ -186,10 +186,10 @@ def test_abi_refuses_progressive_headers_and_bad_offsets():
                                             f.ctypes.data, d_f.data_ptr(), pts.data_ptr(), cnt.data_ptr(), None)
 
     def decode_call(e, f, d_f):
-        return _lib.lib.faa_jpeg_decode_found(dec.handle, e.headers.ctypes.data, e.device_headers().data_ptr(),
-                                              e.device_pool().data_ptr(), len(e.pool), e.storage.data_ptr(), 2,
-                                              h_out.ctypes.data, d_out.data_ptr(), st.data_ptr(), None, None, None,
-                                              f.ctypes.data, d_f.data_ptr(), pts.data_ptr(), cnt.data_ptr(), None)
+        return _lib.lib.faa_jpeg_decode(dec.handle, e.headers.ctypes.data, e.device_headers().data_ptr(),
+                                        e.device_pool().data_ptr(), len(e.pool), e.storage.data_ptr(), 2,
+                                        h_out.ctypes.data, d_out.data_ptr(), st.data_ptr(), None, None, None,
+                                        f.ctypes.data, d_f.data_ptr(), pts.data_ptr(), cnt.data_ptr(), 1, None)
     for call in (find_call, decode_call):
         assert call(enc, good, d_good) == _lib.OK
         assert call(pen, good, d_good) == _lib.ERR_VALUE

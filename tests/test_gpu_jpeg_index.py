@@ -1,5 +1,5 @@
 """The JPEG scan index on the device: ``build_jpeg_index`` (C ABI ``faa_jpeg_index_build``) equals the host build's
-index byte for byte, and ``decode_jpeg`` with an index (``faa_jpeg_decode_indexed``) equals the decode without one, in
+index byte for byte, and ``decode_jpeg`` with an index (``faa_jpeg_decode``'s input points) equals the decode without one, in
 pixels and status, on the decoder grid, the geometry streams, fuzzed indexes, 1, 2 and 128 segments and a batch that
 mixes indexed, stale, restart-marker and point-less files.  Then the index command on an ImageNet tree, and
 ``get_dataloaders('imagenet', ...)`` with and without ``conf['faa_jpeg_index']``."""
@@ -136,11 +136,11 @@ def test_abi_refuses_bad_offsets():
     for bad in ([1, 0, 2], [-1, 0, 0], [0, 2, 1]):
         f = np.array(bad, np.int64)
         d_f = torch.from_numpy(f).cuda()
-        e = _lib.lib.faa_jpeg_decode_indexed(dec.handle, enc.headers.ctypes.data, enc.device_headers().data_ptr(),
-                                             enc.device_pool().data_ptr(), len(enc.pool), enc.storage.data_ptr(), 2,
-                                             h_out.ctypes.data, d_out.data_ptr(), st.data_ptr(),
-                                             enc.with_index(first, points).device_index()[1].data_ptr(),
-                                             f.ctypes.data, d_f.data_ptr(), None)
+        e = _lib.lib.faa_jpeg_decode(dec.handle, enc.headers.ctypes.data, enc.device_headers().data_ptr(),
+                                     enc.device_pool().data_ptr(), len(enc.pool), enc.storage.data_ptr(), 2,
+                                     h_out.ctypes.data, d_out.data_ptr(), st.data_ptr(),
+                                     enc.with_index(first, points).device_index()[1].data_ptr(),
+                                     f.ctypes.data, d_f.data_ptr(), None, None, None, None, 0, None)
         assert e == _lib.ERR_VALUE
         cnt = torch.empty(2, dtype=torch.int32, device="cuda")
         e = _lib.lib.faa_jpeg_index_build(enc.headers.ctypes.data, enc.device_headers().data_ptr(),

@@ -1,4 +1,4 @@
-"""The recording JPEG decode on the device (``decode_jpeg(record=True)``, C ABI ``faa_jpeg_decode_recording``): its
+"""The recording JPEG decode on the device (``decode_jpeg(record=True)``, C ABI ``faa_jpeg_decode`` with its recording outputs): its
 pixels and status equal the plain decode's, and its compacted points equal ``build_jpeg_index``'s byte for byte, on the
 decoder grid, the geometry streams and a batch mixing used, stale, foreign and absent points; a recording call queued
 behind a call that grows the decoder's buffers.  Then ``conf['faa_jpeg_index_learn']`` on an ImageNet tree: the same
@@ -118,10 +118,10 @@ def test_abi_refuses_bad_capacity_offsets():
     for bad in ([1, 0, 2], [-1, 0, 0], [0, 2, 1]):
         f = np.array(bad, np.int64)
         d_f = torch.from_numpy(f).cuda()
-        e = _lib.lib.faa_jpeg_decode_recording(dec.handle, enc.headers.ctypes.data, enc.device_headers().data_ptr(),
-                                               enc.device_pool().data_ptr(), len(enc.pool), enc.storage.data_ptr(), 2,
-                                               h_out.ctypes.data, d_out.data_ptr(), st.data_ptr(), None, None, None,
-                                               f.ctypes.data, d_f.data_ptr(), pts.data_ptr(), cnt.data_ptr(), None)
+        e = _lib.lib.faa_jpeg_decode(dec.handle, enc.headers.ctypes.data, enc.device_headers().data_ptr(),
+                                     enc.device_pool().data_ptr(), len(enc.pool), enc.storage.data_ptr(), 2,
+                                     h_out.ctypes.data, d_out.data_ptr(), st.data_ptr(), None, None, None,
+                                     f.ctypes.data, d_f.data_ptr(), pts.data_ptr(), cnt.data_ptr(), 0, None)
         assert e == _lib.ERR_VALUE
     torch.cuda.synchronize()
 
