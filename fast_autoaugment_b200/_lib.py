@@ -117,11 +117,9 @@ def _load():
         "faa_jpeg_index_build": (C.c_int, [vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp]),
         "faa_jpeg_index_find": (C.c_int, [vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp]),
         "faa_jpeg_decode": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp,
-                                      C.c_int, vp]),
+                                      vp, vp, vp, vp, C.c_int, vp]),
         "faa_jpeg_parse_progressive": (C.c_int, [C.c_char_p, C.c_size_t, vp, vp, C.c_int, P(C.c_int)]),
         "faa_jpeg_scan_tables": (C.c_int, [C.c_char_p, C.c_size_t, vp, vp, C.c_int, vp]),
-        "faa_jpeg_decode_progressive": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp,
-                                                  vp]),
         "faa_launch_count": (u64, []),
     }
     for name, (res, args) in sig.items():

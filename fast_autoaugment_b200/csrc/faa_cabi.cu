@@ -1606,12 +1606,17 @@ static int grow_async(void** ptr, size_t* have, size_t need, cudaStream_t stream
     return FAA_OK;
 }
 
-// a header the decode calls take: baseline (the quantisation and both Huffman pool slots of every component), or with
-// `progressive` a progressive one (quantisation slots only: the Huffman tables are the scans')
-static int check_jpeg_header(const JpegHeader& h, int n_tables, const std::string& who, bool progressive = false) {
-    if (jpeg_is_progressive(h) != progressive)
-        return fail(FAA_ERR_VALUE, who + (progressive ? ": not a progressive header (faa_jpeg_decode takes it)"
-                                                      : ": a progressive header (faa_jpeg_decode_progressive takes it)"));
+// a header the JPEG device calls take: baseline (the quantisation and both Huffman pool slots of every component), or,
+// when the call gives scans, a progressive one (quantisation slots only: the Huffman tables are the scans').  A
+// progressive header's byte ranges and restart intervals are its scans'; its own must be 0, because the find kernel
+// gives it no work only through scan_len == 0 and would otherwise build tables from its unchecked Huffman slots.
+static int check_jpeg_header(const JpegHeader& h, int n_tables, const std::string& who, bool scans = false) {
+    const bool progressive = jpeg_is_progressive(h);
+    if (progressive && !scans)
+        return fail(FAA_ERR_VALUE, who + ": a progressive header needs the scans group (h_scans, d_scans, h_scan_first, "
+                                         "d_scan_first) of faa_jpeg_decode");
+    if (progressive && (h.scan_off != 0 || h.scan_len != 0 || h.restart != 0))
+        return fail(FAA_ERR_VALUE, who + ": a progressive header has no scan range or restart interval of its own");
     if (h.ncomp != 1 && h.ncomp != 3) return fail(FAA_ERR_VALUE, who + ": component count must be 1 or 3");
     if (check_shape(h.h, h.w)) return fail(FAA_ERR_VALUE, who + ": size out of range");
     const bool samp = h.ncomp == 1 ? (h.hs == 1 && h.vs == 1)
@@ -1701,10 +1706,10 @@ static int check_jpeg_batch(int batch) {
 }
 
 // check_jpeg_header of every image of a call
-static int check_jpeg_headers(const faa_jpeg_header_t* h_headers, int batch, int n_tables, bool progressive = false) {
+static int check_jpeg_headers(const faa_jpeg_header_t* h_headers, int batch, int n_tables, bool scans = false) {
     for (int i = 0; i < batch; ++i) {
         JpegHeader h; memcpy(&h, &h_headers[i], sizeof h);
-        if (int e = check_jpeg_header(h, n_tables, "image " + std::to_string(i), progressive)) return e;
+        if (int e = check_jpeg_header(h, n_tables, "image " + std::to_string(i), scans)) return e;
     }
     return FAA_OK;
 }
@@ -1796,8 +1801,9 @@ static int check_jpeg_scans(const JpegHeader& h, const JpegScan* scans, int64_t 
 
 // The JpegJob table of a decode call whose headers are checked: jobs[i] holds where image i's coefficient blocks,
 // restart-segment starts and reconstruct tiles begin, jobs[batch] the totals.  Also checks each image's output
-// descriptor, and with `scans` (a progressive call: image i's scans are scans[scan_first[i], scan_first[i + 1])) its
-// scans, whose segments it counts where a baseline image has jpeg_segments.
+// descriptor and, when the call gives scans (image i's are scans[scan_first[i], scan_first[i + 1])), each image's
+// scans: a progressive image's, whose segments it counts where a baseline image has jpeg_segments, and that a baseline
+// image has none.
 static int plan_jpeg_jobs(const faa_jpeg_header_t* h_headers, const faa_image_t* h_out, int batch, int n_tables,
                           const JpegScan* scans, const int64_t* scan_first, std::vector<JpegJob>& jobs) {
     jobs.resize((size_t)batch + 1);
@@ -1809,9 +1815,11 @@ static int plan_jpeg_jobs(const faa_jpeg_header_t* h_headers, const faa_image_t*
         if (h_out[i].h != h.h || h_out[i].w != h.w) return fail(FAA_ERR_VALUE, "output " + who + " is not the size of its JPEG");
         jobs[(size_t)i] = {blocks, (int32_t)segs, (int32_t)tiles};
         blocks += jpeg_image_blocks(h);
-        if (!scans) {
+        if (!jpeg_is_progressive(h)) {
+            if (scans && scan_first[i + 1] != scan_first[i])
+                return fail(FAA_ERR_VALUE, who + ": a baseline image owns no scans");
             segs += jpeg_segments(h);
-        } else {
+        } else {                                   // (check_jpeg_headers refused it if the call gives no scans)
             const int64_t n = scan_first[i + 1] - scan_first[i];
             if (int e = check_jpeg_scans(h, scans + scan_first[i], n, n_tables, who)) return e;
             for (int64_t k = 0; k < n; ++k) segs += jpeg_scan_segments(h, scans[scan_first[i] + k]);
@@ -1825,8 +1833,8 @@ static int plan_jpeg_jobs(const faa_jpeg_header_t* h_headers, const faa_image_t*
 
 // Binds the handle to the current device, orders this call's use of its scratch after the previous call's, grows the
 // coefficient, segment and job buffers to what the call's job table needs and uploads the table.  Every decode call
-// goes through here, under the handle's lock until its launches are queued, so calls of either kind may follow each
-// other on any streams.
+// goes through here, under the handle's lock until its launches are queued, so calls may follow each other on any
+// streams.
 static int jpeg_call_scratch(faa_jpeg_decoder_t* d, cudaStream_t stream, const std::vector<JpegJob>& jobs) {
     int dev = -1;
     if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); return fail(FAA_ERR_NO_DEVICE, "no current CUDA device"); }
@@ -1854,12 +1862,14 @@ int faa_jpeg_decode(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, c
                     const faa_image_t* h_out, const faa_image_t* d_out, int32_t* d_status,
                     const faa_jpeg_sync_t* d_points, const int64_t* h_first, const int64_t* d_first,
                     const int64_t* h_cap_first, const int64_t* d_cap_first, faa_jpeg_sync_t* d_points_out,
-                    int32_t* d_count, int find, void* stream_v) {
+                    int32_t* d_count, const faa_jpeg_scan_t* h_scans, const faa_jpeg_scan_t* d_scans,
+                    const int64_t* h_scan_first, const int64_t* d_scan_first, int find, void* stream_v) {
     if (!d || ((!h_headers || !d_headers || !d_tables || !d_src || !h_out || !d_out || !d_status) && batch > 0))
         return fail(FAA_ERR_VALUE, "null argument");
     if (int e = check_jpeg_batch(batch)) return e;
     const bool indexed = d_points || h_first || d_first;
     const bool recording = h_cap_first || d_cap_first || d_points_out || d_count;
+    const bool scans = h_scans || d_scans || h_scan_first || d_scan_first;
     if (find && !recording)
         return fail(FAA_ERR_VALUE, "find needs the recording outputs h_cap_first, d_cap_first, d_points_out and d_count");
     if (recording && batch > 0) {
@@ -1872,11 +1882,20 @@ int faa_jpeg_decode(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, c
         if (int e = check_jpeg_first(h_first, batch)) return e;
         if (!d_points && h_first[batch] > h_first[0]) return fail(FAA_ERR_VALUE, "null argument: d_points");
     }
-    if (int e = check_jpeg_headers(h_headers, batch, n_tables)) return e;
+    if (scans && batch > 0) {
+        if (!h_scans || !d_scans || !h_scan_first || !d_scan_first)
+            return fail(FAA_ERR_VALUE, "null argument: scans need h_scans, d_scans, h_scan_first and d_scan_first");
+        if (int e = check_jpeg_first(h_scan_first, batch)) return e;
+    }
+    if (int e = check_jpeg_headers(h_headers, batch, n_tables, scans)) return e;
     std::vector<JpegJob> jobs;
-    if (int e = plan_jpeg_jobs(h_headers, h_out, batch, n_tables, nullptr, nullptr, jobs)) return e;
+    if (int e = plan_jpeg_jobs(h_headers, h_out, batch, n_tables, reinterpret_cast<const JpegScan*>(h_scans), h_scan_first,
+                               jobs))
+        return e;
     if (int e = ensure_device()) return e;
     if (batch == 0) return FAA_OK;
+    const int n_prog = (int)std::count_if(h_headers, h_headers + batch,
+                                          [](const faa_jpeg_header_t& h) { return h.reserved == FAA_JPEG_PROGRESSIVE; });
     cudaStream_t stream = (cudaStream_t)stream_v;
     std::lock_guard<std::mutex> lk(d->mu);
     if (int e = jpeg_call_scratch(d, stream, jobs)) return e;
@@ -1896,12 +1915,20 @@ int faa_jpeg_decode(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, c
     P.rec_first = d_cap_first;
     P.rec_points = reinterpret_cast<JpegSync*>(d_points_out);
     P.count = d_count;
-    if (find) {
-        CK(launch_jpeg_find(P, true, stream));
+    P.scans = reinterpret_cast<const JpegScan*>(d_scans);
+    P.scan_first = d_scan_first;
+    if (n_prog < batch) {
+        if (find) {
+            CK(launch_jpeg_find(P, true, stream));
+            g_launches++;
+        }
+        CK(launch_jpeg_entropy(P, stream, find != 0));
         g_launches++;
     }
-    CK(launch_jpeg_entropy(P, stream, find != 0));
-    g_launches++;
+    if (n_prog > 0) {
+        CK(launch_jpeg_progressive(P, stream));
+        g_launches++;
+    }
     CK(launch_jpeg_reconstruct(P, jobs.back().tile0, stream));
     g_launches++;
     return FAA_OK;
@@ -1909,7 +1936,7 @@ int faa_jpeg_decode(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, c
 
 }  // extern "C"
 
-// ------------------------------------------------------------------ progressive JPEG decode --
+// ------------------------------------------------------------------ progressive JPEG parse --
 static_assert(sizeof(faa_jpeg_scan_t) == sizeof(JpegScan) && sizeof(JpegScan) == 112 &&
               offsetof(faa_jpeg_scan_t, pool) == offsetof(JpegScan, pool) && FAA_JPEG_MAX_SCANS == kJpegMaxScans &&
               FAA_JPEG_PROGRESSIVE == kJpegProgressive, "JPEG scan layout");
@@ -1950,54 +1977,6 @@ int faa_jpeg_scan_tables(const uint8_t* bytes, size_t len, const faa_jpeg_header
             if (total > 256 || (size_t)at + 16 + total > len) return fail(FAA_ERR_VALUE, "Huffman table outside the file");
         }
     jpeg_progressive_tables(bytes, h, s, n_scans, reinterpret_cast<JpegTable*>(out));
-    return FAA_OK;
-}
-
-int faa_jpeg_decode_progressive(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers,
-                                const faa_jpeg_header_t* d_headers, const faa_jpeg_table_t* d_tables, int n_tables,
-                                const uint8_t* d_src, int batch, const faa_image_t* h_out, const faa_image_t* d_out,
-                                int32_t* d_status, const faa_jpeg_scan_t* h_scans, const faa_jpeg_scan_t* d_scans,
-                                const int64_t* h_scan_first, const int64_t* d_scan_first, void* stream_v) {
-    if (!d || ((!h_headers || !d_headers || !d_tables || !d_src || !h_out || !d_out || !d_status || !h_scans || !d_scans ||
-                !h_scan_first || !d_scan_first) && batch > 0))
-        return fail(FAA_ERR_VALUE, "null argument");
-    if (int e = check_jpeg_batch(batch)) return e;
-    if (batch > 0)
-        if (int e = check_jpeg_first(h_scan_first, batch)) return e;
-    if (int e = check_jpeg_headers(h_headers, batch, n_tables, true)) return e;
-    std::vector<JpegJob> jobs;
-    if (int e = plan_jpeg_jobs(h_headers, h_out, batch, n_tables, reinterpret_cast<const JpegScan*>(h_scans), h_scan_first,
-                               jobs))
-        return e;
-    if (int e = ensure_device()) return e;
-    if (batch == 0) return FAA_OK;
-    cudaStream_t stream = (cudaStream_t)stream_v;
-    std::lock_guard<std::mutex> lk(d->mu);
-    if (int e = jpeg_call_scratch(d, stream, jobs)) return e;
-    JpegProgressiveParams Q = {};
-    Q.hdrs = reinterpret_cast<const JpegHeader*>(d_headers);
-    Q.pool = reinterpret_cast<const JpegTable*>(d_tables);
-    Q.src = d_src;
-    Q.jobs = reinterpret_cast<const JpegJob*>(d->d_jobs);
-    Q.scans = reinterpret_cast<const JpegScan*>(d_scans);
-    Q.scan_first = d_scan_first;
-    Q.coef = reinterpret_cast<int16_t*>(d->d_coef);
-    Q.segs = reinterpret_cast<int32_t*>(d->d_segs);
-    Q.status = d_status;
-    Q.batch = batch;
-    CK(launch_jpeg_progressive(Q, stream));
-    g_launches++;
-    JpegDecodeParams P = {};
-    P.hdrs = Q.hdrs;
-    P.pool = Q.pool;
-    P.src = d_src;
-    P.jobs = Q.jobs;
-    P.out = reinterpret_cast<const CropImage*>(d_out);
-    P.coef = Q.coef;
-    P.status = d_status;
-    P.batch = batch;
-    CK(launch_jpeg_reconstruct(P, jobs.back().tile0, stream));
-    g_launches++;
     return FAA_OK;
 }
 

@@ -1,7 +1,9 @@
-// faa_jpeg.cu - sm_90a kernels of the baseline JPEG decoder (faa_jpeg_decode), arithmetic in faa_jpeg.cuh.
+// faa_jpeg.cu - sm_90a kernels of the JPEG decoder (faa_jpeg_decode), arithmetic in faa_jpeg.cuh.
 //
-// Two launches per call, no host wait between them:
-//   faa_jpeg_entropy_kernel      one CTA per image.  The CTA builds the image's Huffman lookup tables in shared
+// A call launches, with no host wait between them, the find kernel (with find), the entropy kernel (when the batch has
+// baseline images), the progressive kernel (when it has progressive images) and the reconstruct kernel over every
+// image.  The two entropy kernels have one CTA per image of the batch; each returns at once on the other's images.
+//   faa_jpeg_entropy_kernel      one CTA per baseline image.  The CTA builds the image's Huffman lookup tables in shared
 //                                memory; when the image has restart markers its threads find them in parallel (a
 //                                count, a prefix sum, then the positions); then one thread per restart segment turns
 //                                the scan into int16 coefficients.  An image without restart markers is one segment,
@@ -14,8 +16,8 @@
 //   faa_jpeg_find_kernel         (faa_jpeg_index_find, faa_jpeg_decode's find) one CTA per image; thread k finds point k
 //                                of the scan index in parallel, and links checked against the next point verify a
 //                                prefix of it.  The found decode's entropy instantiation reads the counts it leaves.
-//   faa_jpeg_progressive_kernel  (faa_jpeg_decode_progressive) one CTA per progressive image: the entropy stage of
-//                                progressive files, scans run wave by wave; the reconstruct kernel follows it.
+//   faa_jpeg_progressive_kernel  one CTA per progressive image: the entropy stage of progressive files, scans run wave
+//                                by wave.
 //   faa_jpeg_reconstruct_kernel  one CTA per 64 x 32 output tile of one image.  It runs the islow IDCT of the tile's
 //                                blocks, with the one-block chroma halo fancy upsampling reads, into shared memory,
 //                                upsamples and converts to RGB, and writes uint8 HWC rows with 32-bit stores where the
@@ -58,6 +60,7 @@ __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_entropy_kernel(const
     __shared__ int32_t s_count[kEntropyThreads];
     __shared__ int32_t s_status;
     const int img = blockIdx.x, tid = threadIdx.x;
+    if (P.hdrs[img].reserved == kJpegProgressive) return;     // faa_jpeg_progressive_kernel's (before h: DESIGN §4.8)
     const JpegHeader h = P.hdrs[img];
     const JpegJob job = P.jobs[img];
     const uint8_t* scan = P.src + h.offset + h.scan_off;
@@ -302,7 +305,7 @@ cudaError_t launch_jpeg_find(const JpegDecodeParams& p, bool mark, cudaStream_t 
 // more than kProgGroup scans) runs as several groups, one after the other.
 constexpr int kProgSlots = 8, kProgGroup = 16;
 
-__global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_progressive_kernel(const __grid_constant__ JpegProgressiveParams P) {
+__global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_progressive_kernel(const __grid_constant__ JpegDecodeParams P) {
     __shared__ JpegHuff s_huff[kProgSlots];
     __shared__ JpegScan s_scan[kJpegMaxScans];
     __shared__ int32_t s_seg[kJpegMaxScans];              // first segment-start entry of each scan
@@ -311,6 +314,7 @@ __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_progressive_kernel(c
     __shared__ int32_t s_gscan[kProgGroup], s_gslot[kProgGroup], s_gitem[kProgGroup + 1], s_gtab[kProgSlots];
     __shared__ int32_t s_ng, s_nslot, s_pos, s_status;
     const int img = blockIdx.x, tid = threadIdx.x;
+    if (P.hdrs[img].reserved != kJpegProgressive) return;     // faa_jpeg_entropy_kernel's
     const JpegHeader h = P.hdrs[img];
     const JpegJob job = P.jobs[img];
     const uint8_t* file = P.src + h.offset;
@@ -400,10 +404,13 @@ __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_progressive_kernel(c
     }
     if (status) atomicOr(&s_status, status);
     __syncthreads();
-    if (tid == 0) P.status[img] = s_status;
+    if (tid == 0) {
+        P.status[img] = s_status;
+        if (P.count) P.count[img] = 0;                  // a recording call's: progressive files have no scan index
+    }
 }
 
-cudaError_t launch_jpeg_progressive(const JpegProgressiveParams& p, cudaStream_t stream) {
+cudaError_t launch_jpeg_progressive(const JpegDecodeParams& p, cudaStream_t stream) {
     if (p.batch <= 0) return cudaSuccess;
     faa_jpeg_progressive_kernel<<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p);
     return cudaGetLastError();

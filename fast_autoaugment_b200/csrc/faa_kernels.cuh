@@ -135,10 +135,10 @@ cudaError_t launch_crop_resize(const uint8_t* in, const CropImage* images, void*
                                const CropCfg& cfg, const CropResizeTile& t, cudaStream_t stream);
 cudaError_t launch_lighting_tables(const float* rgb, float* tabs, int n, const float mean[3], const float std[3], cudaStream_t stream);
 
-// baseline JPEG decode (faa_jpeg.cu): what one faa_jpeg_decode call hands its two kernels
+// JPEG decode (faa_jpeg.cu): what one faa_jpeg_decode call hands its kernels
 struct JpegJob {                // per image of the call, plus one sentinel entry holding the total tile count
     int64_t coef;               // first block of the image's coefficient planes in `coef`
-    int32_t seg;                // first entry of the image's restart-segment starts in `segs`
+    int32_t seg;                // first entry of the image's restart-segment starts in `segs` (all its scans)
     int32_t tile0;              // first reconstruct CTA of the image
 };
 struct JpegDecodeParams {
@@ -159,6 +159,9 @@ struct JpegDecodeParams {
     // recording decode only (null otherwise): image i's recorded points go to rec_points[rec_first[i], rec_first[i + 1])
     const int64_t* rec_first;
     JpegSync* rec_points;
+    // progressive images (null when the call has none): image i's scans are scans[scan_first[i], scan_first[i + 1])
+    const JpegScan* scans;
+    const int64_t* scan_first;
 };
 // found: the found decode's instantiation (counts from faa_jpeg_find_kernel, faa_jpeg_decode's find)
 cudaError_t launch_jpeg_entropy(const JpegDecodeParams& p, cudaStream_t stream, bool found = false);
@@ -167,19 +170,8 @@ cudaError_t launch_jpeg_index(const JpegDecodeParams& p, cudaStream_t stream);
 // finds scan indexes into rec_points / rec_first, counts into count, skipping images with input points (first, may be
 // null); mark: a prefix that did not converge gets count ~n
 cudaError_t launch_jpeg_find(const JpegDecodeParams& p, bool mark, cudaStream_t stream);
-// progressive entropy decode (faa_jpeg_decode_progressive): one CTA per image; the reconstruct kernel follows it
-struct JpegProgressiveParams {
-    const JpegHeader* hdrs;     // [batch] (device copy)
-    const JpegTable* pool;
-    const uint8_t* src;
-    const JpegJob* jobs;        // [batch + 1]; seg: first entry of the image's segment starts (all its scans)
-    const JpegScan* scans;      // image i's scans are scans[scan_first[i], scan_first[i + 1])
-    const int64_t* scan_first;
-    int16_t* coef;
-    int32_t* segs;
-    int32_t* status;
-    int32_t batch;
-};
-cudaError_t launch_jpeg_progressive(const JpegProgressiveParams& p, cudaStream_t stream);
+// progressive entropy decode: one CTA per image, the baseline images' CTAs return at once (as the entropy kernel's do
+// for progressive images)
+cudaError_t launch_jpeg_progressive(const JpegDecodeParams& p, cudaStream_t stream);
 
 }  // namespace faa

@@ -907,9 +907,8 @@ def decode_jpeg(encoded: EncodedImages, out: RaggedImages | None = None, record=
     ``record``.  With ``record``, ``count[i] > 0`` still means "these are file i's points now": the found index when its
     chain converged, or the serial decode's recording when the file's points could not be used.
 
-    Progressive files (``EncodedImages.from_bytes(..., progressive=True)``) are decoded by
-    ``faa_jpeg_decode_progressive`` into the same images, the other files of the batch by the call above (``select``
-    copies no byte of them); status comes back in batch order.  They get no scan index: count 0 with ``record=True``,
+    Progressive files (``EncodedImages.from_bytes(..., progressive=True)``) are decoded by the same call from the scans
+    they carry, one more launch when the batch mixes both kinds.  They get no scan index: count 0 with ``record=True``,
     and points given to them are not used."""
     _require_cuda(encoded.storage, "encoded")
     dev = encoded.device
@@ -917,53 +916,6 @@ def decode_jpeg(encoded: EncodedImages, out: RaggedImages | None = None, record=
         out = RaggedImages.empty(encoded.sizes, dev)
     elif not isinstance(out, RaggedImages) or not np.array_equal(out.sizes, encoded.sizes) or out.device != dev:
         raise ValueError("out must be a RaggedImages of the files' sizes on their device")
-    prog = encoded.progressive()
-    if not prog.any():
-        return _decode_baseline(encoded, out, record, find)
-    B = len(encoded)
-    at = np.flatnonzero(~prog)
-    pat = np.flatnonzero(prog)
-    # The progressive files' scans are contiguous in encoded.scans (the others have none), so their call reuses the
-    # device copy of every scan with offsets scan_first[pat] + [end].  One upload carries those offsets and the
-    # permutation that puts the two calls' status (and counts) back in batch order.
-    p_first = np.concatenate([encoded.scan_first[pat], encoded.scan_first[-1:]]).astype(np.int64)
-    inv = np.argsort(np.concatenate([at, pat]), kind="stable").astype(np.int64)
-    d_small = torch.from_numpy(np.concatenate([inv, p_first])).to(dev)
-    d_scans, _ = encoded.device_scans()
-    p_enc = EncodedImages(encoded.storage, encoded.headers[pat], encoded.pool, encoded.device_pool(),
-                          scans=encoded.scans, scan_first=p_first, _d_scans=d_scans, _d_scan_first=d_small[B:])
-    p_out = out.select(pat)
-    res = _decode_baseline(encoded.select(at), out.select(at), record, find) if len(at) else None
-    p_status = torch.empty(len(pat), dtype=torch.int32, device=dev)
-    h_out, d_out = p_out.descriptors()
-    with torch.cuda.device(dev):
-        check(lib.faa_jpeg_decode_progressive(
-            _decoder(dev).handle, p_enc.headers.ctypes.data, p_enc.device_headers().data_ptr(),
-            p_enc.device_pool().data_ptr(), len(p_enc.pool), p_enc.storage.data_ptr(), len(pat), h_out.ctypes.data,
-            d_out.data_ptr(), p_status.data_ptr(), p_enc.scans.ctypes.data, d_scans.data_ptr(), p_first.ctypes.data,
-            p_enc.device_scans()[1].data_ptr(), _stream_ptr(dev)))
-        status = p_status if res is None else torch.cat([res[1], p_status])[d_small[:B]]
-        if not record:
-            return out, status
-        # a progressive file's capacity is 0, so the baseline files' capacity layout is the batch's
-        cap_first = jpeg_index_capacities(encoded.headers)
-        if res is None:
-            return out, status, torch.zeros(B, dtype=torch.int32, device=dev), \
-                torch.empty(16, dtype=torch.uint8, device=dev), cap_first
-        count = torch.cat([res[2], torch.zeros(len(pat), dtype=torch.int32, device=dev)])[d_small[:B]]
-    return out, status, count, res[3], cap_first
-
-
-def _decoder(dev):
-    dec = _DECODERS.get(dev.index)
-    if dec is None:
-        dec = _DECODERS[dev.index] = _JpegDecoder()
-    return dec
-
-
-def _decode_baseline(encoded: EncodedImages, out: RaggedImages, record, find=False):
-    """``decode_jpeg`` of a batch without progressive files"""
-    dev = encoded.device
     B = len(encoded)
     status = torch.empty(max(B, 1), dtype=torch.int32, device=dev)[:B]
     if record or find:
@@ -974,18 +926,30 @@ def _decode_baseline(encoded: EncodedImages, out: RaggedImages, record, find=Fal
         return (out, status, count, points, cap_first) if record else (out, status)
     h_out, d_out = out.descriptors()
     with torch.cuda.device(dev):
-        index, rec = (None,) * 3, (None,) * 4            # the C call's optional groups: scan index in, recording out
+        # the C call's optional groups: scan index in, recording out, scans in
+        index, rec, scans = (None,) * 3, (None,) * 4, (None,) * 4
         if encoded.first is not None:
             d_first, d_points = encoded.device_index()
             index = (d_points.data_ptr(), encoded.first.ctypes.data, d_first.data_ptr())
         if record or find:
             d_cap_first = torch.from_numpy(cap_first).to(dev)
             rec = (cap_first.ctypes.data, d_cap_first.data_ptr(), points.data_ptr(), count.data_ptr())
+        if encoded.scans is not None:
+            d_scans, d_scan_first = encoded.device_scans()
+            scans = (encoded.scans.ctypes.data, d_scans.data_ptr(), encoded.scan_first.ctypes.data,
+                     d_scan_first.data_ptr())
         check(lib.faa_jpeg_decode(_decoder(dev).handle, encoded.headers.ctypes.data, encoded.device_headers().data_ptr(),
                                   encoded.device_pool().data_ptr(), len(encoded.pool), encoded.storage.data_ptr(), B,
-                                  h_out.ctypes.data, d_out.data_ptr(), status.data_ptr(), *index, *rec, int(find),
-                                  _stream_ptr(dev)))
+                                  h_out.ctypes.data, d_out.data_ptr(), status.data_ptr(), *index, *rec, *scans,
+                                  int(find), _stream_ptr(dev)))
     return (out, status, count, points, cap_first) if record else (out, status)
+
+
+def _decoder(dev):
+    dec = _DECODERS.get(dev.index)
+    if dec is None:
+        dec = _DECODERS[dev.index] = _JpegDecoder()
+    return dec
 
 
 def _augment_ragged(policy, batch: RaggedImages, tail, samples, boxes, rng, out):

@@ -1,12 +1,13 @@
 """The JPEG decoder on the device (``EncodedImages`` / ``decode_jpeg``, C ABI ``faa_jpeg_decode``): the whole file grid
 of tests/jpeg_cases.py decoded as ragged batches that mix sizes, subsamplings, grayscale and restart intervals, against
 Pillow and the host build, into sentinel-filled storage at every offset mod 16; a b512 batch of photo-sized files; a
-truncated file among valid ones; the launch count; and the ImageNet loaders and chains over JPEG bytes against the same
-over Pillow-decoded pixels."""
+truncated file among valid ones; the launch count, with progressive files too; and the ImageNet loaders and chains
+over JPEG bytes against the same over Pillow-decoded pixels."""
 import numpy as np
 import pytest
 import torch
 
+import jpeg_progressive_cases as jp
 from helpers import seed_all
 from jpeg_cases import GRID, content, emu_decode, encode, load_emu_jpeg, make, pillow
 
@@ -114,6 +115,16 @@ def test_each_call_is_two_launches():
     c0 = launches()
     decode_jpeg(enc.select([2, 0]))
     assert launches() - c0 == 2
+    # progressive files: two launches for a batch of them, three for one that mixes them with baseline files
+    prog = [jp.encode(content("photo", 64 + 16 * i, 48 + 8 * i, i), progressive=True, quality=80, subsampling=2)
+            for i in range(3)]
+    for batch, n in ((prog, 2), (files[:2] + prog + files[2:], 3)):
+        e = EncodedImages.from_bytes(batch, progressive=True)
+        out = RaggedImages.empty(e.sizes)
+        decode_jpeg(e, out)
+        c0 = launches()
+        decode_jpeg(e, out)
+        assert launches() - c0 == n
 
 
 def test_from_bytes_names_every_refused_file():

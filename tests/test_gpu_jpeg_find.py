@@ -4,7 +4,8 @@ host build's (tests/emu/faa_emu_jpeg_find.cpp at the kernel's window and rounds)
 ``build_jpeg_index``'s where the chain converged; the found decode's pixels and status equal the plain decode's on the
 grid, the geometry streams, the adversarial streams and corrupt files; a batch mixing given, stale, foreign and absent
 points with progressive files gets the counts of ``record=True`` right; a call queued behind one that grows the
-decoder's buffers; three launches per call; the ABI's refusals; and ``conf['faa_jpeg_index_find']`` in the loaders."""
+decoder's buffers; three launches per call, four with progressive files among baseline ones; the ABI's refusals; and
+``conf['faa_jpeg_index_find']`` in the loaders."""
 import os
 
 import numpy as np
@@ -164,9 +165,19 @@ def test_three_launches_per_found_decode_and_one_per_find():
     c0 = launches()
     build_jpeg_index(enc, find=True)
     assert launches() - c0 == 1
+    # with progressive files: a mixed batch takes four launches, a batch of progressive files no find and two
+    prog = [jp.encode(content("photo", 120, 160, i), progressive=True, quality=85, subsampling=2) for i in range(2)]
+    for batch, n in ((files[:2] + prog + files[2:], 4), (prog, 2)):
+        e = EncodedImages.from_bytes(batch, progressive=True)
+        out = engine.RaggedImages.empty(e.sizes)
+        decode_jpeg(e, out, find=True)
+        for kw in ({}, {"record": True}):
+            c0 = launches()
+            decode_jpeg(e, out, find=True, **kw)
+            assert launches() - c0 == n
 
 
-def test_abi_refuses_progressive_headers_and_bad_offsets():
+def test_abi_refuses_progressive_headers_without_scans_and_bad_offsets():
     enc = EncodedImages.from_bytes([encode(content("photo", 96, 128, 2), quality=95)] * 2)
     pen = EncodedImages.from_bytes([jp.encode(content("photo", 96, 128, 2), progressive=True, quality=95)] * 2,
                                    progressive=True)
@@ -189,7 +200,8 @@ def test_abi_refuses_progressive_headers_and_bad_offsets():
         return _lib.lib.faa_jpeg_decode(dec.handle, e.headers.ctypes.data, e.device_headers().data_ptr(),
                                         e.device_pool().data_ptr(), len(e.pool), e.storage.data_ptr(), 2,
                                         h_out.ctypes.data, d_out.data_ptr(), st.data_ptr(), None, None, None,
-                                        f.ctypes.data, d_f.data_ptr(), pts.data_ptr(), cnt.data_ptr(), 1, None)
+                                        f.ctypes.data, d_f.data_ptr(), pts.data_ptr(), cnt.data_ptr(),
+                                        None, None, None, None, 1, None)
     for call in (find_call, decode_call):
         assert call(enc, good, d_good) == _lib.OK
         assert call(pen, good, d_good) == _lib.ERR_VALUE

@@ -124,7 +124,7 @@ def test_mixed_batch_only_the_stale_file_falls_back(emu):
     assert torch.equal(sx, sy) and torch.equal(x, y) and sx.tolist() == [0] * 4
 
 
-def test_abi_refuses_bad_offsets():
+def test_abi_refuses_bad_point_offsets():
     b = [encode(content("photo", 96, 128, 2), quality=95)] * 2
     enc = EncodedImages.from_bytes(b)
     first, points = build_jpeg_index(enc)
@@ -140,7 +140,7 @@ def test_abi_refuses_bad_offsets():
                                      enc.device_pool().data_ptr(), len(enc.pool), enc.storage.data_ptr(), 2,
                                      h_out.ctypes.data, d_out.data_ptr(), st.data_ptr(),
                                      enc.with_index(first, points).device_index()[1].data_ptr(),
-                                     f.ctypes.data, d_f.data_ptr(), None, None, None, None, 0, None)
+                                     f.ctypes.data, d_f.data_ptr(), *(None,) * 8, 0, None)
         assert e == _lib.ERR_VALUE
         cnt = torch.empty(2, dtype=torch.int32, device="cuda")
         e = _lib.lib.faa_jpeg_index_build(enc.headers.ctypes.data, enc.device_headers().data_ptr(),

@@ -1,5 +1,5 @@
 """The progressive JPEG decoder on the device (``decode_jpeg`` of ``EncodedImages.from_bytes(..., progressive=True)``,
-C ABI ``faa_jpeg_decode_progressive``): pixels and status equal the host build's and Pillow's on the Pillow grid, at
+C ABI ``faa_jpeg_decode`` with scans): pixels and status equal the host build's and Pillow's on the Pillow grid, at
 every reconstruct-tile residue, at restart segment counts 1, 127 to 129 and thousands (waves with more work items than
 threads); corrupt streams give the host build's status; batches mixing progressive files with baseline, indexed and
 restart-interval files give every file the pixels and status of its decode alone; a call on a second stream grows

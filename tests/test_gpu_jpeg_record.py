@@ -106,7 +106,7 @@ def test_recording_queued_behind_a_call_that_grows_the_buffers():
     assert int(np.diff(want_l[0]).min()) > 0
 
 
-def test_abi_refuses_bad_capacity_offsets():
+def test_decode_refuses_bad_capacity_offsets():
     enc = EncodedImages.from_bytes([encode(content("photo", 96, 128, 2), quality=95)] * 2)
     out = sentinel_out(enc.sizes)
     h_out, d_out = out.descriptors()
@@ -121,7 +121,8 @@ def test_abi_refuses_bad_capacity_offsets():
         e = _lib.lib.faa_jpeg_decode(dec.handle, enc.headers.ctypes.data, enc.device_headers().data_ptr(),
                                      enc.device_pool().data_ptr(), len(enc.pool), enc.storage.data_ptr(), 2,
                                      h_out.ctypes.data, d_out.data_ptr(), st.data_ptr(), None, None, None,
-                                     f.ctypes.data, d_f.data_ptr(), pts.data_ptr(), cnt.data_ptr(), 0, None)
+                                     f.ctypes.data, d_f.data_ptr(), pts.data_ptr(), cnt.data_ptr(),
+                                     None, None, None, None, 0, None)
         assert e == _lib.ERR_VALUE
     torch.cuda.synchronize()
 
