@@ -39,7 +39,7 @@ JPEG_SCAN_DTYPE = np.dtype([("off", "<i8"), ("len", "<i8"), ("restart", "<i4"), 
                             ("ss", "<i4"), ("se", "<i4"), ("ah", "<i4"), ("al", "<i4"), ("wave", "<i4"),
                             ("dc_at", "<i4", (3,)), ("ac_at", "<i4", (3,)), ("pool", "<i4", (6,)),
                             ("reserved", "<i4", (2,))])                                            # faa_jpeg_scan_t
-JPEG_PROGRESSIVE, JPEG_MAX_SCANS = 1, 64
+JPEG_PROGRESSIVE, JPEG_SCAN_INDEXED, JPEG_MAX_SCANS = 1, 2, 64
 assert SAMPLE_DTYPE.itemsize == 16 and BOX_DTYPE.itemsize == 8 and IMAGE_DTYPE.itemsize == 16
 assert JPEG_HEADER_DTYPE.itemsize == 144 and JPEG_TABLE_DTYPE.itemsize == 400 and JPEG_SYNC_DTYPE.itemsize == 16
 assert JPEG_SCAN_DTYPE.itemsize == 112

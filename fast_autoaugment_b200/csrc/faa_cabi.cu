@@ -1608,14 +1608,15 @@ static int grow_async(void** ptr, size_t* have, size_t need, cudaStream_t stream
 
 // a header the JPEG device calls take: baseline (the quantisation and both Huffman pool slots of every component), or,
 // when the call gives scans, a progressive one (quantisation slots only: the Huffman tables are the scans').  A
-// progressive header's byte ranges and restart intervals are its scans'; its own must be 0, because the find kernel
-// gives it no work only through scan_len == 0 and would otherwise build tables from its unchecked Huffman slots.
+// progressive header's byte ranges and restart intervals are its scans'; its own must be 0, except the scan_len of a
+// kJpegScanIndexed header, which is the length of its scan axis (plan_jpeg_jobs checks it against the scans).  The
+// entropy and find kernels skip progressive headers by their reserved field.
 static int check_jpeg_header(const JpegHeader& h, int n_tables, const std::string& who, bool scans = false) {
     const bool progressive = jpeg_is_progressive(h);
     if (progressive && !scans)
         return fail(FAA_ERR_VALUE, who + ": a progressive header needs the scans group (h_scans, d_scans, h_scan_first, "
                                          "d_scan_first) of faa_jpeg_decode");
-    if (progressive && (h.scan_off != 0 || h.scan_len != 0 || h.restart != 0))
+    if (progressive && (h.scan_off != 0 || (h.scan_len != 0 && !jpeg_prog_indexed(h)) || h.restart != 0))
         return fail(FAA_ERR_VALUE, who + ": a progressive header has no scan range or restart interval of its own");
     if (h.ncomp != 1 && h.ncomp != 3) return fail(FAA_ERR_VALUE, who + ": component count must be 1 or 3");
     if (check_shape(h.h, h.w)) return fail(FAA_ERR_VALUE, who + ": size out of range");
@@ -1683,7 +1684,7 @@ int faa_jpeg_decoder_destroy(faa_jpeg_decoder_t* d) {
 int faa_jpeg_index_capacity(const faa_jpeg_header_t* hdr) {
     if (!hdr) return 0;
     JpegHeader h; memcpy(&h, hdr, sizeof h);
-    return jpeg_is_progressive(h) ? 0 : jpeg_index_capacity(h);
+    return h.reserved == kJpegProgressive ? 0 : jpeg_index_capacity(h);
 }
 
 }  // extern "C"
@@ -1822,7 +1823,14 @@ static int plan_jpeg_jobs(const faa_jpeg_header_t* h_headers, const faa_image_t*
         } else {                                   // (check_jpeg_headers refused it if the call gives no scans)
             const int64_t n = scan_first[i + 1] - scan_first[i];
             if (int e = check_jpeg_scans(h, scans + scan_first[i], n, n_tables, who)) return e;
-            for (int64_t k = 0; k < n; ++k) segs += jpeg_scan_segments(h, scans[scan_first[i] + k]);
+            int64_t axis = 0;
+            for (int64_t k = 0; k < n; ++k) {
+                segs += jpeg_scan_segments(h, scans[scan_first[i] + k]);
+                axis += scans[scan_first[i] + k].len;
+            }
+            if (jpeg_prog_indexed(h) && h.scan_len != axis)
+                return fail(FAA_ERR_VALUE, who + ": a scan-indexed progressive header's scan_len must be the sum of its "
+                                                 "scans' lengths");
         }
         tiles += (int64_t)((h.w + kJpegTileW - 1) / kJpegTileW) * ((h.h + kJpegTileH - 1) / kJpegTileH);
         if (segs > INT32_MAX || tiles > INT32_MAX) return fail(FAA_ERR_UNSUPPORTED, "batch too large: split it");
@@ -1895,7 +1903,10 @@ int faa_jpeg_decode(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, c
     if (int e = ensure_device()) return e;
     if (batch == 0) return FAA_OK;
     const int n_prog = (int)std::count_if(h_headers, h_headers + batch,
-                                          [](const faa_jpeg_header_t& h) { return h.reserved == FAA_JPEG_PROGRESSIVE; });
+                                          [](const faa_jpeg_header_t& h) {
+                                              return (h.reserved | FAA_JPEG_SCAN_INDEXED) ==
+                                                     (FAA_JPEG_PROGRESSIVE | FAA_JPEG_SCAN_INDEXED);
+                                          });
     cudaStream_t stream = (cudaStream_t)stream_v;
     std::lock_guard<std::mutex> lk(d->mu);
     if (int e = jpeg_call_scratch(d, stream, jobs)) return e;
@@ -1939,7 +1950,7 @@ int faa_jpeg_decode(faa_jpeg_decoder_t* d, const faa_jpeg_header_t* h_headers, c
 // ------------------------------------------------------------------ progressive JPEG parse --
 static_assert(sizeof(faa_jpeg_scan_t) == sizeof(JpegScan) && sizeof(JpegScan) == 112 &&
               offsetof(faa_jpeg_scan_t, pool) == offsetof(JpegScan, pool) && FAA_JPEG_MAX_SCANS == kJpegMaxScans &&
-              FAA_JPEG_PROGRESSIVE == kJpegProgressive, "JPEG scan layout");
+              FAA_JPEG_PROGRESSIVE == kJpegProgressive && FAA_JPEG_SCAN_INDEXED == kJpegScanIndexed, "JPEG scan layout");
 
 extern "C" {
 

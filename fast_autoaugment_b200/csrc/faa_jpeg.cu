@@ -17,7 +17,8 @@
 //                                of the scan index in parallel, and links checked against the next point verify a
 //                                prefix of it.  The found decode's entropy instantiation reads the counts it leaves.
 //   faa_jpeg_progressive_kernel  one CTA per progressive image: the entropy stage of progressive files, scans run wave
-//                                by wave.
+//                                by wave.  Its indexed instantiation splits a kJpegScanIndexed file's restart-free scans
+//                                at their points and checks every split; its recording one places those points.
 //   faa_jpeg_reconstruct_kernel  one CTA per 64 x 32 output tile of one image.  It runs the islow IDCT of the tile's
 //                                blocks, with the one-block chroma halo fancy upsampling reads, into shared memory,
 //                                upsamples and converts to RGB, and writes uint8 HWC rows with 32-bit stores where the
@@ -60,7 +61,8 @@ __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_entropy_kernel(const
     __shared__ int32_t s_count[kEntropyThreads];
     __shared__ int32_t s_status;
     const int img = blockIdx.x, tid = threadIdx.x;
-    if (P.hdrs[img].reserved == kJpegProgressive) return;     // faa_jpeg_progressive_kernel's (before h: DESIGN §4.8)
+    if ((P.hdrs[img].reserved | kJpegScanIndexed) == (kJpegProgressive | kJpegScanIndexed))
+        return;                                              // faa_jpeg_progressive_kernel's (before h: DESIGN §4.8)
     const JpegHeader h = P.hdrs[img];
     const JpegJob job = P.jobs[img];
     const uint8_t* scan = P.src + h.offset + h.scan_off;
@@ -262,7 +264,7 @@ __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_find_kernel(const __
     const int img = blockIdx.x, tid = threadIdx.x;
     const JpegHeader h = P.hdrs[img];
     const bool given = P.first && P.first[img + 1] > P.first[img];
-    const int parts = given ? 0 : jpeg_index_parts(h);
+    const int parts = given || jpeg_is_progressive(h) ? 0 : jpeg_index_parts(h);     // (progressive: not found here)
     if (parts == 0) {
         if (tid == 0) P.count[img] = 0;
         return;
@@ -303,8 +305,16 @@ cudaError_t launch_jpeg_find(const JpegDecodeParams& p, bool mark, cudaStream_t 
 // wave.  A wave's scans share no (component, coefficient), so its work items, one per (scan, restart segment), run on
 // all threads at once; a barrier separates waves.  A wave whose scans need more Huffman tables than kProgSlots (or has
 // more than kProgGroup scans) runs as several groups, one after the other.
+// kIndexed: the call gives scan indexes (P.first, P.points).  A kJpegScanIndexed image whose points pass their check
+// runs a restart-free scan with k points as k + 1 work items, each comparing its end state with the next point
+// (jpeg_prog_item); any failure marks the image at the group's barrier, and a marked image zeroes its planes and runs
+// again without its points.  kRecord (with kIndexed, whose P.first may then be null): a kJpegScanIndexed image decoded
+// without usable points places the rule's points of each restart-free scan while decoding it whole, thread 0 compacts
+// them into P.rec_points[P.rec_first[i], P.rec_first[i + 1]), and P.count[i] gets their number; every other image of
+// this kernel gets count 0.
 constexpr int kProgSlots = 8, kProgGroup = 16;
 
+template <bool kIndexed, bool kRecord>
 __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_progressive_kernel(const __grid_constant__ JpegDecodeParams P) {
     __shared__ JpegHuff s_huff[kProgSlots];
     __shared__ JpegScan s_scan[kJpegMaxScans];
@@ -313,8 +323,10 @@ __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_progressive_kernel(c
     __shared__ int32_t s_count[kEntropyThreads];
     __shared__ int32_t s_gscan[kProgGroup], s_gslot[kProgGroup], s_gitem[kProgGroup + 1], s_gtab[kProgSlots];
     __shared__ int32_t s_ng, s_nslot, s_pos, s_status;
+    __shared__ int32_t s_pfirst[kJpegMaxScans + 1];       // (kIndexed) first point of each scan
+    __shared__ JpegSync s_rec[kJpegIndexMaxParts];        // (kRecord) point k of the rule at [k], mcu -1 if none
     const int img = blockIdx.x, tid = threadIdx.x;
-    if (P.hdrs[img].reserved != kJpegProgressive) return;     // faa_jpeg_entropy_kernel's
+    if ((P.hdrs[img].reserved | kJpegScanIndexed) != (kJpegProgressive | kJpegScanIndexed)) return;  // the entropy kernel's
     const JpegHeader h = P.hdrs[img];
     const JpegJob job = P.jobs[img];
     const uint8_t* file = P.src + h.offset;
@@ -327,6 +339,7 @@ __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_progressive_kernel(c
         const int64_t n16 = jpeg_image_blocks(h) * 8;
         for (int64_t k = tid; k < n16; k += kEntropyThreads) z[k] = make_uint4(0, 0, 0, 0);
     }
+    if constexpr (kRecord) s_rec[tid].mcu = -1;
     __syncthreads();
     if (tid == 0) {
         s_status = 0;
@@ -359,60 +372,114 @@ __global__ void __launch_bounds__(kEntropyThreads) faa_jpeg_progressive_kernel(c
         jpeg_markers(r, scan, a, b, s.len, ss, 1 + s_count[tid], n_seg);
         __syncthreads();
     }
+    // the image's points, when it takes them and they pass their check
+    const JpegSync* pts = nullptr;
+    bool use = false;
+    if constexpr (kIndexed) {
+        const int64_t n_pts = jpeg_prog_indexed(h) && (!kRecord || P.first) ? P.first[img + 1] - P.first[img] : 0;
+        if (n_pts > 0) {
+            pts = P.points + P.first[img];
+            bool ok = jpeg_index_count_ok(h, n_pts);
+            if (ok && tid < n_pts) ok = jpeg_prog_point_ok(h, s_scan, n, pts, tid);
+            use = __syncthreads_and(ok);
+            if (use && tid == 0) jpeg_prog_point_first(s_scan, n, pts, (int)n_pts, s_pfirst);
+        }
+    }
     int status = 0;
-    for (int pos = 0; pos < n;) {
-        if (tid == 0) {                                  // the next group: scans of one wave, tables in kProgSlots
-            int ng = 0, slots = 0, items = 0, q = pos;
-            const int w = s_scan[s_order[pos]].wave;
-            while (q < n && ng < kProgGroup) {
-                const int k = s_order[q];
-                const JpegScan& s = s_scan[k];
-                const int need = jpeg_scan_tables(s);
-                if (s.wave != w || slots + need > kProgSlots) break;
-                s_gscan[ng] = k; s_gslot[ng] = slots; s_gitem[ng] = items;
-                for (int t = 0; t < need; ++t) s_gtab[slots + t] = s.pool[s.ss == 0 ? t : 3];
-                slots += need;
-                items += (int)jpeg_scan_segments(h, s);
-                ++ng; ++q;
+    bool marked = false;
+    for (int pass = use ? 0 : 1; pass < 2; ++pass) {     // 0: with the points; 1: without (the plain decode)
+        const bool indexed = kIndexed && pass == 0;
+        if (kIndexed && pass == 1 && use) {              // a marked image: its work so far is thrown away
+            uint4* z = reinterpret_cast<uint4*>(coef);
+            const int64_t n16 = jpeg_image_blocks(h) * 8;
+            for (int64_t k = tid; k < n16; k += kEntropyThreads) z[k] = make_uint4(0, 0, 0, 0);
+            status = 0;
+            __syncthreads();
+        }
+        for (int pos = 0; pos < n;) {
+            if (tid == 0) {                              // the next group: scans of one wave, tables in kProgSlots
+                int ng = 0, slots = 0, items = 0, q = pos;
+                const int w = s_scan[s_order[pos]].wave;
+                while (q < n && ng < kProgGroup) {
+                    const int k = s_order[q];
+                    const JpegScan& s = s_scan[k];
+                    const int need = jpeg_scan_tables(s);
+                    if (s.wave != w || slots + need > kProgSlots) break;
+                    s_gscan[ng] = k; s_gslot[ng] = slots; s_gitem[ng] = items;
+                    for (int t = 0; t < need; ++t) s_gtab[slots + t] = s.pool[s.ss == 0 ? t : 3];
+                    slots += need;
+                    items += indexed && s.restart == 0 ? s_pfirst[k + 1] - s_pfirst[k] + 1 : (int)jpeg_scan_segments(h, s);
+                    ++ng; ++q;
+                }
+                s_gitem[ng] = items; s_ng = ng; s_nslot = slots; s_pos = q;
             }
-            s_gitem[ng] = items; s_ng = ng; s_nslot = slots; s_pos = q;
+            __syncthreads();
+            const int ng = s_ng, nslot = s_nslot, items = s_gitem[ng];
+            pos = s_pos;
+            if (tid < nslot) jpeg_huff_codes(P.pool[s_gtab[tid]], s_huff[tid]);
+            __syncthreads();
+            for (int e = tid; e < nslot << kJpegLookBits; e += kEntropyThreads) {
+                const int t = e >> kJpegLookBits;
+                s_huff[t].look[e & ((1 << kJpegLookBits) - 1)] = jpeg_huff_look(s_huff[t], e & ((1 << kJpegLookBits) - 1));
+            }
+            __syncthreads();
+            bool linked = true;
+            for (int it = tid; it < items; it += kEntropyThreads) {
+                int g = 0;
+                while (it >= s_gitem[g + 1]) ++g;
+                const int k = s_gscan[g];
+                const JpegScan& s = s_scan[k];
+                const int64_t j = it - s_gitem[g], units = jpeg_scan_units(h, s);
+                const JpegHuff* hp[3] = {&s_huff[s_gslot[g]], &s_huff[min(s_gslot[g] + 1, kProgSlots - 1)],
+                                         &s_huff[min(s_gslot[g] + 2, kProgSlots - 1)]};
+                const uint8_t* scan = file + s.off;
+                if (indexed && s.restart == 0) {
+                    bool ok = true;
+                    status |= jpeg_prog_item(h, s, hp, scan, jpeg_prog_axis(s_scan, k), pts + s_pfirst[k],
+                                             s_pfirst[k + 1] - s_pfirst[k], (int)j, coef, &ok);
+                    linked = linked && ok;
+                    continue;
+                }
+                const int64_t u0 = s.restart > 0 ? j * s.restart : 0, u1 = s.restart > 0 ? min(u0 + s.restart, units) : units;
+                const int32_t at = segs[s_seg[k] + j];
+                if constexpr (kRecord) {
+                    JpegProgSink sink;
+                    const bool r = jpeg_prog_indexed(h) && jpeg_prog_sink(h, s_scan, k, s_rec, sink);
+                    status |= jpeg_prog_segment(h, s, hp, scan, at < 0 ? scan + s.len : scan + at, scan + s.len, u0, u1,
+                                                coef, nullptr, nullptr, r ? &sink : nullptr);
+                } else {
+                    status |= jpeg_prog_segment(h, s, hp, scan, at < 0 ? scan + s.len : scan + at, scan + s.len, u0, u1, coef);
+                }
+            }
+            // the wave's coefficients are complete; s_huff is free.  An indexed pass stops at the first failed link.
+            if (indexed) {
+                marked = __syncthreads_or(!linked);
+                if (marked) break;
+            } else {
+                __syncthreads();
+            }
         }
-        __syncthreads();
-        const int ng = s_ng, nslot = s_nslot, items = s_gitem[ng];
-        pos = s_pos;
-        if (tid < nslot) jpeg_huff_codes(P.pool[s_gtab[tid]], s_huff[tid]);
-        __syncthreads();
-        for (int e = tid; e < nslot << kJpegLookBits; e += kEntropyThreads) {
-            const int t = e >> kJpegLookBits;
-            s_huff[t].look[e & ((1 << kJpegLookBits) - 1)] = jpeg_huff_look(s_huff[t], e & ((1 << kJpegLookBits) - 1));
-        }
-        __syncthreads();
-        for (int it = tid; it < items; it += kEntropyThreads) {
-            int g = 0;
-            while (it >= s_gitem[g + 1]) ++g;
-            const int k = s_gscan[g];
-            const JpegScan& s = s_scan[k];
-            const int64_t j = it - s_gitem[g], units = jpeg_scan_units(h, s);
-            const int64_t u0 = s.restart > 0 ? j * s.restart : 0, u1 = s.restart > 0 ? min(u0 + s.restart, units) : units;
-            const JpegHuff* hp[3] = {&s_huff[s_gslot[g]], &s_huff[min(s_gslot[g] + 1, kProgSlots - 1)],
-                                     &s_huff[min(s_gslot[g] + 2, kProgSlots - 1)]};
-            const uint8_t* scan = file + s.off;
-            const int32_t at = segs[s_seg[k] + j];
-            status |= jpeg_prog_segment(h, s, hp, scan, at < 0 ? scan + s.len : scan + at, scan + s.len, u0, u1, coef);
-        }
-        __syncthreads();                                 // the wave's coefficients are complete; s_huff is free
+        if (!marked) break;
     }
     if (status) atomicOr(&s_status, status);
     __syncthreads();
     if (tid == 0) {
         P.status[img] = s_status;
-        if (P.count) P.count[img] = 0;                  // a recording call's: progressive files have no scan index
+        if constexpr (kRecord) {                         // points of the rule when it decoded without usable ones
+            const bool rec = jpeg_prog_indexed(h) && (!use || marked) && s_status == 0;
+            P.count[img] = rec ? jpeg_prog_compact(s_rec, jpeg_index_parts(h), P.rec_points + P.rec_first[img],
+                                                   P.rec_first[img + 1] - P.rec_first[img]) : 0;
+        } else {
+            if (P.count) P.count[img] = 0;              // (a recording call launches the recording instantiation)
+        }
     }
 }
 
 cudaError_t launch_jpeg_progressive(const JpegDecodeParams& p, cudaStream_t stream) {
     if (p.batch <= 0) return cudaSuccess;
-    faa_jpeg_progressive_kernel<<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p);
+    if (p.rec_first) faa_jpeg_progressive_kernel<true, true><<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p);
+    else if (p.first) faa_jpeg_progressive_kernel<true, false><<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p);
+    else faa_jpeg_progressive_kernel<false, false><<<(unsigned)p.batch, kEntropyThreads, 0, stream>>>(p);
     return cudaGetLastError();
 }
 

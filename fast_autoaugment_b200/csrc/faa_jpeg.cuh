@@ -1041,8 +1041,11 @@ inline void jpeg_reconstruct_host(const JpegHeader& h, const JpegTable* tabs, co
 // reconstruct stage reads.  parse_jpeg_progressive takes what parse_jpeg takes (8-bit, 1 or 3 components, 4:4:4 / 4:2:2 /
 // 4:2:0) when it is coded progressively and every coefficient of every component ends at bit 0; libjpeg smooths the
 // blocks of an incomplete progression, which is not modelled, so those files are refused.  Its header has
-// reserved = kJpegProgressive, restart = 0 and no scan_off / scan_len; the scans are a separate list.
+// reserved = kJpegProgressive, restart = 0 and no scan_off / scan_len; the scans are a separate list.  A caller that
+// wants the file to take a scan index marks it reserved = kJpegProgressive | kJpegScanIndexed and sets scan_len to the
+// sum of its scans' lengths (the scan axis below), so that the placement rule of a baseline file applies unchanged.
 constexpr int32_t kJpegProgressive = 1;      // JpegHeader::reserved of a progressive file (0 for every other)
+constexpr int32_t kJpegScanIndexed = 2;      // with kJpegProgressive: the file takes a scan index
 constexpr int kJpegMaxScans = 64;
 
 // layout of faa_jpeg_scan_t
@@ -1059,7 +1062,10 @@ struct JpegScan {
     int32_t reserved[2];
 };
 
-FAA_JHD bool jpeg_is_progressive(const JpegHeader& h) { return h.reserved == kJpegProgressive; }
+FAA_JHD bool jpeg_is_progressive(const JpegHeader& h) {
+    return (h.reserved | kJpegScanIndexed) == (kJpegProgressive | kJpegScanIndexed);
+}
+FAA_JHD bool jpeg_prog_indexed(const JpegHeader& h) { return h.reserved == (kJpegProgressive | kJpegScanIndexed); }
 
 // Huffman tables a scan uses: DC first: one per component; DC refinement: none; AC: one
 FAA_JHD int jpeg_scan_tables(const JpegScan& s) { return s.ss == 0 ? (s.ah == 0 ? s.ns : 0) : 1; }
@@ -1319,18 +1325,126 @@ FAA_JHD uint32_t jpeg_bit(JpegBits& r) {
     return jpeg_get(r, 1);
 }
 
-// Decodes units [u0, u1) of scan s (a restart segment: its data from `data`, EOBRUN and predictors zero) of the scan
-// bytes [lo, end) into coef, accumulating into what earlier waves wrote.  huff[k]: the table of slot k
-// (jpeg_scan_tables).  Stops at the first error; returns JpegStatus.
+// ------------------------------------------------------------------------------------------------ progressive index --
+// The scan index of a progressive file (reserved = kJpegProgressive | kJpegScanIndexed).
+//   Scan axis: the file's scans, concatenated in file order, form one byte axis of length h.scan_len; scan s occupies
+//   [A_s, A_s + len_s).  The placement rule of jpeg_index_parts applies to the axis unchanged (P parts, thresholds T_k).
+//   Points: a JpegSync whose `byte` is the axis offset of the data byte holding the next bit (canonical, as
+//   jpeg_bits_pos gives it) and `bit` the bits of it consumed; the scan holding `byte` is the point's scan.  `mcu` is the
+//   next unit of that scan (jpeg_scan_units).  `pred`: a DC first scan's predictors of its components; an AC scan's
+//   (first pass or refinement) EOBRUN in pred[0]; zeros for a DC refinement and in every unused entry.
+//   Placement: point k is the first unit boundary u >= 1 of the scan that holds T_k whose start byte is >= T_k and
+//   inside that scan.  It is dropped when the scan has no such boundary, when the scan has a restart interval (restart
+//   markers split it already) and when it coincides with the previous point.
+//   Check: at most 127 points, bytes strictly increasing, each in a restart-free scan, unit in [1, units) and strictly
+//   increasing among one scan's points, bit 0..7.  Anything else decodes the file without its index.
+// A restart-free scan with k points is k + 1 work items of its wave; each ends by comparing its end state with the next
+// point.  By induction over the waves, and over the items of each scan, every item starts in the serial decode's state
+// when every comparison holds (DESIGN §4.8); an image where one does not is decoded again, whole, without its index.
+
+// Where a recording progressive decode puts the points of the rule that fall in one restart-free scan: at[k] for
+// threshold k in [next, last), the others untouched (the caller sets every mcu to -1 first).
+struct JpegProgSink {
+    JpegSync* at;
+    int64_t base, len;           // the scan's place on the axis
+    int32_t parts, next, last;
+};
+
+// A_s: axis offset of scan k
+FAA_JHD int64_t jpeg_prog_axis(const JpegScan* scans, int k) {
+    int64_t a = 0;
+    for (int i = 0; i < k; ++i) a += scans[i].len;
+    return a;
+}
+
+// the scan that holds axis byte b, or n
+FAA_JHD int jpeg_prog_scan_of(const JpegScan* scans, int n, int64_t b) {
+    int64_t a = 0;
+    for (int k = 0; k < n; ++k) {
+        if (b >= a && b < a + scans[k].len) return k;
+        a += scans[k].len;
+    }
+    return n;
+}
+
+// the check of point i of pts (the ones before it included through pts[i - 1])
+FAA_JHD bool jpeg_prog_point_ok(const JpegHeader& h, const JpegScan* scans, int n, const JpegSync* pts, int i) {
+    const JpegSync& p = pts[i];
+    if (p.bit < 0 || p.bit > 7 || p.byte < 0 || (i > 0 && p.byte <= pts[i - 1].byte)) return false;
+    const int k = jpeg_prog_scan_of(scans, n, p.byte);
+    if (k == n || scans[k].restart > 0 || p.mcu < 1 || (int64_t)p.mcu >= jpeg_scan_units(h, scans[k])) return false;
+    return i == 0 || pts[i - 1].byte < jpeg_prog_axis(scans, k) || pts[i - 1].mcu < p.mcu;
+}
+
+// first[k]: the first of the n_pts checked points in scan k (first[n] = n_pts)
+FAA_JHD void jpeg_prog_point_first(const JpegScan* scans, int n, const JpegSync* pts, int n_pts, int32_t* first) {
+    int64_t a = 0;
+    int i = 0;
+    for (int k = 0; k < n; ++k) {
+        while (i < n_pts && pts[i].byte < a) ++i;
+        first[k] = i;
+        a += scans[k].len;
+    }
+    first[n] = n_pts;
+}
+
+// The sink of scan k of a file whose points a recording decode places into at[] (indexed by threshold).  False, and no
+// sink, when the rule gives the file no points, the scan has a restart interval or no threshold falls in it.
+FAA_JHD bool jpeg_prog_sink(const JpegHeader& h, const JpegScan* scans, int k, JpegSync* at, JpegProgSink& s) {
+    const int parts = jpeg_index_parts(h);
+    if (!parts || scans[k].restart > 0) return false;
+    const int64_t a = jpeg_prog_axis(scans, k), e = a + scans[k].len;
+    int next = 1, last;
+    while (next < parts && jpeg_index_threshold(h, parts, next) < a) ++next;
+    for (last = next; last < parts && jpeg_index_threshold(h, parts, last) < e; ++last) {}
+    s = {at, a, scans[k].len, parts, next, last};
+    return next < last;
+}
+
+// A decoder state in point form: position, then the predictors (DC first), EOBRUN (AC) or nothing (DC refinement)
+FAA_JHD void jpeg_prog_state(const JpegScan& s, JpegBits& r, int64_t u, const int* pred, int eobrun, JpegSync* p) {
+    p->mcu = (int32_t)u;
+    jpeg_bits_pos(r, &p->byte, &p->bit);
+    for (int c = 0; c < 3; ++c)
+        p->pred[c] = (int16_t)(s.ss == 0 ? (s.ah == 0 && c < s.ns ? pred[c] : 0) : (c == 0 ? eobrun : 0));
+}
+
+// Decodes units [u0, u1) of scan s of the scan bytes [lo, end) into coef, accumulating into what earlier waves wrote,
+// reading from `data`.  Without `from` it is a restart segment (EOBRUN and predictors zero, bit 0 of `data`); with it the
+// segment starts in that point's state (its bit and predictors or EOBRUN; `data` is its byte).  With `to`, a segment
+// that decodes cleanly reports the state it ends in (unit u1, byte relative to lo).  With `rec` (a whole restart-free
+// scan of a recording decode) it places the points of the rule at the unit boundaries it passes.  huff[k]: the table
+// of slot k (jpeg_scan_tables).  Stops at the first error; returns JpegStatus.
 FAA_JHD int jpeg_prog_segment(const JpegHeader& h, const JpegScan& s, const JpegHuff* const* huff, const uint8_t* lo,
-                              const uint8_t* data, const uint8_t* end, int64_t u0, int64_t u1, int16_t* coef) {
+                              const uint8_t* data, const uint8_t* end, int64_t u0, int64_t u1, int16_t* coef,
+                              const JpegSync* from = nullptr, JpegSync* to = nullptr, JpegProgSink* rec = nullptr) {
     JpegBits r;
-    jpeg_bits_init(r, lo, data, end);
     int pred[3] = {0, 0, 0};
     int eobrun = 0;
+    if (from) {
+        jpeg_bits_start(r, lo, data, end, *from);
+        for (int c = 0; c < 3; ++c) pred[c] = from->pred[c];
+        if (s.ss > 0) eobrun = from->pred[0];
+    } else {
+        jpeg_bits_init(r, lo, data, end);
+    }
     const int p1 = 1 << s.al, m1 = -p1;
     const int bw = s.ns == 1 ? jpeg_comp_bw(h, s.comp[0]) : 1;
     for (int64_t u = u0; u < u1; ++u) {
+        if (rec && u > u0) {                             // a unit boundary: the thresholds it reaches
+            JpegSync p;
+            jpeg_prog_state(s, r, u, pred, eobrun, &p);
+            const bool inside = p.byte < rec->len;       // (a boundary at the scan's end is no point of it)
+            p.byte = (int32_t)(rec->base + p.byte);
+            bool placed = false;
+            while (rec->next < rec->last && (int64_t)p.byte >= jpeg_index_threshold(h, rec->parts, rec->next)) {
+                if (!placed && inside) {
+                    rec->at[rec->next] = p;
+                    placed = true;                       // (the later thresholds it reaches coincide: dropped)
+                }
+                ++rec->next;
+            }
+        }
         if (s.ss == 0) {                                 // DC: every block of the MCU (one block without interleaving)
             for (int k = 0; k < s.ns; ++k) {
                 const int c = s.comp[k];
@@ -1419,35 +1533,105 @@ FAA_JHD int jpeg_prog_segment(const JpegHeader& h, const JpegScan& s, const Jpeg
         }
         if (r.n < r.fake) return JPEG_TRUNCATED;        // this unit used bits past the data
     }
+    if (to) jpeg_prog_state(s, r, u1, pred, eobrun, to);
     return JPEG_OK;
 }
 
-// The progressive kernel's entropy work on the host, one scan after another in file order (waves are an order the
-// kernel may use instead: they give the same coefficients).  coef: jpeg_image_blocks(h) blocks, zeroed here.  tabs: the
-// scans' tables in jpeg_progressive_tables' layout.  Returns JpegStatus bits.
+// Work item j of restart-free scan s (at axis offset a, its bytes [lo, lo + s.len)) of an indexed decode whose points in
+// that scan are q[0, np): units [q[j - 1].mcu, q[j].mcu) from point j - 1's state (the scan's start for j = 0) to point j
+// (the scan's end for j = np).  *linked: it ended cleanly in point j's state (the last item always does).  Returns the
+// last item's status (an earlier item's failure shows in *linked).
+FAA_JHD int jpeg_prog_item(const JpegHeader& h, const JpegScan& s, const JpegHuff* const* huff, const uint8_t* lo,
+                           int64_t a, const JpegSync* q, int np, int j, int16_t* coef, bool* linked) {
+    JpegSync from = {0, 0, 0, {0, 0, 0}};
+    if (j > 0) { from = q[j - 1]; from.byte = (int32_t)(from.byte - a); }
+    const int64_t u1 = j < np ? (int64_t)q[j].mcu : jpeg_scan_units(h, s);
+    JpegSync to;
+    const int st = jpeg_prog_segment(h, s, huff, lo, lo + from.byte, lo + s.len, from.mcu, u1, coef, &from, &to);
+    if (j == np) { *linked = true; return st; }
+    to.byte = (int32_t)(to.byte + a);
+    *linked = st == 0 && jpeg_sync_same(to, q[j]);
+    return 0;
+}
+
+// the placed points of at[1, parts) into out[0, cap) in axis order; returns their number
+FAA_JHD int jpeg_prog_compact(const JpegSync* at, int parts, JpegSync* out, int64_t cap) {
+    int n = 0;
+    for (int k = 1; k < parts; ++k)
+        if (at[k].mcu >= 0 && n < cap) out[n++] = at[k];
+    return n;
+}
+
+// The progressive kernel's entropy work on the host.  coef: jpeg_image_blocks(h) blocks, zeroed here.  tabs: the scans'
+// tables in jpeg_progressive_tables' layout.  Returns JpegStatus bits.
+// Without usable points (pts, npts: a scan index of a kJpegScanIndexed file that passes the check) it decodes one scan
+// after another in file order (waves are an order the kernel may use instead: they give the same coefficients).  With
+// them it runs as the indexed kernel does: wave by wave, a restart-free scan as one item per point plus one, the
+// items' end states checked at the end of each wave; when one fails it zeroes the planes and decodes the file again
+// without them.  With rec_count (a recording decode), a kScanIndexed file decoded without usable points places its
+// points into rec_at[0, rec_cap) and *rec_count gets their number (0 when it has a status or the rule gives none).
 inline int jpeg_progressive_entropy_host(const uint8_t* file, const JpegHeader& h, const JpegScan* scans, int n,
-                                         const JpegTable* tabs, int16_t* coef) {
-    memset(coef, 0, (size_t)jpeg_image_blocks(h) * 128);
-    int status = 0;
+                                         const JpegTable* tabs, int16_t* coef, const JpegSync* pts = nullptr,
+                                         int64_t npts = 0, JpegSync* rec_at = nullptr, int64_t rec_cap = 0,
+                                         int32_t* rec_count = nullptr) {
+    if (rec_count) *rec_count = 0;
     JpegHuff* huffs = new JpegHuff[3];
-    for (int i = 0; i < n; ++i) {
+    const JpegHuff* hp[3] = {&huffs[0], &huffs[1], &huffs[2]};
+    bool use = pts && jpeg_prog_indexed(h) && jpeg_index_count_ok(h, npts);
+    for (int i = 0; use && i < (int)npts; ++i) use = jpeg_prog_point_ok(h, scans, n, pts, i);
+    int32_t first[kJpegMaxScans + 1];
+    if (use) jpeg_prog_point_first(scans, n, pts, (int)npts, first);
+    JpegSync at[kJpegIndexMaxParts];
+    for (int k = 0; k < kJpegIndexMaxParts; ++k) at[k].mcu = -1;
+    int status = 0;
+    // scan i: its restart segments, its items (indexed), or itself whole (with a sink when recording)
+    auto run = [&](int i, bool indexed, bool* linked) {
         const JpegScan& s = scans[i];
-        const JpegHuff* hp[3] = {&huffs[0], &huffs[1], &huffs[2]};
         for (int k = 0; k < jpeg_scan_tables(s); ++k) jpeg_huff_build(tabs[3 + 6 * i + (s.ss == 0 ? k : 3)], huffs[k]);
         const uint8_t* scan = file + s.off;
         const uint8_t* end = scan + s.len;
         const int64_t n_seg = jpeg_scan_segments(h, s), units = jpeg_scan_units(h, s);
-        int32_t* at = new int32_t[(size_t)n_seg];
-        for (int64_t k = 0; k < n_seg; ++k) at[k] = k ? -1 : 0;
+        if (indexed && n_seg == 1) {
+            const int np = first[i + 1] - first[i];
+            for (int j = 0; j <= np; ++j) {
+                bool ok = true;
+                status |= jpeg_prog_item(h, s, hp, scan, jpeg_prog_axis(scans, i), pts + first[i], np, j, coef, &ok);
+                *linked = *linked && ok;
+            }
+            return;
+        }
+        int32_t* seg = new int32_t[(size_t)n_seg];
+        for (int64_t k = 0; k < n_seg; ++k) seg[k] = k ? -1 : 0;
         if (n_seg > 1) {
             JpegBits r; jpeg_bits_init(r, scan, scan, end);
-            if (jpeg_markers(r, scan, 0, s.len, s.len, at, 1, n_seg) != n_seg - 1) status |= JPEG_BAD_RESTART;
+            if (jpeg_markers(r, scan, 0, s.len, s.len, seg, 1, n_seg) != n_seg - 1) status |= JPEG_BAD_RESTART;
         }
+        JpegProgSink sink;
+        JpegProgSink* rec = rec_count && jpeg_prog_indexed(h) && jpeg_prog_sink(h, scans, i, at, sink) ? &sink : nullptr;
         for (int64_t k = 0; k < n_seg; ++k) {
             const int64_t u0 = k * (n_seg > 1 ? s.restart : 0), u1 = n_seg == 1 ? units : (u0 + s.restart < units ? u0 + s.restart : units);
-            status |= jpeg_prog_segment(h, s, hp, scan, at[k] < 0 ? end : scan + at[k], end, u0, u1, coef);
+            status |= jpeg_prog_segment(h, s, hp, scan, seg[k] < 0 ? end : scan + seg[k], end, u0, u1, coef, nullptr,
+                                        nullptr, rec);
         }
-        delete[] at;
+        delete[] seg;
+    };
+    memset(coef, 0, (size_t)jpeg_image_blocks(h) * 128);
+    bool linked = true;
+    if (use) {
+        int waves = 0;
+        for (int i = 0; i < n; ++i) waves = scans[i].wave + 1 > waves ? scans[i].wave + 1 : waves;
+        for (int w = 0; w < waves && linked; ++w)
+            for (int i = 0; i < n; ++i)
+                if (scans[i].wave == w) run(i, true, &linked);
+        if (!linked) {                                   // the whole image again, without the index
+            memset(coef, 0, (size_t)jpeg_image_blocks(h) * 128);
+            status = 0;
+        }
+    }
+    if (!use || !linked) {
+        for (int i = 0; i < n; ++i) run(i, false, &linked);
+        if (rec_count && jpeg_prog_indexed(h) && !status)
+            *rec_count = jpeg_prog_compact(at, jpeg_index_parts(h), rec_at, rec_cap);
     }
     delete[] huffs;
     return status;
@@ -1455,11 +1639,14 @@ inline int jpeg_progressive_entropy_host(const uint8_t* file, const JpegHeader& 
 
 // The whole decode of one progressive file on the host (the progressive entropy kernel, then the reconstruct kernel).
 // out: h.h * h.w * 3 bytes; coef_out: the coefficients, when given.  Returns JpegStatus bits.
+// pts / npts / rec_*: as jpeg_progressive_entropy_host.
 inline int jpeg_decode_progressive_host(const uint8_t* file, const JpegHeader& h, const JpegScan* scans, int n,
-                                        const JpegTable* tabs, uint8_t* out, int16_t* coef_out = nullptr) {
+                                        const JpegTable* tabs, uint8_t* out, int16_t* coef_out = nullptr,
+                                        const JpegSync* pts = nullptr, int64_t npts = 0, JpegSync* rec_at = nullptr,
+                                        int64_t rec_cap = 0, int32_t* rec_count = nullptr) {
     const int64_t nblk = jpeg_image_blocks(h);
     int16_t* coef = new int16_t[(size_t)nblk * 64];
-    const int status = jpeg_progressive_entropy_host(file, h, scans, n, tabs, coef);
+    const int status = jpeg_progressive_entropy_host(file, h, scans, n, tabs, coef, pts, npts, rec_at, rec_cap, rec_count);
     if (coef_out) memcpy(coef_out, coef, (size_t)nblk * 128);
     jpeg_reconstruct_host(h, tabs, coef, out);
     delete[] coef;

@@ -588,10 +588,14 @@ class EncodedDeviceDataset:
     once here) and every batch is decoded on the device before its chain runs.  ``progressive``: progressive files
     are taken too (``EncodedImages.from_bytes(..., progressive=True)``).  ``find``: each batch's restart-free files
     without a scan index get one found on the device first (``decode_jpeg(find=True)``), so they decode on many
-    threads; the pixels are the same."""
+    threads; the pixels are the same.  ``progressive_index``: progressive files take a scan index
+    (``from_bytes(..., progressive_index=True)``), so the ones that carry or find none decode as they do without it."""
 
-    def __init__(self, files, targets, device="cuda", progressive=False, find=False):
-        self.images = files if isinstance(files, EncodedImages) else EncodedImages.from_bytes(files, device, progressive)
+    def __init__(self, files, targets, device="cuda", progressive=False, find=False, progressive_index=False):
+        if progressive_index and not progressive:
+            raise ValueError("progressive_index needs progressive")
+        self.images = files if isinstance(files, EncodedImages) else EncodedImages.from_bytes(
+            files, device, progressive, progressive_index)
         self.find = bool(find)
         self.targets = [int(t) for t in targets]
         if len(self.targets) != len(self.images):
@@ -707,11 +711,17 @@ class JpegFileDataset:
     epoch decodes it on many threads; subsets share the index, and ``index.save`` writes it.  ``progressive``: the
     loaders decode progressive files on the device instead of with Pillow (``read_jpeg_batch``).  ``find``: the loaders
     find the scan index of every restart-free file the index does not list on the device, in parallel, before decoding
-    it on many threads (``decode_jpeg(find=True)``); with ``learn`` the found points are what the index learns."""
+    it on many threads (``decode_jpeg(find=True)``); with ``learn`` the found points are what the index learns.
+    ``progressive_index`` (with ``progressive``): progressive files take a scan index as baseline files do, looked up
+    in ``index`` and, with ``learn``, learned from the loaders' recording decodes."""
 
-    def __init__(self, paths, targets, device="cuda", index=None, learn=False, progressive=False, find=False):
+    def __init__(self, paths, targets, device="cuda", index=None, learn=False, progressive=False, find=False,
+                 progressive_index=False):
         if learn and index is None:
             raise ValueError("learn needs an index to enter the files' points into (JpegIndex.empty)")
+        if progressive_index and not progressive:
+            raise ValueError("progressive_index needs progressive")
+        self.progressive_index = bool(progressive_index)
         self.paths = [os.fspath(p) for p in paths]
         self.index = index
         self.learn = bool(learn)
@@ -735,6 +745,7 @@ class JpegFileDataset:
         d = JpegFileDataset.__new__(JpegFileDataset)
         d.paths = self.select(idx)
         d.index, d.learn, d.progressive, d.find = self.index, self.learn, self.progressive, self.find
+        d.progressive_index = self.progressive_index
         d.targets = [self.targets[i] for i in idx]
         d.labels = self.labels.index_select(0, torch.as_tensor(idx, dtype=torch.int64, device=self.labels.device))
         d.device = self.device
@@ -782,16 +793,17 @@ class HostBatch:
         return s
 
 
-def read_jpeg_batch(paths, map=map, index=None, progressive=False):
+def read_jpeg_batch(paths, map=map, index=None, progressive=False, progressive_index=False):
     """Read a batch of files and parse their headers (``parse_jpeg_headers``); decode the files the device decoder
     refuses with Pillow; with a ``JpegIndex``, gather the accepted files' scan indexes.  No device is touched.  ``map``:
     an executor's ``map`` reads, parses and decodes in parallel.  ``progressive=True``: progressive files are accepted
-    with their scans instead of decoded by Pillow."""
+    with their scans instead of decoded by Pillow; ``progressive_index=True``: they take a scan index too."""
     paths = list(paths)
     files = list(map(_read_file, paths))
     scans = scan_first = None
     if progressive:
-        headers, pool, refused, scans, scan_first = parse_jpeg_headers(files, map, progressive=True)
+        headers, pool, refused, scans, scan_first = parse_jpeg_headers(files, map, progressive=True,
+                                                                       progressive_index=progressive_index)
     else:
         headers, pool, refused = parse_jpeg_headers(files, map)
     bad = np.array([i for i, _ in refused], np.int64)
@@ -891,14 +903,19 @@ class FileBatchStream:
     the index (``JpegIndex.add``), so the batches read after that decode them on many threads.  With ``progressive``,
     progressive files are decoded on the device too: their scans travel in the same slot.  With ``find``, every batch
     is decoded by ``decode_jpeg(find=True)``: files without points get a scan index found on the device first and
-    decode on many threads; with ``learn``, the files whose found index converged are entered with those points."""
+    decode on many threads; with ``learn``, the files whose found index converged are entered with those points.
+    With ``progressive_index`` as well as ``progressive``, progressive files are looked up and learned like the others.
+    """
 
     SLOTS = 2
     WORKERS = 2
 
-    def __init__(self, workers=None, index=None, learn=False, progressive=False, find=False):
+    def __init__(self, workers=None, index=None, learn=False, progressive=False, find=False, progressive_index=False):
         if learn and index is None:
             raise ValueError("learn needs an index")
+        if progressive_index and not progressive:
+            raise ValueError("progressive_index needs progressive")
+        self.progressive_index = bool(progressive_index)
         self.workers = int(workers or self.WORKERS)
         self.index = index
         self.learn = bool(learn)
@@ -909,7 +926,7 @@ class FileBatchStream:
 
     def _stage(self, paths, slot, pool, dev):
         hb = read_jpeg_batch(paths, chunked_map(pool.map, self.workers) if self.workers > 1 else map, self.index,
-                             self.progressive)
+                             self.progressive, self.progressive_index)
         lay = _Layout(hb)
         if self.copied[slot] is not None:
             self.copied[slot].synchronize()
@@ -1052,7 +1069,8 @@ class GpuAugmentedLoader:
             dev = self.dataset.device
             batches = [idx_all[k * self.batch_size:(k + 1) * self.batch_size] for k in range(len(self))]
             self.staging = FileBatchStream(index=self.dataset.index, learn=self.dataset.learn,
-                                           progressive=self.dataset.progressive, find=self.dataset.find)
+                                           progressive=self.dataset.progressive, find=self.dataset.find,
+                                           progressive_index=getattr(self.dataset, "progressive_index", False))
             files = self.staging([self.dataset.select(idx) for idx in batches], dev)
         else:
             dev = self.dataset.images.device
@@ -1280,7 +1298,10 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
     restart-free file that has none (``decode_jpeg(find=True)``), so even the first epoch and files no index lists
     decode on many threads, with the same pixels; with ``faa_jpeg_index_learn`` the index learns the found points, and
     the first epoch pays no serial decode.  A find that does not converge within its rounds still splits the file at
-    the points it verified (DESIGN §4.8)."""
+    the points it verified (DESIGN §4.8).  ``faa_jpeg_progressive_index`` (default False; needs
+    ``faa_jpeg_progressive``): progressive files take a scan index too, so with ``faa_jpeg_index`` or
+    ``faa_jpeg_index_learn`` their restart-free scans decode on many threads from points looked up or learned like any
+    other file's, with the same pixels (``python -m fast_autoaugment_b200.jpeg_index --progressive`` writes them)."""
     from sklearn.model_selection import StratifiedShuffleSplit
 
     conf = C.get()
@@ -1307,6 +1328,9 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
     learn = bool(conf.get("faa_jpeg_index_learn", False))
     progressive = bool(conf.get("faa_jpeg_progressive", False))
     find = bool(conf.get("faa_jpeg_index_find", False))
+    progressive_index = bool(conf.get("faa_jpeg_progressive_index", False))
+    if progressive_index and not progressive:
+        raise ValueError("conf['faa_jpeg_progressive_index'] needs conf['faa_jpeg_progressive']")
 
     def device_dataset(x, y):
         if isinstance(x, FilePaths):
@@ -1319,9 +1343,10 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
                 index = JpegIndex.load(path, x.folder)
             if learn and index is None:
                 index = JpegIndex.empty(x.folder)
-            return JpegFileDataset(x, y, index=index, learn=learn, progressive=progressive, find=find)
+            return JpegFileDataset(x, y, index=index, learn=learn, progressive=progressive, find=find,
+                                   progressive_index=progressive_index)
         if isinstance(x, list) and len(x) and isinstance(x[0], bytes):
-            return EncodedDeviceDataset(x, y, progressive=progressive, find=find)
+            return EncodedDeviceDataset(x, y, progressive=progressive, find=find, progressive_index=progressive_index)
         return RaggedDeviceDataset(x, y) if isinstance(x, list) else DeviceDataset(x, y)
     if dataset in ("cifar10", "cifar100", "svhn", "imagenet"):
         total_trainset, testset = device_dataset(tr_x, tr_y), device_dataset(te_x, te_y)

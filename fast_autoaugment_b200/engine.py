@@ -604,7 +604,7 @@ def _parse_any(f):
     return hdr, tabs, None
 
 
-def parse_jpeg_headers(files, map=map, progressive=False):
+def parse_jpeg_headers(files, map=map, progressive=False, progressive_index=False):
     """JPEG files (``bytes``) -> (headers [N], table pool, refused [(position, reason)]).  The tables the files use are
     deduplicated into the pool in order of first use, which the headers' ``pool`` slots index; a refused file's header
     row stays zero and adds nothing to the pool.  ``offset`` is left 0: the caller places the files.  ``map`` runs the
@@ -613,7 +613,13 @@ def parse_jpeg_headers(files, map=map, progressive=False):
     ``progressive=True`` also takes progressive files (``parse_jpeg_progressive``; their headers' ``reserved`` is
     ``JPEG_PROGRESSIVE``), their scans' Huffman tables going into the same pool, and returns ``(headers, pool, refused,
     scans, scan_first)``: ``JPEG_SCAN_DTYPE`` scans with pool slots set, file i's being
-    ``scans[scan_first[i]:scan_first[i + 1]]`` (none for the other files)."""
+    ``scans[scan_first[i]:scan_first[i + 1]]`` (none for the other files).
+
+    ``progressive_index=True`` (with ``progressive``) marks progressive files as taking a scan index: ``reserved`` is
+    ``JPEG_PROGRESSIVE | JPEG_SCAN_INDEXED`` and ``scan_len`` the sum of their scans' lengths (the scan axis of
+    ``faa_jpeg.cuh``), so they are indexed, recorded and learned as baseline files are."""
+    if progressive_index and not progressive:
+        raise ValueError("progressive_index needs progressive=True")
     headers = np.zeros(len(files), dtype=_lib.JPEG_HEADER_DTYPE)
     pool, index, refused = [], {}, []
     scans, counts = [], np.zeros(len(files), np.int64)
@@ -642,6 +648,9 @@ def parse_jpeg_headers(files, map=map, progressive=False):
                         sc["pool"][k, t] = slot_of(tabs[3 + 6 * k + t])
             scans.append(sc)
             counts[i] = len(sc)
+            if progressive_index:
+                headers["reserved"][i] = _lib.JPEG_PROGRESSIVE | _lib.JPEG_SCAN_INDEXED
+                headers["scan_len"][i] = int(sc["len"].sum())
             continue
         for slot in range(9):
             if slot % 3 >= nc:
@@ -712,14 +721,18 @@ class EncodedImages:
         self._d_scan_first = _d_scan_first
 
     @staticmethod
-    def from_bytes(files, device="cuda", progressive=False):
+    def from_bytes(files, device="cuda", progressive=False, progressive_index=False):
         """JPEG files (``bytes``) -> EncodedImages on ``device``.  Raises ValueError naming every file the decoder
         does not take (progressive, arithmetic, 12-bit, CMYK, other sampling, malformed ...) and why.
-        ``progressive=True`` takes progressive files too (``parse_jpeg_headers``)."""
+        ``progressive=True`` takes progressive files too, and ``progressive_index=True`` lets them take a scan index
+        (``parse_jpeg_headers``)."""
+        if progressive_index and not progressive:
+            raise ValueError("progressive_index needs progressive=True")
         files = [bytes(f) for f in files]
         scans = scan_first = None
         if progressive:
-            headers, pool, refused, scans, scan_first = parse_jpeg_headers(files, progressive=True)
+            headers, pool, refused, scans, scan_first = parse_jpeg_headers(files, progressive=True,
+                                                                           progressive_index=progressive_index)
         else:
             headers, pool, refused = parse_jpeg_headers(files)
         if refused:
@@ -745,7 +758,11 @@ class EncodedImages:
 
     def progressive(self):
         """bool [N]: which files are progressive"""
-        return self.headers["reserved"] == _lib.JPEG_PROGRESSIVE
+        return (self.headers["reserved"] & _lib.JPEG_PROGRESSIVE) != 0
+
+    def progressive_indexed(self):
+        """bool [N]: which files are progressive and take a scan index (``progressive_index=True``)"""
+        return self.headers["reserved"] == _lib.JPEG_PROGRESSIVE | _lib.JPEG_SCAN_INDEXED
 
     def with_index(self, first, points):
         """the same files carrying the scan index (first, points), e.g. ``build_jpeg_index``'s"""
@@ -806,19 +823,30 @@ def build_jpeg_index(encoded: EncodedImages, find=False):
     """The scan index of every file of ``encoded`` (C ABI ``faa_jpeg_index_build``: one serial decode per file on the
     device, one thread per file): ``(first, points)``, int64 [N + 1] offsets into ``JPEG_SYNC_DTYPE`` points, file i's
     being ``points[first[i]:first[i + 1]]``.  Files with restart markers, scans under 2 KiB and files whose scan does
-    not decode cleanly get none, and so do progressive files.  Waits for the device.
+    not decode cleanly get none, and so do progressive files that take no scan index.  Progressive files that take one
+    (``from_bytes(..., progressive_index=True)``) get the points a recording ``decode_jpeg`` places, without the points
+    they carry: the index of a progressive file needs its coefficient planes, which only a decode fills.  Waits for the
+    device.
 
     ``find=True`` finds the index in parallel instead (``faa_jpeg_index_find``: one CTA per file, no serial decode).
     Each file's points are then the verified prefix of the chain: always the first points of the serial build's for a
-    file that decodes cleanly, and all of them when the chain converged (DESIGN §4.8)."""
+    file that decodes cleanly, and all of them when the chain converged (DESIGN §4.8).  Progressive files get none."""
     _require_cuda(encoded.storage, "encoded")
     prog = encoded.progressive()
     if prog.any():
-        at = np.flatnonzero(~prog)
-        first, points = build_jpeg_index(encoded.select(at), find)
-        counts = np.zeros(len(encoded), np.int64)
-        counts[at] = np.diff(first)
-        return np.concatenate([[0], np.cumsum(counts)]).astype(np.int64), points
+        parts = [None] * len(encoded)
+        groups = [(np.flatnonzero(~prog), lambda e: build_jpeg_index(e, find))]
+        if not find:
+            groups.append((np.flatnonzero(encoded.progressive_indexed()), _record_progressive_index))
+        for at, build in groups:
+            if len(at):
+                first, points = build(encoded.select(at))
+                for k, i in enumerate(at):
+                    parts[i] = points[first[k]:first[k + 1]]
+        counts = np.array([0 if q is None else len(q) for q in parts], np.int64)
+        got = [q for q in parts if q is not None and len(q)]
+        return np.concatenate([[0], np.cumsum(counts)]).astype(np.int64), \
+            (np.concatenate(got) if got else np.zeros(0, _lib.JPEG_SYNC_DTYPE))
     dev = encoded.device
     B = len(encoded)
     if B == 0:
@@ -841,6 +869,14 @@ def build_jpeg_index(encoded: EncodedImages, find=False):
         count = d_count.cpu().numpy()
         pts = d_points.cpu().numpy()[:total * 16].view(_lib.JPEG_SYNC_DTYPE)
     return compact_jpeg_index(cap_first, count, pts)
+
+
+def _record_progressive_index(encoded: EncodedImages):
+    """``build_jpeg_index`` of scan-indexed progressive files: a recording decode without the points they carry"""
+    bare = EncodedImages(encoded.storage, encoded.headers, encoded.pool, encoded.device_pool(), scans=encoded.scans,
+                         scan_first=encoded.scan_first)
+    _, _, count, points, cap_first = decode_jpeg(bare, record=True)
+    return compact_jpeg_index(cap_first, count.cpu().numpy(), points.cpu().numpy())
 
 
 def jpeg_index_capacities(headers):
@@ -909,7 +945,9 @@ def decode_jpeg(encoded: EncodedImages, out: RaggedImages | None = None, record=
 
     Progressive files (``EncodedImages.from_bytes(..., progressive=True)``) are decoded by the same call from the scans
     they carry, one more launch when the batch mixes both kinds.  They get no scan index: count 0 with ``record=True``,
-    and points given to them are not used."""
+    and points given to them are not used.  Unless they take one (``progressive_index=True``): their restart-free
+    scans then decode on many threads from the points they carry, checked as a baseline file's are, and ``record``
+    records their points as it records a baseline file's.  Same pixels and status, same launches."""
     _require_cuda(encoded.storage, "encoded")
     dev = encoded.device
     if out is None:

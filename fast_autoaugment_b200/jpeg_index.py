@@ -4,7 +4,9 @@ For each split of ``DATAROOT/imagenet-pytorch/{train,val}`` (the reference's sam
 reads the files as the loaders do, records each file's scan index on the device (``engine.build_jpeg_index``: one
 serial decode per file) and writes ``OUTDIR/<split>.npz`` (``data.JpegIndex``).  Give ``OUTDIR`` to
 ``get_dataloaders('imagenet', ...)`` as ``conf['faa_jpeg_index']``: the files listed there are then decoded on many
-threads each, with the same pixels.  The files themselves are not changed."""
+threads each, with the same pixels.  The files themselves are not changed.  With ``--progressive`` it also indexes
+progressive files (their points come from a recording decode on the device), for loaders run with
+``conf['faa_jpeg_progressive']`` and ``conf['faa_jpeg_progressive_index']``; without it they are listed with no points."""
 from __future__ import annotations
 
 import argparse
@@ -22,9 +24,10 @@ from .engine import EncodedImages, build_jpeg_index, parse_jpeg_headers
 CHUNK_BYTES = 256 << 20           # file bytes on the device at a time
 
 
-def index_files(paths, folder, device="cuda", workers=4, log=None):
+def index_files(paths, folder, device="cuda", workers=4, log=None, progressive=False):
     """The ``data.JpegIndex`` of ``paths`` (files under ``folder``).  Files the device decoder refuses are listed with
-    no points."""
+    no points; so are progressive files, unless ``progressive`` (``build_jpeg_index`` of files parsed with
+    ``progressive_index=True``)."""
     paths = [os.fspath(p) for p in paths]
     sizes, firsts, points = [], [np.zeros(1, np.int64)], []
     t0, done = time.perf_counter(), 0
@@ -37,12 +40,12 @@ def index_files(paths, folder, device="cuda", workers=4, log=None):
                 nbytes += os.path.getsize(paths[k])
                 k += 1
             files = list(ex.map(data._read_file, chunk))
-            headers, pool, refused = parse_jpeg_headers(files, ex.map)
+            headers, pool, refused = parse_jpeg_headers(files, ex.map, progressive, progressive)[:3]
             bad = {i for i, _ in refused}
             ok = [i for i in range(len(files)) if i not in bad]
             counts = np.zeros(len(files), np.int64)
             if ok:
-                enc = EncodedImages.from_bytes([files[i] for i in ok], device)
+                enc = EncodedImages.from_bytes([files[i] for i in ok], device, progressive, progressive)
                 first, pts = build_jpeg_index(enc)
                 counts[ok] = np.diff(first)
                 points.append(pts)
@@ -62,6 +65,8 @@ def main(argv=None):
     ap.add_argument("outdir", help="directory for train.npz and val.npz (conf['faa_jpeg_index'])")
     ap.add_argument("--splits", default="train,val")
     ap.add_argument("--workers", type=int, default=4, help="reader threads")
+    ap.add_argument("--progressive", action="store_true",
+                    help="index progressive files too (conf['faa_jpeg_progressive_index'])")
     a = ap.parse_args(argv)
     if not torch.cuda.is_available():
         raise SystemExit("the scan index is recorded on the device: no CUDA device")
@@ -70,7 +75,8 @@ def main(argv=None):
         samples = data.imagenet_index(a.dataroot, split)
         folder = data.imagenet_split_folder(a.dataroot, split)
         idx = index_files([p for p, _ in samples], folder, workers=a.workers,
-                          log=lambda m, s=split: print("[jpeg_index] %s: %s" % (s, m), file=sys.stderr, flush=True))
+                          log=lambda m, s=split: print("[jpeg_index] %s: %s" % (s, m), file=sys.stderr, flush=True),
+                          progressive=a.progressive)
         out = os.path.join(a.outdir, "%s.npz" % split)
         idx.save(out)
         print("[jpeg_index] %s: %d files, %d indexed, %d points -> %s" % (

@@ -412,9 +412,21 @@ int faa_jpeg_index_find(const faa_jpeg_header_t* h_headers, const faa_jpeg_heade
  * FAA_JPEG_MAX_SCANS scans; multi-scan sequential, arithmetic coding and the rest stay refused.  Its header has
  * reserved = FAA_JPEG_PROGRESSIVE, restart = 0 and no scan_off / scan_len, and its quantisation tables are those in force at
  * each component's first scan.  faa_jpeg_decode takes such a header with its scans (below); faa_jpeg_index_build and
- * faa_jpeg_index_find refuse it with FAA_ERR_VALUE, and faa_jpeg_index_capacity gives it 0: progressive files have no
- * scan index. */
+ * faa_jpeg_index_find refuse it with FAA_ERR_VALUE, and faa_jpeg_index_capacity gives it 0: such a file has no scan index.
+ *
+ * A caller that wants a progressive file to take a scan index sets reserved = FAA_JPEG_PROGRESSIVE | FAA_JPEG_SCAN_INDEXED
+ * and scan_len = the sum of its scans' len (faa_jpeg_decode refuses any other scan_len); scan_off and restart stay 0.
+ * Its scans, concatenated in file order, form one byte axis of scan_len bytes, and the placement rule above applies to
+ * that axis: faa_jpeg_index_capacity gives P - 1.  A point of such a file (faa_jpeg_sync_t) holds: byte, the axis offset
+ * of the data byte holding the next bit (the scan holding it is the point's scan); bit; mcu, the next unit of that scan
+ * (an MCU of an interleaved DC scan, else a block of the component's ceil(w/8) x ceil(h/8) grid); pred, the DC
+ * predictors of a DC first scan's components, or EOBRUN in pred[0] for an AC scan, zeros otherwise.  Point k is the
+ * first unit boundary u >= 1 of the scan holding threshold k whose byte is >= the threshold and inside that scan;
+ * scans with a restart interval get no points.  faa_jpeg_index_build and faa_jpeg_index_find refuse such a header too
+ * (a progressive index is recorded by a recording faa_jpeg_decode, which fills the coefficient planes refinement scans
+ * read). */
 #define FAA_JPEG_PROGRESSIVE 1
+#define FAA_JPEG_SCAN_INDEXED 2
 #define FAA_JPEG_MAX_SCANS 64
 typedef struct faa_jpeg_scan {
     int64_t off;              /* entropy-coded data: bytes [off, off + len) of the file                              */
@@ -465,8 +477,11 @@ int faa_jpeg_scan_tables(const uint8_t* bytes, size_t len, const faa_jpeg_header
  *   - scans in (h_scans, d_scans, h_scan_first, d_scan_first), needed for progressive files (FAA_ERR_VALUE without it):
  *     image i's scans are scans[scan_first[i], scan_first[i + 1]), 1 to FAA_JPEG_MAX_SCANS for a progressive file and
  *     none for a baseline one; every scan, its wave included, is checked on the host.  A progressive header's
- *     pool[0, ncomp) index its quantisation tables; its scan_off, scan_len and restart must be 0.  Progressive files
- *     have no scan index: points given to them are not used, and their count is 0.
+ *     pool[0, ncomp) index its quantisation tables; its scan_off, scan_len and restart must be 0 (scan_len: the scan
+ *     axis's length with FAA_JPEG_SCAN_INDEXED).  A FAA_JPEG_PROGRESSIVE file has no scan index: points given to it are
+ *     not used, and its count is 0.  A scan-indexed one takes points and records them as a baseline file does: a
+ *     restart-free scan is split at its points, every split is checked against the next point, and a file where one
+ *     check fails is decoded again, whole, without its points.
  * find != 0 needs the recording group (FAA_ERR_VALUE without it): the files without input points first get their scan
  * index found in parallel (faa_jpeg_index_find, into d_points_out), so that a restart-free file decodes on many threads
  * without a saved index; files with input points keep them.  count[i] > 0 still means these are file i's points now:
