@@ -92,6 +92,8 @@ def _load():
         "faa_policy_set_overlap": (C.c_int, [vp, C.c_int]),
         "faa_augment_many": (C.c_int, [vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, P(Tail), P(Rng), C.c_uint64, vp]),
         "faa_augment_tta": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, P(Tail), P(Rng), vp]),
+        "faa_augment_tta_policies": (C.c_int, [vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, P(Tail), P(Rng),
+                                               vp]),
         "faa_augment_mixup": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, C.c_int, P(Tail),
                                         vp, vp, P(Rng), vp, f32, f32, vp]),
         "faa_augment_host": (C.c_int, [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, P(Tail), P(Rng), vp]),
@@ -109,6 +111,7 @@ def _load():
         "faa_crop_resize": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, P(Tail), vp, P(CropCfg), vp]),
         "faa_crop_resize_ragged": (C.c_int, [vp, vp, C.c_int, vp, P(Tail), vp, P(CropCfg), vp]),
         "faa_augment_ragged": (C.c_int, [vp, vp, vp, C.c_int, vp, vp, vp, vp, P(Rng), C.c_int, vp]),
+        "faa_augment_ragged_policies": (C.c_int, [vp, C.c_int, vp, vp, vp, C.c_int, vp, vp, P(Rng), vp]),
         "faa_jpeg_parse": (C.c_int, [C.c_char_p, C.c_size_t, vp]),
         "faa_jpeg_tables": (C.c_int, [C.c_char_p, C.c_size_t, vp, vp]),
         "faa_jpeg_decoder_create": (C.c_int, [P(vp)]),

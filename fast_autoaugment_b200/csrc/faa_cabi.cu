@@ -243,6 +243,8 @@ struct faa_policy {
     void* d_rg_progs = nullptr; size_t d_rg_progs_bytes = 0;
     void* d_rg_scratch = nullptr; size_t d_rg_scratch_bytes = 0;
     void* d_rg_copy = nullptr; size_t d_rg_copy_bytes = 0;
+    // faa_augment_tta_policies: the candidates' PolicyRef array of the call (grown, never shrunk; stream-ordered reuse)
+    void* d_cands = nullptr; size_t d_cands_bytes = 0;
 };
 
 // All device state of a policy handle lives on ONE device: the one current at its first device call.
@@ -337,7 +339,7 @@ int faa_policy_destroy(faa_policy_t* p) {
     if (p->d_norm_img) cudaFree(p->d_norm_img);
     if (p->d_in) cudaFree(p->d_in);
     if (p->d_out) cudaFree(p->d_out);
-    for (void* b : {p->d_rg_tab, p->d_rg_progs, p->d_rg_scratch, p->d_rg_copy}) if (b) cudaFree(b);
+    for (void* b : {p->d_rg_tab, p->d_rg_progs, p->d_rg_scratch, p->d_rg_copy, p->d_cands}) if (b) cudaFree(b);
     if (p->h_in_stage) cudaFreeHost(p->h_in_stage);
     if (p->h_out_stage) cudaFreeHost(p->h_out_stage);
     for (int i = 0; i < 2; ++i) {
@@ -902,7 +904,39 @@ struct AugRequest {
     int in_mod = 0;                                 // > 0: replicated launch (TTA), entry v reads input image v % in_mod
     bool own_stream = true;                         // false: a chunk of faa_augment_host on one of its side streams,
                                                     // which that call orders itself
+    // multi-policy TTA (faa_augment_tta_policies): entry v draws with candidate cands[v / per_cand]; cands[0] is the
+    // handle the call runs on, the others only lend their device tables
+    faa_policy_t* const* cands = nullptr; int n_cands = 0, per_cand = 0;
 };
+
+// grows one of the handle's per-call table buffers; earlier calls' kernels that may still use it are ordered on `stream`
+// (follow_stream), so waiting for it before the free is enough
+static int grow_on_stream(void** ptr, size_t* have, size_t need, cudaStream_t stream) {
+    if (*have >= need) return FAA_OK;
+    if (*ptr) { CK(cudaStreamSynchronize(stream)); CK(cudaFree(*ptr)); *ptr = nullptr; *have = 0; }
+    need = std::max(need, (size_t)65536);
+    CK(cudaMalloc(ptr, need));
+    *have = need;
+    return FAA_OK;
+}
+
+// The candidates' device tables at h x w (each taken under its own handle's mu), uploaded as the call's PolicyRef array
+// on `stream`.
+static int upload_candidates(faa_policy* p, faa_policy_t* const* cands, int n_cands, int h, int w, cudaStream_t stream,
+                             const PolicyRef** d_refs) {
+    std::vector<PolicyRef> refs((size_t)n_cands);
+    for (int t = 0; t < n_cands; ++t) {
+        faa_policy* c = cands[t];
+        if (int e = bind_device(c)) return e;
+        if (int e = device_table(c, h, w, true, &refs[(size_t)t].ops)) return e;
+        refs[(size_t)t].probs = c->d_probs; refs[(size_t)t].n_sub = c->n_sub; refs[(size_t)t].reserved = 0;
+    }
+    const size_t bytes = refs.size() * sizeof(PolicyRef);
+    if (int e = grow_on_stream(&p->d_cands, &p->d_cands_bytes, bytes, stream)) return e;
+    CK(cudaMemcpyAsync(p->d_cands, refs.data(), bytes, cudaMemcpyHostToDevice, stream));   // (pageable: staged at once)
+    *d_refs = reinterpret_cast<const PolicyRef*>(p->d_cands);
+    return FAA_OK;
+}
 
 static int augment_common(faa_policy_t* p, const AugRequest& q) {
     const faa_tail_t* tail = q.tail;
@@ -949,6 +983,7 @@ static int augment_common(faa_policy_t* p, const AugRequest& q) {
     in.batch = batch; in.crop_pad = std::min(h, std::max({0, tail->crop_pad, q.rng ? q.rng->crop_pad : 0}));
     in.in_mod16 = (uint32_t)((uintptr_t)q.in % 16); in.out_mod16 = (uint32_t)((uintptr_t)q.out % 16);
     in.two_src = q.partner != nullptr; in.apply_tail = q.apply_tail != 0; in.has_sg = p->has_sg;
+    for (int t = 1; t < q.n_cands; ++t) in.has_sg = in.has_sg || q.cands[t]->has_sg;
     in.split_min = kSplitMin;
     if (const char* e = getenv("FAA_SPLIT_MIN")) in.split_min = strtoull(e, nullptr, 10);   // tests: force either path
     in.philox = q.rng && !q.samples; in.allow_ahead = q.allow_ahead;
@@ -975,6 +1010,12 @@ static int augment_common(faa_policy_t* p, const AugRequest& q) {
     R.H = h; R.W = w; R.out_h = tail->out_h; R.out_w = tail->out_w;
     R.n_sub = p->n_sub; R.n_op = p->n_op; R.op_base = q.op_base; R.apply_tail = q.apply_tail;
     R.allow = s.allow; R.split = s.split;
+    if (q.n_cands > 1) {
+        if (int e = upload_candidates(p, q.cands, q.n_cands, h, w, stream, &R.cands)) return e;
+        R.per_cand = q.per_cand;
+        // the cluster kernel's self-resolving path draws from one policy: a multi-policy call always resolves first
+        s.self_resolving = false;
+    }
     if (s.scratch) {            // one scratch image per image, per program slot in the chained schedule
         s.scratch_slot_bytes = (size_t)q.n_all * h * w * 3;
         const size_t need = s.scratch_slot_bytes * (s.use_chain ? 2 : 1);
@@ -1082,6 +1123,43 @@ int faa_augment_tta(faa_policy_t* p, const uint8_t* d_in, void* d_out, int batch
     AugRequest q;
     q.in = d_in; q.out = d_out; q.n_all = q.batch = batch * replicas; q.h = h; q.w = w; q.tail = tail; q.rng = rng;
     q.allow_ahead = true; q.stream = stream; q.in_mod = replicas > 1 ? batch : 0;
+    return augment_common(p, q);
+}
+
+// The candidate list of a multi-policy TTA call, checked on the host before anything touches the device.
+static int check_candidates(faa_policy_t* const* policies, int n_policies) {
+    if (!policies || n_policies < 1) return fail(FAA_ERR_VALUE, "need a non-empty list of candidate policies");
+    for (int t = 0; t < n_policies; ++t) {
+        if (!policies[t]) return fail(FAA_ERR_VALUE, "candidate " + std::to_string(t) + " is null");
+        for (int u = 0; u < t; ++u)
+            if (policies[u] == policies[t])
+                return fail(FAA_ERR_VALUE, "candidates " + std::to_string(u) + " and " + std::to_string(t) + " are the same handle");
+        if (policies[t]->n_op != policies[0]->n_op)
+            return fail(FAA_ERR_VALUE, "every candidate needs the same n_op (candidate " + std::to_string(t) + " has " +
+                                       std::to_string(policies[t]->n_op) + ", candidate 0 " + std::to_string(policies[0]->n_op) + ")");
+    }
+    if (policies[0]->n_op > FAA_MAX_FUSED_OPS)
+        return fail(FAA_ERR_UNSUPPORTED, "replicated launches support policies of at most 2 ops");
+    return FAA_OK;
+}
+
+int faa_augment_tta_policies(faa_policy_t* const* policies, int n_policies, const uint8_t* d_in, void* d_out, int batch,
+                             int replicas, int h, int w, const faa_tail_t* tail, const faa_rng_t* rng, void* stream) {
+    if (int e = check_candidates(policies, n_policies)) return e;
+    if (!rng) return fail(FAA_ERR_VALUE, "null argument");
+    if (batch < 0 || replicas < 1) return fail(FAA_ERR_VALUE, "bad batch / replicas");
+    if ((long long)n_policies * batch * replicas > 65535)
+        return fail(FAA_ERR_UNSUPPORTED, "n_policies * replicas * batch must be <= 65535");
+    if (n_policies == 1) return faa_augment_tta(policies[0], d_in, d_out, batch, replicas, h, w, tail, rng, stream);
+    faa_policy* p = policies[0];
+    std::lock_guard<std::mutex> call_lk(p->call_mu);
+    // one launch over n_policies * replicas * batch entries; entry v = (t * replicas + r) * batch + i reads image i and
+    // draws the decisions of global sample first_index + v from candidate t.  No resolve-ahead: its speculation is keyed
+    // by the handle's own policy.
+    AugRequest q;
+    q.in = d_in; q.out = d_out; q.n_all = q.batch = n_policies * replicas * batch; q.h = h; q.w = w; q.tail = tail;
+    q.rng = rng; q.stream = stream; q.in_mod = batch;
+    q.cands = policies; q.n_cands = n_policies; q.per_cand = replicas * batch;
     return augment_common(p, q);
 }
 
@@ -1231,22 +1309,14 @@ int faa_crop_resize_ragged(const faa_image_t* h_images, const faa_image_t* d_ima
     return FAA_OK;
 }
 
-// grows one of the handle's ragged-launch buffers; earlier calls' kernels that may still use it are ordered on `stream`
-// (follow_stream), so waiting for it before the free is enough
-static int grow_on_stream(void** ptr, size_t* have, size_t need, cudaStream_t stream) {
-    if (*have >= need) return FAA_OK;
-    if (*ptr) { CK(cudaStreamSynchronize(stream)); CK(cudaFree(*ptr)); *ptr = nullptr; *have = 0; }
-    need = std::max(need, (size_t)65536);
-    CK(cudaMalloc(ptr, need));
-    *have = need;
-    return FAA_OK;
-}
-
 static size_t align16(size_t v) { return (v + 15) & ~(size_t)15; }
 
-int faa_augment_ragged(faa_policy_t* p, const faa_image_t* h_in, const faa_image_t* d_in, int batch,
-                       const faa_image_t* h_out, const faa_image_t* d_out, const faa_sample_t* d_samples,
-                       const faa_box_t* d_boxes, const faa_rng_t* rng, int op_base, void* stream_v) {
+// faa_augment_ragged, and faa_augment_ragged_policies when n_cands > 1: image i then draws with candidate
+// cands[h_cand[i]] (cands[0] == p runs the call, the others lend their device tables)
+static int augment_ragged(faa_policy_t* p, faa_policy_t* const* cands, int n_cands, const int32_t* h_cand,
+                          const faa_image_t* h_in, const faa_image_t* d_in, int batch, const faa_image_t* h_out,
+                          const faa_image_t* d_out, const faa_sample_t* d_samples, const faa_box_t* d_boxes,
+                          const faa_rng_t* rng, int op_base, void* stream_v) {
     if (!p || ((!h_in || !d_in || !h_out || !d_out) && batch > 0)) return fail(FAA_ERR_VALUE, "null argument");
     if (batch < 0) return fail(FAA_ERR_VALUE, "negative batch");
     if (batch > 65535) return fail(FAA_ERR_UNSUPPORTED, "at most 65535 images per call (one grid row per image): split the batch");
@@ -1268,22 +1338,34 @@ int faa_augment_ragged(faa_policy_t* p, const faa_image_t* h_in, const faa_image
                                              "(vector stores)");
         ins[(size_t)i] = {a.h, a.w, (uint32_t)((uintptr_t)a.data % 16), (uint32_t)((uintptr_t)o.data % 16)};
     }
+    const bool multi = n_cands > 1;
+    if (multi)
+        for (int i = 0; i < batch; ++i)
+            if (h_cand[i] < 0 || h_cand[i] >= n_cands)
+                return fail(FAA_ERR_VALUE, "image " + std::to_string(i) + " names candidate " + std::to_string(h_cand[i]) +
+                                           " of " + std::to_string(n_cands));
     if (int e = ensure_device()) return e;
     if (batch == 0) return FAA_OK;
     if (int e = bind_device(p)) return e;
+    for (int t = 1; t < n_cands; ++t) { if (int e = bind_device(cands[t])) return e; }
     std::lock_guard<std::mutex> call_lk(p->call_mu);
     cudaStream_t stream = (cudaStream_t)stream_v;
     if (int e = follow_stream(p, stream)) return e;
-    const RaggedPlan plan = plan_ragged(ins.data(), batch, p->has_sg);
+    bool has_sg = p->has_sg;
+    for (int t = 1; t < n_cands; ++t) has_sg = has_sg || cands[t]->has_sg;
+    const RaggedPlan plan = plan_ragged(ins.data(), batch, has_sg);
 
     // per-size launch parameters (in / out / progs / scratch are patched in per image by the kernel)
     const size_t n_geo = plan.geoms.size();
-    std::vector<const OpRec*> geo_ops(n_geo);
+    const int n_tab = multi ? n_cands : 1;
+    std::vector<const OpRec*> geo_ops((size_t)n_tab * n_geo);      // [candidate][size]
     std::vector<AugParams> geo(n_geo);
     for (size_t k = 0; k < n_geo; ++k) {
         const RaggedGeom& g = plan.geoms[k];
         // resolved samples can only reference ops the host sampler validated; Philox can pick anything
-        if (int e = device_table(p, g.H, g.W, d_samples == nullptr, &geo_ops[k])) return e;
+        for (int t = 0; t < n_tab; ++t)
+            if (int e = device_table(multi ? cands[t] : p, g.H, g.W, d_samples == nullptr, &geo_ops[(size_t)t * n_geo + k]))
+                return e;
         AugParams& a = geo[k];
         memset(&a, 0, sizeof a);
         a.B = 1; a.H = a.out_h = g.H; a.W = a.out_w = g.W;
@@ -1313,7 +1395,10 @@ int faa_augment_ragged(faa_policy_t* p, const faa_image_t* h_in, const faa_image
     const size_t off_img = align16(n_geo * sizeof(AugParams));
     const size_t off_list = off_img + align16((size_t)batch * sizeof(RaggedImg));
     const size_t off_copy = off_list + align16((size_t)batch * sizeof(int32_t));
-    const size_t tab_bytes = off_copy + (size_t)n_copy * sizeof(RaggedCopy);
+    // multi-policy calls: the candidates' probabilities and n_sub, and each image's candidate
+    const size_t off_refs = align16(off_copy + (size_t)n_copy * sizeof(RaggedCopy));
+    const size_t off_cand = off_refs + align16((size_t)n_tab * sizeof(PolicyRef));
+    const size_t tab_bytes = multi ? off_cand + (size_t)batch * sizeof(int32_t) : off_copy + (size_t)n_copy * sizeof(RaggedCopy);
     if (int e = grow_on_stream(&p->d_rg_tab, &p->d_rg_tab_bytes, tab_bytes, stream)) return e;
     if (int e = grow_on_stream(&p->d_rg_progs, &p->d_rg_progs_bytes, (size_t)batch * sizeof(Prog), stream)) return e;
     if (scratch_bytes) { if (int e = grow_on_stream(&p->d_rg_scratch, &p->d_rg_scratch_bytes, scratch_bytes, stream)) return e; }
@@ -1326,7 +1411,7 @@ int faa_augment_ragged(faa_policy_t* p, const faa_image_t* h_in, const faa_image
     for (int i = 0; i < batch; ++i) {
         const int k = plan.geom_of[(size_t)i];
         RaggedImg& m = imgs[i];
-        m.ops = geo_ops[(size_t)k]; m.H = plan.geoms[(size_t)k].H; m.W = plan.geoms[(size_t)k].W;
+        m.ops = geo_ops[(size_t)(multi ? h_cand[i] : 0) * n_geo + k]; m.H = plan.geoms[(size_t)k].H; m.W = plan.geoms[(size_t)k].W;
         m.allow = plan.geoms[(size_t)k].plan.allow; m.geom = k;
         m.scratch = scratch_at[(size_t)i] < 0 ? nullptr : (uint8_t*)p->d_rg_scratch + scratch_at[(size_t)i];
         m.realigned = copy_at[(size_t)i] < 0 ? nullptr : (uint8_t*)p->d_rg_copy + copy_at[(size_t)i];
@@ -1336,6 +1421,11 @@ int faa_augment_ragged(faa_policy_t* p, const faa_image_t* h_in, const faa_image
         copies[c] = {h_in[i].data, (uint8_t*)p->d_rg_copy + copy_at[(size_t)i], (uint64_t)imgs[i].H * imgs[i].W * 3};
     }
     memcpy(host.data() + off_list, plan.order.data(), (size_t)batch * sizeof(int32_t));
+    if (multi) {
+        PolicyRef* refs = reinterpret_cast<PolicyRef*>(host.data() + off_refs);
+        for (int t = 0; t < n_cands; ++t) refs[t] = {nullptr, cands[t]->d_probs, cands[t]->n_sub, 0};
+        memcpy(host.data() + off_cand, h_cand, (size_t)batch * sizeof(int32_t));
+    }
     CK(cudaMemcpyAsync(d_tab, host.data(), tab_bytes, cudaMemcpyHostToDevice, stream));   // (pageable: staged at once)
     const RaggedImg* d_imgs = reinterpret_cast<const RaggedImg*>(d_tab + off_img);
     if (n_copy) {
@@ -1350,6 +1440,10 @@ int faa_augment_ragged(faa_policy_t* p, const faa_image_t* h_in, const faa_image
     R.progs = reinterpret_cast<Prog*>(p->d_rg_progs); R.first = 0; R.n = batch;
     R.n_sub = p->n_sub; R.n_op = p->n_op; R.op_base = op_base;
     R.apply_tail = (op_base + FAA_MAX_FUSED_OPS >= p->n_op) ? 1 : 0;
+    if (multi) {
+        R.cands = reinterpret_cast<const PolicyRef*>(d_tab + off_refs);
+        R.cand_of = reinterpret_cast<const int32_t*>(d_tab + off_cand);
+    }
     CK(launch_resolve_ragged(R, d_imgs, stream));
     g_launches++;
     // pixels: one cluster-kernel launch per band count, largest images first
@@ -1364,6 +1458,27 @@ int faa_augment_ragged(faa_policy_t* p, const faa_image_t* h_in, const faa_image
     }
     p->chain_live = false;                  // the next chained step follows this call in stream order
     return FAA_OK;
+}
+
+int faa_augment_ragged(faa_policy_t* p, const faa_image_t* h_in, const faa_image_t* d_in, int batch,
+                       const faa_image_t* h_out, const faa_image_t* d_out, const faa_sample_t* d_samples,
+                       const faa_box_t* d_boxes, const faa_rng_t* rng, int op_base, void* stream) {
+    return augment_ragged(p, nullptr, 1, nullptr, h_in, d_in, batch, h_out, d_out, d_samples, d_boxes, rng, op_base, stream);
+}
+
+int faa_augment_ragged_policies(faa_policy_t* const* policies, int n_policies, const faa_image_t* h_in,
+                                const faa_image_t* d_in, const int32_t* h_policy, int batch, const faa_image_t* h_out,
+                                const faa_image_t* d_out, const faa_rng_t* rng, void* stream) {
+    if (int e = check_candidates(policies, n_policies)) return e;
+    if (!rng || (!h_policy && batch > 0)) return fail(FAA_ERR_VALUE, "null argument");
+    if (n_policies == 1) {
+        for (int i = 0; i < batch; ++i)
+            if (h_policy[i] != 0) return fail(FAA_ERR_VALUE, "image " + std::to_string(i) + " names candidate " +
+                                                              std::to_string(h_policy[i]) + " of 1");
+        return faa_augment_ragged(policies[0], h_in, d_in, batch, h_out, d_out, nullptr, nullptr, rng, 0, stream);
+    }
+    return augment_ragged(policies[0], policies, n_policies, h_policy, h_in, d_in, batch, h_out, d_out, nullptr, nullptr,
+                          rng, 0, stream);
 }
 
 int faa_mix_u8(faa_policy_t* p, const uint8_t* d_a, const uint8_t* d_b, const int32_t* d_partner, const int16_t* d_zero_box_a,

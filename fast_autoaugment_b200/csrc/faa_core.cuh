@@ -401,6 +401,15 @@ FAA_HD void philox_sample(const RngCfg& r, uint64_t index, const OpRec* ops, con
     s.gate = (uint8_t)gate; s.sign = (uint8_t)sign;
 }
 
+// One candidate policy of a multi-policy TTA call (faa_augment_tta_policies, faa_augment_ragged_policies): its compiled
+// table at the launch's size (the ragged resolve takes each image's table from its RaggedImg instead), probabilities and
+// sub-policy count.  Candidates share n_op; only the table, the probabilities and n_sub the decisions are drawn from
+// differ per entry, never the Philox keys.
+struct PolicyRef { const OpRec* ops; const double* probs; int32_t n_sub; int32_t reserved; };
+
+// schedule entry v of a uniform multi-policy TTA call, v = (t * K + r) * B + i, belongs to candidate t = v / (K * B)
+FAA_HD int tta_candidate(int v, int per_candidate) { return v / per_candidate; }
+
 // fast exact division of q by d via a 32-bit reciprocal (valid while q*d < 2^32)
 FAA_HD uint32_t recip32(uint32_t d) { return (uint32_t)((0x100000000ull + d - 1) / d); }
 FAA_HD uint32_t fastdiv(uint32_t q, uint32_t rcp) { return umulhi32(q, rcp); }

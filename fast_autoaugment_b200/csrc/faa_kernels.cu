@@ -97,6 +97,9 @@ __device__ __forceinline__ int cost_bucket(uint32_t cost) {     // 0 = most expe
     return b;
 }
 
+// kMulti: a multi-policy TTA call (P.cands); entry i takes candidate tta_candidate(i, per_cand)'s table, probabilities
+// and n_sub.  The single-policy instantiation is the kernel of every other call.
+template <bool kMulti>
 __global__ void __launch_bounds__(1024) faa_resolve_kernel(const __grid_constant__ ResolveParams P) {
     __shared__ int s_count[3 * kCostBuckets], s_base[3 * kCostBuckets];
     // let the dependent pixel kernel start launching (its prologue overlaps this kernel)
@@ -109,6 +112,13 @@ __global__ void __launch_bounds__(1024) faa_resolve_kernel(const __grid_constant
     __syncthreads();
     for (int t = threadIdx.x; t < P.n; t += blockDim.x) {
         const int i = P.first + t;
+        const OpRec* ops = P.ops;
+        const double* probs = P.probs;
+        int n_sub = P.n_sub;
+        if (kMulti) {
+            const PolicyRef c = P.cands[tta_candidate(i, P.per_cand)];
+            ops = c.ops; probs = c.probs; n_sub = c.n_sub;
+        }
         Sample s;
         Box bx[8];
         if (P.samples != nullptr) {
@@ -119,12 +129,12 @@ __global__ void __launch_bounds__(1024) faa_resolve_kernel(const __grid_constant
             }
         } else {
             const uint64_t at = P.pos != nullptr ? (uint64_t)(uint32_t)P.pos[i] : (uint64_t)i;
-            philox_sample(P.rng, P.rng.first_index + at, P.ops, P.probs, P.n_sub, P.n_op, P.H, P.W,
+            philox_sample(P.rng, P.rng.first_index + at, ops, probs, n_sub, P.n_op, P.H, P.W,
                           P.out_h, P.out_w, s, bx);
         }
         if (P.progs != nullptr) {
             Prog g;
-            build_prog(s, bx, P.ops, P.n_op, P.op_base, P.apply_tail, P.H, P.W, P.out_w, P.allow, g);
+            build_prog(s, bx, ops, P.n_op, P.op_base, P.apply_tail, P.H, P.W, P.out_w, P.allow, g);
             lean_order(g, P.allow);
             // weight class: 0 heavy (cluster kernel), 1 mid (statistics / Sharpness kernel, three-way split only), 2 light
             const int wc = !P.split ? 0 : prog_is_light(g, P.allow) ? 2 : (P.split == 2 && prog_is_mid(g, P.allow)) ? 1 : 0;
@@ -166,9 +176,18 @@ __global__ void __launch_bounds__(1024) faa_resolve_kernel(const __grid_constant
 
 // ragged launch (faa_augment_ragged): the same decisions -> program step, image i at its own size with its own op
 // table and allow bits (imgs[i]); Philox draws global sample rng.first_index + i.  No schedule: the host orders the images.
+// kMulti: a multi-policy TTA call; image i draws with candidate cand_of[i]'s probabilities and n_sub (imgs[i].ops is that
+// candidate's table at the image's size).
+template <bool kMulti>
 __global__ void __launch_bounds__(1024) faa_resolve_ragged_kernel(const __grid_constant__ ResolveParams P, const RaggedImg* imgs) {
     for (int i = threadIdx.x; i < P.n; i += blockDim.x) {
         const RaggedImg m = imgs[i];
+        const double* probs = P.probs;
+        int n_sub = P.n_sub;
+        if (kMulti) {
+            const PolicyRef c = P.cands[P.cand_of[i]];
+            probs = c.probs; n_sub = c.n_sub;
+        }
         Sample s;
         Box bx[8];
         if (P.samples != nullptr) {
@@ -178,7 +197,7 @@ __global__ void __launch_bounds__(1024) faa_resolve_ragged_kernel(const __grid_c
                 else { bx[j].x0 = bx[j].y0 = 0; bx[j].x1 = bx[j].y1 = -1; }
             }
         } else {
-            philox_sample(P.rng, P.rng.first_index + (uint64_t)i, m.ops, P.probs, P.n_sub, P.n_op, m.H, m.W, m.H, m.W, s, bx);
+            philox_sample(P.rng, P.rng.first_index + (uint64_t)i, m.ops, probs, n_sub, P.n_op, m.H, m.W, m.H, m.W, s, bx);
         }
         Prog g;
         build_prog(s, bx, m.ops, P.n_op, P.op_base, P.apply_tail, m.H, m.W, m.W, m.allow, g);
@@ -2515,13 +2534,15 @@ cudaError_t launch_resolve(const ResolveParams& p, cudaStream_t stream) {
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = p.pdl ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, faa_resolve_kernel, p);
+    return p.cands != nullptr ? cudaLaunchKernelEx(&cfg, faa_resolve_kernel<true>, p)
+                              : cudaLaunchKernelEx(&cfg, faa_resolve_kernel<false>, p);
 }
 
 cudaError_t launch_resolve_ragged(const ResolveParams& p, const RaggedImg* imgs, cudaStream_t stream) {
     if (p.n <= 0) return cudaSuccess;
     const int threads = p.n >= 1024 ? 1024 : ((p.n + 31) / 32) * 32;
-    faa_resolve_ragged_kernel<<<1, threads, 0, stream>>>(p, imgs);
+    if (p.cands != nullptr) faa_resolve_ragged_kernel<true><<<1, threads, 0, stream>>>(p, imgs);
+    else faa_resolve_ragged_kernel<false><<<1, threads, 0, stream>>>(p, imgs);
     return cudaGetLastError();
 }
 

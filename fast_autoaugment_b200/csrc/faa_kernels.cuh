@@ -31,7 +31,14 @@ struct ResolveParams {
     int32_t pdl;                // launch with programmatic stream serialization (chained steps)
     const uint32_t* wait_done;  // optional: before writing anything, spin until *wait_done has reached wait_target (the pixel
     uint32_t wait_target;       // CTAs that read this slot's previous programs count themselves there when they finish)
+    // multi-policy TTA calls (null otherwise: ops / probs / n_sub above serve every entry): entry i draws and builds with
+    // candidate cands[c]'s table, probabilities and n_sub, c = tta_candidate(i, per_cand) (faa_resolve_kernel) or
+    // cand_of[i] (faa_resolve_ragged_kernel)
+    const PolicyRef* cands;
+    const int32_t* cand_of;
+    int32_t per_cand;
 };
+// a non-null cands launches the multi-policy instantiation
 cudaError_t launch_resolve(const ResolveParams& p, cudaStream_t stream);
 
 // AugParams::chain: how a pixel launch is ordered against the kernel in front of it in its stream

@@ -27,8 +27,9 @@ from torch.utils.data import Sampler, SubsetRandomSampler
 from . import _lib, archive
 from .conf import Config as C
 from .engine import (CIFAR_MEAN, CIFAR_STD, IMAGENET_MEAN, IMAGENET_STD, CompiledPolicy, EncodedImages, RaggedImages,
-                     TailSpec, augment_batch, augment_tta, center_crop_box, check_tta, compact_jpeg_index, crop_cfg,
-                     crop_resize, decode_jpeg, make_rng, parse_jpeg_headers, sample_philox_at, tta_positions, tta_select)
+                     TailSpec, augment_batch, augment_tta, augment_tta_policies, center_crop_box, check_tta,
+                     check_tta_policies, compact_jpeg_index, compile_policies, crop_cfg, crop_resize, decode_jpeg, make_rng,
+                     parse_jpeg_headers, sample_philox_at, tta_positions, tta_select)
 
 
 class Augmentation(object):
@@ -479,27 +480,62 @@ class ImageNetChain(object):
         self.check_tta(B, replicas, parity)
         K = int(replicas)
         x = self._decoded(batch)
-        dev = x.device
-        raw = TailSpec.raw_u8()
+        y = None
         if self.aug is not None:
-            y = augment_tta(self.aug.compiled, x, raw, K, seed, first_index)
+            y = augment_tta(self.aug.compiled, x, TailSpec.raw_u8(), K, seed, first_index)
             if not isinstance(y, RaggedImages):
                 y = y.view(K * B, *y.shape[2:])
-        elif isinstance(x, RaggedImages):
-            y = tta_select(x, K)
-        else:                                               # the sources themselves, K descriptors each
+        out = self._tta_stages(x, y, B, K, seed, first_index)
+        return out.view(K, B, *out.shape[1:])
+
+    def _tta_stages(self, x, y, B, n, seed, first_index):
+        """crop + resize, ColorJitter and HFlip + Lighting + Normalize, one launch each over the n * B entries of a TTA
+        call: the policy's outputs ``y`` (n * B images in entry order), or, without a policy (``y`` None), the B
+        sources ``x`` read n times through replicated descriptors -> [n * B, 3, s, s]"""
+        dev = x.device
+        if y is None and isinstance(x, RaggedImages):
+            y = tta_select(x, n)
+        elif y is None:                                     # the sources themselves, n descriptors each
             x = x.contiguous()
             h, w = int(x.shape[1]), int(x.shape[2])
-            y = RaggedImages(x.view(-1), tta_positions(B, K) * (h * w * 3), [(h, w)] * (K * B))
+            y = RaggedImages(x.view(-1), tta_positions(B, n) * (h * w * 3), [(h, w)] * (n * B))
         s = self.input_size
         z = crop_resize(y, s, rng=self.crop.cfg(seed, first_index))
-        recs, rgb = self._device_records_tta(B, dev, seed, first_index, K)
+        recs, rgb = self._device_records_tta(B, dev, seed, first_index, n)
         with torch.cuda.device(dev):
             import ctypes as C
-            _lib.check(_lib.lib.faa_color_jitter(z.data_ptr(), z.data_ptr(), K * B, s, s, recs.data_ptr(),
+            _lib.check(_lib.lib.faa_color_jitter(z.data_ptr(), z.data_ptr(), n * B, s, s, recs.data_ptr(),
                                                  C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
-        out = augment_batch(self.flip_policy, z, self.tail, rng=make_rng(seed, first_index, self.tail), lighting_rgb=rgb)
-        return out.view(K, B, *out.shape[1:])
+        return augment_batch(self.flip_policy, z, self.tail, rng=make_rng(seed, first_index, self.tail), lighting_rgb=rgb)
+
+    def check_tta_policies(self, n, policies, replicas, parity=False):
+        """ValueError for a ``train_tta_policies`` call this chain refuses (``policies``: ``CompiledPolicy`` handles):
+        parity draws and what ``check_tta_policies`` refuses"""
+        if parity:
+            raise ValueError("train_tta draws with Philox only: K reference loaders have no single parity draw order")
+        check_tta_policies(policies, n, replicas)
+
+    def train_tta_policies(self, batch, policies, replicas, seed=0, first_index=0, parity=False):
+        """``train_tta`` for T candidate policies in place of the chain's own (the policy search scoring several
+        suggestions against one fold): uint8 [B,H,W,3] CUDA, ``RaggedImages`` or ``EncodedImages`` (decoded once) ->
+        [T, replicas, B, 3, s, s] ``out_dtype`` with
+
+            out[t] == ImageNetChain(policies[t]).train_tta(batch, replicas, seed, first_index + t * replicas * B)
+
+        Each stage is one launch (group) over all T * replicas * B entries, entry v = (t * replicas + r) * B + i drawing
+        the Philox keys of global sample first_index + v: the policy (``augment_tta_policies``), crop + resize,
+        ColorJitter and HFlip + Lighting + Normalize.  ``policies``: what ``compile_policies`` takes.  Raises ValueError
+        before any device work for what ``check_tta_policies`` refuses."""
+        pols = compile_policies(policies)
+        B = len(batch) if isinstance(batch, (RaggedImages, EncodedImages)) else int(batch.shape[0])
+        self.check_tta_policies(B, pols, replicas, parity)
+        T, K = len(pols), int(replicas)
+        x = self._decoded(batch)
+        y = augment_tta_policies(pols, x, TailSpec.raw_u8(), K, seed, first_index)
+        if not isinstance(y, RaggedImages):
+            y = y.view(T * K * B, *y.shape[3:])
+        out = self._tta_stages(x, y, B, T * K, seed, first_index)
+        return out.view(T, K, B, *out.shape[1:])
 
     def test(self, batch_u8, out=None):
         """uint8 [B,H,W,3] CUDA (or ``RaggedImages``) -> [B, 3, s, s]: center crop + resize + ToTensor + Normalize, one
@@ -1106,19 +1142,30 @@ class GpuAugmentedLoader:
                 self._drawn += len(t)
                 yield data, self.dataset.labels.index_select(0, t)
 
-    def tta(self, replicas):
+    def tta(self, replicas, policies=None):
         """The policy search's test-time augmentation (reference search.py:87-125, ``eval_tta``) from one loader: an
         iterator over one epoch of this loader's index stream yielding ``(data[replicas, B, ...], labels[B])``, replica r
         of batch k being what this loader's own ``__iter__`` would yield for it with the Philox keys of
         ``first_index = drawn + r * B`` (``drawn``: samples drawn before the batch).  Each batch is gathered, read or
         decoded once; the replicas come from ``augment_tta`` (no chain) or ``ImageNetChain.train_tta``.  The batch
         draws replicas * B keys, so no key repeats within or across batches or epochs, unlike replicas separate loaders
-        built with one seed.  Raises ValueError for parity draws, a test-chain loader and what ``check_tta`` refuses."""
+        built with one seed.  Raises ValueError for parity draws, a test-chain loader and what ``check_tta`` refuses.
+
+        ``policies``: T candidate policies (what ``compile_policies`` takes: archive lists, ``CompiledPolicy``) scored in
+        place of the loader's own.  Each batch then yields ``(data[T, replicas, B, ...], labels[B])`` from one read or
+        decode, candidate t's block being what ``tta(replicas)`` of a loader with policy t would yield with the keys of
+        ``first_index = drawn + t * replicas * B`` (``augment_tta_policies`` or ``ImageNetChain.train_tta_policies``),
+        and ``drawn`` advances by T * replicas * B.  It also raises ValueError for what ``check_tta_policies``
+        refuses."""
         if self.parity:
             raise ValueError("tta draws with Philox only: K reference loaders have no single parity draw order")
         if self.chain is not None and self.chain_mode != "train":
             raise ValueError("tta replicates the train chain: a %r chain loader draws nothing" % self.chain_mode)
         n = min(self.batch_size, self._n())
+        if policies is not None:
+            pols = compile_policies(policies)
+            check_tta_policies(pols, n, replicas)
+            return self._tta(int(replicas), pols)
         if self.chain is not None:
             self.chain.check_tta(n, replicas)
         else:
@@ -1128,14 +1175,18 @@ class GpuAugmentedLoader:
                                  % _lib.MAX_FUSED_OPS)
         return self._tta(int(replicas))
 
-    def _tta(self, K):
+    def _tta(self, K, pols=None):
         with contextlib.closing(self._batches()) as batches:
             for t, raw in batches:
-                if self.chain is None:
+                if pols is not None and self.chain is None:
+                    data = augment_tta_policies(pols, raw, self.tail, K, self.seed, self._drawn)
+                elif pols is not None:
+                    data = self.chain.train_tta_policies(raw, pols, K, seed=self.seed, first_index=self._drawn)
+                elif self.chain is None:
                     data = augment_tta(self.aug.compiled, raw, self.tail, K, self.seed, self._drawn)
                 else:
                     data = self.chain.train_tta(raw, K, seed=self.seed, first_index=self._drawn)
-                self._drawn += K * len(t)
+                self._drawn += (len(pols) if pols is not None else 1) * K * len(t)
                 yield data, self.dataset.labels.index_select(0, t)
 
 

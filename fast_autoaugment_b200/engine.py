@@ -450,6 +450,103 @@ def check_tta(batch, replicas):
                                                                                 MAX_LAUNCH_IMAGES))
 
 
+def compile_policies(policies):
+    """The candidates of a multi-policy TTA call as ``CompiledPolicy`` handles: each item is a ``CompiledPolicy``, an
+    object holding one as ``compiled`` (``data.Augmentation``) or a reference-format policy list (what the search's
+    ``policy_decoder`` returns for one hyperopt suggestion)."""
+    out = []
+    for p in policies:
+        if isinstance(p, CompiledPolicy):
+            out.append(p)
+        elif isinstance(getattr(p, "compiled", None), CompiledPolicy):
+            out.append(p.compiled)
+        else:
+            out.append(CompiledPolicy(p))
+    return out
+
+
+def check_tta_policies(policies, batch, replicas):
+    """ValueError for a multi-policy TTA call (``augment_tta_policies``) of ``CompiledPolicy`` candidates that the
+    library refuses: what ``check_tta`` refuses, no candidate, one handle given twice, candidates of different op counts
+    or of more than one fused window, and more than 65535 entries (candidates * replicas * batch) per launch"""
+    check_tta(batch, replicas)
+    if len(policies) == 0:
+        raise ValueError("need at least one candidate policy")
+    if len({id(p) for p in policies}) != len(policies):
+        raise ValueError("a candidate policy is given twice: build one CompiledPolicy per candidate")
+    n_op = sorted({p.n_op for p in policies})
+    if len(n_op) != 1:
+        raise ValueError("every candidate needs the same number of ops per sub-policy, not %s" % n_op)
+    if n_op[0] > _lib.MAX_FUSED_OPS:
+        raise ValueError("tta supports policies of at most %d ops per sub-policy (replicated launches)"
+                         % _lib.MAX_FUSED_OPS)
+    n = len(policies) * int(replicas) * int(batch)
+    if n > MAX_LAUNCH_IMAGES:
+        raise ValueError("candidates * replicas * batch = %d images: at most %d per launch" % (n, MAX_LAUNCH_IMAGES))
+
+
+def tta_policy_entries(n_policies, batch, replicas):
+    """(candidate, replica, image) int64 arrays of the n_policies * replicas * batch schedule entries of a multi-policy
+    TTA call: entry v = (t * replicas + r) * batch + i"""
+    v = np.arange(int(n_policies) * int(replicas) * int(batch), dtype=np.int64)
+    return v // (int(replicas) * int(batch)), (v // int(batch)) % int(replicas), v % int(batch)
+
+
+def augment_tta_policies(policies, batch_u8, tail: TailSpec, replicas: int, seed: int, first_index: int = 0, out=None):
+    """``augment_tta`` for T candidate policies at once (the policy search scoring several suggestions against one
+    validation fold): ONE resolve launch and the pixel launches of one replicated launch over T * replicas * B entries
+    (C ABI ``faa_augment_tta_policies``).  ``policies``: what ``compile_policies`` takes.
+
+        out[t] == augment_tta(policies[t], batch_u8, tail, replicas, seed, first_index + t * replicas * B)
+
+    uint8 [B,H,W,3] CUDA batch -> [T, replicas, B, 3, out_h, out_w] (or [T, replicas, B, out_h, out_w, 3] uint8).
+    A ``RaggedImages`` batch (``tail`` must be ``TailSpec.raw_u8()``) gives a ``RaggedImages`` of T * replicas * B
+    images in that entry order, each at its source size (``faa_augment_ragged_policies`` over replicated descriptors).
+    Raises ValueError before any device work for what ``check_tta_policies`` refuses."""
+    pols = compile_policies(policies)
+    B = len(batch_u8) if isinstance(batch_u8, RaggedImages) else int(batch_u8.shape[0])
+    check_tta_policies(pols, B, replicas)
+    T, K = len(pols), int(replicas)
+    handles = (C.c_void_p * T)(*[p.handle.value for p in pols])
+    rng = make_rng(seed, first_index, tail)
+    if isinstance(batch_u8, RaggedImages):
+        raw = TailSpec.raw_u8()
+        if (tail.out_size, tail.crop_pad, tail.hflip, tail.cutout, tail.out_dtype) != \
+                (raw.out_size, raw.crop_pad, raw.hflip, raw.cutout, raw.out_dtype):
+            raise ValueError("a ragged batch is augmented at each image's own size into uint8: the tail must be "
+                             "TailSpec.raw_u8()")
+        src = tta_select(batch_u8, T * K)
+        _require_cuda(src.storage, "batch")
+        if out is None:
+            out = RaggedImages.empty(src.sizes, src.device)
+        elif not isinstance(out, RaggedImages) or not np.array_equal(out.sizes, src.sizes) or out.device != src.device:
+            raise ValueError("out must be a RaggedImages of the replicated batch's sizes on its device")
+        if len(src) == 0:
+            return out
+        cand = np.ascontiguousarray(tta_policy_entries(T, B, K)[0].astype(np.int32))
+        (h_in, d_in), (h_out, d_out) = src.descriptors(), out.descriptors()
+        with torch.cuda.device(src.device):
+            check(lib.faa_augment_ragged_policies(handles, T, h_in.ctypes.data, d_in.data_ptr(), cand.ctypes.data, len(src),
+                                                  h_out.ctypes.data, d_out.data_ptr(), C.byref(rng),
+                                                  _stream_ptr(src.device)))
+        return out
+    _require_cuda(batch_u8, "batch")
+    if batch_u8.dtype != torch.uint8 or batch_u8.dim() != 4 or batch_u8.shape[-1] != 3:
+        raise ValueError("batch must be uint8 [B, H, W, 3]")
+    batch_u8 = batch_u8.contiguous()
+    _, H, W, _ = batch_u8.shape
+    t = tail.c_struct(H, W)
+    shape = (T, K, B, t.out_h, t.out_w, 3) if tail.out_dtype == torch.uint8 else (T, K, B, 3, t.out_h, t.out_w)
+    if out is None:
+        out = torch.empty(shape, dtype=tail.out_dtype, device=batch_u8.device)
+    elif tuple(out.shape) != shape or out.dtype != tail.out_dtype or not out.is_contiguous():
+        raise ValueError("out has the wrong shape/dtype")
+    with torch.cuda.device(batch_u8.device):
+        check(lib.faa_augment_tta_policies(handles, T, batch_u8.data_ptr(), out.data_ptr(), B, K, H, W, C.byref(t),
+                                           C.byref(rng), _stream_ptr(batch_u8.device)))
+    return out
+
+
 def tta_positions(batch, replicas):
     """int64 [replicas * batch]: the batch position each TTA schedule entry v = r * batch + i reads (i)"""
     return np.tile(np.arange(int(batch), dtype=np.int64), int(replicas))

@@ -202,6 +202,18 @@ int faa_augment_many(faa_policy_t* p, int n_steps, const uint8_t* const* d_in, v
 int faa_augment_tta(faa_policy_t* p, const uint8_t* d_in, void* d_out, int batch, int replicas,
                     int h, int w, const faa_tail_t* tail, const faa_rng_t* rng, void* stream);
 
+/* ---- the same for n_policies candidate policies at once (the policy search scores several hyperopt suggestions
+ * against one validation fold): d_out [n_policies][replicas][batch][3][out_h][out_w]; entry
+ * v = (t*replicas + r)*batch + i reads image i and draws the decisions of global sample rng->first_index + v from
+ * candidate t, so block t equals faa_augment_tta(policies[t], ..., first_index + t*replicas*batch).  ONE resolve launch
+ * and the pixel launches of one replicated launch over all entries.  policies[0] runs the call (its scratch, streams
+ * and stream-ordering rules); the others only lend their compiled tables.  Refused before any device work:
+ * FAA_ERR_VALUE for a null or empty list, a null or repeated handle, or candidates whose n_op differ;
+ * FAA_ERR_UNSUPPORTED for n_op > FAA_MAX_FUSED_OPS or n_policies*replicas*batch > 65535.  Candidates may differ in
+ * n_sub.  n_policies == 1 is faa_augment_tta. */
+int faa_augment_tta_policies(faa_policy_t* const* policies, int n_policies, const uint8_t* d_in, void* d_out, int batch,
+                             int replicas, int h, int w, const faa_tail_t* tail, const faa_rng_t* rng, void* stream);
+
 /* same call with HOST buffers: pinned staging, chunked H2D / kernel / D2H pipeline inside.
  * h_out may be NULL (result stays on the device in d_out_keep, which may also be NULL). */
 int faa_augment_host(faa_policy_t* p, const uint8_t* h_in, void* h_out, void* d_out_keep,
@@ -315,6 +327,15 @@ int faa_crop_resize_ragged(const faa_image_t* h_images, const faa_image_t* d_ima
 int faa_augment_ragged(faa_policy_t* p, const faa_image_t* h_in, const faa_image_t* d_in, int batch,
                        const faa_image_t* h_out, const faa_image_t* d_out, const faa_sample_t* d_samples,
                        const faa_box_t* d_boxes, const faa_rng_t* rng, int op_base, void* stream);
+
+/* ---- faa_augment_ragged with Philox draws from one of n_policies candidate policies per image: image i draws the
+ * decisions of global sample rng->first_index + i from policies[h_policy[i]] (host array, each in [0, n_policies)), so
+ * it equals faa_augment_ragged(policies[h_policy[i]], ...) on the same descriptors at that position.  The same launches
+ * as faa_augment_ragged.  The candidate list is refused as in faa_augment_tta_policies; n_policies == 1 is
+ * faa_augment_ragged. */
+int faa_augment_ragged_policies(faa_policy_t* const* policies, int n_policies, const faa_image_t* h_in,
+                                const faa_image_t* d_in, const int32_t* h_policy, int batch, const faa_image_t* h_out,
+                                const faa_image_t* d_out, const faa_rng_t* rng, void* stream);
 
 /* ---- baseline JPEG decode: replaces torchvision's default_loader (imagenet.py:80, `Image.open(f).convert('RGB')`, Pillow
  * on libjpeg-turbo with its default islow IDCT, fancy upsampling and fixed-point YCbCr->RGB) for a batch of files, bit-exact.
