@@ -22,10 +22,13 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import PIL.Image
 import torch
+import torch.distributed as dist
 from torch.utils.data import Sampler, SubsetRandomSampler
+from torch.utils.data.distributed import DistributedSampler
 
 from . import _lib, archive
 from .conf import Config as C
+from .distributed import share_jpeg_index
 from .engine import (CIFAR_MEAN, CIFAR_STD, IMAGENET_MEAN, IMAGENET_STD, CompiledPolicy, EncodedImages, RaggedImages,
                      TailSpec, augment_batch, augment_tta, augment_tta_policies, center_crop_box, check_tta,
                      check_tta_policies, compact_jpeg_index, compile_policies, crop_cfg, crop_resize, decode_jpeg, make_rng,
@@ -668,12 +671,17 @@ class JpegIndex:
     rewritten at the same length) is caught by the decoder, which then decodes that file serially.
 
     ``add`` enters files' points found later (``conf['faa_jpeg_index_learn']``: a loader's recording decodes); they
-    replace the ones listed for the same path.  In memory an index takes about what its file takes on disk: 16 bytes a
-    point, up to 127 points a file (about 1.7 KB at ImageNet's mean file size of about 110 KB)."""
+    replace the ones listed for the same path.  ``delta`` hands out what ``add`` entered since the last ``delta`` and
+    ``merge`` enters another process's delta with the same replace semantics (``distributed.share_jpeg_index``); merged
+    entries are never part of a later delta, so a rank sends only what it learned itself.  In memory an index takes
+    about what its file takes on disk: 16 bytes a point, up to 127 points a file (about 1.7 KB at ImageNet's mean file
+    size of about 110 KB)."""
 
     def __init__(self, folder, paths, sizes, first, points):
         self.folder = os.fspath(folder)
         self._added = {}                           # relative path -> (length, points) entered by add
+        self._merged = {}                          # relative path -> (length, points) entered by merge
+        self._unsent = {}                          # relative paths add entered since the last delta (ordered set)
         self.sizes = np.asarray(sizes, np.int64).reshape(-1)
         self.first = np.asarray(first, np.int64).reshape(-1)
         self.points = np.ascontiguousarray(points, dtype=_lib.JPEG_SYNC_DTYPE).reshape(-1)
@@ -697,11 +705,12 @@ class JpegIndex:
         return JpegIndex(folder, [], np.zeros(0, np.int64), np.zeros(1, np.int64), np.zeros(0, _lib.JPEG_SYNC_DTYPE))
 
     def save(self, path):
-        """write the index, ``add``'s files included, as ``<split>.npz`` of ``python -m fast_autoaugment_b200.jpeg_index``"""
+        """write the index, ``add``'s and ``merge``'s files included, as ``<split>.npz`` of ``python -m
+        fast_autoaugment_b200.jpeg_index``"""
         rel = sorted(self._at, key=self._at.get)
         sizes, first, points = self.sizes, self.first, self.points
-        if self._added:
-            added = dict(self._added)
+        if self._added or self._merged:
+            added = {**self._merged, **self._added}
             rel = [p for p in rel if p not in added]
             at = [self._at[p] for p in rel]
             parts = [self.points[self.first[i]:self.first[i + 1]] for i in at] + [q for _, q in added.values()]
@@ -718,12 +727,53 @@ class JpegIndex:
         1]]`` (``build_jpeg_index``'s form); they replace what the index lists for those paths"""
         for k, p in enumerate(paths):
             q = np.array(points[int(first[k]):int(first[k + 1])], dtype=_lib.JPEG_SYNC_DTYPE)
-            self._added[os.path.relpath(os.fspath(p), self.folder)] = (int(lengths[k]), q)
+            rel = os.path.relpath(os.fspath(p), self.folder)
+            self._added[rel] = (int(lengths[k]), q)
+            self._merged.pop(rel, None)
+            self._unsent[rel] = None
+
+    def delta(self):
+        """``(paths, lengths, first, points)``: the entries ``add`` entered since the last ``delta``, as ``save`` writes
+        them (relative paths as bytes, file lengths, point offsets, points); what ``merge`` takes.  The call starts the
+        next delta."""
+        rel = list(self._unsent)
+        self._unsent = {}
+        parts = [self._added[p][1] for p in rel]
+        first = np.zeros(len(rel) + 1, np.int64)
+        first[1:] = np.cumsum([len(q) for q in parts])
+        return (np.array([os.fsencode(p) for p in rel], dtype=bytes),
+                np.array([self._added[p][0] for p in rel], np.int64), first,
+                np.concatenate(parts) if parts else self.points[:0].copy())
+
+    def merge(self, paths, lengths, first, points):
+        """enter another index's ``delta``: file k (``paths[k]`` relative to the folder, bytes or str) of ``lengths[k]``
+        bytes has points ``points[first[k]:first[k + 1]]``; they replace what the index lists for those paths.  Raises
+        ValueError, entering nothing, for a delta whose parts do not fit together."""
+        n = len(paths)
+        lengths = np.asarray(lengths, np.int64).reshape(-1)
+        first = np.asarray(first, np.int64).reshape(-1)
+        points = np.asarray(points)
+        if points.dtype != _lib.JPEG_SYNC_DTYPE:
+            raise ValueError("JPEG index delta: points must be of JPEG_SYNC_DTYPE")
+        rel = [os.fsdecode(bytes(p)) if isinstance(p, (bytes, np.bytes_)) else os.fspath(p) for p in paths]
+        if len(lengths) != n or len(first) != n + 1 or first[0] != 0 or (np.diff(first) < 0).any() or \
+                first[-1] != points.size or (lengths < 0).any():
+            raise ValueError("JPEG index delta: inconsistent parts")
+        if any(not p or os.path.isabs(p) for p in rel):
+            raise ValueError("JPEG index delta: paths must be relative to the split folder")
+        points = points.reshape(-1).copy()             # one copy; the entries are views of it
+        first, lengths = first.tolist(), lengths.tolist()
+        for k, p in enumerate(rel):
+            self._merged[p] = (lengths[k], points[first[k]:first[k + 1]])
+            self._added.pop(p, None)
+            self._unsent.pop(p, None)
 
     def lookup(self, path, length):
         """the points of the file at ``path`` (of ``length`` bytes), empty when it has none here"""
         rel = os.path.relpath(os.fspath(path), self.folder)
         e = self._added.get(rel)
+        if e is None:
+            e = self._merged.get(rel)
         if e is not None:
             return e[1] if e[0] == int(length) else self.points[:0]
         i = self._at.get(rel)
@@ -1069,7 +1119,10 @@ class GpuAugmentedLoader:
         """``chain``: an ``ImageNetChain`` that transforms the batches instead of the fused policy launch
         (``chain_mode`` 'train' or 'test'); a ``RaggedDeviceDataset``, ``EncodedDeviceDataset`` or ``JpegFileDataset``
         needs one.  A ``JpegFileDataset``'s batches are read from disk one batch ahead (``FileBatchStream``; the stream
-        of the latest epoch is ``staging``)."""
+        of the latest epoch is ``staging``).  When that dataset learns its index and ``sampler`` is a
+        ``DistributedSampler`` under an initialised ``torch.distributed`` of more than one process, ``__iter__``
+        starts every epoch with ``share_jpeg_index`` of the index, a collective, before any file is staged; ``tta``
+        exchanges nothing."""
         if not torch.cuda.is_available():
             raise _lib.FaaRuntimeError("fast_autoaugment_b200 needs a CUDA device (no CPU fallback)")
         self.dataset, self.batch_size, self.tail = dataset, int(batch), tail
@@ -1130,7 +1183,16 @@ class GpuAugmentedLoader:
             if files is not None:
                 files.close()
 
+    def _shares_index(self):
+        """a learning ``JpegFileDataset`` sharded by a ``DistributedSampler`` over more than one process: the ranks
+        exchange what their indexes learned at the start of every epoch"""
+        return isinstance(self.dataset, JpegFileDataset) and self.dataset.learn and \
+            isinstance(self.sampler, DistributedSampler) and dist.is_available() and dist.is_initialized() and \
+            dist.get_world_size() > 1
+
     def __iter__(self):
+        if self._shares_index():                                 # before the staging thread reads the index
+            share_jpeg_index(self.dataset.index)
         with contextlib.closing(self._batches()) as batches:
             for t, raw in batches:
                 if self.chain is None:
@@ -1341,8 +1403,10 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
     same pixels.  ``faa_jpeg_index_learn``: the datasets start from that index, or from an empty one, and the loaders
     enter the scan index of every file they decode serially, so from the second epoch on the files the loaders have
     seen are decoded on many threads, with the same pixels; the train and valid loaders share what they learn
-    (``trainloader.dataset.index.save(path)`` writes it as ``faa_jpeg_index`` reads it).  It costs host memory: 16
-    bytes a point, about 1.7 KB a file at ImageNet's mean file size.  ``faa_jpeg_progressive`` (default False): the
+    (``trainloader.dataset.index.save(path)`` writes it as ``faa_jpeg_index`` reads it).  With ``multinode=True``
+    the train loader's ranks exchange what they learned at the start of every epoch (``share_jpeg_index``), so each
+    rank's index lists what any rank learned.  It costs host memory: 16 bytes a point, about 1.7 KB a file at
+    ImageNet's mean file size.  ``faa_jpeg_progressive`` (default False): the
     train, valid, test and ``tta`` loaders decode progressive JPEG files on the device, bit-exact with Pillow, instead of
     with Pillow on the host; files whose progression is incomplete still go to Pillow.  They get no scan index.
     ``faa_jpeg_index_find`` (default False): the loaders find, on the device and in parallel, the scan index of every

@@ -237,6 +237,115 @@ def mixup_global(policy: CompiledPolicy, local_u8: torch.Tensor, targets: torch.
     return data, targets, (all_targets[tgt_idx_dev] if all_targets.is_cuda else all_targets[perm[lo:lo + b]]), lam
 
 
+JPEG_INDEX_CHUNK = 16 << 20                    # bytes of each rank's delta per all-gather round of share_jpeg_index
+
+
+def _pack_delta(paths, lengths, first, points):
+    """a ``JpegIndex.delta`` as one uint8 array: int64 [files, path bytes, points], the file lengths, the path lengths
+    and the point offsets (int64 each), the points (16 bytes each), then the paths back to back.  A delta of no file
+    packs to no bytes."""
+    if not len(paths):
+        return np.zeros(0, np.uint8)
+    plen = np.array([len(p) for p in paths], np.int64)
+    head = np.array([len(paths), int(plen.sum()), len(points)], np.int64)
+    return np.concatenate([head.view(np.uint8), np.ascontiguousarray(lengths, np.int64).view(np.uint8),
+                           plen.view(np.uint8), np.ascontiguousarray(first, np.int64).view(np.uint8),
+                           np.ascontiguousarray(points).view(np.uint8).reshape(-1),
+                           np.frombuffer(b"".join(bytes(p) for p in paths), np.uint8)])
+
+
+def _unpack_delta(buf):
+    """``_pack_delta``'s ``(paths, lengths, first, points)`` of ``buf``; ValueError when its sizes do not add up"""
+    if buf.size < 24:
+        raise ValueError("%d bytes, shorter than its header" % buf.size)
+    n, nb, npt = (int(v) for v in np.frombuffer(buf, np.int64, 3))
+    if min(n, nb, npt) < 0 or buf.size != 24 + 8 * (3 * n + 1) + _lib.JPEG_SYNC_DTYPE.itemsize * npt + nb:
+        raise ValueError("%d bytes do not hold %d files, %d path bytes and %d points" % (buf.size, n, nb, npt))
+    ints = np.frombuffer(buf, np.int64, 3 * n + 1, 24)
+    lengths, plen, first = ints[:n], ints[n:2 * n], ints[2 * n:]
+    at = 24 + 8 * (3 * n + 1)
+    points = np.frombuffer(buf, _lib.JPEG_SYNC_DTYPE, npt, at)
+    names = buf[at + points.nbytes:].tobytes()
+    if (plen < 0).any() or int(plen.sum()) != nb:
+        raise ValueError("path lengths do not add up to %d bytes" % nb)
+    ends = np.cumsum(plen).tolist()
+    return [names[e - k:e] for e, k in zip(ends, plen.tolist())], lengths, first, points
+
+
+def _fail_everywhere(err, group):
+    """called on every rank at once when the flags of a collective step showed a failure: raise on every rank, naming
+    each rank's error"""
+    msgs = [None] * dist.get_world_size(group)
+    dist.all_gather_object(msgs, None if err is None else "%s: %s" % (type(err).__name__, err), group=group)
+    raise RuntimeError("JPEG index exchange failed: " + "; ".join(
+        "rank %d: %s" % (r, m) for r, m in enumerate(msgs) if m is not None)) from err
+
+
+def share_jpeg_index(index, group=None, chunk_bytes=JPEG_INDEX_CHUNK):
+    """Collective: every rank of ``group`` sends the entries its ``JpegIndex`` learned since the last exchange
+    (``index.delta()``) to every other rank, and enters the other ranks' deltas in rank order (``index.merge``), so
+    every rank's index ends up listing what any rank learned.  Returns the number of entries merged here.
+
+    One all-gather of the packed deltas' sizes, then, when any is not empty, rounds of all-gathers of at most
+    ``chunk_bytes`` of every rank's delta (so no rank ever holds world x its delta in flight), then one all-gather of
+    success flags.  Device tensors on the current device with NCCL, host tensors otherwise.  Every rank enters the
+    same collectives whatever fails locally: a delta that cannot be packed, one that does not unpack or merge (the
+    same verdict on every rank that reads it) or any other local error raises RuntimeError on every rank, naming each
+    rank's error, instead of leaving the others waiting.  Entries merged before a failure stay (a point only decides
+    how a file's decode is split, never its pixels)."""
+    rank, world = dist.get_rank(group), dist.get_world_size(group)
+    dev = torch.device("cuda", torch.cuda.current_device()) if dist.get_backend(group) == "nccl" else torch.device("cpu")
+    err = mine = None
+    try:
+        mine = _pack_delta(*index.delta())
+    except Exception as e:                                       # noqa: BLE001
+        err = e
+    sizes = gather_pool(torch.tensor([-1 if mine is None else mine.size], dtype=torch.int64, device=dev), group)
+    sizes = sizes.cpu().tolist()
+    if min(sizes) < 0:
+        _fail_everywhere(err, group)
+    top = max(sizes)
+    if top == 0:
+        return 0
+    step = max(1, min(int(chunk_bytes), top))
+    bufs = None
+    try:
+        bufs = [mine if r == rank else np.empty(sizes[r], np.uint8) for r in range(world)]
+    except Exception as e:                                       # noqa: BLE001
+        err = e
+    for at in range(0, top, step):
+        m = min(step, top - at)
+        send = torch.zeros(m, dtype=torch.uint8)
+        send[:max(0, min(m, sizes[rank] - at))] = torch.from_numpy(mine[at:at + m])
+        got = gather_pool(send.to(dev), group).cpu().numpy()
+        if err is None:
+            try:
+                for r in range(world):
+                    k = min(m, sizes[r] - at)
+                    if r != rank and k > 0:
+                        bufs[r][at:at + k] = got[r * m:r * m + k]
+            except Exception as e:                               # noqa: BLE001
+                err = e
+    merged = 0
+    if err is None:
+        try:
+            for r in range(world):
+                if r == rank or sizes[r] == 0:
+                    continue
+                try:
+                    delta = _unpack_delta(bufs[r])
+                    index.merge(*delta)
+                except ValueError as e:
+                    raise ValueError("rank %d's JPEG index delta is malformed: %s" % (r, e)) from e
+                merged += len(delta[0])
+        except Exception as e:                                   # noqa: BLE001
+            err = e
+    oks = gather_pool(torch.tensor([int(err is None)], dtype=torch.int64, device=dev), group)
+    if not bool(oks.all()):
+        _fail_everywhere(err, group)
+    return merged
+
+
 class _RawCuda:
     """zero-copy torch view of a raw device allocation (``__cuda_array_interface__``)"""
     def __init__(self, ptr, shape):
