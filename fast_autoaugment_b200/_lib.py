@@ -40,6 +40,7 @@ JPEG_SCAN_DTYPE = np.dtype([("off", "<i8"), ("len", "<i8"), ("restart", "<i4"), 
                             ("dc_at", "<i4", (3,)), ("ac_at", "<i4", (3,)), ("pool", "<i4", (6,)),
                             ("reserved", "<i4", (2,))])                                            # faa_jpeg_scan_t
 JPEG_PROGRESSIVE, JPEG_SCAN_INDEXED, JPEG_MAX_SCANS = 1, 2, 64
+COPY_DTYPE = np.dtype([("src", "<u8"), ("dst", "<u8"), ("bytes", "<u8")])                          # faa_copy_t
 assert SAMPLE_DTYPE.itemsize == 16 and BOX_DTYPE.itemsize == 8 and IMAGE_DTYPE.itemsize == 16
 assert JPEG_HEADER_DTYPE.itemsize == 144 and JPEG_TABLE_DTYPE.itemsize == 400 and JPEG_SYNC_DTYPE.itemsize == 16
 assert JPEG_SCAN_DTYPE.itemsize == 112
@@ -104,6 +105,7 @@ def _load():
         "faa_peer_open": (C.c_int, [vp, P(C.c_void_p)]),
         "faa_peer_close": (C.c_int, [vp]),
         "faa_peer_free": (C.c_int, [vp]),
+        "faa_gather": (C.c_int, [vp, vp, C.c_int, vp]),
         "faa_mix_u8_peer": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, P(Tail), f32, f32, vp]),
         "faa_color_jitter": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp]),
         "faa_policy_set_lighting": (C.c_int, [vp, vp, C.c_int]),

@@ -1546,6 +1546,27 @@ int faa_peer_open(const unsigned char* handle64, void** d_ptr) {
 int faa_peer_close(void* d_ptr) { if (d_ptr) CK(cudaIpcCloseMemHandle(d_ptr)); return FAA_OK; }
 int faa_peer_free(void* d_ptr) { if (d_ptr) CK(cudaFree(d_ptr)); return FAA_OK; }
 
+static_assert(sizeof(faa_copy_t) == sizeof(RaggedCopy) && sizeof(faa_copy_t) == 24, "copy job layout");
+
+int faa_gather(const faa_copy_t* h_jobs, const faa_copy_t* d_jobs, int n, void* stream) {
+    if (!h_jobs || !d_jobs) return fail(FAA_ERR_VALUE, "null argument");
+    if (n <= 0) return fail(FAA_ERR_VALUE, "faa_gather needs at least one job");
+    uint64_t pieces = 0;
+    for (int i = 0; i < n; ++i) {
+        if (!h_jobs[i].src || !h_jobs[i].dst) return fail(FAA_ERR_VALUE, "job " + std::to_string(i) + ": null src or dst");
+        pieces += (h_jobs[i].bytes + kGatherUnit - 1) / kGatherUnit;
+    }
+    if (int e = ensure_device()) return e;
+    if (pieces == 0) return FAA_OK;
+    int dev = 0, sms = 0;
+    CK(cudaGetDevice(&dev));
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    const uint64_t ctas = std::min<uint64_t>(pieces, (uint64_t)sms * 8);    // 8 CTAs of 256 threads fill an SM
+    CK(launch_gather(reinterpret_cast<const RaggedCopy*>(d_jobs), n, (int)ctas, (cudaStream_t)stream));
+    g_launches++;
+    return FAA_OK;
+}
+
 int faa_mix_u8_peer(faa_policy_t* p, const uint8_t* d_a, const uint8_t* const* d_partner_ptrs, const int16_t* d_zero_box_a,
                     const int16_t* d_zero_box_b, void* d_out, int batch, int h, int w, const faa_tail_t* tail, float lam,
                     float one_minus_lam, void* stream) {

@@ -217,6 +217,83 @@ __global__ void __launch_bounds__(256) faa_realign_kernel(const RaggedCopy* jobs
     }
 }
 
+// faa_gather: every job is cut into kGatherUnit-byte pieces and piece u of the whole list (jobs in order) is copied by
+// CTA u % gridDim.x, so a multi-MB job is spread over the SMs and a list of 400-byte jobs over the CTAs.  The list is
+// read in tiles of kGatherTile jobs: the CTA scans the tile's piece counts into shared memory and finds its pieces'
+// jobs by binary search.  Within a piece, src and dst that agree modulo 16 (modulo 4) move 16-byte (4-byte) words after
+// a byte head; anything else moves bytes.  No byte outside [dst, dst + bytes) is written.
+constexpr int kGatherTile = 1024;
+
+__device__ __forceinline__ void gather_piece(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, uint64_t n) {
+    const int t = threadIdx.x;
+    const uintptr_t rel = ((uintptr_t)src ^ (uintptr_t)dst);
+    const int vec = (rel & 15) == 0 ? 16 : (rel & 3) == 0 ? 4 : 1;
+    uint64_t head = vec == 1 ? 0 : ((uint64_t)vec - ((uintptr_t)dst & (vec - 1))) & (vec - 1);
+    if (head > n) head = n;
+    const uint64_t body = (n - head) / vec;
+    if ((uint64_t)t < head) dst[t] = src[t];
+    if (vec == 16) {
+        const uint4* s = reinterpret_cast<const uint4*>(src + head);
+        uint4* d = reinterpret_cast<uint4*>(dst + head);
+        for (uint64_t k = t; k < body; k += kGatherThreads) d[k] = s[k];
+    } else if (vec == 4) {
+        const uint32_t* s = reinterpret_cast<const uint32_t*>(src + head);
+        uint32_t* d = reinterpret_cast<uint32_t*>(dst + head);
+        for (uint64_t k = t; k < body; k += kGatherThreads) d[k] = s[k];
+    } else {
+        for (uint64_t k = t; k < n; k += kGatherThreads) dst[k] = src[k];
+        return;
+    }
+    for (uint64_t k = head + body * vec + t; k < n; k += kGatherThreads) dst[k] = src[k];
+}
+
+__global__ void __launch_bounds__(kGatherThreads) faa_gather_kernel(const RaggedCopy* __restrict__ jobs, int n) {
+    __shared__ uint64_t s_end[kGatherTile];          // inclusive prefix of the tile's piece counts
+    __shared__ uint64_t s_warp[kGatherThreads / 32];
+    constexpr int kPer = kGatherTile / kGatherThreads;
+    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    uint64_t before = 0;                             // pieces of the tiles before this one
+    for (int base = 0; base < n; base += kGatherTile) {
+        uint64_t c[kPer], sum = 0;
+#pragma unroll
+        for (int q = 0; q < kPer; ++q) {
+            const int j = base + t * kPer + q;
+            c[q] = j < n ? (jobs[j].bytes + kGatherUnit - 1) / kGatherUnit : 0;
+            sum += c[q];
+        }
+        uint64_t x = sum;                            // inclusive scan of the threads' sums
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint64_t y = __shfl_up_sync(0xffffffffu, x, o);
+            if (lane >= o) x += y;
+        }
+        if (lane == 31) s_warp[warp] = x;
+        __syncthreads();
+        uint64_t off = 0;
+        for (int w = 0; w < warp; ++w) off += s_warp[w];
+        uint64_t run = off + x - sum;
+#pragma unroll
+        for (int q = 0; q < kPer; ++q) { run += c[q]; s_end[t * kPer + q] = run; }
+        __syncthreads();
+        const uint64_t total = s_end[kGatherTile - 1];
+        const int m = min(kGatherTile, n - base);
+        // the first piece of this tile that is this CTA's: global piece (before + u) % gridDim.x == blockIdx.x
+        uint64_t u = ((uint64_t)blockIdx.x + gridDim.x - before % gridDim.x) % gridDim.x;
+        for (; u < total; u += gridDim.x) {
+            int lo = 0, hi = m - 1;                  // the job whose pieces hold u: first with s_end > u
+            while (lo < hi) {
+                const int mid = (lo + hi) >> 1;
+                if (s_end[mid] > u) hi = mid; else lo = mid + 1;
+            }
+            const RaggedCopy j = jobs[base + lo];
+            const uint64_t at = (u - (s_end[lo] - (j.bytes + kGatherUnit - 1) / kGatherUnit)) * kGatherUnit;
+            gather_piece(j.src + at, j.dst + at, min(kGatherUnit, j.bytes - at));
+        }
+        before += total;
+        __syncthreads();                             // s_end and s_warp are rewritten by the next tile
+    }
+}
+
 #endif  // !FAA_TU_OUT
 
 // ---------------------------------------------------------------------------------------
@@ -2549,6 +2626,12 @@ cudaError_t launch_resolve_ragged(const ResolveParams& p, const RaggedImg* imgs,
 cudaError_t launch_realign(const RaggedCopy* jobs, int n, cudaStream_t stream) {
     if (n <= 0) return cudaSuccess;
     faa_realign_kernel<<<dim3(64, (unsigned)n, 1), 256, 0, stream>>>(jobs);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_gather(const RaggedCopy* jobs, int n, int ctas, cudaStream_t stream) {
+    if (n <= 0 || ctas <= 0) return cudaSuccess;
+    faa_gather_kernel<<<ctas, kGatherThreads, 0, stream>>>(jobs, n);
     return cudaGetLastError();
 }
 

@@ -124,6 +124,10 @@ cudaError_t launch_augment_ragged(const RaggedParams& r, int bands, int count, s
 // copies n images to 4-byte aligned buffers: src[k] -> dst[k], bytes[k] (device arrays) in one launch
 struct RaggedCopy { const uint8_t* src; uint8_t* dst; uint64_t bytes; };
 cudaError_t launch_realign(const RaggedCopy* jobs, int n, cudaStream_t stream);
+// faa_gather: n jobs (device array, faa_copy_t's layout) of `units` kGatherUnit-byte pieces in all, over `ctas` CTAs
+constexpr int kGatherThreads = 256;
+constexpr uint64_t kGatherUnit = 16384;      // bytes of one piece: four 16-byte stores per thread
+cudaError_t launch_gather(const RaggedCopy* jobs, int n, int ctas, cudaStream_t stream);
 
 cudaError_t launch_mixup(const void* data, void* out, const int64_t* perm, int batch, int64_t n_per_sample,
                          int dtype, float lam, float one_minus_lam, cudaStream_t stream);

@@ -8,15 +8,18 @@
   the augmented, normalised CUDA tensor, so the caller's ``.cuda()`` (``train.py:49``) is a
   no-op.  The raw uint8 dataset lives on the device; no CUDA is touched in worker processes
   because there are none.  The one exception is the ImageNet directory (``JpegFileDataset``): its files stay on disk
-  and are read, staged and decoded batch by batch, one batch ahead (``FileBatchStream``).
+  and are read, staged and decoded batch by batch, one batch ahead (``FileBatchStream``), unless they are held in
+  device memory (``ResidentJpegDataset``) and gathered per batch on the device.
 """
 from __future__ import annotations
 
 import contextlib
+import ctypes
 import io
 import math
 import os
 import random
+import time
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
@@ -28,11 +31,13 @@ from torch.utils.data.distributed import DistributedSampler
 
 from . import _lib, archive
 from .conf import Config as C
-from .distributed import share_jpeg_index
+from .distributed import _RawCuda, agree, check_fit, fit_error, gather_bytes, host_ranks, share_jpeg_index
 from .engine import (CIFAR_MEAN, CIFAR_STD, IMAGENET_MEAN, IMAGENET_STD, CompiledPolicy, EncodedImages, RaggedImages,
-                     TailSpec, augment_batch, augment_tta, augment_tta_policies, center_crop_box, check_tta,
-                     check_tta_policies, compact_jpeg_index, compile_policies, crop_cfg, crop_resize, decode_jpeg, make_rng,
-                     parse_jpeg_headers, sample_philox_at, tta_positions, tta_select)
+                     TailSpec, augment_batch, augment_tta, augment_tta_policies, build_jpeg_index, center_crop_box,
+                     check_tta, check_tta_policies, compact_jpeg_index, compile_policies, crop_cfg, crop_resize,
+                     decode_jpeg, gather, jpeg_index_capacities, make_rng, parse_jpeg_headers, sample_philox_at,
+                     tta_positions, tta_select)
+from .engine import _gather_ranges as engine_gather_ranges
 
 
 class Augmentation(object):
@@ -1048,32 +1053,14 @@ class FileBatchStream:
                 learned = (h_count, h_points, cap_first, [len(f) for f in hb.files])
             else:
                 _, status = decode_jpeg(enc, out.select(hb.accepted), **find)
-            st = torch.empty(len(hb.accepted), dtype=torch.int32, pin_memory=True)
-            st.copy_(status, non_blocking=True)
-            ev = torch.cuda.Event()
-            ev.record(torch.cuda.current_stream(dev))
-            pending.append((ev, st, [hb.paths[i] for i in hb.accepted], learned))
+            queue_status(status, [hb.paths[i] for i in hb.accepted], dev, pending, learned)
         for i, o in zip(hb.refused, lay.pixels):
             h, w = (int(v) for v in sizes[i])
             out.image(int(i)).copy_(dbuf[o:o + h * w * 3].view(h, w, 3))
         return out
 
     def _check(self, pending, keep=0):
-        """check (and drop) every pending status but the last ``keep``; enter what recording decodes found"""
-        while len(pending) > keep:
-            ev, st, paths, learned = pending.pop(0)
-            ev.synchronize()
-            if learned is not None:
-                h_count, h_points, cap_first, lengths = learned
-                count = h_count.numpy()
-                first, points = compact_jpeg_index(cap_first, count, h_points.numpy())
-                got = np.flatnonzero(count > 0)
-                self.index.add([paths[i] for i in got], [lengths[i] for i in got],
-                               np.concatenate([[0], np.cumsum(count[got])]), points)
-            bad = [(p, int(s)) for p, s in zip(paths, st.numpy().tolist()) if s]
-            if bad:
-                raise OSError("corrupt JPEG files (decode status): " + "; ".join(
-                    "%s: 0x%x (%s)" % (p, s, ", ".join(n for b, n in _STATUS_BITS if s & b)) for p, s in bad))
+        check_decodes(pending, keep, self.index)
 
     def __call__(self, batches, device):
         """generator of one ``RaggedImages`` per batch of paths in ``batches``"""
@@ -1101,6 +1088,518 @@ class FileBatchStream:
             pool.shutdown(wait=True, cancel_futures=True)
 
 
+def queue_status(status, paths, dev, pending, learned=None):
+    """copy a decode's status (and what a recording decode recorded, ``learned``) to pinned memory behind the decode and
+    append it to ``pending`` for ``check_decodes``, so no batch waits on its own decode"""
+    st = torch.empty(len(paths), dtype=torch.int32, pin_memory=True)
+    st.copy_(status, non_blocking=True)
+    ev = torch.cuda.Event()
+    ev.record(torch.cuda.current_stream(dev))
+    pending.append((ev, st, paths, learned))
+
+
+def check_decodes(pending, keep=0, index=None):
+    """check (and drop) every pending status but the last ``keep``: OSError naming every file whose status is not 0;
+    enter into ``index`` what recording decodes found"""
+    while len(pending) > keep:
+        ev, st, paths, learned = pending.pop(0)
+        ev.synchronize()
+        if learned is not None:
+            h_count, h_points, cap_first, lengths = learned
+            count = h_count.numpy()
+            first, points = compact_jpeg_index(cap_first, count, h_points.numpy())
+            got = np.flatnonzero(count > 0)
+            index.add([paths[i] for i in got], [lengths[i] for i in got],
+                      np.concatenate([[0], np.cumsum(count[got])]), points)
+        codes = st.numpy()
+        bad = [(paths[i], int(codes[i])) for i in np.flatnonzero(codes)]
+        if bad:
+            raise OSError("corrupt JPEG files (decode status): " + "; ".join(
+                "%s: 0x%x (%s)" % (p, s, ", ".join(n for b, n in _STATUS_BITS if s & b)) for p, s in bad))
+
+
+RESIDENT_CHUNK = 256                   # files per read_jpeg_batch call while a resident store is built
+RESIDENT_INDEX_CHUNK = 1024            # files per build_jpeg_index call over a shard
+RESIDENT_STAGE = 64 << 20              # bytes of host staging per upload of a shard's parts
+# host metadata of one file of a resident store: its header (``offset``: its bytes in the owner's shard; ``pool``: rows
+# of the owner's table region), its tables (``n_tables`` rows from row ``table_at``), its points (``n_points`` from
+# byte ``points_at`` of the shard), a refused file's pixels (``refused``, h x w x 3 bytes from byte ``pixels_at``) and
+# the number of its progressive scans
+RESIDENT_META_DTYPE = np.dtype([("hdr", _lib.JPEG_HEADER_DTYPE), ("table_at", "<i8"), ("n_tables", "<i8"),
+                                ("points_at", "<i8"), ("n_points", "<i8"), ("pixels_at", "<i8"), ("h", "<i4"),
+                                ("w", "<i4"), ("refused", "<i4"), ("n_scans", "<i4")])
+_TABLE_BYTES = _lib.JPEG_TABLE_DTYPE.itemsize
+
+
+def resident_owned(n, local_rank, n_local):
+    """the files of an n-file split that local rank ``local_rank`` of ``n_local`` ranks on its host holds: file i
+    belongs to local rank i mod n_local"""
+    return np.arange(int(local_rank), int(n), int(n_local), dtype=np.int64)
+
+
+def _used_slots(hdr, sc):
+    """(header slots, [(scan, slot)]) of a parsed file that name a table: a baseline file's slots s with s % 3 <
+    ncomp; a progressive file's first ncomp header slots and its scans' slots whose DC or AC table exists"""
+    nc = int(hdr["ncomp"])
+    if not int(hdr["reserved"]) & _lib.JPEG_PROGRESSIVE:
+        return [s for s in range(9) if s % 3 < nc], []
+    return list(range(nc)), [(k, t) for k in range(len(sc)) for t in range(6)
+                             if (sc["dc_at"][k] if t < 3 else sc["ac_at"][k])[t % 3] != -1]
+
+
+class ShardPlan:
+    """The host half of one rank's shard of a resident store, from its files' ``read_jpeg_batch`` results (``hbs``, in
+    ownership order): ``meta`` (``RESIDENT_META_DTYPE`` [n]), ``scans`` (the progressive files' scans, file order, pool
+    slots in shard rows), ``tables`` (``JPEG_TABLE_DTYPE``: each accepted file's own tables, in file order) and the
+    byte layout of the shard: the accepted files' bytes from byte 0, the tables from ``tables_off``, room for the points
+    from ``points_off``, the refused files' pixels from ``pixels_off``, each item on a 16-byte boundary; ``need`` bytes.
+
+    ``index``: a ``JpegIndex`` whose points the files take (``points``), exactly sized; without one each accepted file
+    gets room for the most points it can get (``jpeg_index_capacities``) and ``n_points`` 0 until ``build_points``."""
+
+    def __init__(self, hbs, index=None):
+        metas, scans, tables, points = [], [], [], []
+        self.files, self.pixels = [], []
+        n_tab = 0
+        for hb in hbs:
+            m = np.zeros(len(hb.paths), RESIDENT_META_DTYPE)
+            m["refused"][hb.refused] = 1
+            for i, px in zip(hb.refused, hb.pixels):
+                m["h"][i], m["w"][i] = px.shape[:2]
+            for a, i in enumerate(hb.accepted):
+                hdr = hb.headers[a].copy()
+                sc = hb.scans[hb.scan_first[a]:hb.scan_first[a + 1]].copy() if hb.scans is not None else hb.scans
+                used_h, used_s = _used_slots(hdr, sc)
+                uniq = sorted({int(hdr["pool"][s]) for s in used_h} | {int(sc["pool"][k, t]) for k, t in used_s})
+                row = {s: n_tab + j for j, s in enumerate(uniq)}
+                pool = np.full(9, n_tab, np.int32)            # slots that name no table point at the file's first row
+                pool[used_h] = [row[int(hdr["pool"][s])] for s in used_h]
+                hdr["pool"] = pool
+                if sc is not None and len(sc):
+                    sp = np.full((len(sc), 6), n_tab, np.int32)
+                    for k, t in used_s:
+                        sp[k, t] = row[int(sc["pool"][k, t])]
+                    sc["pool"] = sp
+                    scans.append(sc)
+                    m["n_scans"][i] = len(sc)
+                tables.append(hb.pool[uniq])
+                m["hdr"][i] = hdr
+                m["table_at"][i], m["n_tables"][i] = n_tab, len(uniq)
+                m["h"][i], m["w"][i] = hdr["h"], hdr["w"]
+                n_tab += len(uniq)
+            if index is not None:
+                first, pts = index.gather([hb.paths[i] for i in hb.accepted], [len(f) for f in hb.files])
+                m["n_points"][hb.accepted] = np.diff(first)
+                points.append(pts)
+            metas.append(m)
+            self.files += hb.files
+            self.pixels += hb.pixels
+        self.meta = np.concatenate(metas) if metas else np.zeros(0, RESIDENT_META_DTYPE)
+        self.scans = np.concatenate(scans) if scans else np.zeros(0, _lib.JPEG_SCAN_DTYPE)
+        self.tables = np.concatenate(tables) if tables else np.zeros(0, _lib.JPEG_TABLE_DTYPE)
+        self.points = np.concatenate(points) if points else np.zeros(0, _lib.JPEG_SYNC_DTYPE)
+        m = self.meta
+        acc = np.flatnonzero(m["refused"] == 0)
+        self.accepted = acc
+        slot = (m["hdr"]["len"][acc] + 15) // 16 * 16
+        m["hdr"]["offset"][acc] = np.cumsum(slot) - slot
+        self.tables_off = int(slot.sum())
+        self.points_off = self.tables_off + len(self.tables) * _TABLE_BYTES
+        room = m["n_points"][acc] if index is not None else np.diff(jpeg_index_capacities(m["hdr"][acc]))
+        m["points_at"][acc] = self.points_off + 16 * (np.cumsum(room) - room)
+        self.pixels_off = self.points_off + 16 * int(room.sum())
+        ref = np.flatnonzero(m["refused"] != 0)
+        px = (m["h"][ref].astype(np.int64) * m["w"][ref] * 3 + 15) // 16 * 16
+        m["pixels_at"][ref] = self.pixels_off + np.cumsum(px) - px
+        self.need = max(16, self.pixels_off + int(px.sum()))
+
+    def headers(self):
+        """the accepted files' headers, ``offset`` and ``pool`` in the shard (file order)"""
+        return self.meta["hdr"][self.accepted]
+
+    def scan_first(self):
+        n = self.meta["n_scans"][self.accepted].astype(np.int64)
+        return np.concatenate([[0], np.cumsum(n)]).astype(np.int64)
+
+    def parts(self):
+        """[(shard byte offset, uint8 array)] of everything but room for points not yet built, in offset order"""
+        m = self.meta
+        out = [(int(o), np.frombuffer(f, np.uint8)) for o, f in zip(m["hdr"]["offset"][self.accepted], self.files)]
+        out.append((self.tables_off, self.tables.view(np.uint8).reshape(-1)))
+        if len(self.points):
+            at = np.repeat(m["points_at"][self.accepted], m["n_points"][self.accepted])
+            first = np.cumsum(m["n_points"][self.accepted]) - m["n_points"][self.accepted]
+            rows = np.zeros(self.pixels_off - self.points_off, np.uint8).view(_lib.JPEG_SYNC_DTYPE)
+            k = np.arange(len(self.points)) - np.repeat(first, m["n_points"][self.accepted])
+            rows[(at - self.points_off) // 16 + k] = self.points
+            out.append((self.points_off, rows.view(np.uint8)))
+        ref = np.flatnonzero(m["refused"] != 0)
+        out += [(int(o), p.reshape(-1)) for o, p in zip(m["pixels_at"][ref], self.pixels)]
+        return out
+
+
+def _upload(dst, parts):
+    """copy ``parts`` ([(byte offset, uint8 array)] in offset order) into the device tensor ``dst`` through host
+    staging spans of at most ``RESIDENT_STAGE`` bytes (larger parts go alone)"""
+    k = 0
+    while k < len(parts):
+        start, j = parts[k][0], k
+        while j < len(parts) and parts[j][0] + len(parts[j][1]) - start <= max(RESIDENT_STAGE, len(parts[k][1])):
+            j += 1
+        end = parts[j - 1][0] + len(parts[j - 1][1])
+        buf = np.zeros(end - start, np.uint8)
+        for o, a in parts[k:j]:
+            buf[o - start:o - start + len(a)] = a
+        dst[start:end].copy_(torch.from_numpy(buf))
+        k = j
+
+
+def pack_shard_meta(meta, scans, handle, device, tables_off):
+    """one rank's part of a resident store's metadata exchange: int64 [files, scans, device, table region offset], the
+    64-byte IPC handle, the files' ``RESIDENT_META_DTYPE`` rows, their scans"""
+    head = np.array([len(meta), len(scans), int(device), int(tables_off)], np.int64)
+    return np.concatenate([head.view(np.uint8), np.frombuffer(bytes(handle), np.uint8),
+                           np.ascontiguousarray(meta).view(np.uint8).reshape(-1),
+                           np.ascontiguousarray(scans).view(np.uint8).reshape(-1)])
+
+
+def unpack_shard_meta(buf):
+    """``pack_shard_meta``'s (meta, scans, handle, device, tables_off) of ``buf``; ValueError when its sizes do not
+    add up"""
+    if buf.size < 96:
+        raise ValueError("%d bytes, shorter than a shard's metadata header" % buf.size)
+    n, ns, device, tables_off = (int(v) for v in np.frombuffer(buf, np.int64, 4))
+    if min(n, ns) < 0 or buf.size != 96 + n * RESIDENT_META_DTYPE.itemsize + ns * _lib.JPEG_SCAN_DTYPE.itemsize:
+        raise ValueError("%d bytes do not hold %d files' metadata and %d scans" % (buf.size, n, ns))
+    meta = np.frombuffer(buf, RESIDENT_META_DTYPE, n, 96)
+    scans = np.frombuffer(buf, _lib.JPEG_SCAN_DTYPE, ns, 96 + meta.nbytes)
+    if int(meta["n_scans"].sum()) != ns:
+        raise ValueError("scan counts do not add up to %d scans" % ns)
+    return meta, scans, buf[32:96].tobytes(), device, tables_off
+
+
+class ResidentBatch:
+    """The host plan of one batch of a resident store (``ResidentJpegStore.plan``): the output sizes (``sizes``), the
+    batch positions of the accepted and refused files, the accepted files' headers (``offset`` in the batch's file
+    region, ``pool`` in its table region), scan index (``first``; None when no file has points) and scans (``scans``,
+    ``scan_first``; None when no file is progressive), the batch buffer's layout (tables from 0, files from
+    ``files_at``, points from ``points_at``, ``total`` bytes) and the copies that fill it, ``jobs``."""
+
+    def __init__(self, meta, src, scan_first, scans, sel):
+        sel = np.asarray(sel, np.int64).reshape(-1)
+        m = meta[sel]
+        self.sizes = np.stack([m["h"], m["w"]], axis=1).astype(np.int32).reshape(-1, 2)
+        self.accepted = np.flatnonzero(m["refused"] == 0)
+        self.refused = np.flatnonzero(m["refused"] != 0)
+        a = m[self.accepted]
+        s_a, s_r = src[sel[self.accepted]], src[sel[self.refused]]
+        n_tab = a["n_tables"]
+        row0 = np.cumsum(n_tab) - n_tab
+        self.n_tables = int(n_tab.sum())
+        flen = a["hdr"]["len"]
+        slot = (flen + 15) // 16 * 16
+        self.files_at = self.n_tables * _TABLE_BYTES
+        self.points_at = self.files_at + int(slot.sum())
+        n_pts = a["n_points"]
+        self.total = max(16, self.points_at + 16 * int(n_pts.sum()))
+        self.headers = a["hdr"].copy()
+        self.headers["offset"] = np.cumsum(slot) - slot
+        self.headers["pool"] += (row0 - a["table_at"]).astype(np.int32)[:, None]
+        self.first = None
+        if n_pts.any():
+            self.first = np.concatenate([[0], np.cumsum(n_pts)]).astype(np.int64)
+        self.scans = self.scan_first = None
+        n_sc = a["n_scans"].astype(np.int64)
+        if n_sc.any():
+            self.scan_first, self.scans = engine_gather_ranges(scan_first, scans, sel[self.accepted])
+            self.scans["pool"] += np.repeat((row0 - a["table_at"]).astype(np.int32), n_sc)[:, None]
+        tab_dst = _TABLE_BYTES * row0
+        self._rel = (np.concatenate([s_a["tables"], s_a["file"], s_a["points"]]),
+                     np.concatenate([tab_dst, self.files_at + self.headers["offset"],
+                                     self.points_at + 16 * (np.cumsum(n_pts) - n_pts)]).astype(np.uint64),
+                     np.concatenate([_TABLE_BYTES * n_tab, flen, 16 * n_pts]))
+        self._pixels = (s_r["pixels"], m["h"][self.refused].astype(np.int64) * m["w"][self.refused] * 3)
+
+    def jobs(self, buf_ptr, image_ptrs):
+        """``COPY_DTYPE`` jobs of the batch: the accepted files' tables, bytes and points into the batch buffer at
+        ``buf_ptr``, each refused file's pixels into its output image (``image_ptrs``: the refused files' image
+        addresses, batch order).  Jobs of no byte are left out."""
+        src, dst, n = self._rel
+        out = np.zeros(len(src) + len(self._pixels[0]), _lib.COPY_DTYPE)
+        out["src"] = np.concatenate([src, self._pixels[0]])
+        out["dst"] = np.concatenate([dst + np.uint64(buf_ptr), np.asarray(image_ptrs, np.uint64).reshape(-1)])
+        out["bytes"] = np.concatenate([n, self._pixels[1]])
+        return out[out["bytes"] > 0]
+
+
+_SRC_DTYPE = np.dtype([("file", "<u8"), ("tables", "<u8"), ("points", "<u8"), ("pixels", "<u8")])
+
+
+class ResidentJpegStore:
+    """A split's JPEG files held in device memory, sharded over the ranks of each host (``ResidentJpegDataset``).
+
+    Construction is collective under ``multinode`` (every rank of the default group, or ``group``, calls it): the
+    ranks on one host (``host_ranks``) split the files by ``resident_owned``; each reads and parses only its own
+    (``read_jpeg_batch``, Pillow decoding the files the device decoder refuses), plans its shard (``ShardPlan``),
+    checks it fits (``check_fit``), allocates it as one buffer the host's other processes can map (``faa_peer_alloc``),
+    uploads it and, without ``index``, builds its files' scan indexes on its device (``build_jpeg_index``).  The ranks
+    then all-gather their files' metadata (``gather_bytes``) and each maps its host peers' shards (``faa_peer_open``).
+    Every rank enters the same collectives whatever fails locally, and a failure raises on every rank.
+
+    After that no file is read: ``batches`` plans each batch on the host with vectorised numpy (``ResidentBatch``),
+    uploads its job table, headers and scans in one pinned copy, fills the batch buffer and the refused files' output
+    images with one ``faa_gather`` launch and decodes the accepted files as ``FileBatchStream`` does.  ``close`` is
+    collective too."""
+
+    def __init__(self, paths, device="cuda", index=None, progressive=False, progressive_index=False, multinode=False,
+                 group=None, workers=4):
+        self.paths = np.array([os.fspath(p) for p in paths], dtype=object)
+        self.device = torch.device(device)
+        if self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        self.multinode, self.group = bool(multinode), group
+        self._own_ptr, self._opened = 0, []
+        n = len(self.paths)
+        rank = dist.get_rank(group) if self.multinode else 0
+        peers = host_ranks(group) if self.multinode else [0]
+        self.n_local, self.local_rank = len(peers), peers.index(rank)
+        self.own = resident_owned(n, self.local_rank, self.n_local)
+        t0 = time.perf_counter()
+        err = plan = None
+        try:
+            with ThreadPoolExecutor(workers, thread_name_prefix="faa-resident") as pool:
+                read = chunked_map(pool.map, workers)
+                hbs = [read_jpeg_batch(self.paths[self.own[k:k + RESIDENT_CHUNK]], read, None, progressive,
+                                       progressive_index) for k in range(0, len(self.own), RESIDENT_CHUNK)]
+            plan = ShardPlan(hbs, index)
+        except Exception as e:                                   # noqa: BLE001
+            err = e
+        self.timing = {"read": time.perf_counter() - t0}
+        free = torch.cuda.mem_get_info(self.device)[0]
+        if self.multinode:
+            check_fit(None if plan is None else plan.need, free, err, group)
+        elif err is not None:
+            raise err
+        elif plan.need > free:
+            raise RuntimeError(fit_error([plan.need], [free]))
+        self.device_bytes = plan.need
+        self.n_tables = len(plan.tables)
+        handle = None
+        try:
+            t0 = time.perf_counter()
+            with torch.cuda.device(self.device):
+                ptr, h = ctypes.c_void_p(), (ctypes.c_ubyte * 64)()
+                _lib.check(_lib.lib.faa_peer_alloc(plan.need, ctypes.byref(ptr), h))
+                self._own_ptr, handle = ptr.value, bytes(h)
+                self.shard = torch.as_tensor(_RawCuda(self._own_ptr, (plan.need,)), device=self.device)
+                _upload(self.shard, plan.parts())
+                torch.cuda.synchronize(self.device)
+                self.timing["upload"] = time.perf_counter() - t0
+                t0 = time.perf_counter()
+                if index is None:
+                    self._build_points(plan)
+                self.timing["index"] = time.perf_counter() - t0
+        except Exception as e:                                   # noqa: BLE001
+            err = e
+        if not self.multinode:
+            if err is not None:
+                self._release()
+                raise err
+            self._install([(plan.meta, plan.scans, self._own_ptr, plan.tables_off)], [0])
+            return
+        t0 = time.perf_counter()
+        try:
+            self._exchange(plan, handle, err, peers, rank)
+        except RuntimeError:
+            self._release()
+            raise
+        self.timing["exchange"] = time.perf_counter() - t0
+
+    def _exchange(self, plan, handle, err, peers, rank):
+        """the collective metadata exchange and the mapping of the host peers' shards"""
+        mine = None
+        if err is None:
+            try:
+                mine = pack_shard_meta(plan.meta, plan.scans, handle, self.device.index, plan.tables_off)
+            except Exception as e:                               # noqa: BLE001
+                err = e
+        bufs, err = gather_bytes(mine, err, self.group)
+        if err is None:
+            try:
+                shards = []
+                for r in peers:
+                    meta, scans, h, dev, tables_off = unpack_shard_meta(bufs[r])
+                    if r == rank:
+                        base = self._own_ptr
+                    else:
+                        with torch.cuda.device(self.device):
+                            _lib.check(_lib.lib.faa_enable_peer_access(dev))
+                            p = ctypes.c_void_p()
+                            _lib.check(_lib.lib.faa_peer_open((ctypes.c_ubyte * 64).from_buffer_copy(h), ctypes.byref(p)))
+                        base = p.value
+                        self._opened.append(base)
+                    shards.append((meta, scans, base, tables_off))
+                self._install(shards, peers)
+            except Exception as e:                               # noqa: BLE001
+                err = e
+        agree(err, self.group, "resident JPEG store")
+
+    def _build_points(self, plan):
+        """the accepted files' scan indexes, built over the uploaded shard, written into their room"""
+        acc = plan.accepted
+        if not len(acc):
+            return
+        m = plan.meta
+        scans = {}
+        if len(plan.scans):
+            scans = dict(scans=plan.scans, scan_first=plan.scan_first())
+        enc = EncodedImages(self.shard[:plan.tables_off], plan.headers(), plan.tables,
+                            _d_pool=self.shard[plan.tables_off:plan.points_off], **scans)
+        counts, parts = [], []
+        for k in range(0, len(acc), RESIDENT_INDEX_CHUNK):
+            first, pts = build_jpeg_index(enc.select(np.arange(k, min(len(acc), k + RESIDENT_INDEX_CHUNK))))
+            counts.append(np.diff(first))
+            parts.append(pts)
+        count = np.concatenate(counts)
+        m["n_points"][acc] = count
+        pts = np.concatenate(parts)
+        if len(pts):
+            rows = np.zeros((plan.pixels_off - plan.points_off) // 16, _lib.JPEG_SYNC_DTYPE)
+            k = np.arange(len(pts)) - np.repeat(np.cumsum(count) - count, count)
+            rows[(np.repeat(m["points_at"][acc], count) - plan.points_off) // 16 + k] = pts
+            self.shard[plan.points_off:plan.pixels_off].copy_(torch.from_numpy(rows.view(np.uint8)))
+
+    def _install(self, shards, peers):
+        """the split-wide host arrays from every host peer's (meta, scans, base address, table region offset)"""
+        n = len(self.paths)
+        self.meta = np.zeros(n, RESIDENT_META_DTYPE)
+        self.src = np.zeros(n, _SRC_DTYPE)
+        self.owner = np.zeros(n, np.int64)
+        own = [resident_owned(n, j, len(peers)) for j in range(len(peers))]
+        for j, (meta, _, base, tables_off) in enumerate(shards):
+            if len(meta) != len(own[j]):
+                raise ValueError("local rank %d holds %d files, not %d" % (j, len(meta), len(own[j])))
+            at = own[j]
+            self.meta[at] = meta
+            self.owner[at] = j
+            b = np.uint64(base)
+            self.src["file"][at] = b + meta["hdr"]["offset"].astype(np.uint64)
+            self.src["tables"][at] = b + np.uint64(tables_off) + (meta["table_at"] * _TABLE_BYTES).astype(np.uint64)
+            self.src["points"][at] = b + meta["points_at"].astype(np.uint64)
+            self.src["pixels"][at] = b + meta["pixels_at"].astype(np.uint64)
+        self.scan_first = np.concatenate([[0], np.cumsum(self.meta["n_scans"])]).astype(np.int64)
+        self.scans = np.zeros(int(self.scan_first[-1]), _lib.JPEG_SCAN_DTYPE)
+        for j, (meta, scans, _, _) in enumerate(shards):
+            cnt = meta["n_scans"].astype(np.int64)
+            to = np.repeat(self.scan_first[own[j]], cnt) + np.arange(len(scans)) - np.repeat(np.cumsum(cnt) - cnt, cnt)
+            self.scans[to] = scans
+
+    def plan(self, sel):
+        """``ResidentBatch`` of the split's files ``sel``"""
+        return ResidentBatch(self.meta, self.src, self.scan_first, self.scans, sel)
+
+    def batches(self, batches):
+        """generator of one ``RaggedImages`` per batch of split positions in ``batches``; each batch's decode status is
+        checked once the next batch is queued, and at the end (``check_decodes``)"""
+        dev = self.device
+        pending = []
+        for sel in batches:
+            p = self.plan(sel)
+            out = RaggedImages.empty(p.sizes, dev)
+            buf = torch.empty(p.total, dtype=torch.uint8, device=dev)
+            jobs = p.jobs(buf.data_ptr(), out.storage.data_ptr() + out.offsets[p.refused].astype(np.uint64))
+            parts = [jobs, p.headers] + ([p.first] if p.first is not None else []) + \
+                ([p.scan_first, p.scans] if p.scans is not None else [])
+            at = np.cumsum([0] + [_up16(a.nbytes) for a in parts])
+            host = torch.empty(int(at[-1]), dtype=torch.uint8, pin_memory=True)
+            h = host.numpy()
+            for o, a in zip(at, parts):
+                h[o:o + a.nbytes] = a.view(np.uint8).reshape(-1)
+            d = torch.empty(int(at[-1]), dtype=torch.uint8, device=dev)
+            d.copy_(host, non_blocking=True)
+            views = [d[o:o + a.nbytes] for o, a in zip(at, parts)]
+            gather(jobs, views[0], dev)
+            if len(p.accepted):
+                kw = {}
+                if p.first is not None:
+                    kw.update(first=p.first, points=np.empty(int(p.first[-1]), _lib.JPEG_SYNC_DTYPE),
+                              _d_first=views[2].view(torch.int64), _d_points=buf[p.points_at:p.total])
+                if p.scans is not None:
+                    k = 3 if p.first is not None else 2
+                    kw.update(scans=p.scans, scan_first=p.scan_first, _d_scan_first=views[k].view(torch.int64),
+                              _d_scans=views[k + 1])
+                enc = EncodedImages(buf[p.files_at:p.points_at], p.headers, np.empty(p.n_tables, _lib.JPEG_TABLE_DTYPE),
+                                    _d_pool=buf[:p.files_at], _d_headers=views[1], **kw)
+                _, status = decode_jpeg(enc, out.select(p.accepted))
+                queue_status(status, self.paths[np.asarray(sel, np.int64)[p.accepted]], dev, pending)
+            check_decodes(pending, keep=1 if len(p.accepted) else 0)
+            yield out
+        check_decodes(pending)
+
+    def _release(self):
+        with torch.cuda.device(self.device):
+            for p in self._opened:
+                _lib.lib.faa_peer_close(ctypes.c_void_p(p))
+            self._opened = []
+            if self.multinode:
+                dist.barrier(group=self.group)                   # no peer maps this rank's shard any more
+            if self._own_ptr:
+                self.shard = None
+                _lib.lib.faa_peer_free(ctypes.c_void_p(self._own_ptr))
+                self._own_ptr = 0
+
+    def close(self):
+        """free the store: collective under ``multinode``.  Every rank waits for its device, unmaps its peers' shards
+        and, once no rank maps it any more, frees its own."""
+        if self._own_ptr or self._opened:
+            torch.cuda.synchronize(self.device)
+            self._release()
+
+
+class ResidentJpegDataset:
+    """``JpegFileDataset`` whose files are held in device memory (``conf['faa_jpeg_resident']``): a
+    ``ResidentJpegStore`` of the split, sharded over the ranks of each host under ``multinode``, so the loaders read no
+    file after construction (collective under ``multinode``).  ``index``: a ``JpegIndex`` whose points the files take;
+    without one each rank builds its files' scan indexes on its device.  ``progressive`` / ``progressive_index``: as
+    ``JpegFileDataset``'s.  Subsets share the store; ``close`` frees it (collective under ``multinode``).
+    ``device_bytes``: the bytes of this rank's shard."""
+
+    def __init__(self, paths, targets, device="cuda", index=None, progressive=False, progressive_index=False,
+                 multinode=False, group=None):
+        if progressive_index and not progressive:
+            raise ValueError("progressive_index needs progressive")
+        self.targets = [int(t) for t in targets]
+        if len(self.targets) != len(paths):
+            raise ValueError("need one target per image")
+        self.store = ResidentJpegStore(paths, device, index, progressive, progressive_index, multinode, group)
+        self.files = np.arange(len(paths), dtype=np.int64)
+        self.labels = torch.as_tensor(self.targets, dtype=torch.int64, device=self.store.device)
+        self.device = self.labels.device
+
+    @property
+    def device_bytes(self):
+        return self.store.device_bytes
+
+    def __len__(self):
+        return len(self.files)
+
+    def select(self, idx):
+        """the split positions of a batch"""
+        return self.files[np.asarray(idx, np.int64)]
+
+    def subset(self, idx):
+        idx = [int(i) for i in idx]
+        d = ResidentJpegDataset.__new__(ResidentJpegDataset)
+        d.store, d.files = self.store, self.select(idx)
+        d.targets = [self.targets[i] for i in idx]
+        d.labels = self.labels.index_select(0, torch.as_tensor(idx, dtype=torch.int64, device=self.labels.device))
+        d.device = self.device
+        return d
+
+    def close(self):
+        self.store.close()
+
+
 class GpuAugmentedLoader:
     """What ``get_dataloaders`` hands to ``train.py:47`` / ``search.py:101`` instead of a torch ``DataLoader``:
     an iterable of ``(data, label)`` whose ``data`` is the augmented, normalised CUDA batch (``.cuda()`` at
@@ -1122,7 +1621,8 @@ class GpuAugmentedLoader:
         of the latest epoch is ``staging``).  When that dataset learns its index and ``sampler`` is a
         ``DistributedSampler`` under an initialised ``torch.distributed`` of more than one process, ``__iter__``
         starts every epoch with ``share_jpeg_index`` of the index, a collective, before any file is staged; ``tta``
-        exchanges nothing."""
+        exchanges nothing.  A ``ResidentJpegDataset``'s batches are gathered from its store and decoded
+        (``ResidentJpegStore.batches``)."""
         if not torch.cuda.is_available():
             raise _lib.FaaRuntimeError("fast_autoaugment_b200 needs a CUDA device (no CPU fallback)")
         self.dataset, self.batch_size, self.tail = dataset, int(batch), tail
@@ -1130,7 +1630,8 @@ class GpuAugmentedLoader:
         self.aug = Augmentation(policies) if policies is not None else Augmentation([[("Invert", 0.0, 0.0)]])
         self.seed = int(torch.initial_seed() if seed is None else seed) & 0x7FFFFFFFFFFFFFFF
         self.chain, self.chain_mode = chain, chain_mode
-        if isinstance(dataset, (RaggedDeviceDataset, EncodedDeviceDataset, JpegFileDataset)) and chain is None:
+        if isinstance(dataset, (RaggedDeviceDataset, EncodedDeviceDataset, JpegFileDataset, ResidentJpegDataset)) and \
+                chain is None:
             raise ValueError("images of different sizes need an ImageNetChain (conf['faa_crop_resize'])")
         self._drawn = 0                   # samples drawn so far: the Philox counter never repeats across epochs
         self.staging = None
@@ -1161,6 +1662,10 @@ class GpuAugmentedLoader:
                                            progressive=self.dataset.progressive, find=self.dataset.find,
                                            progressive_index=getattr(self.dataset, "progressive_index", False))
             files = self.staging([self.dataset.select(idx) for idx in batches], dev)
+        elif isinstance(self.dataset, ResidentJpegDataset):
+            dev = self.dataset.device
+            batches = [idx_all[k * self.batch_size:(k + 1) * self.batch_size] for k in range(len(self))]
+            files = self.dataset.store.batches([self.dataset.select(idx) for idx in batches])
         else:
             dev = self.dataset.images.device
         try:
@@ -1416,7 +1921,12 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
     the points it verified (DESIGN §4.8).  ``faa_jpeg_progressive_index`` (default False; needs
     ``faa_jpeg_progressive``): progressive files take a scan index too, so with ``faa_jpeg_index`` or
     ``faa_jpeg_index_learn`` their restart-free scans decode on many threads from points looked up or learned like any
-    other file's, with the same pixels (``python -m fast_autoaugment_b200.jpeg_index --progressive`` writes them)."""
+    other file's, with the same pixels (``python -m fast_autoaugment_b200.jpeg_index --progressive`` writes them).
+    ``faa_jpeg_resident`` (default False): the directory's splits are read, parsed and uploaded once, here, and held in
+    device memory (``ResidentJpegDataset``; with ``multinode=True`` a collective, the ranks of each host sharing each
+    split), so the loaders read no file; every file's scan index comes from ``faa_jpeg_index`` or is built on the device
+    here, and ``faa_jpeg_index_learn`` / ``faa_jpeg_index_find`` are refused.  ``dataset.device_bytes`` is what a
+    rank's shard takes, ``dataset.close()`` frees it."""
     from sklearn.model_selection import StratifiedShuffleSplit
 
     conf = C.get()
@@ -1446,16 +1956,26 @@ def get_dataloaders(dataset, batch, dataroot, split=0.15, split_idx=0, multinode
     progressive_index = bool(conf.get("faa_jpeg_progressive_index", False))
     if progressive_index and not progressive:
         raise ValueError("conf['faa_jpeg_progressive_index'] needs conf['faa_jpeg_progressive']")
+    resident = bool(conf.get("faa_jpeg_resident", False))
+    if resident and (learn or find):
+        raise ValueError("conf['faa_jpeg_resident'] builds every file's scan index on the device when the store is made: "
+                         "conf['faa_jpeg_index_learn'] and conf['faa_jpeg_index_find'] have nothing left to do")
+
+    def saved_index(x):
+        if not index_dir:
+            return None
+        path = os.path.join(os.fspath(index_dir), "%s.npz" % x.split)
+        if not os.path.exists(path):
+            raise FileNotFoundError("conf['faa_jpeg_index']: no index of the %s split at %s (write it with "
+                                    "python -m fast_autoaugment_b200.jpeg_index)" % (x.split, path))
+        return JpegIndex.load(path, x.folder)
 
     def device_dataset(x, y):
+        if isinstance(x, FilePaths) and resident:
+            return ResidentJpegDataset(x, y, index=saved_index(x), progressive=progressive,
+                                       progressive_index=progressive_index, multinode=multinode)
         if isinstance(x, FilePaths):
-            index = None
-            if index_dir:
-                path = os.path.join(os.fspath(index_dir), "%s.npz" % x.split)
-                if not os.path.exists(path):
-                    raise FileNotFoundError("conf['faa_jpeg_index']: no index of the %s split at %s (write it with "
-                                            "python -m fast_autoaugment_b200.jpeg_index)" % (x.split, path))
-                index = JpegIndex.load(path, x.folder)
+            index = saved_index(x)
             if learn and index is None:
                 index = JpegIndex.empty(x.folder)
             return JpegFileDataset(x, y, index=index, learn=learn, progressive=progressive, find=find,

@@ -272,41 +272,36 @@ def _unpack_delta(buf):
     return [names[e - k:e] for e, k in zip(ends, plen.tolist())], lengths, first, points
 
 
-def _fail_everywhere(err, group):
+def _fail_everywhere(err, group, what="JPEG index exchange"):
     """called on every rank at once when the flags of a collective step showed a failure: raise on every rank, naming
     each rank's error"""
     msgs = [None] * dist.get_world_size(group)
     dist.all_gather_object(msgs, None if err is None else "%s: %s" % (type(err).__name__, err), group=group)
-    raise RuntimeError("JPEG index exchange failed: " + "; ".join(
+    raise RuntimeError("%s failed: " % what + "; ".join(
         "rank %d: %s" % (r, m) for r, m in enumerate(msgs) if m is not None)) from err
 
 
-def share_jpeg_index(index, group=None, chunk_bytes=JPEG_INDEX_CHUNK):
-    """Collective: every rank of ``group`` sends the entries its ``JpegIndex`` learned since the last exchange
-    (``index.delta()``) to every other rank, and enters the other ranks' deltas in rank order (``index.merge``), so
-    every rank's index ends up listing what any rank learned.  Returns the number of entries merged here.
+def _exchange_device(group):
+    """where the exchanges' tensors live: the current device under NCCL, the host otherwise"""
+    return torch.device("cuda", torch.cuda.current_device()) if dist.get_backend(group) == "nccl" else torch.device("cpu")
 
-    One all-gather of the packed deltas' sizes, then, when any is not empty, rounds of all-gathers of at most
-    ``chunk_bytes`` of every rank's delta (so no rank ever holds world x its delta in flight), then one all-gather of
-    success flags.  Device tensors on the current device with NCCL, host tensors otherwise.  Every rank enters the
-    same collectives whatever fails locally: a delta that cannot be packed, one that does not unpack or merge (the
-    same verdict on every rank that reads it) or any other local error raises RuntimeError on every rank, naming each
-    rank's error, instead of leaving the others waiting.  Entries merged before a failure stay (a point only decides
-    how a file's decode is split, never its pixels)."""
-    rank, world = dist.get_rank(group), dist.get_world_size(group)
-    dev = torch.device("cuda", torch.cuda.current_device()) if dist.get_backend(group) == "nccl" else torch.device("cpu")
-    err = mine = None
-    try:
-        mine = _pack_delta(*index.delta())
-    except Exception as e:                                       # noqa: BLE001
-        err = e
+
+def _gather_sizes(mine, err, dev, group, what):
+    """all-gather of every rank's byte count (-1: the rank has nothing to send, ``err`` says why); raises on every rank
+    when any rank failed"""
     sizes = gather_pool(torch.tensor([-1 if mine is None else mine.size], dtype=torch.int64, device=dev), group)
     sizes = sizes.cpu().tolist()
     if min(sizes) < 0:
-        _fail_everywhere(err, group)
+        _fail_everywhere(err, group, what)
+    return sizes
+
+
+def _gather_rounds(mine, sizes, err, dev, group, chunk_bytes):
+    """every rank's uint8 array ``mine`` (of ``sizes[rank]`` bytes) to every rank, in all-gather rounds of at most
+    ``chunk_bytes`` per rank: (arrays in rank order, own one included, error).  Every rank enters every round whatever
+    fails locally; a failure is returned, not raised."""
+    rank, world = dist.get_rank(group), dist.get_world_size(group)
     top = max(sizes)
-    if top == 0:
-        return 0
     step = max(1, min(int(chunk_bytes), top))
     bufs = None
     try:
@@ -326,6 +321,40 @@ def share_jpeg_index(index, group=None, chunk_bytes=JPEG_INDEX_CHUNK):
                         bufs[r][at:at + k] = got[r * m:r * m + k]
             except Exception as e:                               # noqa: BLE001
                 err = e
+    return bufs, err
+
+
+def agree(err, group=None, what="collective step"):
+    """Collective: all-gather of every rank's success; when any rank failed (``err`` not None there), RuntimeError on
+    every rank naming each rank's error"""
+    oks = gather_pool(torch.tensor([int(err is None)], dtype=torch.int64, device=_exchange_device(group)), group)
+    if not bool(oks.all()):
+        _fail_everywhere(err, group, what)
+
+
+def share_jpeg_index(index, group=None, chunk_bytes=JPEG_INDEX_CHUNK):
+    """Collective: every rank of ``group`` sends the entries its ``JpegIndex`` learned since the last exchange
+    (``index.delta()``) to every other rank, and enters the other ranks' deltas in rank order (``index.merge``), so
+    every rank's index ends up listing what any rank learned.  Returns the number of entries merged here.
+
+    One all-gather of the packed deltas' sizes, then, when any is not empty, rounds of all-gathers of at most
+    ``chunk_bytes`` of every rank's delta (so no rank ever holds world x its delta in flight), then one all-gather of
+    success flags.  Device tensors on the current device with NCCL, host tensors otherwise.  Every rank enters the
+    same collectives whatever fails locally: a delta that cannot be packed, one that does not unpack or merge (the
+    same verdict on every rank that reads it) or any other local error raises RuntimeError on every rank, naming each
+    rank's error, instead of leaving the others waiting.  Entries merged before a failure stay (a point only decides
+    how a file's decode is split, never its pixels)."""
+    rank, world = dist.get_rank(group), dist.get_world_size(group)
+    dev = _exchange_device(group)
+    err = mine = None
+    try:
+        mine = _pack_delta(*index.delta())
+    except Exception as e:                                       # noqa: BLE001
+        err = e
+    sizes = _gather_sizes(mine, err, dev, group, "JPEG index exchange")
+    if max(sizes) == 0:
+        return 0
+    bufs, err = _gather_rounds(mine, sizes, err, dev, group, chunk_bytes)
     merged = 0
     if err is None:
         try:
@@ -340,10 +369,54 @@ def share_jpeg_index(index, group=None, chunk_bytes=JPEG_INDEX_CHUNK):
                 merged += len(delta[0])
         except Exception as e:                                   # noqa: BLE001
             err = e
-    oks = gather_pool(torch.tensor([int(err is None)], dtype=torch.int64, device=dev), group)
-    if not bool(oks.all()):
-        _fail_everywhere(err, group)
+    agree(err, group, "JPEG index exchange")
     return merged
+
+
+def local_ranks(hosts, rank):
+    """the ranks whose host name (``hosts``, one per rank) is ``rank``'s, in rank order"""
+    return [r for r, h in enumerate(hosts) if h == hosts[rank]]
+
+
+def host_ranks(group=None):
+    """Collective: all-gathers ``socket.gethostname()`` and returns ``local_ranks`` of this rank"""
+    import socket
+    hosts = [None] * dist.get_world_size(group)
+    dist.all_gather_object(hosts, socket.gethostname(), group=group)
+    return local_ranks(hosts, dist.get_rank(group))
+
+
+def fit_error(needs, frees):
+    """the RuntimeError message when any rank's need (bytes) exceeds its free device memory, else None"""
+    if all(n <= f for n, f in zip(needs, frees)):
+        return None
+    return "the resident JPEG store does not fit: " + "; ".join(
+        "rank %d needs %d bytes, %d free%s" % (r, n, f, " (too little)" if n > f else "")
+        for r, (n, f) in enumerate(zip(needs, frees)))
+
+
+def check_fit(need, free, err=None, group=None):
+    """Collective: every rank's device-memory need and free bytes (``need`` None: the rank failed before it knew,
+    ``err`` says why).  RuntimeError on every rank when any rank failed or any shard does not fit (``fit_error``)."""
+    dev = _exchange_device(group)
+    got = gather_pool(torch.tensor([-1 if need is None else int(need), int(free)], dtype=torch.int64, device=dev)
+                      .view(1, 2), group).cpu().tolist()
+    if min(n for n, _ in got) < 0:
+        _fail_everywhere(err, group, "resident JPEG store")
+    msg = fit_error([n for n, _ in got], [f for _, f in got])
+    if msg is not None:
+        raise RuntimeError(msg)
+
+
+def gather_bytes(mine, err=None, group=None, chunk_bytes=JPEG_INDEX_CHUNK, what="resident JPEG store"):
+    """Collective: every rank's uint8 array ``mine`` (None when the rank failed to make it, ``err`` then its error) to
+    every rank, in ``share_jpeg_index``'s rounds.  Returns ``(arrays in rank order, error)``; the caller reads them and
+    ends with ``agree``.  Raises on every rank when any rank had nothing to send."""
+    dev = _exchange_device(group)
+    sizes = _gather_sizes(mine, err, dev, group, what)
+    if max(sizes) == 0:
+        return [np.zeros(0, np.uint8) for _ in sizes], err
+    return _gather_rounds(mine, sizes, err, dev, group, chunk_bytes)
 
 
 class _RawCuda:

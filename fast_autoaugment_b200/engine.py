@@ -1087,6 +1087,16 @@ def _decoder(dev):
     return dec
 
 
+def gather(jobs, d_jobs, device):
+    """One launch of the byte copies ``jobs`` (host ``COPY_DTYPE`` [n]: addresses in this process, local or IPC
+    mappings) on ``device``'s current stream (C ABI ``faa_gather``).  ``d_jobs``: the same table's bytes on the device,
+    uploaded by the caller.  Raises ValueError before any device work for an empty table or a null address."""
+    jobs = np.ascontiguousarray(jobs, dtype=_lib.COPY_DTYPE).reshape(-1)
+    dev = torch.device(device)
+    with torch.cuda.device(dev):
+        check(lib.faa_gather(jobs.ctypes.data, d_jobs.data_ptr(), len(jobs), _stream_ptr(dev)))
+
+
 def _augment_ragged(policy, batch: RaggedImages, tail, samples, boxes, rng, out):
     """augment_batch on a RaggedImages batch (C ABI ``faa_augment_ragged``); policies of more than two ops run window
     by window through uint8 intermediates, as ``_augment_launch`` does"""

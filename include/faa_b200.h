@@ -251,6 +251,14 @@ int faa_peer_alloc(size_t bytes, void** d_ptr, unsigned char* handle64);
 int faa_peer_open(const unsigned char* handle64, void** d_ptr);
 int faa_peer_close(void* d_ptr);
 int faa_peer_free(void* d_ptr);
+
+/* ---- one launch of many byte copies (the resident JPEG store's per-batch gather): job i copies exactly d_jobs[i].bytes
+ * bytes from src to dst, either of which may be an IPC mapping of another GPU's buffer (faa_peer_open).  h_jobs is a
+ * host copy of the same table, used to validate and to size the grid: null tables, n <= 0 or a job with a null src
+ * or dst fail with FAA_ERR_VALUE before any device work.  Jobs must not overlap each other's destinations.  Addresses
+ * that agree modulo 16 move as 16-byte words; any alignment is allowed. */
+typedef struct faa_copy { const void* src; void* dst; uint64_t bytes; } faa_copy_t;
+int faa_gather(const faa_copy_t* h_jobs, const faa_copy_t* d_jobs, int n, void* stream);
 int faa_mix_u8_peer(faa_policy_t* p, const uint8_t* d_a, const uint8_t* const* d_partner_ptrs,
                     const int16_t* d_zero_box_a, const int16_t* d_zero_box_b, void* d_out, int batch, int h, int w,
                     const faa_tail_t* tail, float lam, float one_minus_lam, void* stream);
